@@ -1,21 +1,25 @@
 #!/usr/bin/env python
 """bench.py -- candidate windows/s of the PICO cascade scan (RunCascade, core/pigo.go:212-258) on 1080p frames.
 
-Contract (driver): `python bench.py --gpus N --steps K --warmup W` (N>1 under torchrun, one rank per GPU) prints ONE JSON
-line on rank 0.  A "step" = one pass of the hot path (scan of every (scale,row,col) window + emission-order finalize,
+Usage: `python bench.py --gpus N --steps K --warmup W` (N>1 under torchrun, one rank per GPU) prints ONE JSON
+line on rank 0.  K is the number of timed steps of the headline metric.  A "step" = one pass of the hot path (scan of every (scale,row,col) window + emission-order finalize,
 then for N>1 the single NCCL gather of the detection slices) over one batch of synthetic frames.
 
 Workload = BASELINE.json configs[2]: batch of 256 x 1920x1080 uint8 frames PER GPU (weak scaling), facefinder cascade,
 reference test parameters MinSize 20 / MaxSize 1000 / ShiftFactor 0.2 / ScaleFactor 1.1 (core/pigo_test.go:44-50),
 894,448 windows per frame.  configs[1] (one 1080p frame) is a pure latency case (one frame is ~6 us of issue work);
 it is measured too and reported under "single_frame", but the metric -- a throughput -- is quoted on the batch.
-Inputs (530 MB per GPU) exceed the 126 MB L2, so no L2 flush is needed between iterations.
+Inputs (530 MB per GPU) exceed the 50 MB L2 of an H100, so no L2 flush is needed between iterations.
+
+`--dump-outputs DIR` writes what the last timed step computed (rank 0's frames) as DIR/counts.npy (float64 [frames], the
+per-frame detection counts) and DIR/detections.npy (float32 [n, 5]: frame, row, col, scale, q of every stored detection, in
+the library's output order), so that two builds can be compared output for output on identical seeded inputs.
 
   value     : windows/s, frames already resident in HBM, timed with CUDA events on the launching stream, max over ranks
   e2e       : same metric through the public host API (pigo_run_cascade_batch with HOST buffers): pinned H2D of the
               frames and D2H of counts+detections inside the timed region
   roofline  : the scan kernel's ALGORITHMIC bytes (frames*rows*dim + 16*n_det + cascade bytes; SURVEY.md section 8d)
-              over its CUDA-event duration, against MEASURED_PEAKS.json hbm_gbs.  This path is issue/latency bound,
+              over its CUDA-event duration, against MEASURED_PEAKS.json hbm_gbs (else the H100 SXM data sheet's 3350 GB/s).  This path is issue/latency bound,
               NOT HBM bound (2.3 B/window): the fraction is reported as it is.
   cpu_baseline / --impl reference : the CPU restatement of the reference (oracle/, kind "port" -- the reference is Go
               and no Go toolchain exists here) on the host cores, frame-parallel, bounded sample.
@@ -57,7 +61,7 @@ def make_frames(nframes: int, seed0: int) -> np.ndarray:
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (read-only queries)."""
 
     def __init__(self, index: int):
         self.rows, self.proc, self.index = [], None, index
@@ -79,6 +83,7 @@ class ClockSampler:
     def stop(self):
         if self.proc:
             self.proc.terminate()
+            self.proc.wait()
         sm = [float(r[0]) for r in self.rows if len(r) >= 7 and r[0].replace(".", "").isdigit()]
         mx = [float(r[1]) for r in self.rows if len(r) >= 7 and r[1].replace(".", "").isdigit()]
         reasons = set()
@@ -133,6 +138,21 @@ def cpu_sample_frames(nthreads: int, requested: int) -> int:
     return requested or max(16, min(512, 4 * nthreads))
 
 
+def dump_outputs(path: str, out: np.ndarray, cnt: np.ndarray) -> None:
+    """Writes the detections a caller of the timed path receives: per frame the first min(count, cap) rows of `out`
+    (int32 row, col, scale and the float32 bits of q), flattened with the frame index in front."""
+    os.makedirs(path, exist_ok=True)
+    nf, cap = out.shape[0], out.shape[1]
+    stored = np.minimum(cnt, cap)
+    rows = []
+    for f in range(nf):
+        d = out[f, :stored[f]]
+        rows.append(np.column_stack([np.full(len(d), f, np.float32), d[:, :3].astype(np.float32), d[:, 3].view(np.float32)]))
+    dets = np.concatenate(rows) if rows else np.zeros((0, 5), np.float32)
+    np.save(os.path.join(path, "counts.npy"), cnt.astype(np.float64))
+    np.save(os.path.join(path, "detections.npy"), dets.astype(np.float32))
+
+
 def _claim_stdout():
     """The contract is ONE JSON line on stdout: everything else any library writes to fd 1 (NCCL prints its version
     banner there at WARN level, torchrun children inherit the fd) is sent to stderr; the line itself goes to the saved fd."""
@@ -159,7 +179,11 @@ def main():
     ap.add_argument("--no-extra", action="store_true", help="skip the configs[3] / configs[4] blocks (developer runs)")
     ap.add_argument("--pipeline-frames", type=int, default=64, help="frames per GPU per step of the configs[4] pipeline block")
     ap.add_argument("--opts", default="", help="developer sweeps: library options as name=value,... (default: none)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the detections of the last timed step (rank 0) as .npy files under DIR")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     out_fd = _claim_stdout()
 
     rank = int(os.environ.get("RANK", "0"))
@@ -261,6 +285,8 @@ def main():
     barrier()
     ms_total = max_over_ranks(e0.elapsed_time(e1))
     launches = pigo_b200.launch_count() - launches0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, d_out.cpu().numpy(), d_cnt.cpu().numpy())
     for _ in range(args.steps):   # keep the GPU under the same load while the sampler collects a few more points
         step_device()
     torch.cuda.synchronize()
@@ -294,8 +320,8 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "MEASURED_PEAKS.json hbm_gbs (of measured)" if "hbm_gbs" in peaks else "6650 GB/s (of fallback)"
+    peak = float(peaks.get("hbm_gbs", 3350.0))
+    peak_src = "MEASURED_PEAKS.json hbm_gbs (of measured)" if "hbm_gbs" in peaks else "3350 GB/s (H100 SXM data sheet)"
     dom = max(kt.items(), key=lambda kv: kv[1]["total_ms"]) if kt else None
     roofline = None
     if dom:
@@ -307,23 +333,9 @@ def main():
         scan_ms = sum(v["total_ms"] for k, v in kt.items() if k != "finalize") / args.steps
         launch_ms = dom[1]["avg_us"] / 1e3
         achieved = alg_bytes / (launch_ms * 1e-3) / 1e9
-        traffic = None
-        traffic_src = None
-        for name in ("traffic_r02.json", "traffic_r01.json"):
-            try:   # dram__bytes_read.sum + dram__bytes_write.sum of ONE launch from the committed ncu --set full capture
-                tr = json.load(open(os.path.join(ROOT, "profiles", name)))
-                if tr.get("kernel") == dom[0]:
-                    same = tr["frames_per_launch"] == frames_per_launch
-                    traffic = tr["dram_bytes_per_launch"] * (1.0 if same else frames_per_launch / tr["frames_per_launch"])
-                    traffic_src = f"profiles/{name}: ncu dram bytes of one captured launch of {tr['frames_per_launch']} frames" + \
-                        ("" if same else ", scaled by frames per launch")
-                    break
-            except Exception:
-                pass
         roofline = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                    "traffic": traffic, "kernel": dom[0], "kernel_launch_ms": launch_ms, "frames_per_launch": frames_per_launch,
+                    "kernel": dom[0], "kernel_launch_ms": launch_ms, "frames_per_launch": frames_per_launch,
                     "scan_kernels_ms_per_step": scan_ms, "algorithmic_bytes_per_launch": alg_bytes, "peak_source": peak_src,
-                    "traffic_note": traffic_src,
                     "kernels": kt, "tile_role_lanes": lanes, "note": "path is issue/latency/L2-transaction bound (2.3 algorithmic B/window), not HBM "
                     "bound; see DESIGN.md"}
 

@@ -1,6 +1,6 @@
 // Package pigo is the cgo shim that makes libpigo_b200.so a drop-in for the detection path of
 // github.com/esimov/pigo/core (package name "pigo"): same exported types, methods and argument meaning, host
-// code stays in Go, every hot loop runs in hand-written sm_100a CUDA behind the C-ABI of include/pigo_b200.h.
+// code stays in Go, every hot loop runs in hand-written sm_90a CUDA behind the C-ABI of include/pigo_b200.h.
 //
 // NOT COMPILED IN THE BUILD CONTAINER: that image has no Go toolchain (SURVEY.md section 0: go/gccgo/tinygo
 // absent), so this file is the reference-side binding a maintainer adds (INTEGRATION.md), kept beside the

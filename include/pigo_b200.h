@@ -1,5 +1,5 @@
 /*
- * pigo_b200.h -- C-ABI of libpigo_b200.so, the B200 (sm_100a) drop-in for the
+ * pigo_b200.h -- C-ABI of libpigo_b200.so, the H100 (sm_90a) drop-in for the
  * detection path of esimov/pigo (package "pigo", import github.com/esimov/pigo/core).
  *
  * Every entry point states the reference interface it replaces (file:line under the
@@ -11,7 +11,7 @@
  *  - plain pointers and sizes only; no CUDA/torch types (streams travel as void*).
  *  - every function returns a pigo_status (0 = ok, <0 = error); pigo_last_error() returns
  *    a thread-local message for the last failure on the calling thread.
- *  - the library NEVER falls back to a CPU path: without a usable sm_100 device every
+ *  - the library NEVER falls back to a CPU path: without a usable sm_90 device every
  *    compute entry point fails with PIGO_E_NODEVICE / PIGO_E_CUDA.
  *  - the caller owns all input/output buffers.  Host buffers are copied inside the call
  *    (cgo rule: C keeps no Go pointer after return).  Handles own their device tables and
@@ -48,7 +48,7 @@ typedef enum {
   PIGO_E_CUDA = -2,     /* CUDA runtime failure; see pigo_last_error() */
   PIGO_E_CAP = -3,      /* output capacity too small; n_out holds the required count */
   PIGO_E_NOMEM = -4,
-  PIGO_E_NODEVICE = -5  /* no sm_100 device visible: there is no CPU fallback */
+  PIGO_E_NODEVICE = -5  /* no sm_90 device visible: there is no CPU fallback */
 } pigo_status;
 
 /* Where the caller's frame / output buffers live. */

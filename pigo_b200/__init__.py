@@ -1,8 +1,7 @@
 """pigo_b200 -- host-side mirror (Python/ctypes) of the pigo Go API over libpigo_b200.so.
 
-The product is the C-ABI library (include/pigo_b200.h, hand-written sm_100a CUDA).  The reference's
-host language is Go and no Go toolchain exists in this image, so the Go shim lives in go/pigo/
-(uncompiled here; see INTEGRATION.md) and THIS module is the mirror the tests and bench.py drive.
+The product is the C-ABI library (include/pigo_b200.h, hand-written sm_90a CUDA).  The reference's
+host language is Go, so the Go shim lives in go/pigo/ (see INTEGRATION.md) and THIS module is the mirror the tests and bench.py drive.
 Names follow the reference (core/pigo.go, core/puploc.go, core/flploc.go):
 
     Pigo / NewPigo().Unpack(bytes)            core/pigo.go:46-110
@@ -13,7 +12,7 @@ Names follow the reference (core/pigo.go, core/puploc.go, core/flploc.go):
     CascadeParams, ImageParams, Detection, Puploc, FlpCascade     same exported fields
 
 There is NO CPU fallback: importing works anywhere (so that CPU-only checks can verify the exported
-symbols), but every compute call needs the CUDA library and an sm_100 device and raises otherwise.
+symbols), but every compute call needs the CUDA library and an sm_90 (H100) device and raises otherwise.
 """
 from __future__ import annotations
 

@@ -1,4 +1,4 @@
-"""Builds pigo_b200/lib/libpigo_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Builds pigo_b200/lib/libpigo_b200.so in-tree with nvcc for sm_90a (cross-compiles without a GPU)."""
 from __future__ import annotations
 
 import glob
@@ -12,7 +12,7 @@ LIBDIR = os.path.join(HERE, "lib")
 SO = os.path.join(LIBDIR, "libpigo_b200.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
     "-fmad=false",            # Go/amd64 never fuses a*b+c; keep float32/float64 results bit-identical
     "-Xcompiler", "-fPIC,-fvisibility=hidden", "-shared", "-cudart", "static",
     "-Xptxas", "-v",

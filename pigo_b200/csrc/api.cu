@@ -122,7 +122,7 @@ static std::mutex g_dev_mu;
 static int g_sms[kMaxDevices] = {};          // 0 = not validated yet
 static std::atomic<unsigned> g_mask{0};
 
-int device_sms(int dev) { return (dev >= 0 && dev < kMaxDevices && g_sms[dev] > 0) ? g_sms[dev] : 148; }
+int device_sms(int dev) { return (dev >= 0 && dev < kMaxDevices && g_sms[dev] > 0) ? g_sms[dev] : 132; }
 
 int use_device(int dev) {
   if (dev < 0 || dev >= kMaxDevices) return set_err(PIGO_E_INVALID, "device %d out of range", dev);
@@ -139,8 +139,8 @@ int use_device(int dev) {
       if (dev >= n) return set_err(PIGO_E_INVALID, "device %d out of range (0..%d)", dev, n - 1);
       cudaDeviceProp prop;
       CUDA_TRY(cudaGetDeviceProperties(&prop, dev));
-      if (prop.major != 10)
-        return set_err(PIGO_E_NODEVICE, "device %d is sm_%d%d; this library contains sm_100a code only", dev, prop.major, prop.minor);
+      if (prop.major != 9 || prop.minor != 0)
+        return set_err(PIGO_E_NODEVICE, "device %d is sm_%d%d; this library contains sm_90a code only", dev, prop.major, prop.minor);
       g_sms[dev] = prop.multiProcessorCount;
     }
   }
@@ -256,10 +256,9 @@ using namespace pigo;
 // Frames per pipeline group of one batch call.  Resident frames: uniform groups of 128 (fewest kernel tails; the deferred
 // queues of a group stay bounded).  Host frames: 64, with or without in-kernel waiting (host_stream): with it the fused kernel
 // of a group is copy-bound and ends when the group's last chunk arrives, and the group's tail kernels then overlap the next
-// group's copy.  PCIe (49-51 GB/s measured: 10.5-10.8 ms for 256 x 1080p) and the scan (10.4 ms) run at
-// the same rate, so a step costs about  [time the scan idles behind the first copy chunks] + [scan]  and also at least
+// group's copy.  When PCIe and the scan run at about the same rate, a step costs about  [time the scan idles behind the first copy chunks] + [scan]  and also at least
 // [copy] + [tail kernels of the last group]; stream_taper = 1 (128, then half of the rest) shortens the second term but
-// its small groups lengthen the first (measured 13.2 vs 12.6 ms); stream_taper = 2 (1/8, 1/4, 3/8, 3/16, 1/16 of the batch)
+// its small groups lengthen the first; stream_taper = 2 (1/8, 1/4, 3/8, 3/16, 1/16 of the batch)
 // tries to shorten both.
 static std::vector<int> group_schedule(int nframes, bool resident, bool streamed) {
   std::vector<int> g;
@@ -285,7 +284,7 @@ static std::vector<int> group_schedule(int nframes, bool resident, bool streamed
     return g;
   }
   const bool auto_sub = sub <= 0;
-  if (sub <= 0) sub = resident ? 128 : 64;   // streamed host frames: 64 measured best (12.0 vs 12.5 ms with 128: a group's tail kernels overlap the next group's chunks)
+  if (sub <= 0) sub = resident ? 128 : 64;   // streamed host frames: 64 (a group's tail kernels overlap the next group's chunks)
   for (int left = nframes; left > 0; left -= (int)sub) g.push_back((int)std::min<long long>(sub, left));
   if (auto_sub && streamed && taper == 3 && g.size() >= 2 && g.back() >= 32) {
     // the step ends one group's tail kernels after the last chunk: halve the LAST group only
@@ -742,7 +741,6 @@ static WorkspacePool g_misc_pool[kMaxDevices];   // scratch of the handle-less e
 // library can be used again afterwards.
 int pigo_shutdown_impl(void) {
   for (int d = 0; d < kMaxDevices; ++d) {
-    if (device_sms(d) == 148 && g_misc_pool[d].free_list.empty()) continue;
     if (g_misc_pool[d].free_list.empty()) continue;
     if (cudaSetDevice(d) != cudaSuccess) { cudaGetLastError(); continue; }
     cudaDeviceSynchronize();

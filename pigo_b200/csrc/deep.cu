@@ -135,7 +135,7 @@ __global__ void __launch_bounds__(256) deep_kernel(const ScanArgs A, unsigned lo
 // Shared-memory variant (unrotated, large calls): ONE CTA PER SM keeps the tree records [t_lo, t_lo + ktrees) of the tiled table
 // (kTreeRec bytes each: codes, leaves, threshold -- the layout the fused kernel stages) in its 227 KB of shared memory, filled by
 // the TMA bulk engine.  A walk then costs two pixel gathers per level through L1TEX instead of two gathers plus a divergent
-// 64-bit node load: the kernel is bound by L1TEX sectors (ncu r02g: 86 %), and a third of them were node loads.  Consecutive
+// 64-bit node load: the kernel is bound by L1TEX sectors, and a third of them are node loads.  Consecutive
 // trees sit 130 words apart, so the GROUP lanes of a window (consecutive trees, same node index at the root) read distinct banks.
 // Trees below t_lo (thin-tail handoffs of the tile warps, latency-mode items) take the global path of deep_walk.
 __device__ __forceinline__ float deep_walk_smem(const uint8_t* __restrict__ rec, const uint8_t* __restrict__ pc, int s, int dim) {
@@ -222,7 +222,7 @@ __global__ void __launch_bounds__(1024) deep_smem_kernel(const ScanArgs A, unsig
 
 // Resident range [t_lo, t_lo + k): t_lo and k even (16-byte alignment / size of the bulk copy), clipped to the cascade and to what
 // one CTA's shared memory holds.  The launch puts as many CTAs on an SM as the range allows: a smaller range leaves more of the
-// 256 KB L1/shared array to the L1 cache, which the pixel gathers live on (measured: all 446 trees resident = 2x SLOWER).
+// 256 KB L1/shared array to the L1 cache, which the pixel gathers live on.
 static constexpr size_t kDeepSmemMax = 232448;
 void launch_deep_smem(const ScanArgs& A, unsigned long long* counter, const uint8_t* tab_tiled, int num_sms, int threads, int group,
                       int t_lo, int k, cudaStream_t st) {
@@ -249,8 +249,8 @@ void launch_deep_smem(const ScanArgs& A, unsigned long long* counter, const uint
 }
 
 // Flat loop (option deep_flat=1): every iteration each lane group either fetches its next window or walks one step.  No group
-// waits for another at a reconvergence point (ncu round 1: 16.6 of 32 lanes active per instruction in the nested loop), but
-// every fetch now delays the step of the three other groups; measured 3 % slower on the bench workload, kept as a variant.
+// waits for another at a reconvergence point, but every fetch now delays the step of the three other groups; off by default,
+// kept as a variant.
 template <int GROUP, int ROT>
 __global__ void __launch_bounds__(256) deep_flat_kernel(const ScanArgs A, unsigned long long* counter) {
   const unsigned FULL = 0xffffffffu;

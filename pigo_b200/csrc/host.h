@@ -28,7 +28,7 @@ void timing_end(int slot, cudaStream_t st);
 struct Options {
   std::atomic<long long> scan_mode{0};      // 0 auto (fused + gather-v2 + deep), 1 universal gather kernel only, 3 gather-v2 + deep only
   std::atomic<long long> chunk{256};        // windows per work chunk of the universal gather kernel
-  std::atomic<long long> gather_ctas_per_sm{4};   // CTAs per SM of the gather-v2 kernel (0 = occupancy)
+  std::atomic<long long> gather_ctas_per_sm{0};   // CTAs per SM of the gather-v2 kernel (0 = auto: 2 unrotated, 4 rotated; capped at occupancy)
   std::atomic<long long> tile_max_scale{0}; // largest window size routed to the tile warps (0 = auto)
   std::atomic<long long> tile_warps{24};    // warps (= private tile buffers) per CTA of the fused kernel
   std::atomic<long long> tile_ni{1};        // item slots per lane of a tile warp
@@ -66,7 +66,7 @@ struct Options {
   std::atomic<long long> puploc_stage{1};   // pair kernel: 0 = all global, 1 = the current stage's node codes staged in shared memory, 2 = + the stage's pixel patch when it fits
   std::atomic<long long> puploc_mode{0};    // RunDetector kernel: 0 = (perturbation, tree)-pair kernel, 1 = warp-per-perturbation kernel
   std::atomic<long long> lanes{1};          // internal streams the groups alternate between
-  std::atomic<long long> tile_tail_min{10}; // tail policy threshold (sweep r02g: 6 -> 10 is 1 % on the bench workload)
+  std::atomic<long long> tile_tail_min{6};  // tail policy threshold
   std::atomic<long long> tile_band_ratio{0};    // a band spans scales up to ratio/100 x its first scale; 0 = auto (200, or 140 for calls of <= 2 M windows)
   std::atomic<long long> timing{0};         // 1 = bracket every kernel with CUDA events (bench.py roofline pass)
   std::atomic<long long>* find(const std::string& k) {
@@ -252,20 +252,20 @@ struct WsGuard {
 // The library serves up to kMaxDevices GPUs from one process (SURVEY.md section 8e: single process, frames sharded over the
 // devices of a mask).  Handles keep the parsed tables on the host and build one device replica per GPU on first use.
 constexpr int kMaxDevices = 16;
-int use_device(int dev);        // validates (sm_100) + cudaSetDevice on the calling thread
+int use_device(int dev);        // validates (sm_90) + cudaSetDevice on the calling thread
 int default_device();           // device of the non-sharded entry points (pigo_init, implicit device 0)
 int device_sms(int dev);
 std::vector<int> shard_devices();   // devices of the mask given to pigo_init_devices, ascending
 
 struct FaceReplica {            // device copy of one face cascade
-  int device = 0, num_sms = 148;
+  int device = 0, num_sms = 132;
   DevBuf codes, preds, thresh, tiled_tab;
   FaceTables tab{};
   WorkspacePool pool;
   ~FaceReplica() { cudaSetDevice(device); codes.release(); preds.release(); thresh.release(); tiled_tab.release(); }
 };
 struct PuplocReplica {
-  int device = 0, num_sms = 148;
+  int device = 0, num_sms = 132;
   DevBuf codes, preds;
   PuplocTables tab{};
   WorkspacePool pool;

@@ -174,8 +174,7 @@ __device__ __forceinline__ int clamp_coord(float v) { return max(-(1 << 30), min
 
 // STAGED: the node codes of the CURRENT STAGE (trees x 4L bytes: 40 KB for a landmark cascade, 80 KB for the pupil cascade)
 // are copied to shared memory with coalesced loads before the stage's walks, so that the per-level child fetch is a
-// shared-memory load instead of a lane-divergent global one (ncu round 2, unstaged: L1TEX 71 % busy at 25 sectors per
-// request, issue 47 %); the shared copy skews consecutive trees by 8 bytes, otherwise every tree's node i would sit in the
+// shared-memory load instead of a lane-divergent global one (the unstaged kernel is bound by L1TEX sectors); the shared copy skews consecutive trees by 8 bytes, otherwise every tree's node i would sit in the
 // same bank.  The pixel pairs stay global gathers (a landmark seed's patch is up to ~100 KB).
 // PATCH (with STAGED): before a stage whose sample area -- the bounding box of all perturbations' centres +- scale/2, clamped
 // to the image -- fits `patch_cap` bytes, that area is copied to shared memory with coalesced 16-byte loads and the

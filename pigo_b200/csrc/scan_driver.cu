@@ -13,7 +13,7 @@
 
 namespace pigo {
 
-static constexpr size_t kSmemPerCta = 232448;  // 227 KB opt-in maximum on sm_100
+static constexpr size_t kSmemPerCta = 232448;  // 227 KB opt-in maximum on sm_90
 
 // Builds the shared-memory-layout cascade table: one 516-byte record per tree (depth 6 only).
 int build_tiled_tables(const FaceTables& tab, const std::vector<int8_t>& codes, const std::vector<float>& preds,
@@ -144,7 +144,7 @@ static FusedPlan plan_fused(const std::vector<ScaleEntry>& plan, int ntrees, int
   if (P.ni != 1 || P.ks <= P.head || P.ks > 63 || g_opt.tile_prefetch.load()) P.head = 0;
   // Optional cap on the tile core (developer knob; more, shorter tiles).
   long long core_cap = g_opt.tile_core_cap.load();
-  if (core_cap <= 0) core_cap = 512;   // (measured: 16/32-pixel cores for a single frame are SLOWER, 0.26 vs 0.22 ms: tile fills dominate)
+  if (core_cap <= 0) core_cap = 512;   // (16/32-pixel cores mean many more tile fills per frame)
   // per-scale offset tables: NI = 1, no head, its own (shorter) raw prefix for the gather warps
   if (g_opt.tile_ptab.load() != 0 && P.ni == 1 && P.W > 0) {
     P.kt = (int)std::min<long long>(std::min<long long>(std::max<long long>(1, g_opt.ptab_kt.load()), ntrees), 60);
@@ -152,8 +152,7 @@ static FusedPlan plan_fused(const std::vector<ScaleEntry>& plan, int ntrees, int
     P.head = 0;
   }
   // band width: 2x the band's first scale for throughput; a call of <= 2 M windows (one or two 1080p frames) takes narrower bands
-  // (1.4x) -- more, shorter tiles, so that the slowest tile warp of the one partial wave finishes earlier (single 1080p frame:
-  // 0.16-0.20 -> 0.14-0.17 ms; from 4 frames / one 4K frame on the wide bands win again, on the 256-frame batch by 5 %)
+  // (1.4x) -- more, shorter tiles, so that the slowest tile warp of the one partial wave finishes earlier
   unsigned long long call_windows = 0;
   for (const ScaleEntry& e : plan) call_windows += (unsigned long long)e.nrows * (unsigned long long)e.ncols;
   call_windows *= (unsigned long long)std::max(1, batch_frames);
@@ -382,13 +381,12 @@ int run_scan(FaceReplica* c, Workspace* w, int lane, ScanArgs& A, unsigned long 
   T.tile_prefetch = g_opt.tile_prefetch.load() ? 1 : 0;
   T.gather_ni = (int)std::min<long long>(std::max<long long>(1, g_opt.gather_ni.load()), 3);
   // how long a gather-role window stays in the fused kernel before it leaves for the deep kernel (which walks a window with a
-  // lane group and is the cheaper place for long walks).  Measured (profiles/sweeps_r02.txt, "gather_limit"): up to ~32 1080p
-  // frames per call leaving after 8 trees is 10-35 % faster end to end, from 64 frames on 24 trees is best by ~2 %.
+  // lane group and is the cheaper place for long walks): small and mid-sized calls hand over after 8 trees, large ones after 24.
   long long glimit = g_opt.gather_limit.load();
   const unsigned long long call_windows = (unsigned long long)A.wins_per_frame * (unsigned long long)std::max(1, A.batch_frames);
   // "small call" = at most 4 M windows in the whole API call (a 1080p frame has 0.9 M, a 4K frame 3.7 M): latency matters, not throughput
   const bool small_call = call_windows <= 4000000ull;
-  // (the rotated scan has no fused kernel: its block kernel keeps 24 trees unless the call is small, 8 costs it up to 40 %)
+  // (the rotated scan has no fused kernel: its block kernel keeps 24 trees unless the call is small)
   if (glimit <= 0) glimit = (rot ? small_call : call_windows <= 40000000ull) ? 8 : 24;
   T.gather_limit = (int)std::min<long long>(glimit, 1 << 20);
   // small batches (a frame or two) cannot fill the GPU with 256-window blocks: use 64-window blocks then
@@ -486,10 +484,13 @@ int run_scan(FaceReplica* c, Workspace* w, int lane, ScanArgs& A, unsigned long 
     }
     if (G.consume_q1 || G.gather_blocks_per_frame > 0) {
       const size_t smem = ((384 + (size_t)G.ks * kTreeRec + 127) & ~(size_t)127);
+      // unrotated, the kernel drains the tile warps' stragglers and the large scales, and on H100 two CTAs per SM measured faster
+      // than four (256 x 1080p: 11 % less step time together with tile_tail_min 6); rotated, it is the whole scan and keeps four
       int per_sm = (int)g_opt.gather_ctas_per_sm.load();
+      if (per_sm <= 0) per_sm = rot ? 4 : 2;
       if (rot) G.gather_ni = std::min(G.gather_ni, 2);
       const int occ = gather2_ctas_per_sm(smem, G.gather_ni, rot);
-      if (per_sm <= 0 || per_sm > occ) per_sm = occ;
+      if (per_sm > occ) per_sm = occ;
       timing_begin(T_GATHER, st);
       launch_scan_gather2(G, num_sms * per_sm, smem, st);
       timing_end(T_GATHER, st);

@@ -557,8 +557,8 @@ __global__ void __launch_bounds__(MAXT, 1) scan_tiled_kernel(const TiledArgs A, 
           }
         } else {
           // Plain walk: one 32-bit node load per level (fewest shared-memory wavefronts; the kernel is L1TEX-bound).
-          // (Round 2 tried explicit 32-bit shared-window addresses via inline ld.shared and a byte-offset index -- about three
-          // instructions less per level on paper -- and measured 2 % SLOWER: the volatile asm loads pin the schedule.)
+          // (Explicit 32-bit shared-window addresses via inline ld.shared save about three instructions per level on paper,
+          // but the volatile asm loads pin the schedule.)
 #pragma unroll
           for (int u = 0; u < NI; ++u) idx[u] = 1;
 #pragma unroll
@@ -671,7 +671,7 @@ __global__ void __launch_bounds__(MAXT, 1) scan_tiled_kernel(const TiledArgs A, 
 // Per-scale offset tables (round 2, option tile_ptab).  Same warp specialisation, tiles, queues and results as the classic
 // kernel; what changes is WHERE the tile role's node data comes from.  The classic walk derives a node's two sample positions
 // from four int8 codes, the window size and the tile pitch at every level (3 PRMT, 4 IMAD, 3 SHF, 2 LEA, 2 IMAD: 24 instructions
-// per level, ncu r02g: issue 74 %).  Here every tiled ladder entry has its own table of the first kt trees in global memory
+// per level).  Here every tiled ladder entry has its own table of the first kt trees in global memory
 // (ptab_kernel): a node is ONE word holding the two tile offsets ((code*s)>>8)*pitch + ((code*s)>>8), biased by
 // halo*(pitch+1) so that both are unsigned 16-bit, and a level is LDS, LOP, 2 x IADD-class, 2 x LDS.U8, ISETP, index update.
 // A table depends on the scale, so the tile warps of a CTA walk the scales in step: the CTA works in ROUNDS (tile_warps
@@ -680,7 +680,7 @@ __global__ void __launch_bounds__(MAXT, 1) scan_tiled_kernel(const TiledArgs A, 
 // both (lane refill continues across a scale change); it LEAVES a scale when its last lane of that scale is done or evicted
 // (mbarrier arrive), the warp that completes the barrier issues the TMA bulk copy of the table two steps ahead into the freed
 // buffer, and a warp ENTERS the next scale when that copy has landed (mbarrier phase).  Windows alive after kt trees go to the
-// deep queue.  MEASURED (profiles/sweeps_r02.txt): SLOWER than the classic kernel -- see DESIGN.md; kept as a tested option.
+// deep queue.  Off by default (the classic kernel is the default; see DESIGN.md); kept as a tested option.
 constexpr uint32_t kPtCtl = 384;    // full[0..1], empty[0..1] mbarriers (8 bytes each), then the two "filled for sequence" words
 constexpr uint32_t kPtCasc = 448;   // raw cascade prefix of the gather role
 constexpr uint32_t kPtGap = 16;     // bytes between the two table buffers ("one past the last tree" of buffer 0 is not buffer 1)

@@ -1,5 +1,5 @@
 """CPU-side checks of the drop-in boundary: the C-ABI library builds, loads and exports every symbol
-include/pigo_b200.h declares, and fails LOUDLY (no CPU fallback) when no sm_100 device is present."""
+include/pigo_b200.h declares, and fails LOUDLY (no CPU fallback) when no sm_90 device is present."""
 import os
 import re
 

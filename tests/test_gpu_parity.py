@@ -688,7 +688,7 @@ def test_device_pipeline_capacity_and_rng_mode(gpu_face, sample_gray):
 
 
 def test_sharded_scan_matches_single_device(gpu_face, oracle_face):
-    """pigo_run_cascade_batch_sharded over every visible device (1 on the default test box, 2+ under gpurun --gpus N):
+    """pigo_run_cascade_batch_sharded over every visible device (1 on a single-GPU machine, 2+ on a multi-GPU one):
     frame shards, replicas built on first use, results in frame order == the per-frame oracle."""
     n = pigo_b200.device_count()
     pigo_b200.init_devices((1 << n) - 1)
@@ -718,7 +718,7 @@ def test_ycbcr_to_nrgba_matches_oracle(subsample):
 def test_cpp_sharded_over_every_visible_device():
     """tests/cpp/test_sharded.cpp: one process drives every visible GPU through include/pigo_b200.h (pigo_init_devices,
     pigo_run_cascade_batch_sharded, pigo_detect_batch_sharded) and requires byte-identical results to the 1-GPU calls.
-    With one GPU this exercises the same code with a single shard; run under `gpurun --gpus 2` it is the 2-device test."""
+    With one GPU this exercises the same code with a single shard; on a machine with two GPUs it is the 2-device test."""
     import os
     import subprocess
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

@@ -1,7 +1,7 @@
 """CPU-side check of the scan schedule (no GPU): the per-warp tiles of every band must PARTITION the windows of the band's
 scales (each window centre falls into exactly one tile core), every pixel a window of that tile can sample must lie inside
 the tile buffer, and the tile must fit the per-warp shared-memory budget.  Geometry bugs here would silently corrupt the
-GPU result, so they are pinned on the host where the driver runs `-m "not gpu"`."""
+GPU result, so they are pinned on the host, in the `-m "not gpu"` part of the suite."""
 import numpy as np
 import pytest
 

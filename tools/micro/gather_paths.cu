@@ -1,7 +1,7 @@
 // Micro-benchmark: lane-divergent 1-byte gathers (the access pattern of the straggler / deep / rotated / pupil kernels)
 // through (a) ld.global.nc, (b) tex1Dfetch on a linear texture, (c) tex2D on a pitch-linear texture.
 // Each thread emulates tree walks: 6 dependent levels, 2 byte samples per level inside an s x s patch around its window.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o gpurun_out/gather_paths tools/micro/gather_paths.cu
+//   mkdir -p build && nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o build/gather_paths tools/micro/gather_paths.cu
 #include <cuda_runtime.h>
 #include <cstdio>
 #include <cstdint>
@@ -69,7 +69,7 @@ int main() {
     cudaEvent_t a, b; cudaEventCreate(&a); cudaEventCreate(&b);
     for (int s : {24, 100}) for (int coherent : {0, 1}) for (int mode = 0; mode < 3; ++mode) {
       if ((mode == 1 && e1) || (mode == 2 && e2)) continue;
-      const int grid = 148 * 8, walks = 64;
+      const int grid = 132 * 8, walks = 64;
       float best = 1e9;
       for (int rep = 0; rep < 4; ++rep) {
         cudaEventRecord(a);

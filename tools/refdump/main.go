@@ -1,12 +1,12 @@
 // refdump -- runs the UNMODIFIED Go reference (github.com/esimov/pigo/core) on raw grayscale buffers and dumps what it
 // returns, so that the CPU oracle (oracle/pigo_oracle.c) can be pinned to true reference outputs on any box that has a Go
-// toolchain (this repo's build container and GPU box have none: `go version` fails, see DESIGN.md section 2).
+// toolchain (see DESIGN.md section 2).
 //
 // Build / run (offline, against the vendored module; nothing is written into the reference tree):
 //
 //	python tools/refdump/make_inputs.py                      # writes oracle/_ref/inputs/{manifest.json,*.u8}
-//	cd /root/reference && GOFLAGS=-mod=vendor GOCACHE=/tmp/gocache \
-//	    go run /root/repo/tools/refdump/main.go -in /root/repo/oracle/_ref/inputs -out /root/repo/oracle/_ref/refdump.json
+//	cd $PIGO_REF && GOFLAGS=-mod=vendor \
+//	    go run $REPO/tools/refdump/main.go -in $REPO/oracle/_ref/inputs -out $REPO/oracle/_ref/refdump.json
 //	python -m pytest tests/test_refdump.py                   # consumes the dump (skips while it is absent)
 //
 // What is dumped, per input buffer and parameter set of the manifest:
@@ -94,7 +94,7 @@ func drawn(seed int64, n int) []uint32 {
 func main() {
 	in := flag.String("in", "oracle/_ref/inputs", "directory with manifest.json and the raw buffers")
 	out := flag.String("out", "oracle/_ref/refdump.json", "output file")
-	casc := flag.String("cascade", "/root/reference/cascade", "cascade directory of the reference")
+	casc := flag.String("cascade", "cascade", "cascade directory of the reference (run from the reference checkout)")
 	flag.Parse()
 
 	mf, err := os.ReadFile(filepath.Join(*in, "manifest.json"))
