@@ -1,5 +1,6 @@
 // pipeline.go -- additive: the face -> ClusterDetections -> pupils -> landmarks sequence of cmd/pigo/main.go:369-565 /
-// core/flploc_test.go:75-154 for a whole frame batch in ONE library call (pigo_detect_batch: sequenced on the device).
+// core/flploc_test.go:75-154 for a whole frame batch, or for images of different sizes, in ONE library call
+// (pigo_detect_batch / pigo_detect_images: sequenced on the device).
 package pigo
 
 /*
@@ -70,16 +71,8 @@ func (pg *Pigo) DetectBatch(plc *PuplocCascade, calls []LandmarkCall, frames [][
 		copy(host[i*stride:(i+1)*stride], f)
 	}
 	ncalls := len(calls)
-	// C arrays of the call list (cgo: no Go pointers to Go pointers)
-	hs := (*[1 << 10]*C.pigo_puploc)(C.malloc(C.size_t(ncalls+1) * C.size_t(unsafe.Sizeof(uintptr(0)))))
+	hs, fl := callArrays(calls)
 	defer C.free(unsafe.Pointer(hs))
-	fl := make([]C.uint8_t, ncalls+1)
-	for i, c := range calls {
-		hs[i] = c.Cascade.h
-		if c.FlipV {
-			fl[i] = 1
-		}
-	}
 	prm := C.pigo_pipeline_params{min_size: C.int32_t(cp.MinSize), max_size: C.int32_t(cp.MaxSize), shift_factor: C.double(cp.ShiftFactor),
 		scale_factor: C.double(cp.ScaleFactor), angle: C.double(pp.Angle), iou_threshold: C.double(pp.IoU),
 		min_face_scale: C.int32_t(pp.MinFaceScale), eye_perturbs: C.int32_t(pp.EyePerturbs), flp_perturbs: C.int32_t(pp.FlpPerturbs)}
@@ -91,10 +84,10 @@ func (pg *Pigo) DetectBatch(plc *PuplocCascade, calls []LandmarkCall, frames [][
 		points := make([]C.pigo_point, nf*faceCap*(2+ncalls))
 		rc, err := call(func() C.int {
 			if pp.Sharded {
-				return C.pigo_detect_batch_sharded(pg.h, plc.h, (**C.pigo_puploc)(unsafe.Pointer(hs)), &fl[0], C.int(ncalls), (*C.uint8_t)(pinned), C.int(nf),
+				return C.pigo_detect_batch_sharded(pg.h, plc.h, hs, &fl[0], C.int(ncalls), (*C.uint8_t)(pinned), C.int(nf),
 					C.size_t(stride), C.int(cp.Rows), C.int(cp.Cols), C.int(cp.Dim), &prm, nil, C.uint64_t(key), &faces[0], C.int(faceCap), &nfaces[0], &points[0])
 			}
-			return C.pigo_detect_batch(pg.h, plc.h, (**C.pigo_puploc)(unsafe.Pointer(hs)), &fl[0], C.int(ncalls), (*C.uint8_t)(pinned), C.int(nf),
+			return C.pigo_detect_batch(pg.h, plc.h, hs, &fl[0], C.int(ncalls), (*C.uint8_t)(pinned), C.int(nf),
 				C.size_t(stride), C.int(cp.Rows), C.int(cp.Cols), C.int(cp.Dim), &prm, nil, C.uint64_t(key), &faces[0], C.int(faceCap), &nfaces[0], &points[0],
 				C.PIGO_MEM_HOST, nil)
 		})
@@ -113,22 +106,106 @@ func (pg *Pigo) DetectBatch(plc *PuplocCascade, calls []LandmarkCall, frames [][
 		if err != nil {
 			panic(err)
 		}
-		out := make([][]FaceResult, nf)
-		for f := 0; f < nf; f++ {
-			for k := 0; k < int(nfaces[f]); k++ {
-				d := faces[f*faceCap+k]
-				fr := FaceResult{Face: Detection{int(d.row), int(d.col), int(d.scale), float32(d.q)}}
-				if int(d.scale) > pp.MinFaceScale {
-					p := points[(f*faceCap+k)*(2+ncalls):]
-					fr.LeftEye = &Puploc{Row: int(p[0].row), Col: int(p[0].col), Scale: float32(p[0].scale)}
-					fr.RightEye = &Puploc{Row: int(p[1].row), Col: int(p[1].col), Scale: float32(p[1].scale)}
-					for c := 0; c < ncalls; c++ {
-						fr.Landmarks = append(fr.Landmarks, Puploc{Row: int(p[2+c].row), Col: int(p[2+c].col), Scale: float32(p[2+c].scale)})
-					}
-				}
-				out[f] = append(out[f], fr)
-			}
+		return faceResults(faces, nfaces, points, faceCap, ncalls, pp.MinFaceScale)
+	}
+}
+
+// callArrays returns the call list as C arrays (cgo: no Go pointers to Go pointers); the caller frees the handle array.
+func callArrays(calls []LandmarkCall) (**C.pigo_puploc, []C.uint8_t) {
+	hs := unsafe.Slice((**C.pigo_puploc)(C.malloc(C.size_t(len(calls)+1)*C.size_t(unsafe.Sizeof(uintptr(0))))), len(calls)+1)
+	fl := make([]C.uint8_t, len(calls)+1)
+	for i, c := range calls {
+		hs[i] = c.Cascade.h
+		if c.FlipV {
+			fl[i] = 1
 		}
-		return out
+	}
+	return &hs[0], fl
+}
+
+// faceResults converts the [n][faceCap] faces and [n][faceCap][2+ncalls] points of a pipeline call.
+func faceResults(faces []C.pigo_det, nfaces []C.int, points []C.pigo_point, faceCap, ncalls, minFaceScale int) [][]FaceResult {
+	out := make([][]FaceResult, len(nfaces))
+	for f := range out {
+		for k := 0; k < int(nfaces[f]); k++ {
+			d := faces[f*faceCap+k]
+			fr := FaceResult{Face: Detection{int(d.row), int(d.col), int(d.scale), float32(d.q)}}
+			if int(d.scale) > minFaceScale {
+				p := points[(f*faceCap+k)*(2+ncalls):]
+				fr.LeftEye = &Puploc{Row: int(p[0].row), Col: int(p[0].col), Scale: float32(p[0].scale)}
+				fr.RightEye = &Puploc{Row: int(p[1].row), Col: int(p[1].col), Scale: float32(p[1].scale)}
+				for c := 0; c < ncalls; c++ {
+					fr.Landmarks = append(fr.Landmarks, Puploc{Row: int(p[2+c].row), Col: int(p[2+c].col), Scale: float32(p[2+c].scale)})
+				}
+			}
+			out[f] = append(out[f], fr)
+		}
+	}
+	return out
+}
+
+// DetectImages runs the whole sequence for images of different sizes in one call (pigo_detect_images); result[i] lists
+// image i's clusters in the reference's order.  cp's MinSize, MaxSize, ShiftFactor and ScaleFactor are shared by every image
+// (cp's own ImageParams is not used).  There is no sharded mixed-size form: pp.Sharded panics.
+func (pg *Pigo) DetectImages(plc *PuplocCascade, calls []LandmarkCall, images []ImageParams, cp CascadeParams, pp PipelineParams) [][]FaceResult {
+	if pp.Sharded {
+		panic("pigo: DetectImages has no sharded form; use DetectBatch with Sharded for frames of one geometry")
+	}
+	n := len(images)
+	if n == 0 {
+		return nil
+	}
+	// pixels in one pinned buffer (256-byte aligned slices), descriptors in C memory, as RunCascadeImages does
+	offs := make([]int, n)
+	total := 0
+	for i, im := range images {
+		offs[i] = total
+		total += (len(im.Pixels) + 255) &^ 255
+	}
+	var pinned unsafe.Pointer
+	if _, err := call(func() C.int { return C.pigo_alloc_pinned(&pinned, C.size_t(total+256)) }); err != nil {
+		panic(err)
+	}
+	defer C.pigo_free_pinned(pinned)
+	host := unsafe.Slice((*uint8)(pinned), total+256)
+	desc := unsafe.Slice((*C.pigo_image)(C.malloc(C.size_t(n)*C.size_t(unsafe.Sizeof(C.pigo_image{})))), n)
+	defer C.free(unsafe.Pointer(&desc[0]))
+	for i, im := range images {
+		copy(host[offs[i]:], im.Pixels)
+		desc[i] = C.pigo_image{pixels: (*C.uint8_t)(unsafe.Pointer(&host[offs[i]])), rows: C.int32_t(im.Rows), cols: C.int32_t(im.Cols),
+			dim: C.int32_t(im.Dim)}
+	}
+	ncalls := len(calls)
+	hs, fl := callArrays(calls)
+	defer C.free(unsafe.Pointer(hs))
+	prm := C.pigo_pipeline_params{min_size: C.int32_t(cp.MinSize), max_size: C.int32_t(cp.MaxSize), shift_factor: C.double(cp.ShiftFactor),
+		scale_factor: C.double(cp.ScaleFactor), angle: C.double(pp.Angle), iou_threshold: C.double(pp.IoU),
+		min_face_scale: C.int32_t(pp.MinFaceScale), eye_perturbs: C.int32_t(pp.EyePerturbs), flp_perturbs: C.int32_t(pp.FlpPerturbs)}
+	key := atomic.AddUint64(&plc.seed, 1)
+	faceCap := 32
+	for {
+		faces := make([]C.pigo_det, n*faceCap)
+		nfaces := make([]C.int, n)
+		points := make([]C.pigo_point, n*faceCap*(2+ncalls))
+		rc, err := call(func() C.int {
+			return C.pigo_detect_images(pg.h, plc.h, hs, &fl[0], C.int(ncalls), &desc[0], C.int(n), &prm, nil, C.uint64_t(key), &faces[0],
+				C.int(faceCap), &nfaces[0], &points[0], C.PIGO_MEM_HOST, nil)
+		})
+		if rc == C.PIGO_E_CAP {
+			grown := false
+			for _, c := range nfaces {
+				if int(c) > faceCap {
+					faceCap, grown = int(c), true
+				}
+			}
+			if !grown {
+				prm.det_cap = 4 * (prm.det_cap + 512) // raw detections per image exceeded det_cap
+			}
+			continue
+		}
+		if err != nil {
+			panic(err)
+		}
+		return faceResults(faces, nfaces, points, faceCap, ncalls, pp.MinFaceScale)
 	}
 }

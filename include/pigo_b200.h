@@ -193,6 +193,14 @@ int pigo_puploc_run_frames(const pigo_puploc *p, const pigo_point *seeds, int ns
                            size_t frame_stride, int rows, int cols, int dim, double angle, const uint8_t *flipv,
                            pigo_point *out, unsigned flags, void *stream);
 
+/* Additive mixed-size form: seed i refines on images[seed_image[i]] (pigo_image as in pigo_run_cascade_images, each with
+ * its own rows, cols, dim; seed_image may be NULL when nimages == 1).  The descriptor array lives in host memory; with
+ * PIGO_FRAMES_DEVICE every `pixels` is a device pointer holding rows*dim bytes, otherwise host memory holding
+ * (rows-1)*dim + cols bytes.  Everything else as pigo_puploc_run_frames.  1 <= nimages <= 65535, rows, cols >= 1. */
+int pigo_puploc_run_images(const pigo_puploc *p, const pigo_point *seeds, int nseeds, const int32_t *seed_image,
+                           const float *randoms, uint64_t rng_seed, const pigo_image *images, int nimages, double angle,
+                           const uint8_t *flipv, pigo_point *out, unsigned flags, void *stream);
+
 /* ---- (*PuplocCascade).GetLandmarkPoint(leftEye, rightEye *Puploc, img, perturb, flipV) *Puploc,
  * core/flploc.go:36-57: seed arithmetic in float64 on the host, then RunDetector(angle 0). */
 int pigo_get_landmark_point(const pigo_puploc *p, const pigo_point *left_eye, const pigo_point *right_eye,
@@ -234,6 +242,21 @@ int pigo_detect_batch_sharded(const pigo_cascade *face, const pigo_puploc *puplo
                               size_t frame_stride, int rows, int cols, int dim, const pigo_pipeline_params *params,
                               const float *randoms, uint64_t rng_seed, pigo_det *faces, int face_cap, int *n_faces,
                               pigo_point *points);
+
+/* Additive mixed-size form of pigo_detect_batch: `nimages` images of any geometry (photos, thumbnails, several cameras)
+ * in one call, frame f replaced by image i.  Outputs faces[nimages][face_cap], n_faces[nimages],
+ * points[nimages][face_cap][2 + ncalls]; randoms (optional) [nimages][face_cap][2 + ncalls][63][3].  Image i's slices are
+ * byte for byte what pigo_detect_batch(nframes = 1) returns for that image alone given its randoms slice; the library
+ * generator's key is the same (slot = i*face_cap*(2+ncalls) + k*(2+ncalls) + call), so on images of one geometry both
+ * calls agree byte for byte.  det_cap / face_cap, PIGO_E_CAP with the required counts, flags and stream as
+ * pigo_detect_batch.  The descriptor array lives in host memory; pixels as pigo_run_cascade_images.  The CascadeParams
+ * fields and angle of `params` are shared by every image.  0 <= nimages <= 65535, rows, cols >= 1 per image,
+ * nimages*face_cap*(2+ncalls) <= 2^31-1.  Invalid arguments fail with PIGO_E_INVALID before any device work; a stream that
+ * is being captured into a CUDA graph is rejected with PIGO_E_INVALID. */
+int pigo_detect_images(const pigo_cascade *face, const pigo_puploc *puploc, const pigo_puploc *const *flp,
+                       const uint8_t *flp_flip, int ncalls, const pigo_image *images, int nimages,
+                       const pigo_pipeline_params *params, const float *randoms, uint64_t rng_seed, pigo_det *faces,
+                       int face_cap, int *n_faces, pigo_point *points, unsigned flags, void *stream);
 
 /* ---- RgbToGrayscale(src image.Image) []uint8, core/grayscale.go:8-23, for *image.NRGBA input (what GetImage returns,
  * core/image.go:13-33): gray = uint8((0.299 r + 0.587 g + 0.114 b) / 256) in float64 on the 16-bit, alpha-premultiplied

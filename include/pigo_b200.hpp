@@ -210,6 +210,52 @@ inline std::vector<std::vector<FaceResult>> DetectBatch(const Pigo& face, const 
     }
   return out;
 }
+// additive: DetectBatch for images of different sizes in one library call (host pixels; cp.Image is not used).  result[i] lists
+// image i's clusters; on PIGO_E_CAP the call is retried with the reported face count (or a larger det_cap).
+inline std::vector<std::vector<FaceResult>> DetectImages(const Pigo& face, const PuplocCascade& plc,
+                                                         const std::vector<std::pair<const PuplocCascade*, bool>>& calls,
+                                                         const std::vector<ImageParams>& images, const CascadeParams& cp, double iou, int min_face_scale,
+                                                         int eye_perturbs, int flp_perturbs, uint64_t rng_seed, double angle = 0.0, int face_cap = 32) {
+  const int ncalls = (int)calls.size(), n = (int)images.size();
+  std::vector<const pigo_puploc*> hs;
+  std::vector<uint8_t> fl;
+  for (auto& c : calls) { hs.push_back(c.first->handle()); fl.push_back(c.second ? 1 : 0); }
+  std::vector<pigo_image> desc((size_t)n);
+  for (int i = 0; i < n; ++i) desc[i] = pigo_image{images[i].Pixels, images[i].Rows, images[i].Cols, images[i].Dim};
+  pigo_pipeline_params prm{};
+  prm.min_size = cp.MinSize; prm.max_size = cp.MaxSize; prm.shift_factor = cp.ShiftFactor; prm.scale_factor = cp.ScaleFactor; prm.angle = angle;
+  prm.iou_threshold = iou; prm.min_face_scale = min_face_scale; prm.eye_perturbs = eye_perturbs; prm.flp_perturbs = flp_perturbs; prm.det_cap = 0;
+  for (;;) {
+    std::vector<pigo_det> faces((size_t)(n > 0 ? n : 1) * face_cap);
+    std::vector<int> nfaces((size_t)(n > 0 ? n : 1));
+    std::vector<pigo_point> pts((size_t)(n > 0 ? n : 1) * face_cap * (2 + ncalls));
+    const int rc = pigo_detect_images(face.handle(), plc.handle(), hs.data(), fl.data(), ncalls, desc.data(), n, &prm, nullptr, rng_seed, faces.data(),
+                                      face_cap, nfaces.data(), pts.data(), PIGO_MEM_HOST, nullptr);
+    if (rc == PIGO_E_CAP) {
+      bool grown = false;
+      for (int i = 0; i < n; ++i)
+        if (nfaces[i] > face_cap) { face_cap = nfaces[i]; grown = true; }
+      if (!grown) prm.det_cap = 4 * (prm.det_cap + 512);   // raw detections per image exceeded det_cap
+      continue;
+    }
+    check(rc);
+    std::vector<std::vector<FaceResult>> out((size_t)n);
+    for (int f = 0; f < n; ++f)
+      for (int k = 0; k < nfaces[f]; ++k) {
+        const pigo_det& d = faces[(size_t)f * face_cap + k];
+        FaceResult r;
+        r.Face = Detection{d.row, d.col, d.scale, d.q};
+        if (d.scale > min_face_scale) {
+          const pigo_point* p = &pts[((size_t)f * face_cap + k) * (2 + ncalls)];
+          r.Refined = true;
+          r.LeftEye = Puploc{p[0].row, p[0].col, p[0].scale, 0}; r.RightEye = Puploc{p[1].row, p[1].col, p[1].scale, 0};
+          for (int c = 0; c < ncalls; ++c) r.Landmarks.push_back(Puploc{p[2 + c].row, p[2 + c].col, p[2 + c].scale, 0});
+        }
+        out[f].push_back(r);
+      }
+    return out;
+  }
+}
 inline PuplocCascade NewPuplocCascade() { return PuplocCascade(); }   // core/puploc.go:33
 
 }  // namespace pigo

@@ -43,7 +43,7 @@ ABI_SYMBOLS = [
     "pigo_set_option", "pigo_get_option", "pigo_rgba_to_gray", "pigo_puploc_run_frames", "pigo_device_alloc",
     "pigo_device_free", "pigo_device_upload", "pigo_describe_plan", "pigo_init_devices", "pigo_device_count",
     "pigo_device_download", "pigo_run_cascade_batch_sharded", "pigo_detect_batch", "pigo_detect_batch_sharded",
-    "pigo_ycbcr_to_nrgba", "pigo_run_cascade_images",
+    "pigo_ycbcr_to_nrgba", "pigo_run_cascade_images", "pigo_detect_images", "pigo_puploc_run_images",
 ]
 
 
@@ -105,6 +105,8 @@ def lib() -> C.CDLL:
         L.pigo_run_cascade_images.argtypes = [vp, vp, i, i, i, d, d, d, vp, i, vp, C.c_uint, vp]
         L.pigo_detect_batch.argtypes = [vp, vp, vp, vp, i, vp, i, sz, i, i, i, vp, vp, u64, vp, i, vp, vp, C.c_uint, vp]
         L.pigo_detect_batch_sharded.argtypes = [vp, vp, vp, vp, i, vp, i, sz, i, i, i, vp, vp, u64, vp, i, vp, vp]
+        L.pigo_detect_images.argtypes = [vp, vp, vp, vp, i, vp, i, vp, vp, u64, vp, i, vp, vp, C.c_uint, vp]
+        L.pigo_puploc_run_images.argtypes = [vp, vp, i, vp, vp, u64, vp, i, d, vp, vp, C.c_uint, vp]
         L.pigo_ycbcr_to_nrgba.argtypes = [vp, vp, vp, i, i, i, i, i, i, i, vp, vp, C.c_uint, vp]
         L.pigo_set_option.argtypes = [C.c_char_p, C.c_int64]
         L.pigo_get_option.argtypes = [C.c_char_p]
@@ -486,6 +488,30 @@ class PuplocCascade:
                                             rng_seed, fptr, nframes, frame_stride, rows, cols, dim, angle,
                                             fl.ctypes.data if fl is not None else None, out.ctypes.data,
                                             FRAMES_DEVICE if frames_on_device else MEM_HOST, None))
+        return [Puploc(int(o["row"]), int(o["col"]), float(np.float32(o["scale"])), int(o["perturbs"])) for o in out]
+
+    def run_detector_images(self, seeds: Sequence[Puploc], seed_image: Sequence[int], images: Sequence[ImageParams], angle: float = 0.0,
+                            flipv: Optional[Sequence[bool]] = None, randoms: Optional[np.ndarray] = None, rng_seed: int = 0) -> List[Puploc]:
+        """Batch over images of different sizes: seed i refines on images[seed_image[i]].  Pixels are host arrays, or for
+        every image alike device pointers (int) holding Rows*Dim bytes, as in Pigo.RunCascadeImages."""
+        if self._h is None:
+            raise PigoError(PIGO_E_INVALID, "cascade not unpacked")
+        n = len(seeds)
+        if n == 0:
+            return []
+        s = np.zeros(n, dtype=POINT_DTYPE)
+        for k, p in enumerate(seeds):
+            s[k] = (p.Row, p.Col, p.Scale, p.Perturbs)
+        si = np.ascontiguousarray(np.asarray(seed_image, dtype=np.int32))
+        out = np.zeros(n, dtype=POINT_DTYPE)
+        rnd = np.ascontiguousarray(randoms, dtype=np.float32) if randoms is not None else None
+        fl = np.ascontiguousarray(np.asarray(flipv, dtype=np.uint8)) if flipv is not None else None
+        on_dev = len(images) > 0 and all(isinstance(im.Pixels, int) for im in images)
+        keep = [None if on_dev else _pixels(im) for im in images]   # host pixels stay alive for the call
+        desc = image_descs([(im.Pixels if on_dev else p.ctypes.data, im.Rows, im.Cols, im.Dim) for im, p in zip(images, keep)])
+        _check(lib().pigo_puploc_run_images(self._h, s.ctypes.data, n, si.ctypes.data, rnd.ctypes.data if rnd is not None else None, rng_seed,
+                                            desc, len(images), angle, fl.ctypes.data if fl is not None else None, out.ctypes.data,
+                                            FRAMES_DEVICE if on_dev else MEM_HOST, None))
         return [Puploc(int(o["row"]), int(o["col"]), float(np.float32(o["scale"])), int(o["perturbs"])) for o in out]
 
     def RunDetector(self, pl: Puploc, img: ImageParams, angle: float, flipV: bool, randoms: Optional[np.ndarray] = None,

@@ -734,6 +734,145 @@ static int for_each_shard(int nframes, F fn) {
   return rc;
 }
 
+// ---- RunDetector over uniform frames or over an image table (pigo_puploc_run_frames / pigo_puploc_run_images) -----------
+// Host seeds of a standalone RunDetector call: Perturbs range and frame / image index.  *wide = some seed lies outside the
+// 32-bit envelope of the pair kernel (it then runs on the warp-per-perturbation kernel).
+static int check_puploc_seeds(const pigo_point* seeds, int nseeds, const int32_t* seed_frame, int nframes, const char* unit, bool* wide) {
+  for (int i = 0; i < nseeds; ++i) {
+    if (seeds[i].perturbs < 0 || seeds[i].perturbs > 63)
+      return set_err(PIGO_E_INVALID, "seed %d: Perturbs=%d outside 0..63 (the reference panics, core/puploc.go:261)", i, seeds[i].perturbs);
+    if (seed_frame && (seed_frame[i] < 0 || seed_frame[i] >= nframes)) return set_err(PIGO_E_INVALID, "seed %d: %s index out of range", i, unit);
+    if (!(std::fabs(seeds[i].scale) <= 16384.0f)) *wide = true;
+  }
+  return PIGO_OK;
+}
+
+// Geometry of the images of a RunDetector or pipeline call: every image is refined on, so it needs at least one pixel.
+static int check_image_geometry(const pigo_image* images, int nimages) {
+  for (int i = 0; i < nimages; ++i) {
+    const pigo_image& im = images[i];
+    if (im.rows <= 0 || im.cols <= 0 || im.dim < im.cols)
+      return set_err(PIGO_E_INVALID, "image %d: bad geometry rows=%d cols=%d dim=%d", i, im.rows, im.cols, im.dim);
+    if ((uint64_t)im.rows * (uint64_t)im.dim > 0x7fffffffull) return set_err(PIGO_E_INVALID, "image %d: larger than 2^31 bytes", i);
+    if (!im.pixels) return set_err(PIGO_E_INVALID, "image %d: null pixels", i);
+  }
+  return PIGO_OK;
+}
+
+// Pixels of a mixed-size call on the device.  Device images stay where they are; host images go to one 256-byte-aligned
+// arena in w->frames, a round256(rows*dim) slot each, of which only the (rows-1)*dim + cols bytes the reference may index
+// are copied.  The call's ImageDesc table (pixels, rows, cols, pitch) goes to w->img_tab; `staged` receives the device
+// descriptors of the images.
+static int stage_images(Workspace* w, const pigo_image* images, int nimages, bool frames_dev, cudaStream_t st, const ImageDesc** d_desc,
+                        std::vector<pigo_image>& staged) {
+  int rc = PIGO_OK;
+  staged.assign(images, images + nimages);
+  if (!frames_dev) {
+    std::vector<size_t> off(nimages);
+    size_t total = 0;
+    for (int i = 0; i < nimages; ++i) { off[i] = total; total += ((size_t)images[i].rows * images[i].dim + 255) & ~(size_t)255; }
+    if ((rc = w->frames.reserve(total + 256))) return rc;
+    for (int i = 0; i < nimages; ++i) {
+      uint8_t* dst = (uint8_t*)w->frames.p + off[i];
+      CUDA_TRY(cudaMemcpyAsync(dst, images[i].pixels, (size_t)(images[i].rows - 1) * images[i].dim + images[i].cols, cudaMemcpyHostToDevice, st));
+      staged[i].pixels = dst;
+    }
+  }
+  std::vector<ImageDesc> desc(nimages);
+  for (int i = 0; i < nimages; ++i) {
+    desc[i] = ImageDesc{};
+    desc[i].base = staged[i].pixels; desc[i].rows = staged[i].rows; desc[i].cols = staged[i].cols; desc[i].dim = staged[i].dim;
+  }
+  if ((rc = w->img_tab.reserve((size_t)nimages * sizeof(ImageDesc)))) return rc;
+  CUDA_TRY(cudaMemcpyAsync(w->img_tab.p, desc.data(), (size_t)nimages * sizeof(ImageDesc), cudaMemcpyHostToDevice, st));
+  *d_desc = (const ImageDesc*)w->img_tab.p;
+  return PIGO_OK;
+}
+
+// Where the seeds' pixels are: `nframes` uniform frames `stride` bytes apart, or (images != nullptr) an image table of
+// `nframes` entries.  Pointers are host or device memory as the call's flags say.
+struct PuplocPixels {
+  const uint8_t* frames;
+  int nframes;
+  size_t stride;
+  int rows, cols, dim;
+  const pigo_image* images;
+};
+
+static int puploc_run_on(pigo_puploc* p, const pigo_point* seeds, int nseeds, const int32_t* seed_frame, const float* randoms, uint64_t rng_seed,
+                         const PuplocPixels& px, double angle, const uint8_t* flipv, pigo_point* out, bool wide, unsigned flags, void* stream_) {
+  int rc = PIGO_OK;
+  const int dev = default_device();
+  PuplocReplica* R = puploc_replica(p, dev, &rc);
+  if (!R) return rc;
+  const bool frames_dev = flags & PIGO_FRAMES_DEVICE, out_dev = flags & PIGO_OUT_DEVICE;
+  WsGuard g(R->pool);
+  Workspace* w = g.w;
+  if (!w) return set_err(PIGO_E_CUDA, "could not create a CUDA stream");
+  cudaStream_t st = stream_ ? (cudaStream_t)stream_ : w->stream;
+  if ((rc = ws_enter(w, st))) return rc;
+  const uint8_t* d_pix = px.frames;
+  const ImageDesc* d_img = nullptr;
+  if (px.images) {
+    std::vector<pigo_image> staged;
+    if ((rc = stage_images(w, px.images, px.nframes, frames_dev, st, &d_img, staged))) return rc;
+  } else if (!frames_dev) {
+    const size_t bytes = px.stride * (size_t)(px.nframes - 1) + (size_t)(px.rows - 1) * px.dim + px.cols;   // what the reference may index
+    if ((rc = w->frames.reserve(px.stride * (size_t)(px.nframes - 1) + (size_t)px.rows * px.dim))) return rc;
+    CUDA_TRY(cudaMemcpyAsync(w->frames.p, px.frames, bytes, cudaMemcpyHostToDevice, st));
+    d_pix = (const uint8_t*)w->frames.p;
+  }
+  const int32_t* d_sf = seed_frame;
+  const pigo_point* d_seeds = seeds;
+  pigo_point* d_out = out;
+  const float* d_rnd = randoms;
+  const uint8_t* d_flip = flipv;
+  if (!out_dev) {
+    const size_t sb = (size_t)nseeds * sizeof(pigo_point), rb = (size_t)nseeds * 63 * 3 * sizeof(float);
+    if ((rc = w->scratch_a.reserve(2 * sb))) return rc;
+    d_seeds = (const pigo_point*)w->scratch_a.p;
+    d_out = (pigo_point*)((char*)w->scratch_a.p + sb);
+    CUDA_TRY(cudaMemcpyAsync(w->scratch_a.p, seeds, sb, cudaMemcpyHostToDevice, st));
+    if (randoms) {
+      if ((rc = w->scratch_b.reserve(rb))) return rc;
+      CUDA_TRY(cudaMemcpyAsync(w->scratch_b.p, randoms, rb, cudaMemcpyHostToDevice, st));
+      d_rnd = (const float*)w->scratch_b.p;
+    }
+    if (flipv) {
+      if ((rc = w->scratch_c.reserve(nseeds))) return rc;
+      CUDA_TRY(cudaMemcpyAsync(w->scratch_c.p, flipv, nseeds, cudaMemcpyHostToDevice, st));
+      d_flip = (const uint8_t*)w->scratch_c.p;
+    }
+    if (seed_frame) {
+      if ((rc = w->nout.reserve((size_t)nseeds * 4))) return rc;
+      CUDA_TRY(cudaMemcpyAsync(w->nout.p, seed_frame, (size_t)nseeds * 4, cudaMemcpyHostToDevice, st));
+      d_sf = (const int32_t*)w->nout.p;
+    }
+  }
+  int rot_slot = -1;
+  if (angle > 0.0) rot_slot = (int)(32.0 * (angle > 1.0 ? 1.0 : angle));  // core/puploc.go:252-256, :166
+  bool done = false;
+  timing_begin(T_PUPLOC, st);
+  if (g_opt.puploc_mode.load() == 0 && !wide) {
+    if ((rc = w->counters.reserve(64))) return rc;
+    CUDA_TRY(cudaMemsetAsync(w->counters.p, 0, 64, st));
+    PupWork W{};
+    W.seeds = d_seeds; W.out = d_out; W.randoms = d_rnd; W.rng_seed = rng_seed; W.frames = d_pix; W.frame_stride = px.stride;
+    W.slot_frame = d_sf; W.flipv = d_flip; W.slots_per_frame = 0; W.nrows = px.rows; W.ncols = px.cols; W.dim = px.dim; W.rot_slot = rot_slot;
+    W.first = 0; W.span = 1; W.stride = 1; W.nwork = nseeds; W.ntabs = 1; W.tab[0] = R->tab; W.images = d_img;
+    done = launch_puploc_pairs(W, (unsigned int*)w->counters.p, R->num_sms, st) == 0;
+  }
+  if (!done)
+    launch_puploc(R->tab, d_seeds, nseeds, d_rnd, rng_seed, d_pix, d_sf, px.stride, px.rows, px.cols, px.dim, rot_slot, d_flip, d_out, d_img, st);
+  timing_end(T_PUPLOC, st);
+  g_launches++;
+  CUDA_TRY(cudaGetLastError());
+  if (out_dev) return ws_leave_async(w, st);
+  CUDA_TRY(cudaMemcpyAsync(out, d_out, (size_t)nseeds * sizeof(pigo_point), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  return PIGO_OK;
+}
+
 // =========================================================================================================
 extern "C" {
 
@@ -1092,79 +1231,30 @@ int pigo_puploc_run_frames(const pigo_puploc* pc, const pigo_point* seeds, int n
   int rc = ensure_device();
   if (rc) return rc;
   if (nseeds == 0) return PIGO_OK;
-  const int dev = default_device();
-  PuplocReplica* R = puploc_replica(p, dev, &rc);
-  if (!R) return rc;
-  const bool frames_dev = flags & PIGO_FRAMES_DEVICE, out_dev = flags & PIGO_OUT_DEVICE;
-  bool wide = false;   // some seed outside the 32-bit envelope of the pair kernel (only checkable for host seeds)
-  if (!out_dev)
-    for (int i = 0; i < nseeds; ++i) {
-      if (seeds[i].perturbs < 0 || seeds[i].perturbs > 63)
-        return set_err(PIGO_E_INVALID, "seed %d: Perturbs=%d outside 0..63 (the reference panics, core/puploc.go:261)", i, seeds[i].perturbs);
-      if (seed_frame && (seed_frame[i] < 0 || seed_frame[i] >= nframes)) return set_err(PIGO_E_INVALID, "seed %d: frame index out of range", i);
-      if (!(std::fabs(seeds[i].scale) <= 16384.0f)) wide = true;
-    }
-  WsGuard g(R->pool);
-  Workspace* w = g.w;
-  if (!w) return set_err(PIGO_E_CUDA, "could not create a CUDA stream");
-  cudaStream_t st = stream_ ? (cudaStream_t)stream_ : w->stream;
-  if ((rc = ws_enter(w, st))) return rc;
-  const uint8_t* d_pix = pixels;
-  if (!frames_dev) {
-    const size_t bytes = frame_stride * (size_t)(nframes - 1) + (size_t)(rows - 1) * dim + cols;   // what the reference may index
-    if ((rc = w->frames.reserve(frame_stride * (size_t)(nframes - 1) + (size_t)rows * dim))) return rc;
-    CUDA_TRY(cudaMemcpyAsync(w->frames.p, pixels, bytes, cudaMemcpyHostToDevice, st));
-    d_pix = (const uint8_t*)w->frames.p;
-  }
-  const int32_t* d_sf = seed_frame;
-  const pigo_point* d_seeds = seeds;
-  pigo_point* d_out = out;
-  const float* d_rnd = randoms;
-  const uint8_t* d_flip = flipv;
-  if (!out_dev) {
-    const size_t sb = (size_t)nseeds * sizeof(pigo_point), rb = (size_t)nseeds * 63 * 3 * sizeof(float);
-    if ((rc = w->scratch_a.reserve(2 * sb))) return rc;
-    d_seeds = (const pigo_point*)w->scratch_a.p;
-    d_out = (pigo_point*)((char*)w->scratch_a.p + sb);
-    CUDA_TRY(cudaMemcpyAsync(w->scratch_a.p, seeds, sb, cudaMemcpyHostToDevice, st));
-    if (randoms) {
-      if ((rc = w->scratch_b.reserve(rb))) return rc;
-      CUDA_TRY(cudaMemcpyAsync(w->scratch_b.p, randoms, rb, cudaMemcpyHostToDevice, st));
-      d_rnd = (const float*)w->scratch_b.p;
-    }
-    if (flipv) {
-      if ((rc = w->scratch_c.reserve(nseeds))) return rc;
-      CUDA_TRY(cudaMemcpyAsync(w->scratch_c.p, flipv, nseeds, cudaMemcpyHostToDevice, st));
-      d_flip = (const uint8_t*)w->scratch_c.p;
-    }
-    if (seed_frame) {
-      if ((rc = w->nout.reserve((size_t)nseeds * 4))) return rc;
-      CUDA_TRY(cudaMemcpyAsync(w->nout.p, seed_frame, (size_t)nseeds * 4, cudaMemcpyHostToDevice, st));
-      d_sf = (const int32_t*)w->nout.p;
-    }
-  }
-  int rot_slot = -1;
-  if (angle > 0.0) rot_slot = (int)(32.0 * (angle > 1.0 ? 1.0 : angle));  // core/puploc.go:252-256, :166
-  bool done = false;
-  timing_begin(T_PUPLOC, st);
-  if (g_opt.puploc_mode.load() == 0 && !wide) {
-    if ((rc = w->counters.reserve(64))) return rc;
-    CUDA_TRY(cudaMemsetAsync(w->counters.p, 0, 64, st));
-    PupWork W{};
-    W.seeds = d_seeds; W.out = d_out; W.randoms = d_rnd; W.rng_seed = rng_seed; W.frames = d_pix; W.frame_stride = frame_stride;
-    W.slot_frame = d_sf; W.flipv = d_flip; W.slots_per_frame = 0; W.nrows = rows; W.ncols = cols; W.dim = dim; W.rot_slot = rot_slot;
-    W.first = 0; W.span = 1; W.stride = 1; W.nwork = nseeds; W.ntabs = 1; W.tab[0] = R->tab;
-    done = launch_puploc_pairs(W, (unsigned int*)w->counters.p, R->num_sms, st) == 0;
-  }
-  if (!done)
-    launch_puploc(R->tab, d_seeds, nseeds, d_rnd, rng_seed, d_pix, d_sf, frame_stride, rows, cols, dim, rot_slot, d_flip, d_out, st);
-  timing_end(T_PUPLOC, st);
-  g_launches++;
-  CUDA_TRY(cudaGetLastError());
-  if (out_dev) return ws_leave_async(w, st);
-  CUDA_TRY(cudaMemcpyAsync(out, d_out, (size_t)nseeds * sizeof(pigo_point), cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaStreamSynchronize(st));
-  return PIGO_OK;
+  bool wide = false;
+  if (!(flags & PIGO_OUT_DEVICE) && (rc = check_puploc_seeds(seeds, nseeds, seed_frame, nframes, "frame", &wide))) return rc;
+  const PuplocPixels px{pixels, nframes, frame_stride, rows, cols, dim, nullptr};
+  return puploc_run_on(p, seeds, nseeds, seed_frame, randoms, rng_seed, px, angle, flipv, out, wide, flags, stream_);
+}
+
+int pigo_puploc_run_images(const pigo_puploc* pc, const pigo_point* seeds, int nseeds, const int32_t* seed_image, const float* randoms,
+                           uint64_t rng_seed, const pigo_image* images, int nimages, double angle, const uint8_t* flipv, pigo_point* out,
+                           unsigned flags, void* stream_) {
+  if (nseeds < 0) return set_err(PIGO_E_INVALID, "negative nseeds");
+  if (!seeds) return set_err(PIGO_E_INVALID, "null seeds");
+  if (!out) return set_err(PIGO_E_INVALID, "null out");
+  if (nimages < 1 || nimages > 65535) return set_err(PIGO_E_INVALID, "nimages must be 1..65535");
+  if (!images) return set_err(PIGO_E_INVALID, "null images");
+  if (nimages > 1 && !seed_image) return set_err(PIGO_E_INVALID, "seed_image is required when nimages > 1");
+  int rc = check_image_geometry(images, nimages);
+  if (rc) return rc;
+  bool wide = false;
+  if (!(flags & PIGO_OUT_DEVICE) && (rc = check_puploc_seeds(seeds, nseeds, seed_image, nimages, "image", &wide))) return rc;
+  if (!pc) return set_err(PIGO_E_INVALID, "null cascade");
+  if ((rc = ensure_device())) return rc;
+  if (nseeds == 0) return PIGO_OK;
+  const PuplocPixels px{nullptr, nimages, 0, 0, 0, 0, images};
+  return puploc_run_on(const_cast<pigo_puploc*>(pc), seeds, nseeds, seed_image, randoms, rng_seed, px, angle, flipv, out, wide, flags, stream_);
 }
 
 int pigo_get_landmark_point(const pigo_puploc* p, const pigo_point* left_eye, const pigo_point* right_eye, const uint8_t* pixels,
@@ -1190,11 +1280,14 @@ int pigo_get_landmark_point(const pigo_puploc* p, const pigo_point* left_eye, co
 // The reference sequences these calls on the host (core/flploc_test.go:75-154, cmd/pigo/main.go:369-565); here one call
 // runs RunCascade, ClusterDetections, the eye-seed arithmetic, RunDetector for both eyes of every face, the
 // GetLandmarkPoint seed arithmetic and `ncalls` landmark RunDetector calls per face, stream-ordered on the device, with
-// one D2H copy of the results at the end.
-static int detect_batch_on(int dev, pigo_cascade* face, pigo_puploc* puploc, pigo_puploc* const* flp, const uint8_t* flp_flip, int ncalls,
-                           const uint8_t* frames, int nframes, size_t frame_stride, int rows, int cols, int dim, const pigo_pipeline_params& P,
-                           const float* randoms, uint64_t rng_seed, uint64_t slot_base, pigo_det* faces, int face_cap, int* n_faces,
-                           pigo_point* points, unsigned flags, void* stream_) {
+// one D2H copy of the results at the end.  Only the pixel source differs between the uniform batch and the mixed-size
+// call: `scan(w, st, dets, det_cap, cnt, W)` stages the pixels, runs RunCascade into dets[nframes][det_cap] / cnt[nframes]
+// on `st` and points W's pixel fields (uniform frames, or the image table) at the pixels the RunDetector stages read.
+// `unit` names a frame in the capacity messages.
+template <typename ScanFn>
+static int detect_on(int dev, pigo_cascade* face, pigo_puploc* puploc, pigo_puploc* const* flp, const uint8_t* flp_flip, int ncalls, int nframes,
+                     const char* unit, const pigo_pipeline_params& P, const float* randoms, uint64_t rng_seed, uint64_t slot_base, pigo_det* faces,
+                     int face_cap, int* n_faces, pigo_point* points, unsigned flags, void* stream_, ScanFn scan) {
   int rc = PIGO_OK;
   FaceReplica* R = face_replica(face, dev, &rc);
   if (!R) return rc;
@@ -1217,7 +1310,7 @@ static int detect_batch_on(int dev, pigo_cascade* face, pigo_puploc* puploc, pig
     W.tab_of[cidx] = (uint8_t)k; W.flip_of[cidx] = flp_flip && flp_flip[cidx] ? 1 : 0;
   }
   if ((rc = use_device(dev))) return rc;
-  const bool frames_dev = flags & PIGO_FRAMES_DEVICE, out_dev = flags & PIGO_OUT_DEVICE;
+  const bool out_dev = flags & PIGO_OUT_DEVICE;
   const int det_cap = P.det_cap > 0 ? P.det_cap : 2048;
 
   WsGuard g(R->pool);
@@ -1226,16 +1319,6 @@ static int detect_batch_on(int dev, pigo_cascade* face, pigo_puploc* puploc, pig
   cudaStream_t st = stream_ ? (cudaStream_t)stream_ : w->stream;
   if ((rc = ws_enter(w, st))) return rc;
 
-  const size_t frame_bytes = (size_t)rows * dim;
-  const uint8_t* d_frames = frames;
-  size_t d_stride = frame_stride;
-  if (!frames_dev) {
-    // the scan call below streams the host frames into THIS buffer (chunked copy overlapped with the scan kernels); the
-    // pupil / landmark stages gather from it afterwards
-    d_stride = (frame_bytes + 255) & ~(size_t)255;
-    if ((rc = w->frames.reserve(d_stride * nframes + 256))) return rc;
-    d_frames = (const uint8_t*)w->frames.p;
-  }
   const size_t nslots = (size_t)nframes * face_cap * stride;
   // scratch: raw detections + counts, clusters + counts, seeds, points, faces, work counters
   const size_t b_dets = (size_t)nframes * det_cap * sizeof(pigo_det), b_cl = (size_t)nframes * face_cap * sizeof(pigo_det);
@@ -1260,13 +1343,7 @@ static int detect_batch_on(int dev, pigo_cascade* face, pigo_puploc* puploc, pig
   CUDA_TRY(cudaMemsetAsync(w->counters.p, 0, 256, st));
   CUDA_TRY(cudaMemsetAsync(d_points, 0, b_pts, st));
 
-  if (frames_dev)
-    rc = scan_batch_on(face, dev, d_frames, nframes, d_stride, rows, cols, dim, P.min_size, P.max_size, P.shift_factor, P.scale_factor, P.angle,
-                       d_dets, det_cap, d_cnt, PIGO_FRAMES_DEVICE | PIGO_OUT_DEVICE, st);
-  else
-    rc = scan_batch_on(face, dev, frames, nframes, frame_stride, rows, cols, dim, P.min_size, P.max_size, P.shift_factor, P.scale_factor, P.angle,
-                       d_dets, det_cap, d_cnt, PIGO_OUT_DEVICE, st, (uint8_t*)w->frames.p);
-  if (rc) return rc;
+  if ((rc = scan(w, st, d_dets, det_cap, d_cnt, W))) return rc;
   rc = cluster_batch_on(dev, d_dets, d_cnt, nframes, det_cap, P.iou_threshold, d_clusters, face_cap, d_ncl, PIGO_OUT_DEVICE, st);
   if (rc) return rc;
   timing_begin(T_SEEDS, st);
@@ -1277,8 +1354,8 @@ static int detect_batch_on(int dev, pigo_cascade* face, pigo_puploc* puploc, pig
   int rot_slot = -1;
   if (P.angle > 0.0) rot_slot = (int)(32.0 * (P.angle > 1.0 ? 1.0 : P.angle));   // RunDetector(puploc, img, det.angle, false), main.go:422
   W.seeds = d_seeds; W.out = d_points; W.randoms = d_rnd; W.rng_seed = rng_seed; W.slot_base = slot_base;
-  W.frames = d_frames; W.frame_stride = d_stride; W.slot_frame = nullptr; W.flipv = nullptr;
-  W.slots_per_frame = face_cap * stride; W.nrows = rows; W.ncols = cols; W.dim = dim;
+  W.slot_frame = nullptr; W.flipv = nullptr;
+  W.slots_per_frame = face_cap * stride;
   W.stride = stride;
   // (a) both eyes of every face slot
   PupWork E = W;
@@ -1312,10 +1389,51 @@ static int detect_batch_on(int dev, pigo_cascade* face, pigo_puploc* puploc, pig
   CUDA_TRY(cudaMemcpyAsync(points, d_points, b_pts, cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaStreamSynchronize(st));
   for (int f = 0; f < nframes; ++f)
-    if (cnt[f] > det_cap) return set_err(PIGO_E_CAP, "frame %d has %d raw detections, det_cap is %d: raise pigo_pipeline_params.det_cap", f, cnt[f], det_cap);
+    if (cnt[f] > det_cap) return set_err(PIGO_E_CAP, "%s %d has %d raw detections, det_cap is %d: raise pigo_pipeline_params.det_cap", unit, f, cnt[f], det_cap);
   for (int f = 0; f < nframes; ++f)
-    if (n_faces[f] > face_cap) return set_err(PIGO_E_CAP, "frame %d has %d faces, face_cap is %d", f, n_faces[f], face_cap);
+    if (n_faces[f] > face_cap) return set_err(PIGO_E_CAP, "%s %d has %d faces, face_cap is %d", unit, f, n_faces[f], face_cap);
   return PIGO_OK;
+}
+
+static int detect_batch_on(int dev, pigo_cascade* face, pigo_puploc* puploc, pigo_puploc* const* flp, const uint8_t* flp_flip, int ncalls,
+                           const uint8_t* frames, int nframes, size_t frame_stride, int rows, int cols, int dim, const pigo_pipeline_params& P,
+                           const float* randoms, uint64_t rng_seed, uint64_t slot_base, pigo_det* faces, int face_cap, int* n_faces,
+                           pigo_point* points, unsigned flags, void* stream_) {
+  const bool frames_dev = flags & PIGO_FRAMES_DEVICE;
+  auto scan = [&](Workspace* w, cudaStream_t st, pigo_det* d_dets, int det_cap, int32_t* d_cnt, PupWork& W) {
+    int rc = PIGO_OK;
+    W.frames = frames; W.frame_stride = frame_stride; W.nrows = rows; W.ncols = cols; W.dim = dim;
+    if (frames_dev)
+      return scan_batch_on(face, dev, frames, nframes, frame_stride, rows, cols, dim, P.min_size, P.max_size, P.shift_factor, P.scale_factor,
+                           P.angle, d_dets, det_cap, d_cnt, PIGO_FRAMES_DEVICE | PIGO_OUT_DEVICE, st);
+    // the scan call streams the host frames into THIS buffer (chunked copy overlapped with the scan kernels); the
+    // pupil / landmark stages gather from it afterwards
+    W.frame_stride = ((size_t)rows * dim + 255) & ~(size_t)255;
+    if ((rc = w->frames.reserve(W.frame_stride * nframes + 256))) return rc;
+    W.frames = (const uint8_t*)w->frames.p;
+    return scan_batch_on(face, dev, frames, nframes, frame_stride, rows, cols, dim, P.min_size, P.max_size, P.shift_factor, P.scale_factor,
+                         P.angle, d_dets, det_cap, d_cnt, PIGO_OUT_DEVICE, st, (uint8_t*)w->frames.p);
+  };
+  return detect_on(dev, face, puploc, flp, flp_flip, ncalls, nframes, "frame", P, randoms, rng_seed, slot_base, faces, face_cap, n_faces, points,
+                   flags, stream_, scan);
+}
+
+// Mixed-size form: the images' pixels are staged once (stage_images) and both the images scan and the RunDetector stages
+// read them; `plans` / `wins` / `longest` are the call's ladders (build_image_plans).
+static int detect_images_on(int dev, pigo_cascade* face, pigo_puploc* puploc, pigo_puploc* const* flp, const uint8_t* flp_flip, int ncalls,
+                            const pigo_image* images, int nimages, const std::vector<std::vector<ScaleEntry>>& plans,
+                            const std::vector<uint64_t>& wins, int longest, const pigo_pipeline_params& P, const float* randoms, uint64_t rng_seed,
+                            pigo_det* faces, int face_cap, int* n_faces, pigo_point* points, unsigned flags, void* stream_) {
+  const bool frames_dev = flags & PIGO_FRAMES_DEVICE;
+  auto scan = [&](Workspace* w, cudaStream_t st, pigo_det* d_dets, int det_cap, int32_t* d_cnt, PupWork& W) {
+    std::vector<pigo_image> staged;
+    int rc = stage_images(w, images, nimages, frames_dev, st, &W.images, staged);
+    if (rc) return rc;
+    return scan_images_on(face, dev, staged.data(), nimages, plans, wins, longest, P.min_size, P.max_size, P.shift_factor, P.scale_factor,
+                          P.angle, d_dets, det_cap, d_cnt, PIGO_FRAMES_DEVICE | PIGO_OUT_DEVICE, st);
+  };
+  return detect_on(dev, face, puploc, flp, flp_flip, ncalls, nimages, "image", P, randoms, rng_seed, 0, faces, face_cap, n_faces, points, flags,
+                   stream_, scan);
 }
 
 extern "C" {
@@ -1359,6 +1477,49 @@ int pigo_detect_batch_sharded(const pigo_cascade* face, const pigo_puploc* puplo
                            randoms ? randoms + (size_t)lo * per_frame * 189 : nullptr, rng_seed, (uint64_t)lo * per_frame,
                            faces + (size_t)lo * face_cap, face_cap, n_faces + lo, points + (size_t)lo * per_frame, PIGO_MEM_HOST, nullptr);
   });
+}
+
+// Mixed-size pipeline arguments: what check_images_args and check_detect_args check except the uniform geometry, with a
+// message that names the argument; the cascade handles last, so that every other check is reachable without a device.
+static int check_detect_images_args(const pigo_cascade* face, const pigo_puploc* puploc, const pigo_puploc* const* flp, int ncalls,
+                                    const pigo_image* images, int nimages, const pigo_pipeline_params* prm, const pigo_det* faces, int face_cap,
+                                    const int* n_faces, const pigo_point* points) {
+  if (nimages < 0 || nimages > 65535) return set_err(PIGO_E_INVALID, "nimages must be 0..65535");
+  if (nimages > 0 && !images) return set_err(PIGO_E_INVALID, "null images");
+  if (!prm) return set_err(PIGO_E_INVALID, "null params");
+  if (!faces) return set_err(PIGO_E_INVALID, "null faces");
+  if (!n_faces) return set_err(PIGO_E_INVALID, "null n_faces");
+  if (!points) return set_err(PIGO_E_INVALID, "null points");
+  if (ncalls < 0 || ncalls > 30) return set_err(PIGO_E_INVALID, "ncalls must be 0..30");
+  if (ncalls > 0 && !flp) return set_err(PIGO_E_INVALID, "null flp");
+  if (face_cap < 1 || face_cap > 4096) return set_err(PIGO_E_INVALID, "face_cap must be 1..4096");
+  if (prm->eye_perturbs < 0 || prm->eye_perturbs > 63 || prm->flp_perturbs < 0 || prm->flp_perturbs > 63)
+    return set_err(PIGO_E_INVALID, "Perturbs outside 0..63 (the reference panics, core/puploc.go:261)");
+  if ((uint64_t)nimages * (uint64_t)face_cap * (uint64_t)(2 + ncalls) > 0x7fffffffull)
+    return set_err(PIGO_E_INVALID, "nimages*face_cap*(2+ncalls) exceeds 2^31-1 pupil work items");
+  int rc = check_image_geometry(images, nimages);
+  if (rc) return rc;
+  if (!face) return set_err(PIGO_E_INVALID, "null cascade");
+  if (!puploc) return set_err(PIGO_E_INVALID, "null pupil cascade");
+  for (int i = 0; i < ncalls; ++i)
+    if (!flp[i]) return set_err(PIGO_E_INVALID, "null landmark cascade %d", i);
+  return PIGO_OK;
+}
+
+int pigo_detect_images(const pigo_cascade* face, const pigo_puploc* puploc, const pigo_puploc* const* flp, const uint8_t* flp_flip, int ncalls,
+                       const pigo_image* images, int nimages, const pigo_pipeline_params* prm, const float* randoms, uint64_t rng_seed,
+                       pigo_det* faces, int face_cap, int* n_faces, pigo_point* points, unsigned flags, void* stream) {
+  int rc = check_detect_images_args(face, puploc, flp, ncalls, images, nimages, prm, faces, face_cap, n_faces, points);
+  if (rc) return rc;
+  std::vector<std::vector<ScaleEntry>> plans;
+  std::vector<uint64_t> wins;
+  int longest = 0;
+  if ((rc = build_image_plans(images, nimages, prm->min_size, prm->max_size, prm->shift_factor, prm->scale_factor, plans, wins, longest))) return rc;
+  if ((rc = ensure_device())) return rc;
+  if (stream && stream_capturing((cudaStream_t)stream)) return set_err(PIGO_E_INVALID, "pigo_detect_images does not support stream capture");
+  if (nimages == 0) return PIGO_OK;
+  return detect_images_on(default_device(), const_cast<pigo_cascade*>(face), const_cast<pigo_puploc*>(puploc), (pigo_puploc* const*)flp, flp_flip,
+                          ncalls, images, nimages, plans, wins, longest, *prm, randoms, rng_seed, faces, face_cap, n_faces, points, flags, stream);
 }
 
 // ---- RgbToGrayscale, core/grayscale.go:8-23 ----------------------------------------------------------------

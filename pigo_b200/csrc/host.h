@@ -130,6 +130,7 @@ struct PupWork {
   int32_t first, span, stride, nwork, ntabs;
   PuplocTables tab[kMaxPupTabs];
   uint8_t tab_of[32], flip_of[32];
+  const ImageDesc* images;     // mixed-size call: the image table the frame indices refer to (frames .. dim unused); nullptr = uniform frames
 };
 
 
@@ -324,7 +325,7 @@ void launch_cluster(pigo_det* dets, const int32_t* n_in, int cap, double thr, pi
                     pigo_det* out, int out_cap, int32_t* n_out, int nframes, cudaStream_t st);
 void launch_puploc(const PuplocTables& T, const pigo_point* seeds, int nseeds, const float* randoms, uint64_t rng_seed,
                    const uint8_t* frames, const int32_t* seed_frame, size_t frame_stride, int rows, int cols, int dim, int rot_slot,
-                   const uint8_t* flipv, pigo_point* out, cudaStream_t st);
+                   const uint8_t* flipv, pigo_point* out, const ImageDesc* images, cudaStream_t st);
 int launch_puploc_pairs(const PupWork& W, unsigned int* counter, int num_sms, cudaStream_t st);
 void launch_eye_seeds(const pigo_det* clusters, const int32_t* ncl, int cl_cap, int nframes, int face_cap, int stride, int min_face,
                       int eye_perturbs, pigo_det* faces, int32_t* nfaces, pigo_point* seeds, cudaStream_t st);

@@ -35,15 +35,20 @@ __device__ __forceinline__ uint32_t mix64(uint64_t x) {
 // with shuffles, exactly like the reference's sequential loop (core/puploc.go:112-151).  That turns the reference's
 // stages*trees*depth = 1000-deep dependent gather chain into stages*depth = 50; the two children of a node are fetched
 // together with the node's pixel pair (child-pair prefetch).
+// IMG (mixed-size call): seed_frame indexes the image table `images`, whose entry gives the pixels, rows, cols and pitch;
+// frames / frame_stride / nrows / ncols / dim are then unused.
+template <bool IMG = false>
 __global__ void __launch_bounds__(1024, 1) puploc_kernel(PuplocTables T, const pigo_point* __restrict__ seeds, int nseeds,
                                                          const float* __restrict__ randoms, uint64_t rng_seed,
                                                          const uint8_t* __restrict__ frames, const int32_t* __restrict__ seed_frame,
-                                                         size_t frame_stride, int nrows, int ncols, int dim,
+                                                         size_t frame_stride, int frame_rows, int frame_cols, int frame_dim,
                                                          int rot_slot, const uint8_t* __restrict__ flipv_arr,
-                                                         pigo_point* __restrict__ out) {
+                                                         pigo_point* __restrict__ out, const ImageDesc* __restrict__ images) {
   const unsigned FULL = 0xffffffffu;
   const int sidx = blockIdx.x;
-  const uint8_t* __restrict__ pixels = frames + (seed_frame ? (size_t)seed_frame[sidx] * frame_stride : 0);
+  const ImageDesc im = IMG ? images[seed_frame ? seed_frame[sidx] : 0] : ImageDesc{};
+  const uint8_t* __restrict__ pixels = IMG ? im.base : frames + (seed_frame ? (size_t)seed_frame[sidx] * frame_stride : 0);
+  const int nrows = IMG ? im.rows : frame_rows, ncols = IMG ? im.cols : frame_cols, dim = IMG ? im.dim : frame_dim;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   __shared__ float rows_[64], cols_[64], scal_[64];
   const pigo_point seed = seeds[sidx];
@@ -180,7 +185,9 @@ __device__ __forceinline__ int clamp_coord(float v) { return max(-(1 << 30), min
 // to the image -- fits `patch_cap` bytes, that area is copied to shared memory with coalesced 16-byte loads and the
 // stage's pixel pairs become shared-memory loads too (a stage gathers 1260 x depth x 2 lane-divergent bytes from it; the
 // scale shrinks by 0.7-0.8 per stage, so the later stages of a landmark call fit).  Stages that do not fit gather from global memory.
-template <bool STAGED, bool PATCH>
+// IMG (mixed-size call): the slot's frame index selects an entry of the image table W.images, which gives the pixels, the
+// clamps rows-1 / cols-1 and the row pitch (the patch's 16-byte path then needs that image's pitch and base aligned).
+template <bool STAGED, bool PATCH, bool IMG = false>
 __global__ void __launch_bounds__(kPairThreads, PATCH ? 2 : 3) puploc_pair_kernel(const PupWork W, unsigned int* __restrict__ counter, int leaf_bytes,
                                                                                  int codes_bytes, int patch_cap) {
   extern __shared__ __align__(16) uint8_t s_dyn[];
@@ -209,8 +216,9 @@ __global__ void __launch_bounds__(kPairThreads, PATCH ? 2 : 3) puploc_pair_kerne
     const PuplocTables T = W.tab[W.tab_of[j]];
     const bool flip = W.flipv ? (W.flipv[slot] != 0) : (W.flip_of[j] != 0);
     const int frame = W.slots_per_frame > 0 ? slot / W.slots_per_frame : (W.slot_frame ? W.slot_frame[slot] : 0);
-    const uint8_t* __restrict__ pixels = W.frames + (size_t)frame * W.frame_stride;
-    const int L = T.leaves, tree_codes = 4 * L, rlim = W.nrows - 1, clim = W.ncols - 1;   // padded device layout, see PuplocTables
+    const uint8_t* __restrict__ pixels = IMG ? W.images[frame].base : W.frames + (size_t)frame * W.frame_stride;
+    auto dim = [&]() { return IMG ? W.images[frame].dim : W.dim; };   // row pitch (read at each use, as W.dim was before IMG)
+    const int L = T.leaves, tree_codes = 4 * L, rlim = (IMG ? W.images[frame].rows : W.nrows) - 1, clim = (IMG ? W.images[frame].cols : W.ncols) - 1;   // padded device layout, see PuplocTables
     const bool rot = W.rot_slot >= 0;
     const int sstride = tree_codes + 8;                    // shared-memory tree stride (bank skew)
     auto stage_codes = [&](int st) {
@@ -260,14 +268,14 @@ __global__ void __launch_bounds__(kPairThreads, PATCH ? 2 : 3) puploc_pair_kerne
       const int r0 = min(max(s_box[0], 0), rlim), r1 = min(max(s_box[1], 0), rlim);
       const int c0 = min(max(s_box[2], 0), clim) & ~15, c1 = min(max(s_box[3], 0), clim);
       const long long rows = (long long)r1 - r0 + 1, pitch = ((long long)c1 - c0 + 16) & ~15ll;
-      if (rows <= 0 || pitch <= 0 || rows * pitch > patch_cap || (W.dim & 15) || (reinterpret_cast<uintptr_t>(pixels) & 15)) return;
+      if (rows <= 0 || pitch <= 0 || rows * pitch > patch_cap || (dim() & 15) || (reinterpret_cast<uintptr_t>(pixels) & 15)) return;
       p_use = true; p_r0 = r0; p_c0 = c0; p_pitch = (int)pitch;
       const int vec_per_row = (int)(pitch >> 4), total = (int)rows * vec_per_row;
       for (int q = tid; q < total; q += nt) {
         const int y = q / vec_per_row, x = q - y * vec_per_row;
-        if (c0 + 16 * x + 16 <= W.dim)     // (vectors past the end of the row are never sampled: columns are clamped to ncols-1 < dim)
+        if (c0 + 16 * x + 16 <= dim())     // (vectors past the end of the row are never sampled: columns are clamped to ncols-1 < the pitch)
           *reinterpret_cast<uint4*>(s_patch + (size_t)y * pitch + 16 * x) =
-              __ldg(reinterpret_cast<const uint4*>(pixels + (size_t)(r0 + y) * W.dim + c0 + 16 * x));
+              __ldg(reinterpret_cast<const uint4*>(pixels + (size_t)(r0 + y) * dim() + c0 + 16 * x));
       }
     };
     load_patch();
@@ -298,8 +306,8 @@ __global__ void __launch_bounds__(kPairThreads, PATCH ? 2 : 3) puploc_pair_kerne
             const int k3 = flip ? neg_i8(cw >> 24) : (cw >> 24);
             const int r1 = __vimin_s32_relu(ir + ((k0 * rs) >> 8), rlim), r2 = __vimin_s32_relu(ir + ((k2 * rs) >> 8), rlim);   // :118-119
             const int c1 = __vimin_s32_relu(ic + ((k1 * rs) >> 8), clim), c2 = __vimin_s32_relu(ic + ((k3 * rs) >> 8), clim);   // :124/:127
-            const unsigned q1 = (PATCH && p_use) ? s_patch[(r1 - p_r0) * p_pitch + (c1 - p_c0)] : __ldg(pixels + (size_t)r1 * W.dim + c1);
-            const unsigned q2 = (PATCH && p_use) ? s_patch[(r2 - p_r0) * p_pitch + (c2 - p_c0)] : __ldg(pixels + (size_t)r2 * W.dim + c2);
+            const unsigned q1 = (PATCH && p_use) ? s_patch[(r1 - p_r0) * p_pitch + (c1 - p_c0)] : __ldg(pixels + (size_t)r1 * dim() + c1);
+            const unsigned q2 = (PATCH && p_use) ? s_patch[(r2 - p_r0) * p_pitch + (c2 - p_c0)] : __ldg(pixels + (size_t)r2 * dim() + c2);
             const int bit = q1 > q2 ? 1 : 0;                                                                                     // :130-136
             cw = bit ? kr : kl;
             idx = 2 * idx + 1 + bit;
@@ -316,8 +324,8 @@ __global__ void __launch_bounds__(kPairThreads, PATCH ? 2 : 3) puploc_pair_kerne
             const int c1 = __vimin_s32_relu(ic + (int)((iqs * k0 + iqc * k1) >> 16), clim);   // :189
             const int r2 = __vimin_s32_relu(ir + (int)((iqc * k2 - iqs * k3) >> 16), rlim);   // :190
             const int c2 = __vimin_s32_relu(ic + (int)((iqs * k2 + iqc * k3) >> 16), clim);   // :191
-            const unsigned q1 = (PATCH && p_use) ? s_patch[(r1 - p_r0) * p_pitch + (c1 - p_c0)] : __ldg(pixels + (size_t)r1 * W.dim + c1);
-            const unsigned q2 = (PATCH && p_use) ? s_patch[(r2 - p_r0) * p_pitch + (c2 - p_c0)] : __ldg(pixels + (size_t)r2 * W.dim + c2);
+            const unsigned q1 = (PATCH && p_use) ? s_patch[(r1 - p_r0) * p_pitch + (c1 - p_c0)] : __ldg(pixels + (size_t)r1 * dim() + c1);
+            const unsigned q2 = (PATCH && p_use) ? s_patch[(r2 - p_r0) * p_pitch + (c2 - p_c0)] : __ldg(pixels + (size_t)r2 * dim() + c2);
             const int bit = q1 <= q2 ? 1 : 0;                                                                                    // :193-199
             cw = bit ? kr : kl;
             idx = 2 * idx + 1 + bit;
@@ -367,6 +375,21 @@ __global__ void __launch_bounds__(kPairThreads, PATCH ? 2 : 3) puploc_pair_kerne
   }
 }
 
+template <bool IMG>
+static void set_pair_smem(int bytes) {
+  cudaFuncSetAttribute(puploc_pair_kernel<true, true, IMG>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  cudaFuncSetAttribute(puploc_pair_kernel<true, false, IMG>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  cudaFuncSetAttribute(puploc_pair_kernel<false, false, IMG>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+}
+// codes_bytes > 0: the stage's node codes are staged; patch_cap > 0 (with them): so is the stage's pixel patch
+template <bool IMG>
+static void launch_pair_variant(const PupWork& W, unsigned int* counter, int grid, size_t smem, int leaf, int codes_bytes, int patch_cap,
+                                cudaStream_t st) {
+  if (patch_cap > 0) puploc_pair_kernel<true, true, IMG><<<grid, kPairThreads, smem, st>>>(W, counter, leaf, codes_bytes, patch_cap);
+  else if (codes_bytes > 0) puploc_pair_kernel<true, false, IMG><<<grid, kPairThreads, smem, st>>>(W, counter, leaf, codes_bytes, 0);
+  else puploc_pair_kernel<false, false, IMG><<<grid, kPairThreads, smem, st>>>(W, counter, leaf, 0, 0);
+}
+
 int launch_puploc_pairs(const PupWork& W, unsigned int* counter, int num_sms, cudaStream_t st) {
   // shared memory is sized by the cascades THIS launch uses (positions first .. first+span-1), not by every table of the work list
   int trees_max = 0;
@@ -387,15 +410,13 @@ int launch_puploc_pairs(const PupWork& W, unsigned int* counter, int num_sms, cu
   static bool attr_set[kMaxDevices] = {};
   int dev = 0; cudaGetDevice(&dev);
   if (!attr_set[dev]) {
-    cudaFuncSetAttribute(puploc_pair_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBudget);
-    cudaFuncSetAttribute(puploc_pair_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBudget);
-    cudaFuncSetAttribute(puploc_pair_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBudget);
+    set_pair_smem<false>((int)kBudget);
+    set_pair_smem<true>((int)kBudget);
     attr_set[dev] = true;
   }
   const int grid = max(1, min(W.nwork, num_sms * 3));
-  if (patch_cap > 0) puploc_pair_kernel<true, true><<<grid, kPairThreads, smem, st>>>(W, counter, (int)leaf, (int)codes_max, (int)patch_cap);
-  else if (staged) puploc_pair_kernel<true, false><<<grid, kPairThreads, smem, st>>>(W, counter, (int)leaf, (int)codes_max, 0);
-  else puploc_pair_kernel<false, false><<<grid, kPairThreads, smem, st>>>(W, counter, (int)leaf, 0, 0);
+  if (W.images) launch_pair_variant<true>(W, counter, grid, smem, (int)leaf, staged ? (int)codes_max : 0, (int)patch_cap, st);
+  else launch_pair_variant<false>(W, counter, grid, smem, (int)leaf, staged ? (int)codes_max : 0, (int)patch_cap, st);
   return 0;
 }
 
@@ -457,9 +478,13 @@ void launch_landmark_seeds(const pigo_point* points, pigo_point* seeds, int nslo
 
 void launch_puploc(const PuplocTables& T, const pigo_point* seeds, int nseeds, const float* randoms, uint64_t rng_seed,
                    const uint8_t* frames, const int32_t* seed_frame, size_t frame_stride, int rows, int cols, int dim, int rot_slot,
-                   const uint8_t* flipv, pigo_point* out, cudaStream_t st) {
-  puploc_kernel<<<nseeds, 1024, 0, st>>>(T, seeds, nseeds, randoms, rng_seed, frames, seed_frame, frame_stride, rows, cols, dim, rot_slot,
-                                         flipv, out);
+                   const uint8_t* flipv, pigo_point* out, const ImageDesc* images, cudaStream_t st) {
+  if (images)
+    puploc_kernel<true><<<nseeds, 1024, 0, st>>>(T, seeds, nseeds, randoms, rng_seed, frames, seed_frame, frame_stride, rows, cols, dim,
+                                                 rot_slot, flipv, out, images);
+  else
+    puploc_kernel<false><<<nseeds, 1024, 0, st>>>(T, seeds, nseeds, randoms, rng_seed, frames, seed_frame, frame_stride, rows, cols, dim,
+                                                  rot_slot, flipv, out, nullptr);
 }
 
 }  // namespace pigo

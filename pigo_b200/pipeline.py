@@ -154,8 +154,12 @@ def detect_batch_device(clf: Pigo, plc: PuplocCascade, flpcs: Dict[str, PuplocCa
     _check(rc)
     if raw:
         return faces, nfaces[:nf], points
+    return _faces_of(faces, nfaces, points, min_face)
+
+
+def _faces_of(faces, nfaces, points, min_face) -> List[List[Face]]:
     out: List[List[Face]] = []
-    for f in range(nf):
+    for f in range(len(faces)):
         fl_ = []
         for k in range(int(nfaces[f])):
             d = faces[f, k]
@@ -166,3 +170,34 @@ def detect_batch_device(clf: Pigo, plc: PuplocCascade, flpcs: Dict[str, PuplocCa
             fl_.append(fc)
         out.append(fl_)
     return out
+
+
+def detect_images_device(clf: Pigo, plc: PuplocCascade, flpcs: Dict[str, PuplocCascade], images, cp: CascadeParams, iou: float = 0.1,
+                         min_face: int = 50, eye_perturbs: int = 50, flp_perturbs: int = 63, face_cap: int = 32, angle: float = 0.0,
+                         randoms: Optional[np.ndarray] = None, rng_seed: int = 0, det_cap: int = 0, raw: bool = False):
+    """detect_batch_device for images of different sizes in one call (pigo_detect_images).  images: ImageParams with host
+    arrays, or for every image alike device pointers (int) holding Rows*Dim bytes; cp's MinSize / MaxSize / ShiftFactor /
+    ScaleFactor are shared (cp.ImageParams is not used).  randoms: optional [N][face_cap][17][63][3] float32.
+    Returns List[List[Face]] (raw=True: the (faces, n_faces, points) arrays)."""
+    import ctypes as C
+    from . import DET_DTYPE, POINT_DTYPE, FRAMES_DEVICE, MEM_HOST, PipelineParams, _check, _pixels, image_descs, lib
+    hs, fl = landmark_call_arrays(flpcs)
+    ncalls = len(fl)
+    n = len(images)
+    on_dev = n > 0 and all(isinstance(im.Pixels, int) for im in images)
+    keep = [None if on_dev else _pixels(im) for im in images]   # host pixels stay alive for the call
+    desc = image_descs([(im.Pixels if on_dev else p.ctypes.data, im.Rows, im.Cols, im.Dim) for im, p in zip(images, keep)])
+    prm = PipelineParams(cp.MinSize, cp.MaxSize, cp.ShiftFactor, cp.ScaleFactor, angle, iou, min_face, eye_perturbs, flp_perturbs, det_cap)
+    rnd = None
+    if randoms is not None:
+        rnd = np.ascontiguousarray(randoms, dtype=np.float32)
+        assert rnd.size == n * face_cap * (2 + ncalls) * 189, "randoms must be [N][face_cap][2+ncalls][63][3]"
+    faces = np.zeros((n, face_cap), dtype=DET_DTYPE)
+    nfaces = np.zeros(max(n, 1), dtype=np.int32)
+    points = np.zeros((n, face_cap, 2 + ncalls), dtype=POINT_DTYPE)
+    _check(lib().pigo_detect_images(clf._h, plc._h, hs, fl.ctypes.data, ncalls, desc, n, C.byref(prm), rnd.ctypes.data if rnd is not None else None,
+                                    rng_seed, faces.ctypes.data, face_cap, nfaces.ctypes.data, points.ctypes.data,
+                                    FRAMES_DEVICE if on_dev else MEM_HOST, None))
+    if raw:
+        return faces, nfaces[:n], points
+    return _faces_of(faces, nfaces, points, min_face)

@@ -7,7 +7,11 @@ Usage: `python tools/ragged_bench.py [--frames 256]` on one GPU prints one JSON 
   one_images_call_e2e_host : the mixed call from pageable host images, wall clock
   uniform_1080p : the mixed call on --frames identical-geometry 1080p frames (bench.py's batch) against pigo_run_cascade_batch
               with the default schedule and with scan_mode=3 (the gather-v2 + deep pair the mixed call runs), alternated
-Writes nothing to the tree.
+  pipeline : face -> cluster -> pupils -> 15 landmarks on the same 256 images: one pigo_detect_images call against one
+              pigo_detect_batch per geometry and one per image (device resident, CUDA events; faces and counts asserted
+              identical, points compared in an untimed run with injected randoms), and pigo_detect_images against
+              pigo_detect_batch on --pipeline-frames uniform 1080p frames, alternated
+`--sections scan,pipeline` selects the sections.  Writes nothing to the tree.
 """
 import argparse
 import json
@@ -188,18 +192,155 @@ def ragged_bench(clf, dev: int, stream, d_frames, nf: int) -> dict:
                               "note": "median of 5 alternated rounds after 2"}}
 
 
+def pipeline_bench(clf, dev: int, stream, d_frames, nf: int) -> dict:
+    """The whole per-face sequence (pigo_detect_images / pigo_detect_batch, the reference's 15 landmark calls) on the mixed
+    set three ways, and on uniform 1080p frames two ways; see the module docstring."""
+    import ctypes as C
+    import torch
+    import pigo_b200
+    from pigo_b200 import pipeline
+    L = pigo_b200.lib()
+    st = C.c_void_p(stream.cuda_stream)
+    cuda = f"cuda:{dev}"
+    plc = pigo_b200.NewPuplocCascade().UnpackCascade(pigo_b200.load_cascade("puploc"))
+    names = sorted(set(pipeline.EYE_CASCADES + pipeline.MOUTH_CASCADES))
+    flp = {nm: pigo_b200.NewPuplocCascade().UnpackCascade(pigo_b200.load_cascade("lps/" + nm)) for nm in names}
+    hs, fl = pipeline.landmark_call_arrays(flp)
+    ncalls = len(fl)
+    face_cap, det_cap = 128, 4096
+    prm = pigo_b200.PipelineParams(*PARAMS, 0.0, 0.1, 50, 50, 63, det_cap)
+    flags = pigo_b200.FRAMES_DEVICE | pigo_b200.OUT_DEVICE
+    imgs = ragged_images()
+    n = len(imgs)
+    offs, total = [], 0
+    for b, r, c, d in imgs:
+        offs.append(total)
+        total += (r * d + 255) & ~255
+    host = np.zeros(total, dtype=np.uint8)
+    for (b, r, c, d), o in zip(imgs, offs):
+        host[o:o + r * d] = b.reshape(-1)
+    dev_all = torch.from_numpy(host).to(cuda)
+    descs = pigo_b200.image_descs([(dev_all.data_ptr() + o, r, c, d) for (b, r, c, d), o in zip(imgs, offs)])
+    geo = {}
+    for i, (_, r, c, d) in enumerate(imgs):
+        geo.setdefault((r, c, d), []).append(i)
+    geo_frames = {g: torch.stack([dev_all[offs[i]:offs[i] + g[0] * g[2]] for i in idx]) for g, idx in geo.items()}
+    outs = {k: (torch.zeros((n, face_cap, 4), dtype=torch.int32, device=cuda), torch.zeros(n, dtype=torch.int32, device=cuda),
+                torch.zeros((n, face_cap, 2 + ncalls, 4), dtype=torch.int32, device=cuda)) for k in "abc"}
+    geo_out = {g: tuple(torch.zeros((len(idx),) + t.shape[1:], dtype=torch.int32, device=cuda) for t in outs["b"]) for g, idx in geo.items()}
+
+    def check(rc):
+        if rc != 0:
+            raise RuntimeError(L.pigo_last_error().decode())
+
+    def batch(frames_ptr, k, stride, r, c, d, o, rnd):
+        check(L.pigo_detect_batch(clf._h, plc._h, hs, fl.ctypes.data, ncalls, frames_ptr, k, stride, r, c, d, C.byref(prm), rnd, 7,
+                                  o[0].data_ptr(), face_cap, o[1].data_ptr(), o[2].data_ptr(), flags, st))
+
+    def run_a(rnd=None):
+        check(L.pigo_detect_images(clf._h, plc._h, hs, fl.ctypes.data, ncalls, descs, n, C.byref(prm), rnd.data_ptr() if rnd is not None else None,
+                                   7, outs["a"][0].data_ptr(), face_cap, outs["a"][1].data_ptr(), outs["a"][2].data_ptr(), flags, st))
+
+    def run_b(rnd=None):
+        for g, fr in geo_frames.items():
+            rg = rnd[geo[g]].contiguous() if rnd is not None else None
+            batch(fr.data_ptr(), fr.shape[0], g[0] * g[2], *g, geo_out[g], rg.data_ptr() if rg is not None else None)
+            if rnd is not None:
+                torch.cuda.synchronize()   # rg must outlive the asynchronous call
+
+    def run_c(rnd=None):
+        for i, (b, r, c, d) in enumerate(imgs):
+            o = tuple(t[i:i + 1] for t in outs["c"])
+            batch(dev_all.data_ptr() + offs[i], 1, r * d, r, c, d, o, rnd[i].data_ptr() if rnd is not None else None)
+
+    def gather_b():
+        for g, idx in geo.items():
+            for t, u in zip(outs["b"], geo_out[g]):
+                t[idx] = u
+
+    def timed(fn, reps=5, warm=2):
+        for _ in range(warm):
+            fn()
+        torch.cuda.synchronize()
+        ts = []
+        for _ in range(reps):
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            a.record(stream)
+            fn()
+            b.record(stream)
+            torch.cuda.synchronize()
+            ts.append(a.elapsed_time(b))
+        return float(np.median(ts))
+
+    ms = {k: timed(f) for k, f in (("a", run_a), ("b", run_b), ("c", run_c))}
+    gather_b()
+    res = {k: [t.cpu().numpy() for t in outs[k]] for k in "abc"}
+    assert int(res["a"][1].max()) <= face_cap, "raise face_cap: an image has more faces than the bench buffer"
+    for k in "bc":
+        assert np.array_equal(res["a"][1], res[k][1]), f"pipeline: face counts of ({k}) differ"
+        assert res["a"][0].tobytes() == res[k][0].tobytes(), f"pipeline: faces of ({k}) differ"
+    # points: generator keys depend on the frame index, so compare with the same injected randoms (untimed)
+    rnd = torch.from_numpy(np.random.default_rng(11).random((n, face_cap, 2 + ncalls, 63, 3), dtype=np.float32)).to(cuda)
+    run_a(rnd); run_b(rnd); run_c(rnd)
+    torch.cuda.synchronize()
+    gather_b()
+    pts = {k: outs[k][2].cpu().numpy() for k in "abc"}
+    assert pts["a"].tobytes() == pts["b"].tobytes() == pts["c"].tobytes(), "pipeline: points differ with injected randoms"
+    del rnd
+    refined = int((res["a"][0][..., 2] > 50).sum())
+
+    # uniform 1080p: the mixed call against the batch call on the same frames, alternated
+    uo = {k: (torch.zeros((nf, face_cap, 4), dtype=torch.int32, device=cuda), torch.zeros(nf, dtype=torch.int32, device=cuda),
+              torch.zeros((nf, face_cap, 2 + ncalls, 4), dtype=torch.int32, device=cuda)) for k in ("images", "batch")}
+    udesc = pigo_b200.image_descs([(d_frames[i].data_ptr(), ROWS, COLS, COLS) for i in range(nf)])
+
+    def u_run(k):
+        o = uo[k]
+        if k == "images":
+            check(L.pigo_detect_images(clf._h, plc._h, hs, fl.ctypes.data, ncalls, udesc, nf, C.byref(prm), None, 7, o[0].data_ptr(), face_cap,
+                                       o[1].data_ptr(), o[2].data_ptr(), flags, st))
+        else:
+            batch(d_frames.data_ptr(), nf, ROWS * COLS, ROWS, COLS, COLS, o, None)
+
+    uts = {k: [] for k in uo}
+    for r in range(7):
+        for k in uo:
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            a.record(stream)
+            u_run(k)
+            b.record(stream)
+            torch.cuda.synchronize()
+            if r >= 2:
+                uts[k].append(a.elapsed_time(b))
+    ums = {k: float(np.median(v)) for k, v in uts.items()}
+    same_u = all(torch.equal(x, y) for x, y in zip(uo["images"], uo["batch"]))
+    return {"workload": f"{n} images of {len(geo)} geometries (the scan section's set), test parameters, eye Perturbs 50, 15 landmark calls, "
+                        "device resident, device outputs, CUDA events, median of 5 after 2 warm-ups",
+            "one_detect_images_call_ms": ms["a"], "detect_batch_per_geometry_ms": ms["b"], "detect_batch_per_image_ms": ms["c"],
+            "calls": {"a": 1, "b": len(geo), "c": n}, "faces": int(res["a"][1].sum()), "refined_faces": refined,
+            "faces_counts_identical": True, "points_identical_with_injected_randoms": True,
+            "uniform_1080p": {"frames": nf, "ms_detect_images": ums["images"], "ms_detect_batch": ums["batch"],
+                              "images_over_batch": ums["images"] / ums["batch"], "outputs_identical": bool(same_u),
+                              "note": "median of 5 alternated rounds after 2"}}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--frames", type=int, default=256, help="frames of the uniform 1080p comparison")
+    ap.add_argument("--pipeline-frames", type=int, default=64, help="frames of the uniform 1080p pipeline comparison")
+    ap.add_argument("--sections", default="scan,pipeline", help="comma-separated: scan, pipeline")
     args = ap.parse_args()
+    sections = set(args.sections.split(","))
     import torch
     import pigo_b200
     pigo_b200.init(0)
     clf = pigo_b200.NewPigo().Unpack(pigo_b200.load_cascade("facefinder"))
-    d_frames = torch.from_numpy(make_frames(args.frames, seed0=0)).to("cuda:0")
+    d_frames = torch.from_numpy(make_frames(max(args.frames, args.pipeline_frames), seed0=0)).to("cuda:0")
     stream = torch.cuda.Stream(device=0)
     torch.cuda.set_stream(stream)
-    res = ragged_bench(clf, 0, stream, d_frames, args.frames)
+    res = ragged_bench(clf, 0, stream, d_frames[:args.frames], args.frames) if "scan" in sections else {}
+    if "pipeline" in sections:
+        res["pipeline"] = pipeline_bench(clf, 0, stream, d_frames[:args.pipeline_frames], args.pipeline_frames)
     res["gpu"] = torch.cuda.get_device_name(0)
     try:   # read-only query: the power limit belongs beside the numbers
         import subprocess

@@ -7,7 +7,8 @@
 No torch (ctypes mirror only), a few hundred thousand windows in total, so that the instrumented run ends in minutes.
 Covers: fused kernel (tile + gather role, aligned TMA fill and byte-wise fill), gather-v2 with Q1, deep kernel with Q2,
 queue-overflow fallbacks (tiny KS, tail policy on), universal gather kernel (rotated, scan_mode=1), finalize, cluster,
-RunDetector / landmark kernels over resident frames, grayscale.  Prints the detection counts (compare with a plain run).
+RunDetector / landmark kernels over resident frames, grayscale, and the mixed-size pipeline and RunDetector (image-table
+kernel variants; --images runs only those).  Prints the detection counts (compare with a plain run).
 """
 import argparse
 import os
@@ -31,11 +32,16 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--quick", action="store_true", help="scan kernels only, fewer variants (racecheck is slow)")
     ap.add_argument("--new", action="store_true", help="only the kernels added late in round 2 (offset tables, shared-memory deep, queue overflow)")
+    ap.add_argument("--images", action="store_true", help="only the mixed-size pipeline and RunDetector (image-table kernel variants)")
     args = ap.parse_args()
     pigo_b200.init(0)
     clf = pigo_b200.NewPigo().Unpack(pigo_b200.load_cascade("facefinder"))
     sample = synth.sample_gray()
     counts = []
+    if args.images:
+        counts += images_case(clf, sample)
+        print("sanitize_run counts:", counts, "launches:", pigo_b200.launch_count())
+        return
 
     variants = [{}, {"tile_warps": 4, "tile_ks": 5, "gather_ks": 7, "tile_tail_min": 33},
                 {"scan_mode": 3, "gather_ks": 4}, {"scan_mode": 1}, {"tile_ni": 2, "tile_warps": 8, "gather_warps": 0, "tile_prefetch": 1},
@@ -100,7 +106,37 @@ def main():
         cr = np.random.default_rng(3).integers(0, 256, size=(11, 20), dtype=np.uint8)
         out, gy = pigo_b200.YCbCrToNRGBA(yy, cb, cr, 2, 37, 21, want_gray=True)
         counts += [int(out.sum()), int(gy.sum())]
+        counts += images_case(clf, sample)
     print("sanitize_run counts:", counts, "launches:", pigo_b200.launch_count() if hasattr(pigo_b200, "launch_count") else "n/a")
+
+
+def images_case(clf, sample):
+    """pigo_detect_images over images of three geometries (one with Dim % 16 != 0: the patch falls back to global gathers),
+    every puploc_stage; pigo_puploc_run_images with seeds on and past the borders on both RunDetector kernels."""
+    counts = []
+    plc = pigo_b200.NewPuplocCascade().UnpackCascade(pigo_b200.load_cascade("puploc"))
+    names = sorted(set(pipeline.EYE_CASCADES + pipeline.MOUTH_CASCADES))
+    flp = {n: pigo_b200.NewPuplocCascade().UnpackCascade(pigo_b200.load_cascade("lps/" + n)) for n in names}
+    wide = np.zeros((300, 712), dtype=np.uint8)
+    wide[:, :700] = synth.frame_faces(sample, 300, 700, noise_seed=2)
+    images = [ImageParams(sample, 400, 320, 320), ImageParams(wide, 300, 700, 712),
+              ImageParams(synth.frame_faces(sample, 540, 960, shift=(30, 200), noise_seed=4), 540, 960, 960), ImageParams(np.zeros(64, np.uint8), 8, 8, 8)]
+    cp = CascadeParams(ImageParams(), *PRM)
+    for stage, ang in ((2, 0.0), (1, 0.05), (0, 0.0)):
+        pigo_b200.set_option("puploc_stage", stage)
+        f, n, p = pipeline.detect_images_device(clf, plc, flp, images, cp, face_cap=8, rng_seed=3, angle=ang, raw=True)
+        counts += [int(n.sum()), int((p["row"] > 0).sum())]
+    pigo_b200.set_option("puploc_stage", 1)
+    rng = np.random.default_rng(5)
+    seeds = [pigo_b200.Puploc(int(rng.integers(-30, 560)), int(rng.integers(-30, 980)), float(rng.uniform(4, 200)), int(rng.integers(0, 64)))
+             for _ in range(24)]
+    which = [k % 3 for k in range(24)]
+    for mode in (0, 1):
+        pigo_b200.set_option("puploc_mode", mode)
+        out = plc.run_detector_images(seeds, which, images[:3], 0.2, [k % 2 == 0 for k in range(24)], rng_seed=9)
+        counts.append(sum(o.Row for o in out))
+    pigo_b200.set_option("puploc_mode", 0)
+    return counts
 
 
 if __name__ == "__main__":
