@@ -267,6 +267,91 @@ func (pg *Pigo) RunCascadeImages(images []ImageParams, cp CascadeParams, angle f
 	}
 }
 
+// packImages copies the pixels of a mixed-size call to one pinned buffer (256-byte aligned slices; cgo forbids passing Go
+// memory that holds Go pointers) and builds the descriptors that point into it in C memory.  Images that share a pixel
+// slice and geometry are stored once: an angle sweep lists one image once per angle.  free releases both buffers.
+func packImages(images []ImageParams) (desc []C.pigo_image, free func()) {
+	type key struct {
+		p                  *uint8
+		n, rows, cols, dim int
+	}
+	n := len(images)
+	offs := make([]int, n)
+	first := make([]bool, n)
+	seen := make(map[key]int, n)
+	total := 0
+	for i, im := range images {
+		k := key{nil, len(im.Pixels), im.Rows, im.Cols, im.Dim}
+		if len(im.Pixels) > 0 {
+			k.p = &im.Pixels[0]
+		}
+		o, ok := seen[k]
+		if !ok {
+			o, first[i] = total, true
+			seen[k] = o
+			total += (len(im.Pixels) + 255) &^ 255
+		}
+		offs[i] = o
+	}
+	var pinned unsafe.Pointer
+	if _, err := call(func() C.int { return C.pigo_alloc_pinned(&pinned, C.size_t(total+256)) }); err != nil {
+		panic(err)
+	}
+	host := unsafe.Slice((*uint8)(pinned), total+256)
+	desc = unsafe.Slice((*C.pigo_image)(C.malloc(C.size_t(n)*C.size_t(unsafe.Sizeof(C.pigo_image{})))), n)
+	for i, im := range images {
+		if first[i] {
+			copy(host[offs[i]:], im.Pixels)
+		}
+		desc[i] = C.pigo_image{pixels: (*C.uint8_t)(unsafe.Pointer(&host[offs[i]])), rows: C.int32_t(im.Rows), cols: C.int32_t(im.Cols),
+			dim: C.int32_t(im.Dim)}
+	}
+	return desc, func() {
+		C.free(unsafe.Pointer(&desc[0]))
+		C.pigo_free_pinned(pinned)
+	}
+}
+
+// RunCascadeImagesAngles is RunCascadeImages with images[i] scanned at angles[i] (pigo_run_cascade_images_angles): an
+// angle sweep is one call that lists an image once per angle, and a pixel slice listed several times is copied once.
+// It panics unless there is one angle per image.
+func (pg *Pigo) RunCascadeImagesAngles(images []ImageParams, cp CascadeParams, angles []float64) [][]Detection {
+	if len(angles) != len(images) {
+		panic("pigo: RunCascadeImagesAngles needs one angle per image")
+	}
+	n := len(images)
+	if n == 0 {
+		return nil
+	}
+	desc, free := packImages(images)
+	defer free()
+	capacity := 1024
+	for {
+		buf := make([]C.pigo_det, capacity*n)
+		cnt := make([]C.int, n)
+		rc, err := call(func() C.int {
+			return C.pigo_run_cascade_images_angles(pg.h, &desc[0], C.int(n), (*C.double)(unsafe.Pointer(&angles[0])), C.int(cp.MinSize),
+				C.int(cp.MaxSize), C.double(cp.ShiftFactor), C.double(cp.ScaleFactor), &buf[0], C.int(capacity), &cnt[0], C.PIGO_MEM_HOST, nil)
+		})
+		if rc == C.PIGO_E_CAP {
+			for _, c := range cnt {
+				if int(c) > capacity {
+					capacity = int(c)
+				}
+			}
+			continue
+		}
+		if err != nil {
+			panic(err)
+		}
+		out := make([][]Detection, n)
+		for i := range out {
+			out[i] = toGo(buf[i*capacity:(i+1)*capacity], int(cnt[i]))
+		}
+		return out
+	}
+}
+
 // ClusterDetections mirrors core/pigo.go:262-308, including the in-place sort of the caller's slice by Q.
 func (pg *Pigo) ClusterDetections(detections []Detection, iouThreshold float64) []Detection {
 	n := len(detections)

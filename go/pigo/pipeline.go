@@ -209,3 +209,54 @@ func (pg *Pigo) DetectImages(plc *PuplocCascade, calls []LandmarkCall, images []
 		return faceResults(faces, nfaces, points, faceCap, ncalls, pp.MinFaceScale)
 	}
 }
+
+// DetectImagesAngles is DetectImages with image i scanned and its eyes refined at angles[i] (pigo_detect_images_angles);
+// pp.Angle is not used and the landmark calls stay at angle 0, as GetLandmarkPoint does.  A pixel slice listed several
+// times (an angle sweep) is copied once.  It panics unless there is one angle per image, and on pp.Sharded.
+func (pg *Pigo) DetectImagesAngles(plc *PuplocCascade, calls []LandmarkCall, images []ImageParams, cp CascadeParams, pp PipelineParams, angles []float64) [][]FaceResult {
+	if pp.Sharded {
+		panic("pigo: DetectImagesAngles has no sharded form")
+	}
+	if len(angles) != len(images) {
+		panic("pigo: DetectImagesAngles needs one angle per image")
+	}
+	n := len(images)
+	if n == 0 {
+		return nil
+	}
+	desc, free := packImages(images)
+	defer free()
+	ncalls := len(calls)
+	hs, fl := callArrays(calls)
+	defer C.free(unsafe.Pointer(hs))
+	prm := C.pigo_pipeline_params{min_size: C.int32_t(cp.MinSize), max_size: C.int32_t(cp.MaxSize), shift_factor: C.double(cp.ShiftFactor),
+		scale_factor: C.double(cp.ScaleFactor), iou_threshold: C.double(pp.IoU), min_face_scale: C.int32_t(pp.MinFaceScale),
+		eye_perturbs: C.int32_t(pp.EyePerturbs), flp_perturbs: C.int32_t(pp.FlpPerturbs)}
+	key := atomic.AddUint64(&plc.seed, 1)
+	faceCap := 32
+	for {
+		faces := make([]C.pigo_det, n*faceCap)
+		nfaces := make([]C.int, n)
+		points := make([]C.pigo_point, n*faceCap*(2+ncalls))
+		rc, err := call(func() C.int {
+			return C.pigo_detect_images_angles(pg.h, plc.h, hs, &fl[0], C.int(ncalls), &desc[0], C.int(n), (*C.double)(unsafe.Pointer(&angles[0])),
+				&prm, nil, C.uint64_t(key), &faces[0], C.int(faceCap), &nfaces[0], &points[0], C.PIGO_MEM_HOST, nil)
+		})
+		if rc == C.PIGO_E_CAP {
+			grown := false
+			for _, c := range nfaces {
+				if int(c) > faceCap {
+					faceCap, grown = int(c), true
+				}
+			}
+			if !grown {
+				prm.det_cap = 4 * (prm.det_cap + 512) // raw detections per image exceeded det_cap
+			}
+			continue
+		}
+		if err != nil {
+			panic(err)
+		}
+		return faceResults(faces, nfaces, points, faceCap, ncalls, pp.MinFaceScale)
+	}
+}

@@ -151,6 +151,18 @@ int pigo_run_cascade_images(const pigo_cascade *c, const pigo_image *images, int
                             double shift_factor, double scale_factor, double angle, pigo_det *out, int cap_per_image,
                             int *n_out, unsigned flags, void *stream);
 
+/* Per-image angles: pigo_run_cascade_images with image i scanned at angles[i] (`angles` is a host array of nimages
+ * doubles; > 0 rotates, > 1 is clamped to 1, <= 0 and NaN scan unrotated, as core/pigo.go:232-238).  out[i][0..n_out[i])
+ * is byte for byte what pigo_run_cascade returns for image i alone at angles[i]; with every angle equal to a, the call
+ * is pigo_run_cascade_images(..., a, ...).  An angle sweep is one call: list an image once per angle.  Host descriptors
+ * that repeat (pixels, rows, cols, dim) are copied to the device once.  The rotated images keep one node table per
+ * distinct int(32*a) on the device (at most 33, each nscales*ntrees*512 bytes over the call's longest ladder); past
+ * 1 GiB of tables they run in several passes.  Everything else, including errors, as pigo_run_cascade_images; a null
+ * `angles` with nimages > 0 fails with PIGO_E_INVALID. */
+int pigo_run_cascade_images_angles(const pigo_cascade *c, const pigo_image *images, int nimages, const double *angles,
+                                   int min_size, int max_size, double shift_factor, double scale_factor, pigo_det *out,
+                                   int cap_per_image, int *n_out, unsigned flags, void *stream);
+
 /* Multi-GPU form of the batch call: HOST frames (pinned memory from pigo_alloc_pinned recommended), sharded over
  * the devices of pigo_init_devices, one host thread and one stream per device, no data-path collective; every
  * device writes its frames' slices of `out` / `n_out`, so the result is identical to the single-GPU call.
@@ -257,6 +269,17 @@ int pigo_detect_images(const pigo_cascade *face, const pigo_puploc *puploc, cons
                        const uint8_t *flp_flip, int ncalls, const pigo_image *images, int nimages,
                        const pigo_pipeline_params *params, const float *randoms, uint64_t rng_seed, pigo_det *faces,
                        int face_cap, int *n_faces, pigo_point *points, unsigned flags, void *stream);
+
+/* Per-image angles: pigo_detect_images with params->angle replaced by angles[i] for image i (`angles` is a host array of
+ * nimages doubles, rules as pigo_run_cascade_images_angles; params->angle is ignored).  The scan and the eye RunDetector
+ * of image i use angles[i]; the landmark calls stay at angle 0, as GetLandmarkPoint does.  The generator key is
+ * pigo_detect_images' key, so with every angle equal both calls agree byte for byte.  Everything else as
+ * pigo_detect_images; a null `angles` with nimages > 0 fails with PIGO_E_INVALID. */
+int pigo_detect_images_angles(const pigo_cascade *face, const pigo_puploc *puploc, const pigo_puploc *const *flp,
+                              const uint8_t *flp_flip, int ncalls, const pigo_image *images, int nimages,
+                              const double *angles, const pigo_pipeline_params *params, const float *randoms,
+                              uint64_t rng_seed, pigo_det *faces, int face_cap, int *n_faces, pigo_point *points,
+                              unsigned flags, void *stream);
 
 /* ---- RgbToGrayscale(src image.Image) []uint8, core/grayscale.go:8-23, for *image.NRGBA input (what GetImage returns,
  * core/image.go:13-33): gray = uint8((0.299 r + 0.587 g + 0.114 b) / 256) in float64 on the 16-bit, alpha-premultiplied

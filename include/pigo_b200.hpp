@@ -104,6 +104,13 @@ class Pigo {                    // core/pigo.go:37-43
   // additive: RunCascade for images of different sizes in one call (host pixels); result i is what RunCascade returns for
   // images[i] with cp's MinSize / MaxSize / ShiftFactor / ScaleFactor (cp.Image is not used)
   std::vector<std::vector<Detection>> RunCascadeImages(const std::vector<ImageParams>& images, const CascadeParams& cp, double angle) const {
+    return RunCascadeImagesAngles(images, cp, std::vector<double>(images.size(), angle));
+  }
+  // additive: RunCascadeImages with images[i] scanned at angles[i] (one angle per image; an angle sweep lists an image once
+  // per angle, and repeated pixels are copied to the device once)
+  std::vector<std::vector<Detection>> RunCascadeImagesAngles(const std::vector<ImageParams>& images, const CascadeParams& cp,
+                                                             const std::vector<double>& angles) const {
+    if (angles.size() != images.size()) throw std::invalid_argument("RunCascadeImagesAngles needs one angle per image");
     const int n = (int)images.size();
     std::vector<pigo_image> desc((size_t)n);
     for (int i = 0; i < n; ++i) desc[i] = pigo_image{images[i].Pixels, images[i].Rows, images[i].Cols, images[i].Dim};
@@ -111,8 +118,8 @@ class Pigo {                    // core/pigo.go:37-43
     for (;;) {
       std::vector<pigo_det> buf((size_t)cap * (n > 0 ? n : 1));
       std::vector<int> cnt((size_t)(n > 0 ? n : 1));
-      const int rc = pigo_run_cascade_images(h_.get(), desc.data(), n, cp.MinSize, cp.MaxSize, cp.ShiftFactor, cp.ScaleFactor, angle, buf.data(),
-                                             cap, cnt.data(), PIGO_MEM_HOST, nullptr);
+      const int rc = pigo_run_cascade_images_angles(h_.get(), desc.data(), n, angles.data(), cp.MinSize, cp.MaxSize, cp.ShiftFactor, cp.ScaleFactor,
+                                                    buf.data(), cap, cnt.data(), PIGO_MEM_HOST, nullptr);
       if (rc == PIGO_E_CAP) { for (int c : cnt) cap = c > cap ? c : cap; continue; }
       check(rc);
       std::vector<std::vector<Detection>> out((size_t)n);
@@ -210,12 +217,15 @@ inline std::vector<std::vector<FaceResult>> DetectBatch(const Pigo& face, const 
     }
   return out;
 }
-// additive: DetectBatch for images of different sizes in one library call (host pixels; cp.Image is not used).  result[i] lists
-// image i's clusters; on PIGO_E_CAP the call is retried with the reported face count (or a larger det_cap).
-inline std::vector<std::vector<FaceResult>> DetectImages(const Pigo& face, const PuplocCascade& plc,
-                                                         const std::vector<std::pair<const PuplocCascade*, bool>>& calls,
-                                                         const std::vector<ImageParams>& images, const CascadeParams& cp, double iou, int min_face_scale,
-                                                         int eye_perturbs, int flp_perturbs, uint64_t rng_seed, double angle = 0.0, int face_cap = 32) {
+// additive: DetectImages with image i scanned and its eyes refined at angles[i] (one angle per image; the landmark calls stay
+// at angle 0).  result[i] lists image i's clusters; on PIGO_E_CAP the call is retried with the reported face count (or a
+// larger det_cap).
+inline std::vector<std::vector<FaceResult>> DetectImagesAngles(const Pigo& face, const PuplocCascade& plc,
+                                                               const std::vector<std::pair<const PuplocCascade*, bool>>& calls,
+                                                               const std::vector<ImageParams>& images, const CascadeParams& cp, double iou,
+                                                               int min_face_scale, int eye_perturbs, int flp_perturbs, uint64_t rng_seed,
+                                                               const std::vector<double>& angles, int face_cap = 32) {
+  if (angles.size() != images.size()) throw std::invalid_argument("DetectImagesAngles needs one angle per image");
   const int ncalls = (int)calls.size(), n = (int)images.size();
   std::vector<const pigo_puploc*> hs;
   std::vector<uint8_t> fl;
@@ -223,14 +233,14 @@ inline std::vector<std::vector<FaceResult>> DetectImages(const Pigo& face, const
   std::vector<pigo_image> desc((size_t)n);
   for (int i = 0; i < n; ++i) desc[i] = pigo_image{images[i].Pixels, images[i].Rows, images[i].Cols, images[i].Dim};
   pigo_pipeline_params prm{};
-  prm.min_size = cp.MinSize; prm.max_size = cp.MaxSize; prm.shift_factor = cp.ShiftFactor; prm.scale_factor = cp.ScaleFactor; prm.angle = angle;
+  prm.min_size = cp.MinSize; prm.max_size = cp.MaxSize; prm.shift_factor = cp.ShiftFactor; prm.scale_factor = cp.ScaleFactor; prm.angle = 0.0;
   prm.iou_threshold = iou; prm.min_face_scale = min_face_scale; prm.eye_perturbs = eye_perturbs; prm.flp_perturbs = flp_perturbs; prm.det_cap = 0;
   for (;;) {
     std::vector<pigo_det> faces((size_t)(n > 0 ? n : 1) * face_cap);
     std::vector<int> nfaces((size_t)(n > 0 ? n : 1));
     std::vector<pigo_point> pts((size_t)(n > 0 ? n : 1) * face_cap * (2 + ncalls));
-    const int rc = pigo_detect_images(face.handle(), plc.handle(), hs.data(), fl.data(), ncalls, desc.data(), n, &prm, nullptr, rng_seed, faces.data(),
-                                      face_cap, nfaces.data(), pts.data(), PIGO_MEM_HOST, nullptr);
+    const int rc = pigo_detect_images_angles(face.handle(), plc.handle(), hs.data(), fl.data(), ncalls, desc.data(), n, angles.data(), &prm, nullptr,
+                                             rng_seed, faces.data(), face_cap, nfaces.data(), pts.data(), PIGO_MEM_HOST, nullptr);
     if (rc == PIGO_E_CAP) {
       bool grown = false;
       for (int i = 0; i < n; ++i)
@@ -255,6 +265,15 @@ inline std::vector<std::vector<FaceResult>> DetectImages(const Pigo& face, const
       }
     return out;
   }
+}
+// additive: DetectBatch for images of different sizes in one library call (host pixels; cp.Image is not used), every image at
+// `angle`.  result[i] lists image i's clusters; PIGO_E_CAP is retried as in DetectImagesAngles.
+inline std::vector<std::vector<FaceResult>> DetectImages(const Pigo& face, const PuplocCascade& plc,
+                                                         const std::vector<std::pair<const PuplocCascade*, bool>>& calls,
+                                                         const std::vector<ImageParams>& images, const CascadeParams& cp, double iou, int min_face_scale,
+                                                         int eye_perturbs, int flp_perturbs, uint64_t rng_seed, double angle = 0.0, int face_cap = 32) {
+  return DetectImagesAngles(face, plc, calls, images, cp, iou, min_face_scale, eye_perturbs, flp_perturbs, rng_seed,
+                            std::vector<double>(images.size(), angle), face_cap);
 }
 inline PuplocCascade NewPuplocCascade() { return PuplocCascade(); }   // core/puploc.go:33
 

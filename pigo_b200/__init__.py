@@ -44,6 +44,7 @@ ABI_SYMBOLS = [
     "pigo_device_free", "pigo_device_upload", "pigo_describe_plan", "pigo_init_devices", "pigo_device_count",
     "pigo_device_download", "pigo_run_cascade_batch_sharded", "pigo_detect_batch", "pigo_detect_batch_sharded",
     "pigo_ycbcr_to_nrgba", "pigo_run_cascade_images", "pigo_detect_images", "pigo_puploc_run_images",
+    "pigo_run_cascade_images_angles", "pigo_detect_images_angles",
 ]
 
 
@@ -107,6 +108,8 @@ def lib() -> C.CDLL:
         L.pigo_detect_batch_sharded.argtypes = [vp, vp, vp, vp, i, vp, i, sz, i, i, i, vp, vp, u64, vp, i, vp, vp]
         L.pigo_detect_images.argtypes = [vp, vp, vp, vp, i, vp, i, vp, vp, u64, vp, i, vp, vp, C.c_uint, vp]
         L.pigo_puploc_run_images.argtypes = [vp, vp, i, vp, vp, u64, vp, i, d, vp, vp, C.c_uint, vp]
+        L.pigo_run_cascade_images_angles.argtypes = [vp, vp, i, vp, i, i, d, d, vp, i, vp, C.c_uint, vp]
+        L.pigo_detect_images_angles.argtypes = [vp, vp, vp, vp, i, vp, i, vp, vp, vp, u64, vp, i, vp, vp, C.c_uint, vp]
         L.pigo_ycbcr_to_nrgba.argtypes = [vp, vp, vp, i, i, i, i, i, i, i, vp, vp, C.c_uint, vp]
         L.pigo_set_option.argtypes = [C.c_char_p, C.c_int64]
         L.pigo_get_option.argtypes = [C.c_char_p]
@@ -359,6 +362,39 @@ class Pigo:
         self._need()
         _check(lib().pigo_run_cascade_images(self._h, image_descs(images), len(images), min_size, max_size, shift, scale, angle, out_ptr,
                                              cap_per_image, counts_ptr, FRAMES_DEVICE | OUT_DEVICE, stream or None))
+
+    def RunCascadeImagesAngles(self, images: Sequence[ImageParams], cp: CascadeParams, angles: Sequence[float], cap_per_image: int = 1024):
+        """RunCascadeImages with image i scanned at angles[i] (one angle per image).  An angle sweep is one call: list an
+        image once per angle; repeated host pixels are copied to the device once.  Returns (dets[N, cap] DET_DTYPE, counts[N])."""
+        self._need()
+        n = len(images)
+        if len(angles) != n:
+            raise ValueError("angles must have one entry per image")
+        on_dev = n > 0 and all(isinstance(im.Pixels, int) for im in images)
+        keep = [None if on_dev else _pixels(im) for im in images]   # host pixels stay alive for the call
+        desc = image_descs([(im.Pixels if on_dev else p.ctypes.data, im.Rows, im.Cols, im.Dim) for im, p in zip(images, keep)])
+        ang = np.ascontiguousarray(angles, dtype=np.float64)
+        while True:
+            out = np.zeros((n, max(cap_per_image, 1)), dtype=DET_DTYPE)
+            cnt = np.zeros(max(n, 1), dtype=np.int32)
+            rc = lib().pigo_run_cascade_images_angles(self._h, desc, n, ang.ctypes.data, cp.MinSize, cp.MaxSize, cp.ShiftFactor, cp.ScaleFactor,
+                                                      out.ctypes.data, cap_per_image, cnt.ctypes.data, FRAMES_DEVICE if on_dev else MEM_HOST, None)
+            if rc == PIGO_E_CAP:
+                cap_per_image = int(cnt.max())
+                continue
+            _check(rc)
+            return out, cnt[:n]
+
+    def run_cascade_images_angles_device(self, images, angles: Sequence[float], min_size: int, max_size: int, shift: float, scale: float,
+                                         out_ptr: int, cap_per_image: int, counts_ptr: int, stream: int = 0):
+        """Device-resident, asynchronous form of RunCascadeImagesAngles: images = [(device pointer, rows, cols, dim)], angles a
+        host sequence with one entry per image, out [N][cap] and counts [N] device pointers; no host sync."""
+        self._need()
+        if len(angles) != len(images):
+            raise ValueError("angles must have one entry per image")
+        ang = np.ascontiguousarray(angles, dtype=np.float64)
+        _check(lib().pigo_run_cascade_images_angles(self._h, image_descs(images), len(images), ang.ctypes.data, min_size, max_size, shift, scale,
+                                                    out_ptr, cap_per_image, counts_ptr, FRAMES_DEVICE | OUT_DEVICE, stream or None))
 
     # -- ClusterDetections -----------------------------------------------------------------------------------
     def cluster_array(self, dets: np.ndarray, iou: float):

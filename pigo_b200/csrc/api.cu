@@ -10,8 +10,11 @@
 #include <cstring>
 #include <mutex>
 #include <algorithm>
+#include <map>
+#include <numeric>
 #include <string>
 #include <thread>
+#include <tuple>
 #include <vector>
 
 #include "common.cuh"
@@ -547,29 +550,59 @@ static int build_image_plans(const pigo_image* images, int nimages, int min_size
   return PIGO_OK;
 }
 
+// Table slot of a rotated scan, core/pigo.go:159,:232-236: angle > 0 rotates, angle > 1 is clamped to 1, and angle <= 0
+// or NaN scans unrotated (-1).
+static int rot_slot_of(double angle) { return angle > 0.0 ? (int)(32.0 * (angle > 1.0 ? 1.0 : angle)) : -1; }
+
+// Bound on the rotated node tables one pass of a mixed-size call keeps on the device (one table per distinct slot, each
+// over the call's longest ladder, at most 512 MB).  A call whose slots need more runs its rotated images in several passes.
+static constexpr size_t kImagesRotBytes = (size_t)1 << 30;
+
+// Host images of a mixed-size call in one arena of 256-byte-aligned slots.  Descriptors that repeat an earlier
+// (pixels, rows, cols, dim) share its slot, so a sweep that lists one photo once per angle copies it once.
+// off[i] = byte offset of image i's slot; first[i] = image i is the first to use that slot (its bytes are the ones copied).
+static size_t arena_layout(const pigo_image* images, int n, std::vector<size_t>& off, std::vector<char>& first) {
+  std::map<std::tuple<const uint8_t*, int, int, int>, size_t> seen;
+  off.assign(n, 0);
+  first.assign(n, 0);
+  size_t total = 0;
+  for (int i = 0; i < n; ++i) {
+    const pigo_image& im = images[i];
+    const auto ins = seen.emplace(std::make_tuple(im.pixels, im.rows, im.cols, im.dim), total);
+    off[i] = ins.first->second;
+    if (ins.second) { first[i] = 1; total += ((size_t)im.rows * im.dim + 255) & ~(size_t)255; }
+  }
+  return total;
+}
+
+// Image i is scanned at angles[i].  The rotated and the unrotated scan are different kernel variants, so the images run
+// in passes: the unrotated images in caller order, then the rotated ones ordered by (slot, caller index), cut into
+// passes of at most kImagesRotBytes of node tables.  That order does not depend on how the caller interleaves images and
+// angles.  Each pass is grouped and scheduled from its own windows; finalize writes every image to its caller index.
 static int scan_images_on(pigo_cascade* c, int dev, const pigo_image* images, int nimages, const std::vector<std::vector<ScaleEntry>>& plans,
                           const std::vector<uint64_t>& wins, int longest, int min_size, int max_size, double shift_factor, double scale_factor,
-                          double angle, pigo_det* out, int cap_per_image, int* n_out, unsigned flags, void* stream_) {
+                          const double* angles, pigo_det* out, int cap_per_image, int* n_out, unsigned flags, void* stream_) {
   int rc = PIGO_OK;
   FaceReplica* R = face_replica(c, dev, &rc);
   if (!R) return rc;
   if ((rc = use_device(dev))) return rc;
   const bool frames_dev = flags & PIGO_FRAMES_DEVICE, out_dev = flags & PIGO_OUT_DEVICE;
-  int rot_slot = -1;
-  if (angle > 0.0) rot_slot = (int)(32.0 * (angle > 1.0 ? 1.0 : angle));   // core/pigo.go:159,:232-236
+  std::vector<int> slot(nimages);
+  bool any_rot = false;
+  for (int i = 0; i < nimages; ++i) { slot[i] = rot_slot_of(angles[i]); any_rot |= slot[i] >= 0; }
   const int nlad = (int)plans[longest].size();
   const int max_scale = nlad > 0 ? plans[longest].back().s : 0;
   const size_t rot_bytes = (size_t)nlad * (size_t)R->tab.ntrees * 64 * sizeof(RotNode);
   const long long mode = g_opt.scan_mode.load();
   const bool fast = R->tab.depth == 6 && R->tiled_tab.p != nullptr && mode != 1 &&
-                    (rot_slot < 0 || (g_opt.rot_mode.load() == 0 && max_scale <= 32000 && rot_bytes <= ((size_t)1 << 29)));
+                    (!any_rot || (g_opt.rot_mode.load() == 0 && max_scale <= 32000 && rot_bytes <= ((size_t)1 << 29)));
   if (!fast) {
-    // cascades of depth != 6 and the universal-kernel options: the single-image path, image by image
+    // cascades of depth != 6 and the universal-kernel options: the single-image path, image by image at its own angle
     int rc_cap = PIGO_OK;
     for (int i = 0; i < nimages; ++i) {
       const pigo_image& im = images[i];
       rc = scan_batch_on(c, dev, im.pixels, 1, (size_t)im.rows * im.dim, im.rows, im.cols, im.dim, min_size, max_size, shift_factor,
-                         scale_factor, angle, out ? out + (size_t)i * cap_per_image : nullptr, cap_per_image, n_out + i, flags, stream_);
+                         scale_factor, angles[i], out ? out + (size_t)i * cap_per_image : nullptr, cap_per_image, n_out + i, flags, stream_);
       if (rc == PIGO_E_CAP) rc_cap = rc;
       else if (rc) return rc;
     }
@@ -583,50 +616,81 @@ static int scan_images_on(pigo_cascade* c, int dev, const pigo_image* images, in
   if ((rc = ws_enter(w, st))) return rc;
   const int cap = cap_per_image > 0 ? cap_per_image : 1;
 
-  // schedule from the call's total windows; block prefixes per image, groups of consecutive images
-  uint64_t call_windows = 0;
-  for (uint64_t v : wins) call_windows += v;
-  const ImagesSchedule P = images_schedule(call_windows, rot_slot >= 0);
-  const int GB = 1 << P.gb_shift;
-  // groups of about equal window counts (a uniform 1080p batch gets the uniform path's groups of 128)
-  const uint64_t ngroups = std::max<uint64_t>(1, (call_windows + kImagesGroupWindows - 1) / kImagesGroupWindows);
-  const uint64_t group_target = (call_windows + ngroups - 1) / ngroups;
+  // order[j] = caller index of the image at position j of the call's image table; passes are ranges of positions
+  std::vector<int> order(nimages);
+  std::iota(order.begin(), order.end(), 0);
+  std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return slot[a] < slot[b]; });
+  struct Pass { int first, n; std::vector<int> slots; };   // slots: the pass's node tables in order (empty = unrotated)
+  std::vector<Pass> passes;
+  const size_t slots_per_pass = std::max<size_t>(1, kImagesRotBytes / std::max<size_t>(rot_bytes, 1));
+  for (int j = 0; j < nimages; ++j) {
+    const int s = slot[order[j]];
+    const bool new_slot = j == 0 || s != slot[order[j - 1]];
+    if (j == 0 || (s >= 0 && slot[order[j - 1]] < 0) || (new_slot && s >= 0 && passes.back().slots.size() == slots_per_pass))
+      passes.push_back(Pass{j, 0, {}});
+    Pass& p = passes.back();
+    if (new_slot && s >= 0) p.slots.push_back(s);
+    p.n++;
+  }
+  size_t max_tables = 0;
+  for (const Pass& p : passes) max_tables = std::max(max_tables, p.slots.size());
+
+  // per pass: schedule from the pass's windows; block prefixes per image, groups of consecutive images
   std::vector<ImageDesc> desc(nimages);
   std::vector<ScaleEntry> plan_all;
-  struct Group { int first, n; uint32_t blocks; uint64_t windows; };
+  struct Group { int first, n; uint32_t blocks; uint64_t windows; int pass; };
   std::vector<Group> groups;
+  std::vector<ImagesSchedule> sched(passes.size());
   const long long sub = g_opt.sub_batch.load();   // developer knob: at most this many images per group
-  for (int i = 0; i < nimages; ++i) {
-    if (groups.empty() || (groups.back().windows > 0 && groups.back().windows + wins[i] > group_target) ||
-        (sub > 0 && groups.back().n >= sub))
-      groups.push_back(Group{i, 0, 0, 0});
-    Group& G = groups.back();
-    ImageDesc& d = desc[i];
-    d.rows = images[i].rows; d.cols = images[i].cols; d.dim = images[i].dim;
-    d.nscales = (int)plans[i].size();
-    d.plan_off = (uint32_t)plan_all.size();
-    d.block_base = G.blocks;
-    uint32_t nb = 0;
-    for (ScaleEntry e : plans[i]) {
-      e.pad = nb;
-      nb += (uint32_t)((e.ncols + GB - 1) / GB) * (uint32_t)((e.nrows + GB - 1) / GB);
-      plan_all.push_back(e);
+  for (size_t pi = 0; pi < passes.size(); ++pi) {
+    const Pass& p = passes[pi];
+    uint64_t pass_windows = 0;
+    for (int j = p.first; j < p.first + p.n; ++j) pass_windows += wins[order[j]];
+    sched[pi] = images_schedule(pass_windows, !p.slots.empty());
+    const int GB = 1 << sched[pi].gb_shift;
+    // groups of about equal window counts (a uniform 1080p batch gets the uniform path's groups of 128)
+    const uint64_t ngroups = std::max<uint64_t>(1, (pass_windows + kImagesGroupWindows - 1) / kImagesGroupWindows);
+    const uint64_t group_target = (pass_windows + ngroups - 1) / ngroups;
+    const size_t first_group = groups.size();
+    for (int j = p.first; j < p.first + p.n; ++j) {
+      const int i = order[j];
+      if (groups.size() == first_group || (groups.back().windows > 0 && groups.back().windows + wins[i] > group_target) ||
+          (sub > 0 && groups.back().n >= sub))
+        groups.push_back(Group{j, 0, 0, 0, (int)pi});
+      Group& G = groups.back();
+      ImageDesc& d = desc[j];
+      d.rows = images[i].rows; d.cols = images[i].cols; d.dim = images[i].dim;
+      d.nscales = (int)plans[i].size();
+      d.plan_off = (uint32_t)plan_all.size();
+      d.block_base = G.blocks;
+      d.rot_slot = slot[i];
+      d.rot_off = 0;
+      if (slot[i] >= 0)
+        d.rot_off = (uint32_t)((std::find(p.slots.begin(), p.slots.end(), slot[i]) - p.slots.begin()) * (size_t)nlad * R->tab.ntrees);
+      d.out_index = i;
+      uint32_t nb = 0;
+      for (ScaleEntry e : plans[i]) {
+        e.pad = nb;
+        nb += (uint32_t)((e.ncols + GB - 1) / GB) * (uint32_t)((e.nrows + GB - 1) / GB);
+        plan_all.push_back(e);
+      }
+      if ((uint64_t)G.blocks + nb > 0xffffffffull) return set_err(PIGO_E_INVALID, "image %d: too many windows", i);
+      G.blocks += nb; G.windows += wins[i]; G.n++;
     }
-    if ((uint64_t)G.blocks + nb > 0xffffffffull) return set_err(PIGO_E_INVALID, "image %d: too many windows", i);
-    G.blocks += nb; G.windows += wins[i]; G.n++;
   }
 
-  // pixels: device images in place; host images in one 256-byte-aligned arena, reading only what the reference may index
+  // pixels: device images in place; host images in one 256-byte-aligned arena (each distinct image once), reading only
+  // what the reference may index
   if (frames_dev) {
-    for (int i = 0; i < nimages; ++i) desc[i].base = images[i].pixels;
+    for (int j = 0; j < nimages; ++j) desc[j].base = images[order[j]].pixels;
   } else {
-    std::vector<size_t> off(nimages);
-    size_t total = 0;
-    for (int i = 0; i < nimages; ++i) { off[i] = total; total += ((size_t)images[i].rows * images[i].dim + 255) & ~(size_t)255; }
+    std::vector<size_t> off;
+    std::vector<char> first;
+    const size_t total = arena_layout(images, nimages, off, first);
     if ((rc = w->frames.reserve(total + 256))) return rc;
+    for (int j = 0; j < nimages; ++j) desc[j].base = (const uint8_t*)w->frames.p + off[order[j]];
     for (int i = 0; i < nimages; ++i) {
-      desc[i].base = (const uint8_t*)w->frames.p + off[i];
-      if (wins[i] == 0) continue;   // never read
+      if (!first[i] || wins[i] == 0) continue;   // a repeat, or never read
       const size_t frame_min = (size_t)(images[i].rows - 1) * images[i].dim + images[i].cols;
       CUDA_TRY(cudaMemcpyAsync((uint8_t*)w->frames.p + off[i], images[i].pixels, frame_min, cudaMemcpyHostToDevice, st));
     }
@@ -642,22 +706,27 @@ static int scan_images_on(pigo_cascade* c, int dev, const pigo_image* images, in
   CUDA_TRY(cudaMemcpyAsync(w->img_tab.p, tab.data(), tab.size(), cudaMemcpyHostToDevice, st));
   const ImageDesc* d_desc = (const ImageDesc*)w->img_tab.p;
   const ScaleEntry* d_plan = (const ScaleEntry*)((const uint8_t*)w->img_tab.p + desc_bytes);
-
-  // rotated node table over the longest ladder, cached per workspace by (slot, ladder)
-  const RotNode* d_rot = nullptr;
-  if (rot_slot >= 0 && nlad > 0) {
-    if (w->img_rot_slot != rot_slot || w->img_rot_len != nlad || w->img_rot_min != min_size || w->img_rot_scale != scale_factor) {
-      w->img_rot_slot = -1;
-      if ((rc = w->img_rot.reserve(rot_bytes))) return rc;
-      timing_begin(T_ROTTAB, st);
-      launch_rot_table(R->tab, d_plan + desc[longest].plan_off, nlad, rot_slot, (RotNode*)w->img_rot.p, R->num_sms * 8, st);
-      timing_end(T_ROTTAB, st);
-      g_launches++;
-      CUDA_TRY(cudaGetLastError());
-      w->img_rot_slot = rot_slot; w->img_rot_len = nlad; w->img_rot_min = min_size; w->img_rot_scale = scale_factor;
-    }
-    d_rot = (const RotNode*)w->img_rot.p;
+  const int longest_pos = (int)(std::find(order.begin(), order.end(), longest) - order.begin());
+  // the node tables of a pass over the longest ladder, one per slot, cached per workspace by (slots, ladder)
+  if (max_tables > 0 && nlad > 0) {
+    const size_t cap0 = w->img_rot.cap;
+    if ((rc = w->img_rot.reserve(max_tables * rot_bytes))) { w->img_rot_slots.clear(); return rc; }
+    if (w->img_rot.cap != cap0) w->img_rot_slots.clear();   // a new buffer holds no tables
   }
+  auto build_tables = [&](const std::vector<int>& slots) -> int {
+    if (w->img_rot_slots == slots && w->img_rot_len == nlad && w->img_rot_min == min_size && w->img_rot_scale == scale_factor) return PIGO_OK;
+    w->img_rot_slots.clear();
+    timing_begin(T_ROTTAB, st);
+    for (size_t k = 0; k < slots.size(); ++k) {
+      launch_rot_table(R->tab, d_plan + desc[longest_pos].plan_off, nlad, slots[k], (RotNode*)w->img_rot.p + k * (size_t)nlad * R->tab.ntrees * 64,
+                       R->num_sms * 8, st);
+      g_launches++;
+    }
+    timing_end(T_ROTTAB, st);
+    CUDA_TRY(cudaGetLastError());
+    w->img_rot_slots = slots; w->img_rot_len = nlad; w->img_rot_min = min_size; w->img_rot_scale = scale_factor;
+    return PIGO_OK;
+  };
 
   // outputs and counters: [0..nimages) raw counts | 8 x u64 work counters per group
   pigo_det* d_out = out;
@@ -676,20 +745,29 @@ static int scan_images_on(pigo_cascade* c, int dev, const pigo_image* images, in
   int32_t* d_rawcount = (int32_t*)w->counters.p;
   unsigned long long* d_work = (unsigned long long*)((char*)w->counters.p + work_off);
 
+  int tables_of = -1;   // pass whose node tables img_rot holds in this call
   for (size_t k = 0; k < groups.size(); ++k) {
     const Group& G = groups[k];
     if (G.windows == 0 || R->tab.ntrees == 0) continue;
+    const Pass& p = passes[G.pass];
+    if (!p.slots.empty() && tables_of != G.pass) {
+      if ((rc = build_tables(p.slots))) return rc;
+      tables_of = G.pass;
+    }
     int first_live = G.first;
-    while (wins[first_live] == 0) ++first_live;
+    while (wins[order[first_live]] == 0) ++first_live;
     ScanArgs A{};
     A.tab = R->tab;
     A.frames = desc[first_live].base;   // a readable pixel for the idle lanes of the kernels
     A.nframes = G.n;
     A.plan = d_plan;
-    A.rot_slot = rot_slot; A.rot_tab = d_rot; A.batch_frames = nimages;
+    // the images kernels read only whether the pass is rotated; each image's node table comes from its ImageDesc
+    A.rot_slot = p.slots.empty() ? -1 : p.slots[0];
+    A.rot_tab = p.slots.empty() ? nullptr : (const RotNode*)w->img_rot.p;
+    A.batch_frames = nimages;
     A.raw = (RawDet*)w->raw.p + (size_t)G.first * cap; A.raw_count = d_rawcount + G.first; A.cap = cap;
     A.images = d_desc + G.first; A.nimages = G.n;
-    if ((rc = run_scan_images(R, w, A, P, G.blocks, G.windows, d_work + 8 * k, st, R->num_sms))) return rc;
+    if ((rc = run_scan_images(R, w, A, sched[G.pass], G.blocks, G.windows, d_work + 8 * k, st, R->num_sms))) return rc;
   }
   if (!out_dev) CUDA_TRY(cudaMemsetAsync(d_out, 0, (size_t)nimages * cap * sizeof(pigo_det), st));
   timing_begin(T_FINALIZE, st);
@@ -760,21 +838,22 @@ static int check_image_geometry(const pigo_image* images, int nimages) {
 }
 
 // Pixels of a mixed-size call on the device.  Device images stay where they are; host images go to one 256-byte-aligned
-// arena in w->frames, a round256(rows*dim) slot each, of which only the (rows-1)*dim + cols bytes the reference may index
-// are copied.  The call's ImageDesc table (pixels, rows, cols, pitch) goes to w->img_tab; `staged` receives the device
-// descriptors of the images.
-static int stage_images(Workspace* w, const pigo_image* images, int nimages, bool frames_dev, cudaStream_t st, const ImageDesc** d_desc,
-                        std::vector<pigo_image>& staged) {
+// arena in w->frames (arena_layout: a round256(rows*dim) slot per distinct image), of which only the (rows-1)*dim + cols
+// bytes the reference may index are copied.  The call's ImageDesc table (pixels, rows, cols, pitch and, given `angles`,
+// each image's rotation slot) goes to w->img_tab; `staged` receives the device descriptors of the images.
+static int stage_images(Workspace* w, const pigo_image* images, int nimages, const double* angles, bool frames_dev, cudaStream_t st,
+                        const ImageDesc** d_desc, std::vector<pigo_image>& staged) {
   int rc = PIGO_OK;
   staged.assign(images, images + nimages);
   if (!frames_dev) {
-    std::vector<size_t> off(nimages);
-    size_t total = 0;
-    for (int i = 0; i < nimages; ++i) { off[i] = total; total += ((size_t)images[i].rows * images[i].dim + 255) & ~(size_t)255; }
+    std::vector<size_t> off;
+    std::vector<char> first;
+    const size_t total = arena_layout(images, nimages, off, first);
     if ((rc = w->frames.reserve(total + 256))) return rc;
     for (int i = 0; i < nimages; ++i) {
       uint8_t* dst = (uint8_t*)w->frames.p + off[i];
-      CUDA_TRY(cudaMemcpyAsync(dst, images[i].pixels, (size_t)(images[i].rows - 1) * images[i].dim + images[i].cols, cudaMemcpyHostToDevice, st));
+      if (first[i])
+        CUDA_TRY(cudaMemcpyAsync(dst, images[i].pixels, (size_t)(images[i].rows - 1) * images[i].dim + images[i].cols, cudaMemcpyHostToDevice, st));
       staged[i].pixels = dst;
     }
   }
@@ -782,6 +861,8 @@ static int stage_images(Workspace* w, const pigo_image* images, int nimages, boo
   for (int i = 0; i < nimages; ++i) {
     desc[i] = ImageDesc{};
     desc[i].base = staged[i].pixels; desc[i].rows = staged[i].rows; desc[i].cols = staged[i].cols; desc[i].dim = staged[i].dim;
+    desc[i].rot_slot = angles ? rot_slot_of(angles[i]) : -1;
+    desc[i].out_index = i;
   }
   if ((rc = w->img_tab.reserve((size_t)nimages * sizeof(ImageDesc)))) return rc;
   CUDA_TRY(cudaMemcpyAsync(w->img_tab.p, desc.data(), (size_t)nimages * sizeof(ImageDesc), cudaMemcpyHostToDevice, st));
@@ -815,7 +896,7 @@ static int puploc_run_on(pigo_puploc* p, const pigo_point* seeds, int nseeds, co
   const ImageDesc* d_img = nullptr;
   if (px.images) {
     std::vector<pigo_image> staged;
-    if ((rc = stage_images(w, px.images, px.nframes, frames_dev, st, &d_img, staged))) return rc;
+    if ((rc = stage_images(w, px.images, px.nframes, nullptr, frames_dev, st, &d_img, staged))) return rc;
   } else if (!frames_dev) {
     const size_t bytes = px.stride * (size_t)(px.nframes - 1) + (size_t)(px.rows - 1) * px.dim + px.cols;   // what the reference may index
     if ((rc = w->frames.reserve(px.stride * (size_t)(px.nframes - 1) + (size_t)px.rows * px.dim))) return rc;
@@ -849,8 +930,7 @@ static int puploc_run_on(pigo_puploc* p, const pigo_point* seeds, int nseeds, co
       d_sf = (const int32_t*)w->nout.p;
     }
   }
-  int rot_slot = -1;
-  if (angle > 0.0) rot_slot = (int)(32.0 * (angle > 1.0 ? 1.0 : angle));  // core/puploc.go:252-256, :166
+  const int rot_slot = rot_slot_of(angle);  // core/puploc.go:252-256, :166
   bool done = false;
   timing_begin(T_PUPLOC, st);
   if (g_opt.puploc_mode.load() == 0 && !wide) {
@@ -1060,8 +1140,12 @@ int pigo_run_cascade(const pigo_cascade* c, const uint8_t* pixels, int rows, int
                                 scale_factor, angle, out, cap, n_out, PIGO_MEM_HOST, nullptr);
 }
 
-int pigo_run_cascade_images(const pigo_cascade* cc, const pigo_image* images, int nimages, int min_size, int max_size, double shift_factor,
-                            double scale_factor, double angle, pigo_det* out, int cap_per_image, int* n_out, unsigned flags, void* stream_) {
+}  // extern "C"
+
+// pigo_run_cascade_images and pigo_run_cascade_images_angles: image i at angles[i].  `fn` names the entry point in messages.
+static int run_cascade_images(const char* fn, const pigo_cascade* cc, const pigo_image* images, int nimages, const double* angles, int min_size,
+                              int max_size, double shift_factor, double scale_factor, pigo_det* out, int cap_per_image, int* n_out,
+                              unsigned flags, void* stream_) {
   int rc = check_images_args(cc, images, nimages, out, cap_per_image, n_out);
   if (rc) return rc;
   std::vector<std::vector<ScaleEntry>> plans;
@@ -1069,11 +1153,27 @@ int pigo_run_cascade_images(const pigo_cascade* cc, const pigo_image* images, in
   int longest = 0;
   if ((rc = build_image_plans(images, nimages, min_size, max_size, shift_factor, scale_factor, plans, wins, longest))) return rc;
   if ((rc = ensure_device())) return rc;
-  if (stream_ && stream_capturing((cudaStream_t)stream_))
-    return set_err(PIGO_E_INVALID, "pigo_run_cascade_images does not support stream capture");
+  if (stream_ && stream_capturing((cudaStream_t)stream_)) return set_err(PIGO_E_INVALID, "%s does not support stream capture", fn);
   if (nimages == 0) return PIGO_OK;
   return scan_images_on(const_cast<pigo_cascade*>(cc), default_device(), images, nimages, plans, wins, longest, min_size, max_size,
-                        shift_factor, scale_factor, angle, out, cap_per_image, n_out, flags, stream_);
+                        shift_factor, scale_factor, angles, out, cap_per_image, n_out, flags, stream_);
+}
+
+extern "C" {
+
+int pigo_run_cascade_images(const pigo_cascade* cc, const pigo_image* images, int nimages, int min_size, int max_size, double shift_factor,
+                            double scale_factor, double angle, pigo_det* out, int cap_per_image, int* n_out, unsigned flags, void* stream_) {
+  const std::vector<double> angles(nimages > 0 && nimages <= 65535 ? nimages : 0, angle);   // (other counts are rejected)
+  return run_cascade_images("pigo_run_cascade_images", cc, images, nimages, angles.data(), min_size, max_size, shift_factor, scale_factor,
+                            out, cap_per_image, n_out, flags, stream_);
+}
+
+int pigo_run_cascade_images_angles(const pigo_cascade* cc, const pigo_image* images, int nimages, const double* angles, int min_size,
+                                   int max_size, double shift_factor, double scale_factor, pigo_det* out, int cap_per_image, int* n_out,
+                                   unsigned flags, void* stream_) {
+  if (nimages > 0 && !angles) return set_err(PIGO_E_INVALID, "null angles");
+  return run_cascade_images("pigo_run_cascade_images_angles", cc, images, nimages, angles, min_size, max_size, shift_factor, scale_factor,
+                            out, cap_per_image, n_out, flags, stream_);
 }
 
 // Multi-GPU form (SURVEY.md section 8e): HOST frames are sharded over the devices of pigo_init_devices; every device
@@ -1282,8 +1382,8 @@ int pigo_get_landmark_point(const pigo_puploc* p, const pigo_point* left_eye, co
 // GetLandmarkPoint seed arithmetic and `ncalls` landmark RunDetector calls per face, stream-ordered on the device, with
 // one D2H copy of the results at the end.  Only the pixel source differs between the uniform batch and the mixed-size
 // call: `scan(w, st, dets, det_cap, cnt, W)` stages the pixels, runs RunCascade into dets[nframes][det_cap] / cnt[nframes]
-// on `st` and points W's pixel fields (uniform frames, or the image table) at the pixels the RunDetector stages read.
-// `unit` names a frame in the capacity messages.
+// on `st`, points W's pixel fields (uniform frames, or the image table) at the pixels the RunDetector stages read and sets
+// W.rot_slot to the eye stage's rotation (the call's slot, or kRotSlotPerImage).  `unit` names a frame in the capacity messages.
 template <typename ScanFn>
 static int detect_on(int dev, pigo_cascade* face, pigo_puploc* puploc, pigo_puploc* const* flp, const uint8_t* flp_flip, int ncalls, int nframes,
                      const char* unit, const pigo_pipeline_params& P, const float* randoms, uint64_t rng_seed, uint64_t slot_base, pigo_det* faces,
@@ -1351,15 +1451,13 @@ static int detect_on(int dev, pigo_cascade* face, pigo_puploc* puploc, pigo_pupl
   timing_end(T_SEEDS, st);
   g_launches++;
 
-  int rot_slot = -1;
-  if (P.angle > 0.0) rot_slot = (int)(32.0 * (P.angle > 1.0 ? 1.0 : P.angle));   // RunDetector(puploc, img, det.angle, false), main.go:422
   W.seeds = d_seeds; W.out = d_points; W.randoms = d_rnd; W.rng_seed = rng_seed; W.slot_base = slot_base;
   W.slot_frame = nullptr; W.flipv = nullptr;
   W.slots_per_frame = face_cap * stride;
   W.stride = stride;
-  // (a) both eyes of every face slot
+  // (a) both eyes of every face slot, at the scan's angle: RunDetector(puploc, img, det.angle, false), main.go:422
   PupWork E = W;
-  E.rot_slot = rot_slot; E.first = 0; E.span = 2; E.nwork = nframes * face_cap * 2;
+  E.first = 0; E.span = 2; E.nwork = nframes * face_cap * 2;
   E.tab_of[0] = E.tab_of[1] = 0; E.flip_of[0] = E.flip_of[1] = 0;
   timing_begin(T_PUPLOC, st);
   if (launch_puploc_pairs(E, (unsigned int*)w->counters.p, R->num_sms, st) != 0) return set_err(PIGO_E_INVALID, "pupil cascade has too many trees per stage for the pipeline kernel");
@@ -1403,6 +1501,7 @@ static int detect_batch_on(int dev, pigo_cascade* face, pigo_puploc* puploc, pig
   auto scan = [&](Workspace* w, cudaStream_t st, pigo_det* d_dets, int det_cap, int32_t* d_cnt, PupWork& W) {
     int rc = PIGO_OK;
     W.frames = frames; W.frame_stride = frame_stride; W.nrows = rows; W.ncols = cols; W.dim = dim;
+    W.rot_slot = rot_slot_of(P.angle);
     if (frames_dev)
       return scan_batch_on(face, dev, frames, nframes, frame_stride, rows, cols, dim, P.min_size, P.max_size, P.shift_factor, P.scale_factor,
                            P.angle, d_dets, det_cap, d_cnt, PIGO_FRAMES_DEVICE | PIGO_OUT_DEVICE, st);
@@ -1419,18 +1518,20 @@ static int detect_batch_on(int dev, pigo_cascade* face, pigo_puploc* puploc, pig
 }
 
 // Mixed-size form: the images' pixels are staged once (stage_images) and both the images scan and the RunDetector stages
-// read them; `plans` / `wins` / `longest` are the call's ladders (build_image_plans).
+// read them; `plans` / `wins` / `longest` are the call's ladders (build_image_plans).  Image i is scanned and its eyes are
+// refined at angles[i] (P.angle is not used).
 static int detect_images_on(int dev, pigo_cascade* face, pigo_puploc* puploc, pigo_puploc* const* flp, const uint8_t* flp_flip, int ncalls,
-                            const pigo_image* images, int nimages, const std::vector<std::vector<ScaleEntry>>& plans,
+                            const pigo_image* images, int nimages, const double* angles, const std::vector<std::vector<ScaleEntry>>& plans,
                             const std::vector<uint64_t>& wins, int longest, const pigo_pipeline_params& P, const float* randoms, uint64_t rng_seed,
                             pigo_det* faces, int face_cap, int* n_faces, pigo_point* points, unsigned flags, void* stream_) {
   const bool frames_dev = flags & PIGO_FRAMES_DEVICE;
   auto scan = [&](Workspace* w, cudaStream_t st, pigo_det* d_dets, int det_cap, int32_t* d_cnt, PupWork& W) {
     std::vector<pigo_image> staged;
-    int rc = stage_images(w, images, nimages, frames_dev, st, &W.images, staged);
+    int rc = stage_images(w, images, nimages, angles, frames_dev, st, &W.images, staged);
     if (rc) return rc;
+    W.rot_slot = kRotSlotPerImage;
     return scan_images_on(face, dev, staged.data(), nimages, plans, wins, longest, P.min_size, P.max_size, P.shift_factor, P.scale_factor,
-                          P.angle, d_dets, det_cap, d_cnt, PIGO_FRAMES_DEVICE | PIGO_OUT_DEVICE, st);
+                          angles, d_dets, det_cap, d_cnt, PIGO_FRAMES_DEVICE | PIGO_OUT_DEVICE, st);
   };
   return detect_on(dev, face, puploc, flp, flp_flip, ncalls, nimages, "image", P, randoms, rng_seed, 0, faces, face_cap, n_faces, points, flags,
                    stream_, scan);
@@ -1506,9 +1607,12 @@ static int check_detect_images_args(const pigo_cascade* face, const pigo_puploc*
   return PIGO_OK;
 }
 
-int pigo_detect_images(const pigo_cascade* face, const pigo_puploc* puploc, const pigo_puploc* const* flp, const uint8_t* flp_flip, int ncalls,
-                       const pigo_image* images, int nimages, const pigo_pipeline_params* prm, const float* randoms, uint64_t rng_seed,
-                       pigo_det* faces, int face_cap, int* n_faces, pigo_point* points, unsigned flags, void* stream) {
+// pigo_detect_images and pigo_detect_images_angles: image i at angles[i] (nullptr: prm->angle for every image).  `fn`
+// names the entry point in messages.
+static int detect_images(const char* fn, const pigo_cascade* face, const pigo_puploc* puploc, const pigo_puploc* const* flp, const uint8_t* flp_flip,
+                         int ncalls, const pigo_image* images, int nimages, const double* angles, const pigo_pipeline_params* prm,
+                         const float* randoms, uint64_t rng_seed, pigo_det* faces, int face_cap, int* n_faces, pigo_point* points, unsigned flags,
+                         void* stream) {
   int rc = check_detect_images_args(face, puploc, flp, ncalls, images, nimages, prm, faces, face_cap, n_faces, points);
   if (rc) return rc;
   std::vector<std::vector<ScaleEntry>> plans;
@@ -1516,10 +1620,29 @@ int pigo_detect_images(const pigo_cascade* face, const pigo_puploc* puploc, cons
   int longest = 0;
   if ((rc = build_image_plans(images, nimages, prm->min_size, prm->max_size, prm->shift_factor, prm->scale_factor, plans, wins, longest))) return rc;
   if ((rc = ensure_device())) return rc;
-  if (stream && stream_capturing((cudaStream_t)stream)) return set_err(PIGO_E_INVALID, "pigo_detect_images does not support stream capture");
+  if (stream && stream_capturing((cudaStream_t)stream)) return set_err(PIGO_E_INVALID, "%s does not support stream capture", fn);
   if (nimages == 0) return PIGO_OK;
+  std::vector<double> uniform;
+  if (!angles) { uniform.assign(nimages, prm->angle); angles = uniform.data(); }
   return detect_images_on(default_device(), const_cast<pigo_cascade*>(face), const_cast<pigo_puploc*>(puploc), (pigo_puploc* const*)flp, flp_flip,
-                          ncalls, images, nimages, plans, wins, longest, *prm, randoms, rng_seed, faces, face_cap, n_faces, points, flags, stream);
+                          ncalls, images, nimages, angles, plans, wins, longest, *prm, randoms, rng_seed, faces, face_cap, n_faces, points, flags,
+                          stream);
+}
+
+int pigo_detect_images(const pigo_cascade* face, const pigo_puploc* puploc, const pigo_puploc* const* flp, const uint8_t* flp_flip, int ncalls,
+                       const pigo_image* images, int nimages, const pigo_pipeline_params* prm, const float* randoms, uint64_t rng_seed,
+                       pigo_det* faces, int face_cap, int* n_faces, pigo_point* points, unsigned flags, void* stream) {
+  return detect_images("pigo_detect_images", face, puploc, flp, flp_flip, ncalls, images, nimages, nullptr, prm, randoms, rng_seed, faces, face_cap,
+                       n_faces, points, flags, stream);
+}
+
+int pigo_detect_images_angles(const pigo_cascade* face, const pigo_puploc* puploc, const pigo_puploc* const* flp, const uint8_t* flp_flip,
+                              int ncalls, const pigo_image* images, int nimages, const double* angles, const pigo_pipeline_params* prm,
+                              const float* randoms, uint64_t rng_seed, pigo_det* faces, int face_cap, int* n_faces, pigo_point* points,
+                              unsigned flags, void* stream) {
+  if (nimages > 0 && !angles) return set_err(PIGO_E_INVALID, "null angles");
+  return detect_images("pigo_detect_images_angles", face, puploc, flp, flp_flip, ncalls, images, nimages, angles, prm, randoms, rng_seed, faces,
+                       face_cap, n_faces, points, flags, stream);
 }
 
 // ---- RgbToGrayscale, core/grayscale.go:8-23 ----------------------------------------------------------------

@@ -57,14 +57,20 @@ struct RotNode {
 
 // One image of a mixed-size call (pigo_run_cascade_images).  Every image's ladder is a prefix of the call's longest ladder
 // (off = s/2+1 never decreases, so the entries that fit an image come first), so ladder index si means the same
-// (s, step, off) in every image and one rotated node table serves them all; only nrows/ncols/wbase/pad differ.
+// (s, step, off) in every image and one rotated node table per table slot serves them all; only nrows/ncols/wbase/pad differ.
 struct ImageDesc {
   const uint8_t* base;   // the image's pixels on the device, `dim` bytes per row
   int32_t rows, cols, dim;
   int32_t nscales;       // length of this image's ladder (a prefix of the longest ladder of the call)
   uint32_t plan_off;     // index of the image's first ScaleEntry in the call's concatenated plan
   uint32_t block_base;   // index of the image's first gather block in its group (ScaleEntry.pad counts within the image)
+  uint32_t rot_off;      // rotated scan: the image's node table in ScanArgs.rot_tab, in units of 64 RotNode records
+  int32_t rot_slot;      // the image's table slot int(32*a) (-1 = unrotated): RunDetector with PupWork.rot_slot == kRotSlotPerImage
+  int32_t out_index;     // scan: the image's index in the caller's arrays (finalize writes its results there)
 };
+
+// PupWork.rot_slot / puploc_kernel's rot_slot of a call whose images each carry their own angle (ImageDesc.rot_slot).
+constexpr int kRotSlotPerImage = -2;
 
 struct ScanArgs {
   FaceTables tab;

@@ -80,10 +80,12 @@ __device__ __forceinline__ DeepWin deep_fetch(const ScanArgs& A, const FaceTable
   const ScaleEntry* plan = A.plan;
   int nscales = A.nscales;
   DeepWin w;
+  size_t rot_off = 0;   // IMG: the image's node table (units of 64 RotNode records)
   if (IMG) {
     const ImageDesc im = A.images[frame];
     plan += im.plan_off; nscales = im.nscales;
     w.pc = im.base; w.dim = im.dim; w.lim = im.rows - 1;
+    if (ROT) rot_off = im.rot_off;
   } else {
     w.pc = A.frames + (size_t)frame * A.frame_stride; w.dim = A.dim; w.lim = A.rows - 1;
   }
@@ -95,7 +97,7 @@ __device__ __forceinline__ DeepWin deep_fetch(const ScanArgs& A, const FaceTable
   w.s = e.s; w.wid = it.wid; w.frame = frame; w.t0 = it.tree; w.acc = it.acc;
   w.r = e.off + (int)ri * e.step; w.c = e.off + (int)ci * e.step;
   w.rt = A.rot_tab;
-  if (ROT) w.rt = A.rot_tab + (size_t)si * T.ntrees * 64;
+  if (ROT) w.rt = A.rot_tab + (rot_off + (size_t)si * T.ntrees) * 64;
   else w.pc += (size_t)w.r * w.dim + w.c;
   return w;
 }

@@ -7,7 +7,8 @@
 
 namespace pigo {
 
-// IMG = 1 (mixed-size call): frame = image, decoded against that image's plan (images[frame]).
+// IMG = 1 (mixed-size call): frame = image, decoded against that image's plan (images[frame]); the results go to the
+// caller's slot images[frame].out_index of out / n_out.
 template <int IMG>
 __global__ void __launch_bounds__(256) finalize_kernel(const RawDet* __restrict__ raw, const int32_t* __restrict__ raw_count,
                                                        int cap, const ScaleEntry* __restrict__ plan, int nscales,
@@ -16,7 +17,8 @@ __global__ void __launch_bounds__(256) finalize_kernel(const RawDet* __restrict_
   const int frame = blockIdx.y;
   const int total = raw_count[frame];
   const int n = min(total, cap);
-  if (blockIdx.x == 0 && threadIdx.x == 0) n_out[frame] = total;  // required count (may exceed cap)
+  const int dst = IMG ? images[frame].out_index : frame;
+  if (blockIdx.x == 0 && threadIdx.x == 0) n_out[dst] = total;  // required count (may exceed cap)
   if ((int)(blockIdx.x * blockDim.x) >= n) return;
   const RawDet* rf = raw + (size_t)frame * cap;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -43,7 +45,7 @@ __global__ void __launch_bounds__(256) finalize_kernel(const RawDet* __restrict_
     d.col = e.off + (int)ci * e.step;
     d.scale = e.s;
     d.q = me.q;
-    out[(size_t)frame * cap + rank] = d;
+    out[(size_t)dst * cap + rank] = d;
   }
 }
 

@@ -126,7 +126,7 @@ struct PupWork {
   const int32_t* slot_frame;   // frame of each slot (nullptr = frame 0) unless slots_per_frame > 0
   const uint8_t* flipv;        // per-slot flip flags (nullptr: use flip_of[j])
   int32_t slots_per_frame;     // > 0: frame = slot / slots_per_frame
-  int32_t nrows, ncols, dim, rot_slot;
+  int32_t nrows, ncols, dim, rot_slot;   // rot_slot: -1 unrotated; kRotSlotPerImage: images[frame].rot_slot
   int32_t first, span, stride, nwork, ntabs;
   PuplocTables tab[kMaxPupTabs];
   uint8_t tab_of[32], flip_of[32];
@@ -195,10 +195,11 @@ struct Workspace {
   int p_rows = -1, p_cols = -1, p_min = 0, p_max = 0;
   int pad_first_untiled = -1;  // which gather-block prefix is currently stored in the device copy of the plan
   double p_shift = 0, p_scale = 0;
-  // mixed-size calls keep their own device plan / image table and rotated node table, so that they never disturb the
+  // mixed-size calls keep their own device plan / image table and rotated node tables, so that they never disturb the
   // cached uniform plan above (plan_host, pad_first_untiled, rot_slot + rot_tab, ptab_sig)
   DevBuf img_tab, img_rot;
-  int img_rot_slot = -1, img_rot_len = 0, img_rot_min = 0;   // what img_rot was built for (-1 = nothing)
+  std::vector<int> img_rot_slots;                            // what img_rot was built for: one table per slot, in order (empty = nothing)
+  int img_rot_len = 0, img_rot_min = 0;
   double img_rot_scale = 0;
   void* pinned = nullptr;
   size_t pinned_cap = 0;

@@ -36,7 +36,7 @@ __device__ __forceinline__ uint32_t mix64(uint64_t x) {
 // stages*trees*depth = 1000-deep dependent gather chain into stages*depth = 50; the two children of a node are fetched
 // together with the node's pixel pair (child-pair prefetch).
 // IMG (mixed-size call): seed_frame indexes the image table `images`, whose entry gives the pixels, rows, cols and pitch;
-// frames / frame_stride / nrows / ncols / dim are then unused.
+// frames / frame_stride / nrows / ncols / dim are then unused, and rot_slot == kRotSlotPerImage takes the image's slot.
 template <bool IMG = false>
 __global__ void __launch_bounds__(1024, 1) puploc_kernel(PuplocTables T, const pigo_point* __restrict__ seeds, int nseeds,
                                                          const float* __restrict__ randoms, uint64_t rng_seed,
@@ -49,6 +49,7 @@ __global__ void __launch_bounds__(1024, 1) puploc_kernel(PuplocTables T, const p
   const ImageDesc im = IMG ? images[seed_frame ? seed_frame[sidx] : 0] : ImageDesc{};
   const uint8_t* __restrict__ pixels = IMG ? im.base : frames + (seed_frame ? (size_t)seed_frame[sidx] * frame_stride : 0);
   const int nrows = IMG ? im.rows : frame_rows, ncols = IMG ? im.cols : frame_cols, dim = IMG ? im.dim : frame_dim;
+  if (IMG && rot_slot == kRotSlotPerImage) rot_slot = im.rot_slot;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   __shared__ float rows_[64], cols_[64], scal_[64];
   const pigo_point seed = seeds[sidx];
@@ -186,7 +187,8 @@ __device__ __forceinline__ int clamp_coord(float v) { return max(-(1 << 30), min
 // stage's pixel pairs become shared-memory loads too (a stage gathers 1260 x depth x 2 lane-divergent bytes from it; the
 // scale shrinks by 0.7-0.8 per stage, so the later stages of a landmark call fit).  Stages that do not fit gather from global memory.
 // IMG (mixed-size call): the slot's frame index selects an entry of the image table W.images, which gives the pixels, the
-// clamps rows-1 / cols-1 and the row pitch (the patch's 16-byte path then needs that image's pitch and base aligned).
+// clamps rows-1 / cols-1 and the row pitch (the patch's 16-byte path then needs that image's pitch and base aligned), and
+// with W.rot_slot == kRotSlotPerImage the rotation table slot.
 template <bool STAGED, bool PATCH, bool IMG = false>
 __global__ void __launch_bounds__(kPairThreads, PATCH ? 2 : 3) puploc_pair_kernel(const PupWork W, unsigned int* __restrict__ counter, int leaf_bytes,
                                                                                  int codes_bytes, int patch_cap) {
@@ -219,7 +221,8 @@ __global__ void __launch_bounds__(kPairThreads, PATCH ? 2 : 3) puploc_pair_kerne
     const uint8_t* __restrict__ pixels = IMG ? W.images[frame].base : W.frames + (size_t)frame * W.frame_stride;
     auto dim = [&]() { return IMG ? W.images[frame].dim : W.dim; };   // row pitch (read at each use, as W.dim was before IMG)
     const int L = T.leaves, tree_codes = 4 * L, rlim = (IMG ? W.images[frame].rows : W.nrows) - 1, clim = (IMG ? W.images[frame].cols : W.ncols) - 1;   // padded device layout, see PuplocTables
-    const bool rot = W.rot_slot >= 0;
+    const int rot_slot = (IMG && W.rot_slot == kRotSlotPerImage) ? W.images[frame].rot_slot : W.rot_slot;
+    const bool rot = rot_slot >= 0;
     const int sstride = tree_codes + 8;                    // shared-memory tree stride (bank skew)
     auto stage_codes = [&](int st) {
       const uint2* src = reinterpret_cast<const uint2*>(T.codes + (size_t)st * T.trees * tree_codes);
@@ -250,8 +253,8 @@ __global__ void __launch_bounds__(kPairThreads, PATCH ? 2 : 3) puploc_pair_kerne
         c = __fadd_rn((float)seed.col, __fmul_rn(t1, __fsub_rn(0.5f, u1)));   // :249
         s = __fmul_rn(seed.scale, __fadd_rn(0.925f, __fmul_rn(0.15f, u2)));   // :250
         if (rot) {
-          qs = (int)__fmul_rn(s, c_qsinf[W.rot_slot]);     // int(qsin), :166,:188 (from the INITIAL s)
-          qc = (int)__fmul_rn(s, c_qcosf[W.rot_slot]);
+          qs = (int)__fmul_rn(s, c_qsinf[rot_slot]);     // int(qsin), :166,:188 (from the INITIAL s)
+          qc = (int)__fmul_rn(s, c_qcosf[rot_slot]);
         }
       }
       s_r[tid] = r; s_c[tid] = c; s_s[tid] = s; s_qs[tid] = qs; s_qc[tid] = qc;

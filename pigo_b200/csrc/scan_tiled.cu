@@ -114,7 +114,7 @@ __device__ __forceinline__ void gather_role(const TiledArgs& A, const uint8_t* s
   // per-warp block cursor (uniform)
   uint32_t cur = 0, end = 0;
   int b_s = 0, b_step = 0, b_r0 = 0, b_c0 = 0, b_w = 1, b_ncols = 0, cframe = 0, b_si = 0;
-  int b_dim = 0, b_lim = 0;
+  int b_dim = 0, b_lim = 0, b_rot = 0;   // IMG: pitch, rotated clamp and node-table offset of the block's image
   const uint8_t* b_base = S.frames;
   uint32_t b_wid0 = 0;
   bool more = true;
@@ -163,6 +163,7 @@ __device__ __forceinline__ void gather_role(const TiledArgs& A, const uint8_t* s
             plan = S.plan + im.plan_off;
             lo = 0; hi = im.nscales - 1;
             b_base = im.base; b_dim = im.dim; b_lim = im.rows - 1;
+            if (ROT) b_rot = (int)im.rot_off;
           } else {
             cframe = (int)(g / A.gather_blocks_per_frame);
             wait_frames(S.ready, S.frame_base + (unsigned)cframe + 1u);
@@ -210,7 +211,7 @@ __device__ __forceinline__ void gather_role(const TiledArgs& A, const uint8_t* s
             wid[u] = b_wid0 + ly * (uint32_t)b_ncols + lx;
             fr[u] = cframe; wsi[u] = b_si;
             const uint8_t* fb = IMG ? b_base : S.frames + (size_t)cframe * S.frame_stride;
-            if (ROT) { pc[u] = fb; wr[u] = r; wc[u] = c; sv[u] = b_si * T.ntrees; }
+            if (ROT) { pc[u] = fb; wr[u] = r; wc[u] = c; sv[u] = (IMG ? b_rot : 0) + b_si * T.ntrees; }
             else { pc[u] = fb + (size_t)r * (IMG ? b_dim : S.dim) + c; sv[u] = b_s; }
             if (IMG) { dm[u] = b_dim; lm[u] = b_lim; }
             tbo[u] = casc; acc[u] = 0.f;

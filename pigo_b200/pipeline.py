@@ -179,6 +179,23 @@ def detect_images_device(clf: Pigo, plc: PuplocCascade, flpcs: Dict[str, PuplocC
     arrays, or for every image alike device pointers (int) holding Rows*Dim bytes; cp's MinSize / MaxSize / ShiftFactor /
     ScaleFactor are shared (cp.ImageParams is not used).  randoms: optional [N][face_cap][17][63][3] float32.
     Returns List[List[Face]] (raw=True: the (faces, n_faces, points) arrays)."""
+    return _detect_images(clf, plc, flpcs, images, cp, iou, min_face, eye_perturbs, flp_perturbs, face_cap, angle, None, randoms, rng_seed,
+                          det_cap, raw)
+
+
+def detect_images_angles_device(clf: Pigo, plc: PuplocCascade, flpcs: Dict[str, PuplocCascade], images, cp: CascadeParams, angles,
+                                iou: float = 0.1, min_face: int = 50, eye_perturbs: int = 50, flp_perturbs: int = 63, face_cap: int = 32,
+                                randoms: Optional[np.ndarray] = None, rng_seed: int = 0, det_cap: int = 0, raw: bool = False):
+    """detect_images_device with image i scanned and its eyes refined at angles[i] (pigo_detect_images_angles); the landmark
+    calls stay at angle 0.  An angle sweep is one call: list an image once per angle (its host pixels are copied once)."""
+    if len(angles) != len(images):
+        raise ValueError("angles must have one entry per image")
+    return _detect_images(clf, plc, flpcs, images, cp, iou, min_face, eye_perturbs, flp_perturbs, face_cap, 0.0, angles, randoms, rng_seed,
+                          det_cap, raw)
+
+
+def _detect_images(clf, plc, flpcs, images, cp, iou, min_face, eye_perturbs, flp_perturbs, face_cap, angle, angles, randoms, rng_seed, det_cap,
+                   raw):
     import ctypes as C
     from . import DET_DTYPE, POINT_DTYPE, FRAMES_DEVICE, MEM_HOST, PipelineParams, _check, _pixels, image_descs, lib
     hs, fl = landmark_call_arrays(flpcs)
@@ -195,9 +212,15 @@ def detect_images_device(clf: Pigo, plc: PuplocCascade, flpcs: Dict[str, PuplocC
     faces = np.zeros((n, face_cap), dtype=DET_DTYPE)
     nfaces = np.zeros(max(n, 1), dtype=np.int32)
     points = np.zeros((n, face_cap, 2 + ncalls), dtype=POINT_DTYPE)
-    _check(lib().pigo_detect_images(clf._h, plc._h, hs, fl.ctypes.data, ncalls, desc, n, C.byref(prm), rnd.ctypes.data if rnd is not None else None,
-                                    rng_seed, faces.ctypes.data, face_cap, nfaces.ctypes.data, points.ctypes.data,
-                                    FRAMES_DEVICE if on_dev else MEM_HOST, None))
+    flags = FRAMES_DEVICE if on_dev else MEM_HOST
+    rptr = rnd.ctypes.data if rnd is not None else None
+    if angles is None:
+        _check(lib().pigo_detect_images(clf._h, plc._h, hs, fl.ctypes.data, ncalls, desc, n, C.byref(prm), rptr, rng_seed, faces.ctypes.data,
+                                        face_cap, nfaces.ctypes.data, points.ctypes.data, flags, None))
+    else:
+        ang = np.ascontiguousarray(angles, dtype=np.float64)
+        _check(lib().pigo_detect_images_angles(clf._h, plc._h, hs, fl.ctypes.data, ncalls, desc, n, ang.ctypes.data, C.byref(prm), rptr,
+                                               rng_seed, faces.ctypes.data, face_cap, nfaces.ctypes.data, points.ctypes.data, flags, None))
     if raw:
         return faces, nfaces[:n], points
     return _faces_of(faces, nfaces, points, min_face)

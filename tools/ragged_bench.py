@@ -11,7 +11,12 @@ Usage: `python tools/ragged_bench.py [--frames 256]` on one GPU prints one JSON 
               pigo_detect_batch per geometry and one per image (device resident, CUDA events; faces and counts asserted
               identical, points compared in an untimed run with injected randoms), and pigo_detect_images against
               pigo_detect_batch on --pipeline-frames uniform 1080p frames, alternated
-`--sections scan,pipeline` selects the sections.  Writes nothing to the tree.
+  angles : angle sweeps, one per-image-angle call against one call per angle (device resident, CUDA events, outputs
+              asserted identical): (1) one 1080p frame at 0 and k/32 (k = 1..32) against 33 single-frame calls; (2) bench.py's
+              configs[3] batch, 8 x 4K frames at the 32 rotated slots, against 32 batch calls; (3) 16 wide images x 8 angles
+              through the pipeline, listed image-major and angle-major, against 8 pigo_detect_images calls
+`--sections scan,pipeline` (the default) selects the sections; `--sections angles` runs the sweeps alone.  Writes nothing
+to the tree.
 """
 import argparse
 import json
@@ -324,11 +329,167 @@ def pipeline_bench(clf, dev: int, stream, d_frames, nf: int) -> dict:
                               "note": "median of 5 alternated rounds after 2"}}
 
 
+def angles_bench(clf, dev: int, stream) -> dict:
+    """Angle sweeps as one pigo_run_cascade_images_angles / pigo_detect_images_angles call against one call per angle (device
+    resident, CUDA events, outputs asserted identical); see the module docstring."""
+    import ctypes as C
+    import torch
+    import pigo_b200
+    from pigo_b200 import pipeline, synth
+    L = pigo_b200.lib()
+    st = stream.cuda_stream
+    cuda = f"cuda:{dev}"
+
+    def timed(fn, reps=7, warm=2):
+        for _ in range(warm):
+            fn()
+        torch.cuda.synchronize()
+        ts = []
+        for _ in range(reps):
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            a.record(stream)
+            fn()
+            b.record(stream)
+            torch.cuda.synchronize()
+            ts.append(a.elapsed_time(b))
+        return float(np.median(ts))
+
+    def zeros(*shape):
+        return torch.zeros(shape, dtype=torch.int32, device=cuda)
+
+    res = {}
+    # (1) one 1080p frame at angle 0 and k/32, k = 1..32: one call over 33 pointers to the frame against 33 single-frame calls
+    cap = 1024
+    fr = torch.from_numpy(synth.frame_faces(None, 1080, 1920, noise_seed=3)).to(cuda)
+    sweep = [0.0] + [k / 32 for k in range(1, 33)]
+    na = len(sweep)
+    desc = [(fr.data_ptr(), 1080, 1920, 1920)] * na
+    o1, c1, o2, c2 = zeros(na, cap, 4), zeros(na), zeros(na, cap, 4), zeros(na)
+    W1 = pigo_b200.count_windows(1080, 1920, *PARAMS) * na
+    ms_one = timed(lambda: clf.run_cascade_images_angles_device(desc, sweep, *PARAMS, o1.data_ptr(), cap, c1.data_ptr(), st))
+    ms_lone = timed(lambda: [clf.run_cascade_batch_device(fr.data_ptr(), 1, 1080 * 1920, 1080, 1920, 1920, *PARAMS, a, o2[k].data_ptr(), cap,
+                                                          c2.data_ptr() + 4 * k, st) for k, a in enumerate(sweep)])
+    assert torch.equal(c1, c2) and int(c1.max()) <= cap
+    assert all(torch.equal(o1[k, :c1[k]], o2[k, :c1[k]]) for k in range(na)), "angles (1): outputs differ"
+    res["sweep_1080p"] = {"workload": "one 1080p frame (class F) at angle 0 and k/32, k = 1..32", "entries": na, "windows": W1,
+                          "ms_one_call": ms_one, "ms_call_per_angle": ms_lone, "calls": {"one": 1, "per_angle": na},
+                          "speedup": ms_lone / ms_one, "detections": int(c1.sum()), "outputs_identical": True}
+
+    # (2) bench.py's configs[3] workload: 8 x 4K frames at the 32 rotated slots, one call over pointers into the batch against
+    #     one batch call per slot
+    R4, C4, n4, cap4 = 2160, 3840, 8, 4096
+    fr4 = torch.from_numpy(np.stack([synth.frame_faces(None, R4, C4, shift=(31 * i, 17 * i), noise_seed=i) for i in range(n4)])).to(cuda)
+    rot = [k / 32 for k in range(1, 33)]
+    desc4 = [(fr4[i].data_ptr(), R4, C4, C4) for a in rot for i in range(n4)]   # angle-major: slot k's frames contiguous
+    ang4 = [a for a in rot for _ in range(n4)]
+    o1, c1, o2, c2 = zeros(len(desc4), cap4, 4), zeros(len(desc4)), zeros(len(desc4), cap4, 4), zeros(len(desc4))
+    W4 = pigo_b200.count_windows(R4, C4, *PARAMS) * n4 * len(rot)
+    ms_one = timed(lambda: clf.run_cascade_images_angles_device(desc4, ang4, *PARAMS, o1.data_ptr(), cap4, c1.data_ptr(), st), reps=5)
+    ms_lone = timed(lambda: [clf.run_cascade_batch_device(fr4.data_ptr(), n4, R4 * C4, R4, C4, C4, *PARAMS, a, o2[k * n4].data_ptr(), cap4,
+                                                          c2.data_ptr() + 4 * k * n4, st) for k, a in enumerate(rot)], reps=5)
+    assert torch.equal(c1, c2) and int(c1.max()) <= cap4
+    assert all(torch.equal(o1[k, :c1[k]], o2[k, :c1[k]]) for k in range(len(desc4))), "angles (2): outputs differ"
+    res["config4_sweep"] = {"workload": f"{n4} x 3840x2160 frames (class F, bench.py configs[3]) at angle k/32, k = 1..32", "entries": len(desc4),
+                            "windows": W4, "ms_one_call": ms_one, "ms_batch_call_per_angle": ms_lone, "calls": {"one": 1, "per_angle": len(rot)},
+                            "speedup": ms_lone / ms_one, "windows_per_s_one_call": W4 / (ms_one * 1e-3), "detections": int(c1.sum()),
+                            "outputs_identical": True}
+    del fr4, o1, c1, o2, c2
+
+    # (3) pipeline: 16 mixed images x 8 angles, one pigo_detect_images_angles call (listed image-major and angle-major) against
+    #     one pigo_detect_images call per angle
+    plc = pigo_b200.NewPuplocCascade().UnpackCascade(pigo_b200.load_cascade("puploc"))
+    names = sorted(set(pipeline.EYE_CASCADES + pipeline.MOUTH_CASCADES))
+    flp = {nm: pigo_b200.NewPuplocCascade().UnpackCascade(pigo_b200.load_cascade("lps/" + nm)) for nm in names}
+    hs, fl = pipeline.landmark_call_arrays(flp)
+    ncalls = len(fl)
+    face_cap = 256
+    prm = pigo_b200.PipelineParams(*PARAMS, 0.0, 0.1, 50, 50, 63, 4096)
+    flags = pigo_b200.FRAMES_DEVICE | pigo_b200.OUT_DEVICE
+    imgs = [im for im in ragged_images(64, seed=7) if im[2] >= im[1]][:16]   # wide images: the rotated column clamp stays inside
+    offs, total = [], 0
+    for b, r, c, d in imgs:
+        offs.append(total)
+        total += (r * d + 255) & ~255
+    host = np.zeros(total, dtype=np.uint8)
+    for (b, r, c, d), o in zip(imgs, offs):
+        host[o:o + r * d] = b.reshape(-1)
+    dev_all = torch.from_numpy(host).to(cuda)
+    base = [(dev_all.data_ptr() + o, r, c, d) for (b, r, c, d), o in zip(imgs, offs)]
+    pang = [0.0, 0.02, 0.05, 0.1, 0.25, 0.5, 0.75, 1.0]
+    ni, nk = len(base), len(pang)
+    n = ni * nk
+    listings = {"image_major": [(i, k) for i in range(ni) for k in range(nk)], "angle_major": [(i, k) for k in range(nk) for i in range(ni)]}
+    outs = {key: (zeros(n, face_cap, 4), zeros(n), zeros(n, face_cap, 2 + ncalls, 4)) for key in ("image_major", "angle_major", "per_angle")}
+    pdesc = pigo_b200.image_descs(base)
+
+    def check(rc):
+        if rc != 0:
+            raise RuntimeError(L.pigo_last_error().decode())
+
+    def one(key):
+        lst = listings[key]
+        d = pigo_b200.image_descs([base[i] for i, _ in lst])
+        a = np.array([pang[k] for _, k in lst], dtype=np.float64)
+        o = outs[key]
+        return lambda rnd=None: check(L.pigo_detect_images_angles(clf._h, plc._h, hs, fl.ctypes.data, ncalls, d, n, a.ctypes.data, C.byref(prm),
+                                                                  rnd.data_ptr() if rnd is not None else None, 7, o[0].data_ptr(), face_cap,
+                                                                  o[1].data_ptr(), o[2].data_ptr(), flags, C.c_void_p(st)))
+
+    def per_angle(rnd=None):
+        o = outs["per_angle"]   # angle-major slices: angle k's images at rows k*ni .. (k+1)*ni
+        for k, a in enumerate(pang):
+            p = pigo_b200.PipelineParams(*PARAMS, a, 0.1, 50, 50, 63, 4096)
+            check(L.pigo_detect_images(clf._h, plc._h, hs, fl.ctypes.data, ncalls, pdesc, ni, C.byref(p), rnd[k * ni].data_ptr() if rnd is not None else None,
+                                       7, o[0][k * ni].data_ptr(), face_cap, o[1].data_ptr() + 4 * k * ni, o[2][k * ni].data_ptr(), flags,
+                                       C.c_void_p(st)))
+
+    run_im, run_am = one("image_major"), one("angle_major")
+    pms = {"image_major": [], "angle_major": [], "per_angle": []}
+    for f in (run_im, run_am, per_angle):
+        f(); f()
+    torch.cuda.synchronize()
+    for rnd in range(7):   # alternated rounds, so that drift hits the three alike
+        for key, f in (("image_major", run_im), ("angle_major", run_am), ("per_angle", per_angle)):
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            a.record(stream)
+            f()
+            b.record(stream)
+            torch.cuda.synchronize()
+            if rnd >= 2:
+                pms[key].append(a.elapsed_time(b))
+    pm = {k: float(np.median(v)) for k, v in pms.items()}
+    # faces and counts of the timed runs must agree; points (the generator's key is the slot index) are compared in an untimed
+    # run with the same injected randoms per (image, angle)
+    r = {k: [t.cpu().numpy() for t in v] for k, v in outs.items()}
+    assert int(r["per_angle"][1].max()) <= face_cap
+    am_pos = {ik: p for p, ik in enumerate(listings["angle_major"])}
+    for key in ("image_major", "angle_major"):
+        for p, ik in enumerate(listings[key]):
+            q = am_pos[ik]   # the per-angle calls' outputs are angle-major
+            assert r[key][1][p] == r["per_angle"][1][q] and r[key][0][p].tobytes() == r["per_angle"][0][q].tobytes(), f"angles (3): {key} differs"
+    rnd = torch.from_numpy(np.random.default_rng(13).random((n, face_cap, 2 + ncalls, 63, 3), dtype=np.float32)).to(cuda)   # angle-major
+    rnd_im = rnd[[am_pos[ik] for ik in listings["image_major"]]].contiguous()
+    run_im(rnd_im); run_am(rnd); per_angle(rnd)
+    torch.cuda.synchronize()
+    pts = {k: v[2].cpu().numpy() for k, v in outs.items()}
+    assert pts["angle_major"].tobytes() == pts["per_angle"].tobytes(), "angles (3): points differ with injected randoms"
+    assert all(pts["image_major"][p].tobytes() == pts["per_angle"][am_pos[ik]].tobytes() for p, ik in enumerate(listings["image_major"]))
+    del rnd, rnd_im
+    res["pipeline_sweep"] = {"workload": f"{ni} wide images of the scan section's mix x {nk} angles {pang}, 15 landmark calls, device outputs",
+                             "entries": n, "ms_one_call_image_major": pm["image_major"], "ms_one_call_angle_major": pm["angle_major"],
+                             "ms_detect_images_per_angle": pm["per_angle"], "calls": {"one": 1, "per_angle": nk},
+                             "speedup": pm["per_angle"] / pm["angle_major"], "faces": int(r["per_angle"][1].sum()),
+                             "refined_faces": int((r["per_angle"][0][..., 2] > 50).sum()), "outputs_identical": True,
+                             "note": "median of 5 alternated rounds after 2"}
+    res["note"] = "device resident, CUDA events; (1) and (2) median of 7 / 5 after 2 warm-ups"
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--frames", type=int, default=256, help="frames of the uniform 1080p comparison")
     ap.add_argument("--pipeline-frames", type=int, default=64, help="frames of the uniform 1080p pipeline comparison")
-    ap.add_argument("--sections", default="scan,pipeline", help="comma-separated: scan, pipeline")
+    ap.add_argument("--sections", default="scan,pipeline", help="comma-separated: scan, pipeline, angles")
     args = ap.parse_args()
     sections = set(args.sections.split(","))
     import torch
@@ -341,6 +502,8 @@ def main():
     res = ragged_bench(clf, 0, stream, d_frames[:args.frames], args.frames) if "scan" in sections else {}
     if "pipeline" in sections:
         res["pipeline"] = pipeline_bench(clf, 0, stream, d_frames[:args.pipeline_frames], args.pipeline_frames)
+    if "angles" in sections:
+        res["angles"] = angles_bench(clf, 0, stream)
     res["gpu"] = torch.cuda.get_device_name(0)
     try:   # read-only query: the power limit belongs beside the numbers
         import subprocess

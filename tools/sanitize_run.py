@@ -8,7 +8,7 @@ No torch (ctypes mirror only), a few hundred thousand windows in total, so that 
 Covers: fused kernel (tile + gather role, aligned TMA fill and byte-wise fill), gather-v2 with Q1, deep kernel with Q2,
 queue-overflow fallbacks (tiny KS, tail policy on), universal gather kernel (rotated, scan_mode=1), finalize, cluster,
 RunDetector / landmark kernels over resident frames, grayscale, and the mixed-size pipeline and RunDetector (image-table
-kernel variants; --images runs only those).  Prints the detection counts (compare with a plain run).
+kernel variants; --images runs only those), and the per-image angle calls (--angles runs only those).  Prints the detection counts (compare with a plain run).
 """
 import argparse
 import os
@@ -33,13 +33,14 @@ def main():
     ap.add_argument("--quick", action="store_true", help="scan kernels only, fewer variants (racecheck is slow)")
     ap.add_argument("--new", action="store_true", help="only the kernels added late in round 2 (offset tables, shared-memory deep, queue overflow)")
     ap.add_argument("--images", action="store_true", help="only the mixed-size pipeline and RunDetector (image-table kernel variants)")
+    ap.add_argument("--angles", action="store_true", help="only the per-image angle calls (several node tables, unrotated and rotated passes)")
     args = ap.parse_args()
     pigo_b200.init(0)
     clf = pigo_b200.NewPigo().Unpack(pigo_b200.load_cascade("facefinder"))
     sample = synth.sample_gray()
     counts = []
-    if args.images:
-        counts += images_case(clf, sample)
+    if args.images or args.angles:
+        counts += angles_case(clf, sample) if args.angles else images_case(clf, sample)
         print("sanitize_run counts:", counts, "launches:", pigo_b200.launch_count())
         return
 
@@ -107,6 +108,7 @@ def main():
         out, gy = pigo_b200.YCbCrToNRGBA(yy, cb, cr, 2, 37, 21, want_gray=True)
         counts += [int(out.sum()), int(gy.sum())]
         counts += images_case(clf, sample)
+        counts += angles_case(clf, sample)
     print("sanitize_run counts:", counts, "launches:", pigo_b200.launch_count() if hasattr(pigo_b200, "launch_count") else "n/a")
 
 
@@ -136,6 +138,30 @@ def images_case(clf, sample):
         out = plc.run_detector_images(seeds, which, images[:3], 0.2, [k % 2 == 0 for k in range(24)], rng_seed=9)
         counts.append(sum(o.Row for o in out))
     pigo_b200.set_option("puploc_mode", 0)
+    return counts
+
+
+def angles_case(clf, sample):
+    """pigo_run_cascade_images_angles on two wide images and the sample, each listed at several angles (repeated host
+    descriptors, unrotated and rotated passes, one node table per slot), and pigo_detect_images_angles (per-image eye slots)."""
+    counts = []
+    wide = np.zeros((300, 712), dtype=np.uint8)
+    wide[:, :700] = synth.frame_faces(sample, 300, 700, noise_seed=2)
+    base = [ImageParams(sample, 400, 320, 320), ImageParams(wide, 300, 700, 712), ImageParams(np.zeros(64, np.uint8), 8, 8, 8)]
+    angles = [0.0, 0.05, 0.3, 1.0]
+    ims = [im for im in base for _ in angles]
+    ang = [0.0 if im.Cols < im.Rows else a for im in base for a in angles]   # tall images unrotated (the rotated column clamp)
+    cp = CascadeParams(ImageParams(), *PRM)
+    dets, cnt = clf.RunCascadeImagesAngles(ims, cp, ang, 256)
+    counts += [int(c) for c in cnt]
+    plc = pigo_b200.NewPuplocCascade().UnpackCascade(pigo_b200.load_cascade("puploc"))
+    names = sorted(set(pipeline.EYE_CASCADES + pipeline.MOUTH_CASCADES))
+    flp = {n: pigo_b200.NewPuplocCascade().UnpackCascade(pigo_b200.load_cascade("lps/" + n)) for n in names}
+    for stage in (2, 1):
+        pigo_b200.set_option("puploc_stage", stage)
+        f, n, p = pipeline.detect_images_angles_device(clf, plc, flp, ims, cp, ang, face_cap=8, rng_seed=3, raw=True)
+        counts += [int(n.sum()), int((p["row"] > 0).sum())]
+    pigo_b200.set_option("puploc_stage", 1)
     return counts
 
 
