@@ -767,7 +767,9 @@ static int scan_images_on(pigo_cascade* c, int dev, const pigo_image* images, in
     A.batch_frames = nimages;
     A.raw = (RawDet*)w->raw.p + (size_t)G.first * cap; A.raw_count = d_rawcount + G.first; A.cap = cap;
     A.images = d_desc + G.first; A.nimages = G.n;
-    if ((rc = run_scan_images(R, w, A, sched[G.pass], G.blocks, G.windows, d_work + 8 * k, st, R->num_sms))) return rc;
+    int max_rows = 1, max_cols = 1;
+    for (int j = G.first; j < G.first + G.n; ++j) { max_rows = std::max(max_rows, desc[j].rows); max_cols = std::max(max_cols, desc[j].cols); }
+    if ((rc = run_scan_images(R, w, A, sched[G.pass], G.blocks, G.windows, max_rows, max_cols, d_work + 8 * k, st, R->num_sms))) return rc;
   }
   if (!out_dev) CUDA_TRY(cudaMemsetAsync(d_out, 0, (size_t)nimages * cap * sizeof(pigo_det), st));
   timing_begin(T_FINALIZE, st);

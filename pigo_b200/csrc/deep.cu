@@ -63,8 +63,29 @@ __device__ __forceinline__ float deep_walk(const ScanArgs& A, const FaceTables& 
   }
 }
 
-// Decodes a queue item: window geometry from the ladder entry the producer packed (0xffff = not known: search).
-// IMG = 1 (mixed-size call): the frame field is the image of the group; plan, pixels, pitch and clamp are that image's.
+// Where a queue item's window lies: frame (IMG = 1: the image of the group), ladder entry, size and centre (r, c), from the
+// ladder entry the producer packed (0xffff = not known: search).  The deep kernel and the queue sort decode items with it.
+struct DeepPos {
+  int frame, si, s, r, c;
+};
+template <int IMG>
+__device__ __forceinline__ DeepPos deep_pos(const ScanArgs& A, const DeepItem& it) {
+  DeepPos p;
+  p.frame = (int)(it.frame_si & 0xffffu);
+  const ScaleEntry* plan = A.plan;
+  int nscales = A.nscales;
+  if (IMG) { plan += A.images[p.frame].plan_off; nscales = A.images[p.frame].nscales; }
+  p.si = (int)(it.frame_si >> 16);
+  if (p.si == 0xffff) p.si = find_scale(plan, nscales, it.wid);
+  const ScaleEntry e = plan[p.si];
+  const uint32_t local = it.wid - e.wbase;
+  const uint32_t ri = local / (uint32_t)e.ncols, ci = local - ri * (uint32_t)e.ncols;
+  p.s = e.s;
+  p.r = e.off + (int)ri * e.step; p.c = e.off + (int)ci * e.step;
+  return p;
+}
+
+// Decodes a queue item for the walk.  IMG = 1 (mixed-size call): plan, pixels, pitch and clamp are the image's.
 struct DeepWin {
   uint32_t wid;
   int frame, t0, s, r, c;
@@ -76,36 +97,50 @@ struct DeepWin {
 template <int ROT, int IMG = 0>
 __device__ __forceinline__ DeepWin deep_fetch(const ScanArgs& A, const FaceTables& T, unsigned long long g) {
   const DeepItem it = A.longq[g];
-  const int frame = (int)(it.frame_si & 0xffffu);
-  const ScaleEntry* plan = A.plan;
-  int nscales = A.nscales;
+  const DeepPos p = deep_pos<IMG>(A, it);
   DeepWin w;
   size_t rot_off = 0;   // IMG: the image's node table (units of 64 RotNode records)
   if (IMG) {
-    const ImageDesc im = A.images[frame];
-    plan += im.plan_off; nscales = im.nscales;
+    const ImageDesc im = A.images[p.frame];
     w.pc = im.base; w.dim = im.dim; w.lim = im.rows - 1;
     if (ROT) rot_off = im.rot_off;
   } else {
-    w.pc = A.frames + (size_t)frame * A.frame_stride; w.dim = A.dim; w.lim = A.rows - 1;
+    w.pc = A.frames + (size_t)p.frame * A.frame_stride; w.dim = A.dim; w.lim = A.rows - 1;
   }
-  int si = (int)(it.frame_si >> 16);
-  if (si == 0xffff) si = find_scale(plan, nscales, it.wid);
-  const ScaleEntry e = plan[si];
-  const uint32_t local = it.wid - e.wbase;
-  const uint32_t ri = local / (uint32_t)e.ncols, ci = local - ri * (uint32_t)e.ncols;
-  w.s = e.s; w.wid = it.wid; w.frame = frame; w.t0 = it.tree; w.acc = it.acc;
-  w.r = e.off + (int)ri * e.step; w.c = e.off + (int)ci * e.step;
+  w.s = p.s; w.wid = it.wid; w.frame = p.frame; w.t0 = it.tree; w.acc = it.acc;
+  w.r = p.r; w.c = p.c;
   w.rt = A.rot_tab;
-  if (ROT) w.rt = A.rot_tab + (rot_off + (size_t)si * T.ntrees) * 64;
+  if (ROT) w.rt = A.rot_tab + (rot_off + (size_t)p.si * T.ntrees) * 64;
   else w.pc += (size_t)w.r * w.dim + w.c;
   return w;
 }
 
+// Ordered consumption (CHUNK > 0): a CTA claims CHUNK consecutive items of the sorted queue with one global atomic and its
+// lane groups take them one by one from a shared-memory cursor, so that the windows resident on an SM at the same time are
+// neighbours and their pixel footprints share its L1.  `claim` packs (first item of the run << 32) | items handed out of it.
+// The group that draws ticket CHUNK claims the next run and takes its first item; groups that draw a later ticket wait for it.
+// H100, 256 x 1080p: runs of 32 / 128 items, 256-thread CTAs and 32-pixel cells measured slower, 128-pixel cells the same.
+constexpr int kDeepChunk = 64;
+constexpr int kDeepOrdThreads = 1024;
+template <int CHUNK>
+__device__ __forceinline__ unsigned long long deep_claim(unsigned long long* claim, unsigned long long* counter) {
+  for (;;) {
+    const unsigned long long v = atomicAdd(claim, 1ull);
+    const unsigned j = (unsigned)v;
+    if (j < CHUNK) return (v >> 32) + j;
+    if (j == CHUNK) {
+      const unsigned long long base = atomicAdd(counter, (unsigned long long)CHUNK);
+      atomicExch(claim, (base << 32) | 1ull);
+      return base;
+    }
+    __nanosleep(64);
+  }
+}
+
 // Round-1 loop structure: the lane groups of a warp fetch together, then the warp stays in the step loop until its slowest
 // window is done (measured faster than the flat loop below: one fetch latency per 32/GROUP windows instead of one per window).
-template <int GROUP, int ROT, int IMG = 0>
-__global__ void __launch_bounds__(256) deep_kernel(const ScanArgs A, unsigned long long* counter) {
+template <int GROUP, int ROT, int IMG = 0, int CHUNK = 0>
+__global__ void __launch_bounds__(CHUNK ? kDeepOrdThreads : 256, CHUNK ? 2048 / kDeepOrdThreads : 1) deep_kernel(const ScanArgs A, unsigned long long* counter) {
   const int lane = threadIdx.x & 31;
   const int sub = lane & (GROUP - 1);
   const unsigned gmask = GROUP == 32 ? 0xffffffffu : (GROUP == 16 ? (0xffffu << (lane & 16)) : (0xffu << (lane & 24)));
@@ -113,9 +148,18 @@ __global__ void __launch_bounds__(256) deep_kernel(const ScanArgs A, unsigned lo
   const FaceTables T = A.tab;
   const uint32_t qn = min(*A.long_count, A.long_cap);
   const int lim = A.rows - 1;
+  __shared__ unsigned long long claim;
+  if (CHUNK) {
+    if (threadIdx.x == 0) claim = atomicAdd(counter, (unsigned long long)CHUNK) << 32;
+    __syncthreads();
+  }
   for (;;) {
     unsigned long long g = 0;
-    if (sub == 0) g = atomicAdd(counter, 1ull);
+    if constexpr (CHUNK > 0) {
+      if (sub == 0) g = deep_claim<CHUNK>(&claim, counter);
+    } else {
+      if (sub == 0) g = atomicAdd(counter, 1ull);
+    }
     g = __shfl_sync(gmask, g, leader);
     if (g >= qn) break;
     const DeepWin w = deep_fetch<ROT, IMG>(A, T, g);
@@ -336,8 +380,31 @@ static void launch_deep_images(const ScanArgs& A, unsigned long long* counter, i
   else deep_kernel<32, ROT, 1><<<grid, 256, 0, st>>>(A, counter);
 }
 
-void launch_deep(const ScanArgs& A, unsigned long long* counter, int grid, int group, cudaStream_t st) {
+// Ordered consumption: two 1024-thread CTAs per SM (every lane group of an SM draws from one of two runs), the L1/shared
+// split set to the largest L1 (the kernel's only shared memory is its 8-byte cursor).
+template <int GROUP, int ROT, int IMG>
+static void launch_deep_chunked_g(const ScanArgs& A, unsigned long long* counter, int num_sms, cudaStream_t st) {
+  cudaFuncSetAttribute(deep_kernel<GROUP, ROT, IMG, kDeepChunk>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxL1);
+  deep_kernel<GROUP, ROT, IMG, kDeepChunk><<<num_sms * (2048 / kDeepOrdThreads), kDeepOrdThreads, 0, st>>>(A, counter);
+}
+template <int ROT, int IMG>
+static void launch_deep_chunked(const ScanArgs& A, unsigned long long* counter, int num_sms, int group, cudaStream_t st) {
+  if (group == 8) launch_deep_chunked_g<8, ROT, IMG>(A, counter, num_sms, st);
+  else if (group == 16) launch_deep_chunked_g<16, ROT, IMG>(A, counter, num_sms, st);
+  else launch_deep_chunked_g<32, ROT, IMG>(A, counter, num_sms, st);
+}
+
+void launch_deep(const ScanArgs& A, unsigned long long* counter, int num_sms, int group, bool ordered, cudaStream_t st) {
   const bool rot = A.rot_slot >= 0 && A.rot_tab != nullptr;
+  const int grid = num_sms * 8;
+  if (ordered) {
+    if (A.images != nullptr) {
+      if (rot) launch_deep_chunked<1, 1>(A, counter, num_sms, group, st); else launch_deep_chunked<0, 1>(A, counter, num_sms, group, st);
+    } else {
+      if (rot) launch_deep_chunked<1, 0>(A, counter, num_sms, group, st); else launch_deep_chunked<0, 0>(A, counter, num_sms, group, st);
+    }
+    return;
+  }
   if (A.images != nullptr) {
     if (rot) launch_deep_images<1>(A, counter, grid, group, st); else launch_deep_images<0>(A, counter, grid, group, st);
     return;
@@ -345,6 +412,99 @@ void launch_deep(const ScanArgs& A, unsigned long long* counter, int grid, int g
   const bool flat = g_opt.deep_flat.load() != 0;
   if (rot) { if (flat) launch_deep_g<1, 1>(A, counter, grid, group, st); else launch_deep_g<1, 0>(A, counter, grid, group, st); }
   else { if (flat) launch_deep_g<0, 1>(A, counter, grid, group, st); else launch_deep_g<0, 0>(A, counter, grid, group, st); }
+}
+
+// ---- Q2 in image order -------------------------------------------------------------------------------------
+// A counting sort of the queue on (frame, cell of the window centre), cells of 2^shift x 2^shift pixels in row-major order:
+// key + rank within the key's bin, an exclusive scan of the bins, a scatter.  Every kernel reads the item count on the
+// device, so the sequence needs no host synchronisation.  The order within a bin is the order of the rank atomics, which
+// changes nothing: the deep kernel appends detections with atomics and finalize_kernel sorts them.
+struct DeepGrid {
+  int shift, cells_x, cells;   // cell edge 2^shift, cells per row, cells per frame
+};
+static constexpr uint64_t kDeepMaxBins = 1u << 18;   // bins of one sort: the scan is one CTA
+static DeepGrid deep_grid(int rows, int cols, int nframes) {
+  DeepGrid g{6, 0, 0};   // 64-pixel cells, coarser when a group has too many frames for the bin budget
+  for (;;) {
+    g.cells_x = ((std::max(cols, 1) - 1) >> g.shift) + 1;
+    g.cells = (((std::max(rows, 1) - 1) >> g.shift) + 1) * g.cells_x;
+    if ((uint64_t)g.cells * (uint64_t)std::max(nframes, 1) <= kDeepMaxBins || g.shift >= 24) return g;
+    ++g.shift;
+  }
+}
+
+size_t deep_sort_aux_bytes(int rows, int cols, int nframes, size_t qcap) {
+  const DeepGrid g = deep_grid(rows, cols, nframes);
+  return (((size_t)g.cells * std::max(nframes, 1) + 1) & ~(size_t)1) * sizeof(uint32_t) + qcap * sizeof(uint2);
+}
+
+template <int IMG>
+__global__ void __launch_bounds__(256) deep_key_kernel(const ScanArgs A, DeepGrid G, uint32_t* __restrict__ bins, uint2* __restrict__ keyrank) {
+  const uint32_t qn = min(*A.long_count, A.long_cap);
+  for (uint32_t g = blockIdx.x * blockDim.x + threadIdx.x; g < qn; g += gridDim.x * blockDim.x) {
+    const DeepPos p = deep_pos<IMG>(A, A.longq[g]);
+    const uint32_t key = (uint32_t)p.frame * (uint32_t)G.cells + (uint32_t)((p.r >> G.shift) * G.cells_x + (p.c >> G.shift));
+    keyrank[g] = make_uint2(key, atomicAdd(bins + key, 1u));
+  }
+}
+
+// In-place exclusive scan of bins[0, n) by one CTA: each thread a contiguous segment.
+__global__ void __launch_bounds__(1024) deep_scan_kernel(uint32_t* __restrict__ bins, int n) {
+  __shared__ uint32_t warp_sum[32];
+  const int per = (n + 1023) / 1024;
+  const int lo = min(n, (int)threadIdx.x * per), hi = min(n, lo + per);
+  uint32_t sum = 0;
+  for (int i = lo; i < hi; ++i) sum += bins[i];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  uint32_t incl = sum;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const uint32_t v = __shfl_up_sync(0xffffffffu, incl, d);
+    if (lane >= d) incl += v;
+  }
+  if (lane == 31) warp_sum[warp] = incl;
+  __syncthreads();
+  if (warp == 0) {
+    uint32_t w = warp_sum[lane];
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const uint32_t v = __shfl_up_sync(0xffffffffu, w, d);
+      if (lane >= d) w += v;
+    }
+    warp_sum[lane] = w;
+  }
+  __syncthreads();
+  uint32_t run = incl - sum + (warp > 0 ? warp_sum[warp - 1] : 0u);
+  for (int i = lo; i < hi; ++i) {
+    const uint32_t v = bins[i];
+    bins[i] = run;
+    run += v;
+  }
+}
+
+__global__ void __launch_bounds__(256) deep_scatter_kernel(const ScanArgs A, const uint32_t* __restrict__ bins, const uint2* __restrict__ keyrank,
+                                                           DeepItem* __restrict__ sorted) {
+  const uint32_t qn = min(*A.long_count, A.long_cap);
+  for (uint32_t g = blockIdx.x * blockDim.x + threadIdx.x; g < qn; g += gridDim.x * blockDim.x) {
+    const uint2 kr = keyrank[g];
+    sorted[bins[kr.x] + kr.y] = A.longq[g];
+  }
+}
+
+// Sorts A.longq into `sorted`.  rows / cols: the frame size (mixed-size call: the largest of the group); aux: a buffer of
+// deep_sort_aux_bytes(rows, cols, A.nframes, A.long_cap) bytes.
+int launch_deep_sort(const ScanArgs& A, int rows, int cols, DeepItem* sorted, void* aux, int num_sms, cudaStream_t st) {
+  const DeepGrid G = deep_grid(rows, cols, A.nframes);
+  const int nbins = G.cells * std::max(A.nframes, 1);
+  uint32_t* bins = (uint32_t*)aux;
+  uint2* keyrank = (uint2*)(bins + ((nbins + 1) & ~1));
+  if (cudaMemsetAsync(bins, 0, (size_t)nbins * sizeof(uint32_t), st) != cudaSuccess) return set_err(PIGO_E_CUDA, "cudaMemsetAsync failed");
+  if (A.images != nullptr) deep_key_kernel<1><<<num_sms * 8, 256, 0, st>>>(A, G, bins, keyrank);
+  else deep_key_kernel<0><<<num_sms * 8, 256, 0, st>>>(A, G, bins, keyrank);
+  deep_scan_kernel<<<1, 1024, 0, st>>>(bins, nbins);
+  deep_scatter_kernel<<<num_sms * 8, 256, 0, st>>>(A, bins, keyrank, sorted);
+  g_launches += 3;
+  return PIGO_OK;
 }
 
 // ---- rotated node table -------------------------------------------------------------------------------------

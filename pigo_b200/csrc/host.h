@@ -161,6 +161,7 @@ struct Workspace {
   std::vector<int> ptab_sig;                   // geometry the cached per-scale offset tables were built for (empty = none)
   int rot_slot = -1;                           // table slot the cached rotated node table was built for (-1 = none)
   DevBuf deep[kMaxLanes], longq[kMaxLanes];   // Q1 / Q2 per pipeline lane
+  DevBuf longq_sorted[kMaxLanes], longq_aux[kMaxLanes];   // Q2 in image order, and the sort's bins and keys (launch_deep_sort)
   cudaStream_t lane_stream[kMaxLanes] = {nullptr, nullptr, nullptr, nullptr};
   cudaEvent_t ev_fork = nullptr, ev_join[kMaxLanes] = {nullptr, nullptr, nullptr, nullptr};
   cudaEvent_t busy = nullptr;                  // last asynchronous use of this workspace (device-output calls)
@@ -207,7 +208,7 @@ struct Workspace {
   ~Workspace() {
     frames.release(); raw.release(); counters.release(); out.release(); nout.release(); plan.release();
     for (int l = 0; l < kMaxLanes; ++l) {
-      deep[l].release(); longq[l].release();
+      deep[l].release(); longq[l].release(); longq_sorted[l].release(); longq_aux[l].release();
       if (lane_stream[l]) cudaStreamDestroy(lane_stream[l]);
       if (ev_join[l]) cudaEventDestroy(ev_join[l]);
     }
@@ -314,7 +315,9 @@ void launch_ycbcr(const uint8_t* y, const uint8_t* cb, const uint8_t* cr, int y_
 void launch_scan_gather2(const TiledArgs& A, int grid, size_t smem, cudaStream_t st);
 int gather2_ctas_per_sm(size_t smem, int ng, bool rot, bool img = false);
 void launch_rot_table(const FaceTables& T, const ScaleEntry* plan, int nscales, int slot, RotNode* out, int grid, cudaStream_t st);
-void launch_deep(const ScanArgs& A, unsigned long long* counter, int grid, int group, cudaStream_t st);
+void launch_deep(const ScanArgs& A, unsigned long long* counter, int num_sms, int group, bool ordered, cudaStream_t st);
+size_t deep_sort_aux_bytes(int rows, int cols, int nframes, size_t qcap);
+int launch_deep_sort(const ScanArgs& A, int rows, int cols, DeepItem* sorted, void* aux, int num_sms, cudaStream_t st);
 void launch_deep_smem(const ScanArgs& A, unsigned long long* counter, const uint8_t* tab_tiled, int num_sms, int threads, int group, int t_lo, int k,
                       cudaStream_t st);
 int gather_max_ctas_per_sm(int depth, bool rot);
@@ -339,10 +342,11 @@ struct ImagesSchedule {
   int gb_shift;       // log2 of the gather block edge in windows
   int gather_limit;   // trees a window walks in the gather-v2 kernel before it goes to the deep kernel
   int deep_group;     // lanes per window in the deep kernel
+  bool deep_ordered;  // the deep kernel takes its queue in image order (launch_deep_sort)
 };
 ImagesSchedule images_schedule(uint64_t call_windows, bool rot);
 int run_scan_images(FaceReplica* c, Workspace* w, ScanArgs& A, const ImagesSchedule& P, uint32_t group_blocks, uint64_t group_windows,
-                    unsigned long long* d_work, cudaStream_t st, int num_sms);
+                    int max_rows, int max_cols, unsigned long long* d_work, cudaStream_t st, int num_sms);
 FaceReplica* face_replica(pigo_cascade* c, int dev, int* rc);
 PuplocReplica* puploc_replica(pigo_puploc* p, int dev, int* rc);
 }  // namespace pigo

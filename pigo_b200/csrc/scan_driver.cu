@@ -313,6 +313,22 @@ static int check_launch(const char* what) {
   return PIGO_OK;
 }
 
+// The deep kernel takes Q2 in image order (sorted by frame and 64-pixel cell of the window centre, consumed in per-CTA runs of
+// neighbouring windows that share an SM's L1) above this many windows per call.  Smaller calls (up to four 1080p frames or one
+// 4K frame) keep one atomic per item: their queue is short, latency matters, and the ordered path was no faster on one frame.
+static bool deep_ordered(uint64_t call_windows) { return call_windows > 4000000ull; }
+
+// Sorts D.longq into the lane's second queue buffer and points D at it.  rows / cols: the largest frame of the group.
+static int sort_deep_queue(Workspace* w, int lane, ScanArgs& D, int rows, int cols, uint64_t q2_cap, int num_sms, cudaStream_t st) {
+  int rc;
+  if ((rc = w->longq_sorted[lane].reserve(q2_cap * sizeof(DeepItem)))) return rc;
+  if ((rc = w->longq_aux[lane].reserve(deep_sort_aux_bytes(rows, cols, D.nframes, q2_cap)))) return rc;
+  if ((rc = launch_deep_sort(D, rows, cols, (DeepItem*)w->longq_sorted[lane].p, w->longq_aux[lane].p, num_sms, st))) return rc;
+  if ((rc = check_launch("deep queue sort"))) return rc;
+  D.longq = (DeepItem*)w->longq_sorted[lane].p;
+  return PIGO_OK;
+}
+
 int run_scan(FaceReplica* c, Workspace* w, int lane, ScanArgs& A, unsigned long long* d_work, cudaStream_t st, int num_sms) {
   int rc;
   const bool rot = A.rot_slot >= 0;
@@ -499,7 +515,7 @@ int run_scan(FaceReplica* c, Workspace* w, int lane, ScanArgs& A, unsigned long 
     }
   }
 
-  // ---- deep kernel: Q2, one warp per window, 32 trees per step
+  // ---- deep kernel: Q2, one lane group per window
   {
     timing_begin(T_DEEP, st);
     int group = (int)g_opt.deep_group.load();
@@ -513,7 +529,10 @@ int run_scan(FaceReplica* c, Workspace* w, int lane, ScanArgs& A, unsigned long 
                        (int)std::min<long long>(std::max<long long>(2, g_opt.deep_smem_k.load()), 1 << 20), st);
     } else {
       if (group != 8 && group != 16 && group != 32) group = small_call ? 32 : 8;   // small call: the latency of a full survivor matters
-      launch_deep(A, d_work + 3, num_sms * 8, group, st);
+      ScanArgs D = A;
+      const bool ordered = deep_ordered(call_windows);
+      if (ordered && (rc = sort_deep_queue(w, lane, D, A.rows, A.cols, q2_cap, num_sms, st))) return rc;
+      launch_deep(D, d_work + 3, num_sms, group, ordered, st);
     }
     timing_end(T_DEEP, st);
     g_launches++;
@@ -533,6 +552,7 @@ ImagesSchedule images_schedule(uint64_t call_windows, bool rot) {
   P.gb_shift = (g_opt.gather_block.load() == 8 || (g_opt.gather_block.load() == 0 && small_call)) ? 3 : 4;
   P.deep_group = (int)g_opt.deep_group.load();
   if (P.deep_group != 8 && P.deep_group != 16 && P.deep_group != 32) P.deep_group = small_call ? 32 : 8;
+  P.deep_ordered = deep_ordered(call_windows);
   return P;
 }
 
@@ -540,7 +560,7 @@ ImagesSchedule images_schedule(uint64_t call_windows, bool rot) {
 // located through the image table), then the deep kernel over its survivors -- the kernel pair scan_mode=3 runs for a
 // uniform batch.  The caller has set A.images / A.plan (block prefixes built for P.gb_shift) and, rotated, A.rot_tab.
 int run_scan_images(FaceReplica* c, Workspace* w, ScanArgs& A, const ImagesSchedule& P, uint32_t group_blocks, uint64_t group_windows,
-                    unsigned long long* d_work, cudaStream_t st, int num_sms) {
+                    int max_rows, int max_cols, unsigned long long* d_work, cudaStream_t st, int num_sms) {
   int rc;
   const bool rot = A.rot_slot >= 0;
   // d_work (zeroed per call): [0] block cursor  [3] Q2 consumer cursor  [4] Q1 count (unused)  [5] Q2 count
@@ -577,7 +597,9 @@ int run_scan_images(FaceReplica* c, Workspace* w, ScanArgs& A, const ImagesSched
   if ((rc = check_launch("gather-v2 scan (images)"))) return rc;
 
   timing_begin(T_DEEP, st);
-  launch_deep(A, d_work + 3, num_sms * 8, P.deep_group, st);
+  ScanArgs D = A;
+  if (P.deep_ordered && (rc = sort_deep_queue(w, 0, D, max_rows, max_cols, q2_cap, num_sms, st))) return rc;
+  launch_deep(D, d_work + 3, num_sms, P.deep_group, P.deep_ordered, st);
   timing_end(T_DEEP, st);
   g_launches++;
   return check_launch("deep scan (images)");
