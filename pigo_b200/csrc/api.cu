@@ -393,7 +393,7 @@ static int scan_batch_on(pigo_cascade* c, int dev, const uint8_t* frames, int nf
   bool zero_out_staging = !out_dev;   // slots past a frame's count travel back to the host too: keep them defined (zero)
 
   // Sub-batch pipeline: the batch is cut into groups of frames (group_schedule) that alternate between `lanes` internal
-  // streams.  (1) The deferred queues (Q1/Q2) of a group are bounded and consumed soon after they are filled;
+  // streams.  (1) The deferred queue (Q2) of a group is bounded and consumed soon after they are filled;
   // (2) with host frames, the H2D copy of group k+1 overlaps the scan of group k.
   int rot_slot = -1;
   if (angle > 0.0) {                      // core/pigo.go:232-236

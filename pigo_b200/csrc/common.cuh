@@ -95,14 +95,10 @@ struct ScanArgs {
   uint32_t chunks_per_frame;
   // gather-kernel window filter: only scales with index in [scale_lo, scale_hi) (tiled kernel takes the rest)
   int32_t scale_lo, scale_hi;
-  // Q1 "straggler" queue (optional): windows still alive when a tile warp drained its tile; any tree index.
-  // Consumed one-item-per-lane by the gather-v2 kernel.
-  DeepItem* deep;
-  unsigned int* deep_count;
-  uint32_t deep_cap;
   int32_t batch_frames;       // frames of the whole API call (group-independent choices: gather block edge, deep group width)
-  // Q2 "long" queue: windows that survived the KS shared-memory-resident trees.  Consumed one-item-per-WARP
-  // (32 trees evaluated in parallel) by the deep kernel, which bounds the serial chain of a full survivor.
+  // Q2 "long" queue: windows that survived the shared-memory-resident trees, and the stragglers a tile warp still had alive
+  // when it drained its tile (any tree index).  Consumed one item per lane group (GROUP trees evaluated in parallel) by the
+  // deep kernel, which bounds the serial chain of a full survivor.
   DeepItem* longq;
   unsigned int* long_count;
   uint32_t long_cap;
@@ -171,11 +167,9 @@ struct TiledArgs {
   int32_t gather_scale_lo;                // first ladder entry scanned by the gather warps
   uint32_t gather_blocks_per_frame;       // 16x16-window blocks of those scales (ScaleEntry.pad = block prefix)
   unsigned long long* gather_counter;
-  unsigned long long* q1_counter;         // consumer cursor of Q1 (gather-v2 kernel only)
   int32_t gb_shift;                       // log2 of the gather block edge in windows (4 -> 16x16, 3 -> 8x8)
   int32_t tile_prefetch;                  // tile role: fetch both children of a node with one 64-bit load
-  int32_t consume_q1;                     // gather-v2 only: drain the straggler queue Q1 (complete at launch)
-  int32_t gather_ni;                      // windows per lane in the gather role (ILP)
+  int32_t gather_ni;                     // windows per lane in the gather role (ILP)
   // dense-head variant of the tile role (scan_head_kernel): the first `head_trees` trees of every tiled ladder entry have a
   // per-scale node table (two precomputed 16-bit sample offsets per node) at shared-memory offset head_off; survivors of the
   // head travel through a per-warp ring (ring_off, kRing entries of 12 bytes) to the generic lane-refill loop

@@ -54,8 +54,8 @@ struct Options {
   std::atomic<long long> deep_smem_threads{256};
   std::atomic<long long> deep_smem_lo{24};   // first resident tree / number of resident trees of that kernel
   std::atomic<long long> deep_smem_k{128};
-  std::atomic<long long> gather_limit{0};   // trees a gather-role window walks before it goes to the deep kernel; 0 = auto (8 for calls of <= 40 M windows, else 24)
-  std::atomic<long long> queue_cap{0};      // developer knob: cap of the straggler / deep queues in items (0 = sized from the window count)
+  std::atomic<long long> gather_limit{0};   // trees a gather-role window walks before it goes to the deep kernel; 0 = auto (8 for calls of <= 40 M windows, else 16; rotated and mixed-size scans see scan_driver.cu)
+  std::atomic<long long> queue_cap{0};      // developer knob: cap of the deep queue in items (0 = sized from the window count)
   std::atomic<long long> tile_ptab{0};      // fused kernel, tile role: 1 = per-scale offset tables, scale-synchronous rounds (scan_ptab_kernel)
   std::atomic<long long> ptab_kt{16};       // trees per table of that kernel (survivors go to the deep queue)
   std::atomic<long long> ptab_ks{24};       // raw cascade trees its gather warps keep in shared memory
@@ -160,7 +160,7 @@ struct Workspace {
   DevBuf frames, raw, counters, out, nout, plan, tiles, scratch_a, scratch_b, scratch_c, rot_tab, ptab;
   std::vector<int> ptab_sig;                   // geometry the cached per-scale offset tables were built for (empty = none)
   int rot_slot = -1;                           // table slot the cached rotated node table was built for (-1 = none)
-  DevBuf deep[kMaxLanes], longq[kMaxLanes];   // Q1 / Q2 per pipeline lane
+  DevBuf longq[kMaxLanes];                     // the deep queue Q2 per pipeline lane
   DevBuf longq_sorted[kMaxLanes], longq_aux[kMaxLanes];   // Q2 in image order, and the sort's bins and keys (launch_deep_sort)
   cudaStream_t lane_stream[kMaxLanes] = {nullptr, nullptr, nullptr, nullptr};
   cudaEvent_t ev_fork = nullptr, ev_join[kMaxLanes] = {nullptr, nullptr, nullptr, nullptr};
@@ -208,7 +208,7 @@ struct Workspace {
   ~Workspace() {
     frames.release(); raw.release(); counters.release(); out.release(); nout.release(); plan.release();
     for (int l = 0; l < kMaxLanes; ++l) {
-      deep[l].release(); longq[l].release(); longq_sorted[l].release(); longq_aux[l].release();
+      longq[l].release(); longq_sorted[l].release(); longq_aux[l].release();
       if (lane_stream[l]) cudaStreamDestroy(lane_stream[l]);
       if (ev_join[l]) cudaEventDestroy(ev_join[l]);
     }

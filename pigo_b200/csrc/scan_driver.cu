@@ -1,7 +1,9 @@
 // scan_driver.cu -- host-side planning and sequencing of the scan kernels for one RunCascade batch:
 //   fused kernel     : tile warps (scales whose pixel tiles fit a per-warp shared-memory buffer) + gather warps (the rest)
-//   gather-v2 kernel : the straggler queue Q1 (and any blocks the fused kernel did not take)
-//   deep kernel      : queue Q2, one warp (or half warp) per window, 32 (16) trees per step
+//   gather-v2 kernel : the 16x16-window blocks the fused kernel did not take (gather_warps=0, no tile plan, rotated scan)
+//   deep kernel      : queue Q2 (the tile warps' stragglers and every window that outlived the shared-memory trees),
+//                      one lane group per window (8 lanes, 32 for small calls), one tree per lane and step; large calls
+//                      sort Q2 into image order first
 //   gather kernel    : universal fallback -- rotated scan, cascades of depth != 6, scan_mode=1
 #include <algorithm>
 #include <cstdio>
@@ -333,12 +335,11 @@ int run_scan(FaceReplica* c, Workspace* w, int lane, ScanArgs& A, unsigned long 
   int rc;
   const bool rot = A.rot_slot >= 0;
   const long long mode = g_opt.scan_mode.load();
-  // d_work (zeroed per call): [0] gather block cursor  [1] tile cursor  [2] Q1 consumer cursor  [3] Q2 consumer cursor
-  //                           [4] Q1 count (u32)       [5] Q2 count (u32)  [6] chunk cursor of the standalone gather kernel
-  A.deep = nullptr; A.deep_count = (unsigned int*)(d_work + 4); A.deep_cap = 0;
-  A.longq = nullptr; A.long_count = (unsigned int*)(d_work + 5); A.long_cap = 0;
+  // d_work (zeroed per call): [0] gather block cursor  [1] tile cursor  [2] Q2 consumer cursor  [3] Q2 count (u32)
+  //                           [4] chunk cursor of the standalone gather kernel
+  A.longq = nullptr; A.long_count = (unsigned int*)(d_work + 3); A.long_cap = 0;
   A.chunk = (uint32_t)std::max<long long>(32, g_opt.chunk.load());
-  A.chunk_counter = d_work + 6;
+  A.chunk_counter = d_work + 4;
 
   // Rotated scan on the block/deep structure: needs the per-call node table (one RotNode per ladder entry, tree, node).
   const size_t rot_bytes = (size_t)A.nscales * (size_t)A.tab.ntrees * 64 * sizeof(RotNode);
@@ -373,17 +374,14 @@ int run_scan(FaceReplica* c, Workspace* w, int lane, ScanArgs& A, unsigned long 
     A.rot_tab = (const RotNode*)w->rot_tab.p;
   }
 
-  // ---- queues
+  // ---- the deep queue: the tile warps' stragglers (up to 1/16 of the windows) + the windows that outlive the resident trees
+  //      (1/32, 1/16 with the per-scale offset tables)
   const uint64_t total_windows = (uint64_t)A.wins_per_frame * A.nframes;
-  const uint64_t q1_cap = std::min<uint64_t>(total_windows / 16 + 65536, 1ull << 26);
-  const uint64_t q2_cap = std::min<uint64_t>(total_windows / (g_opt.tile_ptab.load() != 0 ? 16 : 32) + 65536, 1ull << 26);
-  // developer knob: tiny queues force the "queue full" paths of every producer (tests)
+  const uint64_t q2_cap = std::min<uint64_t>(total_windows / 16 + total_windows / (g_opt.tile_ptab.load() != 0 ? 16 : 32) + 65536, 1ull << 26);
+  // developer knob: a tiny queue forces the "queue full" paths of every producer (tests)
   const long long qlim = g_opt.queue_cap.load();
-  const uint64_t q1_use = qlim > 0 ? std::min<uint64_t>(q1_cap, (uint64_t)qlim) : q1_cap;
   const uint64_t q2_use = qlim > 0 ? std::min<uint64_t>(q2_cap, (uint64_t)qlim) : q2_cap;
-  if ((rc = w->deep[lane].reserve(q1_cap * sizeof(DeepItem)))) return rc;
   if ((rc = w->longq[lane].reserve(q2_cap * sizeof(DeepItem)))) return rc;
-  A.deep = (DeepItem*)w->deep[lane].p; A.deep_cap = (uint32_t)q1_use;
   A.longq = (DeepItem*)w->longq[lane].p; A.long_cap = (uint32_t)q2_use;
 
   TiledArgs T{};
@@ -391,19 +389,20 @@ int run_scan(FaceReplica* c, Workspace* w, int lane, ScanArgs& A, unsigned long 
   T.scan.chunk_counter = d_work + 1;
   T.tab_tiled = (const uint8_t*)c->tiled_tab.p;
   T.gather_counter = d_work;
-  T.q1_counter = d_work + 2;
   T.gather_scale_lo = 0;
   T.gather_blocks_per_frame = 0;
   T.tile_prefetch = g_opt.tile_prefetch.load() ? 1 : 0;
   T.gather_ni = (int)std::min<long long>(std::max<long long>(1, g_opt.gather_ni.load()), 3);
   // how long a gather-role window stays in the fused kernel before it leaves for the deep kernel (which walks a window with a
-  // lane group and is the cheaper place for long walks): small and mid-sized calls hand over after 8 trees, large ones after 24.
+  // lane group and is the cheaper place for long walks): calls of up to 40 M windows hand over after 8 trees, larger ones after
+  // 16.  (H100, 256 x 1080p: 8 and 16 trees took 0.7 and 0.6 ms off the 24 used before; but 8 made the 64-frame ShiftFactor 0.1
+  // batch 2 % slower than the previous build, and 16 did not.)
   long long glimit = g_opt.gather_limit.load();
   const unsigned long long call_windows = (unsigned long long)A.wins_per_frame * (unsigned long long)std::max(1, A.batch_frames);
   // "small call" = at most 4 M windows in the whole API call (a 1080p frame has 0.9 M, a 4K frame 3.7 M): latency matters, not throughput
   const bool small_call = call_windows <= 4000000ull;
   // (the rotated scan has no fused kernel: its block kernel keeps 24 trees unless the call is small)
-  if (glimit <= 0) glimit = (rot ? small_call : call_windows <= 40000000ull) ? 8 : 24;
+  if (glimit <= 0) glimit = rot ? (small_call ? 8 : 24) : (call_windows <= 40000000ull ? 8 : 16);
   T.gather_limit = (int)std::min<long long>(glimit, 1 << 20);
   // small batches (a frame or two) cannot fill the GPU with 256-window blocks: use 64-window blocks then
   // (decided from the frames of the whole API call, not of this pipeline group: the block prefix lives in the shared plan)
@@ -415,7 +414,7 @@ int run_scan(FaceReplica* c, Workspace* w, int lane, ScanArgs& A, unsigned long 
     return (int)std::min<long long>(std::min<long long>(std::max<long long>(1, v), A.tab.ntrees), fit);
   };
   int first_untiled = 0;
-  bool blocks_done = false, tiled_ran = false;
+  bool blocks_done = false;
   if (mode != 3 && !rot) {
     FusedPlan P = plan_fused(w->plan_host, A.tab.ntrees, A.batch_frames);
     const TilePlan& tp = P.tp;
@@ -429,7 +428,6 @@ int run_scan(FaceReplica* c, Workspace* w, int lane, ScanArgs& A, unsigned long 
       F.tiles_per_frame = tp.tiles_per_frame;
       F.total_tiles = (unsigned long long)tp.tiles_per_frame * A.nframes;
       F.tile_warps = W;
-      F.consume_q1 = 0;
       F.stats = walk_stats_buffer(c->device);
       F.head_trees = P.head; F.head_nscales = tp.first_untiled;
       F.head_off = (uint32_t)P.L.head_off; F.ring_off = (uint32_t)P.L.ring_off; F.tiles_off = (uint32_t)P.L.tiles_off;
@@ -477,7 +475,6 @@ int run_scan(FaceReplica* c, Workspace* w, int lane, ScanArgs& A, unsigned long 
       timing_end(T_TILED, st);
       g_launches++;
       if ((rc = check_launch("fused scan"))) return rc;
-      tiled_ran = true;
     }
   }
 
@@ -487,21 +484,20 @@ int run_scan(FaceReplica* c, Workspace* w, int lane, ScanArgs& A, unsigned long 
   if (A.ready != nullptr && w->group_copied != nullptr) {
     if (cudaStreamWaitEvent(st, w->group_copied, 0) != cudaSuccess) return set_err(PIGO_E_CUDA, "cudaStreamWaitEvent failed");
   }
-  // ---- gather-v2: the Q1 stragglers of the tile warps + the 16x16-window blocks of the untiled scales
-  {
+  // ---- gather-v2: the 16x16-window blocks of the untiled scales, when the fused kernel's gather warps did not take them
+  //      (gather_warps=0, no tile plan fits, or the rotated scan).  On the default path it does not run: the fused kernel is
+  //      followed by the deep kernel alone.
+  if (!blocks_done && first_untiled < A.nscales) {
     TiledArgs G = T;
     G.scan.ready = nullptr;
     G.ks = round_ks(std::min<long long>(g_opt.gather_ks.load(), T.gather_limit));
-    G.consume_q1 = tiled_ran ? 1 : 0;
     G.tile_warps = 0;
-    if (!blocks_done && first_untiled < A.nscales) {
-      if ((rc = upload_block_prefix(w, first_untiled, A.nscales, T.gb_shift, st, &G.gather_blocks_per_frame))) return rc;
-      G.gather_scale_lo = first_untiled;
-    }
-    if (G.consume_q1 || G.gather_blocks_per_frame > 0) {
+    if ((rc = upload_block_prefix(w, first_untiled, A.nscales, T.gb_shift, st, &G.gather_blocks_per_frame))) return rc;
+    G.gather_scale_lo = first_untiled;
+    if (G.gather_blocks_per_frame > 0) {
       const size_t smem = ((384 + (size_t)G.ks * kTreeRec + 127) & ~(size_t)127);
-      // unrotated, the kernel drains the tile warps' stragglers and the large scales, and on H100 two CTAs per SM measured faster
-      // than four (256 x 1080p: 11 % less step time together with tile_tail_min 6); rotated, it is the whole scan and keeps four
+      // unrotated, on H100 two CTAs per SM measured faster than four (256 x 1080p, when the kernel also drained the tile
+      // warps' stragglers: 11 % less step time together with tile_tail_min 6); rotated, it is the whole scan and keeps four
       int per_sm = (int)g_opt.gather_ctas_per_sm.load();
       if (per_sm <= 0) per_sm = rot ? 4 : 2;
       if (rot) G.gather_ni = std::min(G.gather_ni, 2);
@@ -525,14 +521,14 @@ int run_scan(FaceReplica* c, Workspace* w, int lane, ScanArgs& A, unsigned long 
       if (group != 4 && group != 8 && group != 16 && group != 32) group = 8;
       int threads = (int)g_opt.deep_smem_threads.load();
       threads = std::min(1024, std::max(128, threads)) & ~31;
-      launch_deep_smem(A, d_work + 3, (const uint8_t*)c->tiled_tab.p, num_sms, threads, group, (int)std::min<long long>(std::max<long long>(0, g_opt.deep_smem_lo.load()), 1 << 20),
+      launch_deep_smem(A, d_work + 2, (const uint8_t*)c->tiled_tab.p, num_sms, threads, group, (int)std::min<long long>(std::max<long long>(0, g_opt.deep_smem_lo.load()), 1 << 20),
                        (int)std::min<long long>(std::max<long long>(2, g_opt.deep_smem_k.load()), 1 << 20), st);
     } else {
       if (group != 8 && group != 16 && group != 32) group = small_call ? 32 : 8;   // small call: the latency of a full survivor matters
       ScanArgs D = A;
       const bool ordered = deep_ordered(call_windows);
       if (ordered && (rc = sort_deep_queue(w, lane, D, A.rows, A.cols, q2_cap, num_sms, st))) return rc;
-      launch_deep(D, d_work + 3, num_sms, group, ordered, st);
+      launch_deep(D, d_work + 2, num_sms, group, ordered, st);
     }
     timing_end(T_DEEP, st);
     g_launches++;
@@ -547,6 +543,7 @@ ImagesSchedule images_schedule(uint64_t call_windows, bool rot) {
   ImagesSchedule P;
   const bool small_call = call_windows <= 4000000ull;
   long long glimit = g_opt.gather_limit.load();
+  // (not run_scan's rule: here gather-v2 is the whole scan, as on the rotated path, and the hand-over point was not re-measured)
   if (glimit <= 0) glimit = (rot ? small_call : call_windows <= 40000000ull) ? 8 : 24;
   P.gather_limit = (int)std::min<long long>(glimit, 1 << 20);
   P.gb_shift = (g_opt.gather_block.load() == 8 || (g_opt.gather_block.load() == 0 && small_call)) ? 3 : 4;
@@ -563,9 +560,8 @@ int run_scan_images(FaceReplica* c, Workspace* w, ScanArgs& A, const ImagesSched
                     int max_rows, int max_cols, unsigned long long* d_work, cudaStream_t st, int num_sms) {
   int rc;
   const bool rot = A.rot_slot >= 0;
-  // d_work (zeroed per call): [0] block cursor  [3] Q2 consumer cursor  [4] Q1 count (unused)  [5] Q2 count
-  A.deep = nullptr; A.deep_count = (unsigned int*)(d_work + 4); A.deep_cap = 0;
-  A.long_count = (unsigned int*)(d_work + 5);
+  // d_work (zeroed per call): [0] block cursor  [2] Q2 consumer cursor  [3] Q2 count (as run_scan)
+  A.long_count = (unsigned int*)(d_work + 3);
   const uint64_t q2_cap = std::min<uint64_t>(group_windows / 32 + 65536, 1ull << 26);
   const long long qlim = g_opt.queue_cap.load();
   if ((rc = w->longq[0].reserve(q2_cap * sizeof(DeepItem)))) return rc;
@@ -576,7 +572,6 @@ int run_scan_images(FaceReplica* c, Workspace* w, ScanArgs& A, const ImagesSched
   G.scan = A;
   G.tab_tiled = (const uint8_t*)c->tiled_tab.p;
   G.gather_counter = d_work;
-  G.q1_counter = d_work + 2;
   G.gather_scale_lo = 0;
   G.gather_blocks_per_frame = group_blocks;
   G.gather_limit = P.gather_limit;
@@ -599,7 +594,7 @@ int run_scan_images(FaceReplica* c, Workspace* w, ScanArgs& A, const ImagesSched
   timing_begin(T_DEEP, st);
   ScanArgs D = A;
   if (P.deep_ordered && (rc = sort_deep_queue(w, 0, D, max_rows, max_cols, q2_cap, num_sms, st))) return rc;
-  launch_deep(D, d_work + 3, num_sms, P.deep_group, P.deep_ordered, st);
+  launch_deep(D, d_work + 2, num_sms, P.deep_group, P.deep_ordered, st);
   timing_end(T_DEEP, st);
   g_launches++;
   return check_launch("deep scan (images)");

@@ -12,9 +12,9 @@
 //    2 LDS.U8 pixel gathers); lanes whose window was rejected are re-armed with the next window of the tile via
 //    ballot+popc (straight-line fast path), so warps stay full although ~60% of the windows die at tree 0.
 //  * Long-lived windows must not pin a tile: whatever is still alive when fewer than `tail_min` windows remain after
-//    the tile's list ran out goes to the straggler queue Q1 (finished one-per-lane by gather-v2), and a window that
-//    survives the KS resident trees goes to Q2 (finished one-per-WARP, 32/16 trees per step, by deep.cu).  If a queue
-//    is full the lane simply keeps walking (rows beyond KS from global memory): queues are an optimisation only.
+//    the tile's list ran out, and any window that survives the KS resident trees, goes to the deep queue Q2 (finished
+//    one lane group per window, several trees per step, by deep.cu, which can start a window at any tree).  If the queue
+//    is full the lane simply keeps walking (rows beyond KS from global memory): the queue is an optimisation only.
 //  * GATHER WARPS (same CTA, same shared cascade prefix): the scales too large for a per-warp tile, in 16x16-window
 //    blocks, pixels by ld.global.nc.
 //
@@ -79,7 +79,7 @@ __device__ __forceinline__ int walk_rot_nodes(const RotNode* __restrict__ tn, co
 
 // IMG = 1: a mixed-size call (S.images).  The block cursor then maps a global block index to (image, ladder entry, block)
 // of the group, and pixels, row pitch and the rotated clamp come from that image; gather_blocks_per_frame holds the
-// group's total block count and there is no Q1 (no fused kernel runs before it).
+// group's total block count.
 template <int NG, int ROT, int IMG = 0>
 __device__ __forceinline__ void gather_role(const TiledArgs& A, const uint8_t* smem, uint32_t casc, uint32_t casc_end) {
   const unsigned FULL = 0xffffffffu;
@@ -88,11 +88,8 @@ __device__ __forceinline__ void gather_role(const TiledArgs& A, const uint8_t* s
   const FaceTables T = S.tab;
   const unsigned long long total_blocks = IMG ? (unsigned long long)A.gather_blocks_per_frame
                                               : (unsigned long long)A.gather_blocks_per_frame * S.nframes;
-  // Q1 (stragglers of the tile warps) is complete when the gather-v2 kernel starts; the fused kernel never reads it
-  const uint32_t q1n = (!IMG && A.consume_q1) ? min(*S.deep_count, S.deep_cap) : 0u;
-  bool q1_more = q1n > 0, blocks_more = total_blocks > 0;
-  bool from_q1 = false;
-  if (!blocks_more && !q1_more) return;
+  bool blocks_more = total_blocks > 0;
+  if (!blocks_more) return;
   const uint32_t tbo_last = casc + (uint32_t)T.ntrees * kTreeRec;   // record offset "one past the last tree"
   const int lim = S.rows - 1;
 
@@ -127,17 +124,6 @@ __device__ __forceinline__ void gather_role(const TiledArgs& A, const uint8_t* s
       while (need && more) {
         if (cur == end) {
           unsigned long long g = 0;
-          if (q1_more) {                       // stragglers: 32 queue items per grab
-            if (lane == 0) g = atomicAdd(A.q1_counter, 1ull);
-            g = __shfl_sync(FULL, g, 0);
-            if (g * 32ull < q1n) {
-              from_q1 = true;
-              cur = (uint32_t)g * 32u; end = min(cur + 32u, q1n);
-              continue;
-            }
-            q1_more = false;
-          }
-          from_q1 = false;
           if (blocks_more) {
             if (lane == 0) g = atomicAdd(A.gather_counter, 1ull);
             g = __shfl_sync(FULL, g, 0);
@@ -191,31 +177,16 @@ __device__ __forceinline__ void gather_role(const TiledArgs& A, const uint8_t* s
         const uint32_t rank = __popc(need & lanemask_lt());
         if (!alive[u] && rank < avail) {
           const uint32_t k = cur + rank;
-          if (!IMG && from_q1) {
-            const DeepItem it = S.deep[k];
-            int si = (int)(it.frame_si >> 16);
-            const int itf = (int)(it.frame_si & 0xffffu);
-            if (si == 0xffff) si = find_scale(S.plan, S.nscales, it.wid);   // producer did not know the ladder entry
-            const ScaleEntry e = S.plan[si];
-            const uint32_t local = it.wid - e.wbase;
-            const uint32_t ri = local / (uint32_t)e.ncols, ci = local - ri * (uint32_t)e.ncols;
-            wid[u] = it.wid; fr[u] = itf; wsi[u] = si;
-            const int r = e.off + (int)ri * e.step, c = e.off + (int)ci * e.step;
-            if (ROT) { pc[u] = S.frames + (size_t)itf * S.frame_stride; wr[u] = r; wc[u] = c; sv[u] = si * T.ntrees + it.tree; }
-            else { pc[u] = S.frames + (size_t)itf * S.frame_stride + (size_t)r * S.dim + c; sv[u] = e.s; }
-            tbo[u] = casc + (uint32_t)it.tree * kTreeRec; acc[u] = it.acc;
-          } else {
-            const uint32_t ly = b_w == (1 << A.gb_shift) ? (k >> A.gb_shift) : k / (uint32_t)b_w;
-            const uint32_t lx = k - ly * (uint32_t)b_w;
-            const int r = b_r0 + (int)ly * b_step, c = b_c0 + (int)lx * b_step;
-            wid[u] = b_wid0 + ly * (uint32_t)b_ncols + lx;
-            fr[u] = cframe; wsi[u] = b_si;
-            const uint8_t* fb = IMG ? b_base : S.frames + (size_t)cframe * S.frame_stride;
-            if (ROT) { pc[u] = fb; wr[u] = r; wc[u] = c; sv[u] = (IMG ? b_rot : 0) + b_si * T.ntrees; }
-            else { pc[u] = fb + (size_t)r * (IMG ? b_dim : S.dim) + c; sv[u] = b_s; }
-            if (IMG) { dm[u] = b_dim; lm[u] = b_lim; }
-            tbo[u] = casc; acc[u] = 0.f;
-          }
+          const uint32_t ly = b_w == (1 << A.gb_shift) ? (k >> A.gb_shift) : k / (uint32_t)b_w;
+          const uint32_t lx = k - ly * (uint32_t)b_w;
+          const int r = b_r0 + (int)ly * b_step, c = b_c0 + (int)lx * b_step;
+          wid[u] = b_wid0 + ly * (uint32_t)b_ncols + lx;
+          fr[u] = cframe; wsi[u] = b_si;
+          const uint8_t* fb = IMG ? b_base : S.frames + (size_t)cframe * S.frame_stride;
+          if (ROT) { pc[u] = fb; wr[u] = r; wc[u] = c; sv[u] = (IMG ? b_rot : 0) + b_si * T.ntrees; }
+          else { pc[u] = fb + (size_t)r * (IMG ? b_dim : S.dim) + c; sv[u] = b_s; }
+          if (IMG) { dm[u] = b_dim; lm[u] = b_lim; }
+          tbo[u] = casc; acc[u] = 0.f;
           alive[u] = true;
         }
         cur += min((uint32_t)__popc(need), avail);
@@ -269,8 +240,8 @@ __device__ __forceinline__ void gather_role(const TiledArgs& A, const uint8_t* s
         thr[u] = *reinterpret_cast<const float*>(smem + tbo[u] + 512);
       }
     } else {
-      // some window is past the resident prefix and could not be handed over (Q2 full, or a Q1 item already beyond
-      // the prefix): per-slot walk with a table-source switch
+      // some window is past the resident prefix and could not be handed over (Q2 full): per-slot walk with a table-source
+      // switch
 #pragma unroll
       for (int u = 0; u < NG; ++u) {
         const bool res = tbo[u] < casc_end;
@@ -340,8 +311,8 @@ __device__ __forceinline__ void stage_cascade(const TiledArgs& A, uint32_t smem_
   mbar_wait(bar, 0);
 }
 
-// gather-v2: every warp plays the gather role (untiled scales in 16x16-window blocks + the Q1 stragglers), with the
-// cascade prefix in shared memory.  256 threads, several CTAs per SM.
+// gather-v2: every warp plays the gather role (untiled scales in 16x16-window blocks), with the cascade prefix in shared
+// memory.  256 threads, several CTAs per SM.
 template <int NG, int MINB, int ROT, int IMG = 0>
 __global__ void __launch_bounds__(256, MINB) scan_gather2_kernel(const TiledArgs A) {
   extern __shared__ __align__(128) uint8_t smem[];
@@ -377,8 +348,8 @@ __global__ void __launch_bounds__(MAXT, 1) scan_tiled_kernel(const TiledArgs A, 
 
   const ScanArgs& S = A.scan;
   if (warp >= A.tile_warps) {   // warp-specialised: the remaining warps scan the large scales by global-memory gathers
-    // (a gather-role walk is a chain of L2 round trips, ~4000 cycles per tree: with a frame or two in the batch the host lowers
-    // gather_limit so that long-lived windows move early to the deep kernel, which walks 32 trees per step)
+    // (a gather-role walk is a chain of L2 round trips, ~4000 cycles per tree: the host sets a low gather_limit so that
+    // long-lived windows move early to the deep kernel, which walks several trees per step)
     const uint32_t g_end = casc + (uint32_t)min(A.ks, max(1, A.gather_limit)) * kTreeRec;
     if (A.gather_ni >= 2) gather_role<2, 0>(A, smem, casc, g_end);
     else gather_role<1, 0>(A, smem, casc, g_end);
@@ -528,12 +499,12 @@ __global__ void __launch_bounds__(MAXT, 1) scan_tiled_kernel(const TiledArgs A, 
             unsigned live = ~nd;
             if (exhausted && live != 0u && __popc(live) < A.tail_min && !overflow_mode) {
               unsigned qbase = 0;
-              if (lane == 0) qbase = atomicAdd(S.deep_count, (unsigned)__popc(live));
+              if (lane == 0) qbase = atomicAdd(S.long_count, (unsigned)__popc(live));
               qbase = __shfl_sync(FULL, qbase, 0);
               const unsigned pos = qbase + __popc(live & lanemask_lt());
               const int qsi = scale_index_of(smem, sv[u]);
-              if (alive[u] && pos < S.deep_cap) {
-                S.deep[pos] = DeepItem{wid[u], pack_frame_si(frame, qsi), (int)((tbo[u] - casc) / kTreeRec), acc[u]};
+              if (alive[u] && pos < S.long_cap) {
+                S.longq[pos] = DeepItem{wid[u], pack_frame_si(frame, qsi), (int)((tbo[u] - casc) / kTreeRec), acc[u]};
                 alive[u] = false;
               }
               live = __ballot_sync(FULL, alive[u]);
@@ -930,19 +901,19 @@ __global__ void __launch_bounds__(MAXT, 1) scan_ptab_kernel(const TiledArgs A, c
               if (cur_k == cur_n) {
                 // ---- enter the next band scale: needs the older one left and the table landed.  Lanes still in the older
                 //      scale would hold its buffer (and with it every warp of the CTA) for up to kt trees: they are evicted
-                //      to the straggler queue Q1 instead (a few per cent of the windows; gather-v2 finishes them).
+                //      to the deep queue Q2 instead (a few per cent of the windows; the deep kernel finishes them).
                 if (old_open) {
                   const uint32_t old_lo = tab0 + ((q_round + (uint32_t)k - 1u) & 1u) * bstride;
                   const bool mine = alive && (tbo - old_lo) < bstride;
                   const unsigned mm = __ballot_sync(FULL, mine);
                   if (mm) {
                     unsigned qbase = 0;
-                    if (lane == 0) qbase = atomicAdd(S.deep_count, (unsigned)__popc(mm));
+                    if (lane == 0) qbase = atomicAdd(S.long_count, (unsigned)__popc(mm));
                     qbase = __shfl_sync(FULL, qbase, 0);
                     const unsigned pos = qbase + __popc(mm & lanemask_lt());
                     if (mine) {
                       const int tv = A.kt - tleft;
-                      if (pos < S.deep_cap) S.deep[pos] = DeepItem{wid, pack_frame_si(frame, B.scale_lo + k - 1), tv, acc};
+                      if (pos < S.long_cap) S.longq[pos] = DeepItem{wid, pack_frame_si(frame, B.scale_lo + k - 1), tv, acc};
                       else pt_finish_slow(S.tab.codes, S.tab.preds, S.tab.thresh, S.tab.ntrees, S.raw_count, S.raw, S.cap, smem, pb + bias, pitch, u_s_old, tv, acc, frame, wid);
                       alive = false;
                     }
@@ -988,18 +959,18 @@ __global__ void __launch_bounds__(MAXT, 1) scan_ptab_kernel(const TiledArgs A, c
               cur_k += min(__popc(nd), avail);
               nd = __ballot_sync(FULL, !alive);
             }
-            // ---- tail policy: once the tile is drained, a thin slot group is handed to the straggler queue Q1
+            // ---- tail policy: once the tile is drained, a thin slot group is handed to the deep queue Q2
             unsigned live = __ballot_sync(FULL, alive);
             if (exhausted && live != 0u && __popc(live) < A.tail_min) {
               unsigned qbase = 0;
-              if (lane == 0) qbase = atomicAdd(S.deep_count, (unsigned)__popc(live));
+              if (lane == 0) qbase = atomicAdd(S.long_count, (unsigned)__popc(live));
               qbase = __shfl_sync(FULL, qbase, 0);
               const unsigned pos = qbase + __popc(live & lanemask_lt());
               if (alive) {
                 const uint32_t old_lo = tab0 + ((q_round + (uint32_t)k - 1u) & 1u) * bstride;
                 const bool in_old = old_open && (tbo - old_lo) < bstride;
                 const int tv = A.kt - tleft;
-                if (pos < S.deep_cap) S.deep[pos] = DeepItem{wid, pack_frame_si(frame, B.scale_lo + (in_old ? k - 1 : k)), tv, acc};
+                if (pos < S.long_cap) S.longq[pos] = DeepItem{wid, pack_frame_si(frame, B.scale_lo + (in_old ? k - 1 : k)), tv, acc};
                 else pt_finish_slow(S.tab.codes, S.tab.preds, S.tab.thresh, S.tab.ntrees, S.raw_count, S.raw, S.cap, smem, pb + bias, pitch, in_old ? u_s_old : u_s, tv, acc, frame, wid);
                 alive = false;
               }
@@ -1314,14 +1285,14 @@ __global__ void __launch_bounds__(MAXT, 1) scan_head_kernel(const TiledArgs A, c
         continue;
       }
       if (exhausted && ring_cnt == 0 && !overflow_mode && __popc(live) < A.tail_min) {
-        // tile drained: a thin group of stragglers goes to Q1 (finished one-per-lane by gather-v2)
+        // tile drained: a thin group of stragglers goes to Q2 (finished by the deep kernel, one lane group per window)
         unsigned qbase = 0;
-        if (lane == 0) qbase = atomicAdd(S.deep_count, (unsigned)__popc(live));
+        if (lane == 0) qbase = atomicAdd(S.long_count, (unsigned)__popc(live));
         qbase = __shfl_sync(FULL, qbase, 0);
         const unsigned pos = qbase + __popc(live & lanemask_lt());
         const int qsi = scale_index_of(smem, sv);
-        if (alive && pos < S.deep_cap) {
-          S.deep[pos] = DeepItem{wid, pack_frame_si(frame, qsi), (int)((tbo - casc) / kTreeRec), acc};
+        if (alive && pos < S.long_cap) {
+          S.longq[pos] = DeepItem{wid, pack_frame_si(frame, qsi), (int)((tbo - casc) / kTreeRec), acc};
           alive = false;
         }
         live = __ballot_sync(FULL, alive);

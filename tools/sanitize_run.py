@@ -5,7 +5,7 @@
     compute-sanitizer --tool racecheck --error-exitcode 3 python tools/sanitize_run.py --quick
 
 No torch (ctypes mirror only), a few hundred thousand windows in total, so that the instrumented run ends in minutes.
-Covers: fused kernel (tile + gather role, aligned TMA fill and byte-wise fill), gather-v2 with Q1, deep kernel with Q2,
+Covers: fused kernel (tile + gather role, aligned TMA fill and byte-wise fill), gather-v2, deep kernel with Q2,
 queue-overflow fallbacks (tiny KS, tail policy on), universal gather kernel (rotated, scan_mode=1), finalize, cluster,
 RunDetector / landmark kernels over resident frames, grayscale, and the mixed-size pipeline and RunDetector (image-table
 kernel variants; --images runs only those), and the per-image angle calls (--angles runs only those).  Prints the detection counts (compare with a plain run).

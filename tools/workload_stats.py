@@ -2,7 +2,7 @@
 """Workload statistics of the scan (CPU only, numpy restatement of classifyRegion): for one 1080p frame of each synthetic
 content class (pigo_b200/synth.py: U noise, S smooth + faces, F faces on noise) and the reference's test parameters, how
 many trees each window evaluates before it is rejected, per scale.  These numbers are what the kernel schedule is built on
-(which share of the tree walks happens in the tile warps, in Q1/gather-v2, in Q2/deep) -- see DESIGN.md section 7.
+(which share of the tree walks happens in the tile warps, in the gather role, in Q2/deep) -- see DESIGN.md section 7.
 
     python tools/workload_stats.py > profiles/workload_stats_r01.md
 """
