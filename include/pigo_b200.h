@@ -297,6 +297,45 @@ int pigo_ycbcr_to_nrgba(const uint8_t *y, const uint8_t *cb, const uint8_t *cr, 
                         int subsample, int min_x, int min_y, int width, int height, uint8_t *nrgba, uint8_t *gray,
                         unsigned flags, void *stream);
 
+/* ---- RgbToGrayscale(ImgToNRGBA(img)) for a batch of decoded images of any size (core/grayscale.go:8-23, core/image.go:35-90;
+ * what cmd/pigo/main.go:281-286 feeds the detector), straight into device memory for the mixed-size calls.
+ * Each pigo_decoded describes one decoded Go image at its rectangle's origin:
+ *   PIGO_DECODED_YCBCR  *image.YCbCr: plane = Y[YOffset(Rect.Min):], Cb and Cr[COffset(Rect.Min):]; stride = YStride, CStride;
+ *                       subsample = SubsampleRatio (0..5 = 444, 422, 420, 440, 411, 410); (min_x, min_y) = Rect.Min (>= 0)
+ *   PIGO_DECODED_NRGBA  *image.NRGBA: plane[0] = Pix[PixOffset(Rect.Min):], stride[0] = Stride
+ *   PIGO_DECODED_RGBA   *image.RGBA (alpha-premultiplied), laid out as NRGBA
+ *   PIGO_DECODED_GRAY   *image.Gray: plane[0] = Pix[PixOffset(Rect.Min):], stride[0] = Stride
+ * width, height = Rect size.  Fields a format does not use are ignored, but take part in the repeat test below.
+ * Output: `gray` is a device buffer of *gray_bytes bytes.  Source i gets a 256-byte-aligned slot of height rows of exactly
+ * width bytes and images[i] = {slot, height, width, width} (dim == width: the rotated scan's column clamp,
+ * core/pigo.go:168,171, reads past cols on some shapes, so a padded pitch would change results).  Pass `images` unchanged,
+ * with PIGO_FRAMES_DEVICE, to pigo_run_cascade_images[_angles], pigo_detect_images[_angles] or pigo_puploc_run_images.
+ * Slot bytes: YCbCr = the fused `gray` output of pigo_ycbcr_to_nrgba; NRGBA = pigo_rgba_to_gray of the pixels; RGBA =
+ * the same after color.NRGBAModel (c*0xffff/a >> 8 in uint32, a == 0 -> 0; a channel above alpha wraps as in Go);
+ * Gray = Y (luma(Y, Y, Y, 0xff) == Y for every Y).
+ * Descriptors that are byte-identical share one slot and are converted once (an angle sweep of one photo costs one
+ * conversion).  Required size = sum over distinct descriptors of round256(width*height).  If `gray` is NULL or
+ * *gray_bytes is smaller, the call sets *gray_bytes to the required size and returns PIGO_E_CAP; that query, every
+ * argument check and a call with n == 0 (PIGO_OK, required size 0) need no device.  PIGO_E_INVALID: n outside 0..65535, an unknown
+ * format, subsample outside 0..5, a negative YCbCr origin, width or height < 1, width*height >= 2^31, a stride below
+ * width * bytes per pixel (CStride: below the rectangle's chroma width), a null plane, a null src / images / gray_bytes,
+ * or a stream that is being captured into a CUDA graph.
+ * flags: PIGO_FRAMES_DEVICE = the planes are device pointers; on a caller's stream the call then returns without
+ * synchronising.  Host planes are read only during the call: one copy per plane per distinct source, of the bytes the
+ * rectangle covers.  With stream NULL the call synchronises before it returns. */
+#define PIGO_DECODED_YCBCR 0
+#define PIGO_DECODED_NRGBA 1
+#define PIGO_DECODED_RGBA 2
+#define PIGO_DECODED_GRAY 3
+typedef struct {
+  int32_t format, subsample, min_x, min_y, width, height;
+  const uint8_t *plane[3];
+  int32_t stride[2];
+} pigo_decoded;
+
+int pigo_gray_images(const pigo_decoded *src, int n, uint8_t *gray, size_t *gray_bytes, pigo_image *images, unsigned flags,
+                     void *stream);
+
 /* ---- tuning / introspection (not part of the reference surface) ------------------------- */
 /* Process-global developer knobs (kernel variants, group sizes, per-kernel timing): debugging and
  * benchmarking only, NOT per handle -- set them before the first compute call and leave them alone while

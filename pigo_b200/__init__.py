@@ -30,6 +30,7 @@ CASCADE_DIR = os.path.join(DATA_DIR, "cascade")
 
 PIGO_OK, PIGO_E_INVALID, PIGO_E_CUDA, PIGO_E_CAP, PIGO_E_NOMEM, PIGO_E_NODEVICE = 0, -1, -2, -3, -4, -5
 MEM_HOST, FRAMES_DEVICE, OUT_DEVICE = 0, 1, 2
+DECODED_YCBCR, DECODED_NRGBA, DECODED_RGBA, DECODED_GRAY = 0, 1, 2, 3
 
 DET_DTYPE = np.dtype([("row", "<i4"), ("col", "<i4"), ("scale", "<i4"), ("q", "<f4")])
 POINT_DTYPE = np.dtype([("row", "<i4"), ("col", "<i4"), ("scale", "<f4"), ("perturbs", "<i4")])
@@ -44,7 +45,7 @@ ABI_SYMBOLS = [
     "pigo_device_free", "pigo_device_upload", "pigo_describe_plan", "pigo_init_devices", "pigo_device_count",
     "pigo_device_download", "pigo_run_cascade_batch_sharded", "pigo_detect_batch", "pigo_detect_batch_sharded",
     "pigo_ycbcr_to_nrgba", "pigo_run_cascade_images", "pigo_detect_images", "pigo_puploc_run_images",
-    "pigo_run_cascade_images_angles", "pigo_detect_images_angles",
+    "pigo_run_cascade_images_angles", "pigo_detect_images_angles", "pigo_gray_images",
 ]
 
 
@@ -111,6 +112,7 @@ def lib() -> C.CDLL:
         L.pigo_run_cascade_images_angles.argtypes = [vp, vp, i, vp, i, i, d, d, vp, i, vp, C.c_uint, vp]
         L.pigo_detect_images_angles.argtypes = [vp, vp, vp, vp, i, vp, i, vp, vp, vp, u64, vp, i, vp, vp, C.c_uint, vp]
         L.pigo_ycbcr_to_nrgba.argtypes = [vp, vp, vp, i, i, i, i, i, i, i, vp, vp, C.c_uint, vp]
+        L.pigo_gray_images.argtypes = [vp, i, vp, C.POINTER(sz), vp, C.c_uint, vp]
         L.pigo_set_option.argtypes = [C.c_char_p, C.c_int64]
         L.pigo_get_option.argtypes = [C.c_char_p]
         L.pigo_get_option.restype = C.c_int64
@@ -628,6 +630,134 @@ def YCbCrToNRGBA(y: np.ndarray, cb: np.ndarray, cr: np.ndarray, subsample: int, 
                                      cb.shape[1] if cb.ndim == 2 else 0, subsample, min_x, min_y, width, height,
                                      out.ctypes.data if out.size else None, gray.ctypes.data if want_gray and gray.size else None, MEM_HOST, None))
     return (out, gray) if want_gray else out
+
+
+class PigoDecoded(C.Structure):
+    """pigo_decoded (include/pigo_b200.h): one decoded image of a pigo_gray_images call."""
+    _fields_ = [("format", C.c_int32), ("subsample", C.c_int32), ("min_x", C.c_int32), ("min_y", C.c_int32), ("width", C.c_int32),
+                ("height", C.c_int32), ("plane", C.c_void_p * 3), ("stride", C.c_int32 * 2)]
+
+
+def _row_bytes(a, default: int) -> int:
+    """Row pitch in bytes of a uint8 plane given as a numpy array or torch tensor of two or more dimensions, else `default`."""
+    if isinstance(a, np.ndarray) and a.ndim >= 2:
+        return int(a.strides[0])
+    if hasattr(a, "stride") and hasattr(a, "dim") and a.dim() >= 2:
+        return int(a.stride(0))
+    return int(default)
+
+
+def _plane_ptr(a) -> Optional[int]:
+    """Address of a plane: a device pointer (int), a torch tensor, or a host numpy uint8 array."""
+    if a is None:
+        return None
+    if isinstance(a, int):
+        return a
+    if hasattr(a, "data_ptr"):
+        return int(a.data_ptr())
+    if not isinstance(a, np.ndarray) or a.dtype != np.uint8:
+        raise TypeError("a plane is a uint8 numpy array, a torch tensor or a device pointer (int)")
+    return int(a.ctypes.data)
+
+
+@dataclass
+class DecodedImage:
+    """One decoded Go image as pigo_gray_images takes it (pigo_decoded): `planes` start at the rectangle's origin and are
+    host numpy uint8 arrays, or (device_sources) device pointers / torch CUDA tensors.  Build it with one constructor per
+    Go image type; strides default to the arrays' row pitch."""
+    format: int
+    width: int
+    height: int
+    planes: tuple
+    strides: tuple = (0, 0)
+    subsample: int = 0
+    min_x: int = 0
+    min_y: int = 0
+
+    @classmethod
+    def ycbcr(cls, y, cb, cr, subsample: int, width: int, height: int, min_x: int = 0, min_y: int = 0, y_stride: Optional[int] = None,
+              c_stride: Optional[int] = None) -> "DecodedImage":
+        """*image.YCbCr: Y[YOffset(Rect.Min):], Cb / Cr[COffset(Rect.Min):], SubsampleRatio (0..5), Rect.Min (>= 0)."""
+        return cls(DECODED_YCBCR, width, height, (y, cb, cr), (y_stride if y_stride is not None else _row_bytes(y, width),
+                                                               c_stride if c_stride is not None else _row_bytes(cb, 0)), subsample, min_x, min_y)
+
+    @classmethod
+    def nrgba(cls, pix, width: int, height: int, stride: Optional[int] = None) -> "DecodedImage":
+        """*image.NRGBA: Pix[PixOffset(Rect.Min):] and Stride."""
+        return cls(DECODED_NRGBA, width, height, (pix,), (stride if stride is not None else _row_bytes(pix, 4 * width), 0))
+
+    @classmethod
+    def rgba(cls, pix, width: int, height: int, stride: Optional[int] = None) -> "DecodedImage":
+        """*image.RGBA (alpha-premultiplied): Pix[PixOffset(Rect.Min):] and Stride."""
+        return cls(DECODED_RGBA, width, height, (pix,), (stride if stride is not None else _row_bytes(pix, 4 * width), 0))
+
+    @classmethod
+    def gray(cls, pix, width: int, height: int, stride: Optional[int] = None) -> "DecodedImage":
+        """*image.Gray: Pix[PixOffset(Rect.Min):] and Stride."""
+        return cls(DECODED_GRAY, width, height, (pix,), (stride if stride is not None else _row_bytes(pix, width), 0))
+
+    def desc(self) -> PigoDecoded:
+        d = PigoDecoded()
+        d.format, d.subsample, d.min_x, d.min_y, d.width, d.height = self.format, self.subsample, self.min_x, self.min_y, self.width, self.height
+        for k in range(3):
+            d.plane[k] = _plane_ptr(self.planes[k]) if k < len(self.planes) else None
+        d.stride[0], d.stride[1] = int(self.strides[0]), int(self.strides[1])
+        return d
+
+
+class DeviceImage(tuple):
+    """A device image of the gray arena: the (pixels, rows, cols, dim) tuple run_cascade_images[_angles]_device takes, with the
+    ImageParams field names pipeline.detect_images[_angles]_device reads (Pixels is a device pointer)."""
+    def __new__(cls, pixels: int, rows: int, cols: int, dim: int):
+        return super().__new__(cls, (pixels, rows, cols, dim))
+
+    Pixels = property(lambda self: self[0])
+    Rows = property(lambda self: self[1])
+    Cols = property(lambda self: self[2])
+    Dim = property(lambda self: self[3])
+
+
+def decoded_descs(sources: Sequence[DecodedImage]) -> C.Array:
+    arr = (PigoDecoded * max(len(sources), 1))()
+    for k, s in enumerate(sources):
+        arr[k] = s.desc()
+    return arr
+
+
+def gray_images_bytes(sources: Sequence[DecodedImage]) -> int:
+    """Device bytes pigo_gray_images needs for `sources` (no device needed): sum of round256(width*height) over distinct sources."""
+    need = C.c_size_t(0)
+    imgs = (PigoImage * max(len(sources), 1))()
+    rc = lib().pigo_gray_images(decoded_descs(sources), len(sources), None, C.byref(need), imgs, MEM_HOST, None)
+    if rc not in (PIGO_OK, PIGO_E_CAP):
+        _check(rc)
+    return int(need.value)
+
+
+def gray_images(sources: Sequence[DecodedImage], stream=None, device_sources: bool = False):
+    """RgbToGrayscale(ImgToNRGBA(img)) of every source in one call (pigo_gray_images).  Returns (arena, images): the arena is a
+    torch uint8 CUDA tensor and images[i] a DeviceImage {slot, height, width, width} that Pigo.run_cascade_images_angles_device
+    and pipeline.detect_images_angles_device take as it is.  Repeated sources share a slot.  `stream` (a torch.cuda.Stream or
+    a cudaStream_t as int) orders the call on the caller's stream; without it the arena is complete on return.  Host planes
+    are read only during the call; with device_sources every plane is a device pointer or CUDA tensor."""
+    import torch
+    n = len(sources)
+    desc = decoded_descs(sources)
+    imgs = (PigoImage * max(n, 1))()
+    flags = FRAMES_DEVICE if device_sources else MEM_HOST
+    sptr = (stream.cuda_stream if hasattr(stream, "cuda_stream") else int(stream)) if stream is not None else None
+    need = C.c_size_t(0)
+    rc = lib().pigo_gray_images(desc, n, None, C.byref(need), imgs, flags, sptr)
+    if rc not in (PIGO_OK, PIGO_E_CAP):
+        _check(rc)
+    if hasattr(stream, "cuda_stream"):
+        with torch.cuda.stream(stream):
+            arena = torch.empty(need.value, dtype=torch.uint8, device="cuda")
+    else:
+        arena = torch.empty(need.value, dtype=torch.uint8, device="cuda")
+    size = C.c_size_t(arena.numel())
+    _check(lib().pigo_gray_images(desc, n, arena.data_ptr() if arena.numel() else None, C.byref(size), imgs, flags, sptr))
+    return arena, [DeviceImage(imgs[k].pixels, imgs[k].rows, imgs[k].cols, imgs[k].dim) for k in range(n)]
 
 
 class DeviceFrames:

@@ -34,7 +34,7 @@ struct TimingSlot {
 };
 static TimingSlot g_tslot[T_NSLOTS];
 static std::mutex g_tmu;
-static const char* kSlotNames[T_NSLOTS] = {"tiled", "gather", "deep", "finalize", "cluster", "puploc", "gray", "seeds", "rottab", "ycbcr"};
+static const char* kSlotNames[T_NSLOTS] = {"tiled", "gather", "deep", "finalize", "cluster", "puploc", "gray", "seeds", "rottab", "ycbcr", "gray_images"};
 
 void timing_reset() {
   std::lock_guard<std::mutex> g(g_tmu);
@@ -558,21 +558,37 @@ static int rot_slot_of(double angle) { return angle > 0.0 ? (int)(32.0 * (angle 
 // over the call's longest ladder, at most 512 MB).  A call whose slots need more runs its rotated images in several passes.
 static constexpr size_t kImagesRotBytes = (size_t)1 << 30;
 
-// Host images of a mixed-size call in one arena of 256-byte-aligned slots.  Descriptors that repeat an earlier
-// (pixels, rows, cols, dim) share its slot, so a sweep that lists one photo once per angle copies it once.
-// off[i] = byte offset of image i's slot; first[i] = image i is the first to use that slot (its bytes are the ones copied).
-static size_t arena_layout(const pigo_image* images, int n, std::vector<size_t>& off, std::vector<char>& first) {
-  std::map<std::tuple<const uint8_t*, int, int, int>, size_t> seen;
+// The items of a call in one arena of 256-byte-aligned slots of bytes(item) bytes.  Items whose key(item) repeats an earlier
+// one share its slot, so a sweep that lists one photo once per angle copies (or converts) it once.
+// off[i] = byte offset of item i's slot; first[i] = item i is the first to use that slot (its bytes are the ones written).
+template <typename T, typename Key, typename Bytes>
+static size_t arena_layout(const T* items, int n, Key key, Bytes bytes, std::vector<size_t>& off, std::vector<char>& first) {
+  std::map<decltype(key(items[0])), size_t> seen;
   off.assign(n, 0);
   first.assign(n, 0);
   size_t total = 0;
   for (int i = 0; i < n; ++i) {
-    const pigo_image& im = images[i];
-    const auto ins = seen.emplace(std::make_tuple(im.pixels, im.rows, im.cols, im.dim), total);
+    const auto ins = seen.emplace(key(items[i]), total);
     off[i] = ins.first->second;
-    if (ins.second) { first[i] = 1; total += ((size_t)im.rows * im.dim + 255) & ~(size_t)255; }
+    if (ins.second) { first[i] = 1; total += (bytes(items[i]) + 255) & ~(size_t)255; }
   }
   return total;
+}
+
+// Host images of a mixed-size call: descriptors that repeat an earlier (pixels, rows, cols, dim) share its slot.
+static size_t arena_layout(const pigo_image* images, int n, std::vector<size_t>& off, std::vector<char>& first) {
+  return arena_layout(images, n, [](const pigo_image& im) { return std::make_tuple(im.pixels, im.rows, im.cols, im.dim); },
+                      [](const pigo_image& im) { return (size_t)im.rows * im.dim; }, off, first);
+}
+
+// Decoded images of pigo_gray_images: byte-identical descriptors share a slot of width*height gray bytes.
+static size_t arena_layout(const pigo_decoded* src, int n, std::vector<size_t>& off, std::vector<char>& first) {
+  return arena_layout(src, n,
+                      [](const pigo_decoded& d) {
+                        return std::make_tuple(d.format, d.subsample, d.min_x, d.min_y, d.width, d.height, d.plane[0], d.plane[1], d.plane[2],
+                                               d.stride[0], d.stride[1]);
+                      },
+                      [](const pigo_decoded& d) { return (size_t)d.width * d.height; }, off, first);
 }
 
 // Image i is scanned at angles[i].  The rotated and the unrotated scan are different kernel variants, so the images run
@@ -1539,6 +1555,47 @@ static int detect_images_on(int dev, pigo_cascade* face, pigo_puploc* puploc, pi
                    stream_, scan);
 }
 
+// Extent of the planes image.YCbCr holds for Rect (min)-(min + size), min >= 0: bytes from the rectangle's origin to its
+// last sample in the Y plane and in each chroma plane (COffset rows and columns per ratio), and the rectangle's chroma width.
+struct YCbCrExtent {
+  size_t y_bytes, c_bytes;
+  int c_cols;
+};
+static YCbCrExtent ycbcr_extent(int subsample, int min_x, int min_y, int width, int height, int y_stride, int c_stride) {
+  const int xs = chroma_xshift(subsample), ys = chroma_yshift(subsample);
+  const int c_rows = ((min_y + height - 1) >> ys) - (min_y >> ys) + 1, c_cols = ((min_x + width - 1) >> xs) - (min_x >> xs) + 1;
+  return YCbCrExtent{(size_t)(height - 1) * y_stride + width, (size_t)(c_rows - 1) * c_stride + c_cols, c_cols};
+}
+
+static int decoded_bpp(int format) { return format == PIGO_DECODED_NRGBA || format == PIGO_DECODED_RGBA ? 4 : 1; }
+
+// Host bytes of plane k of a decoded source from its rectangle's origin to its last sample (0: the format has no plane k).
+static size_t decoded_plane_bytes(const pigo_decoded& d, int k) {
+  if (d.format == PIGO_DECODED_YCBCR) {
+    const YCbCrExtent e = ycbcr_extent(d.subsample, d.min_x, d.min_y, d.width, d.height, d.stride[0], d.stride[1]);
+    return k == 0 ? e.y_bytes : e.c_bytes;
+  }
+  return k == 0 ? (size_t)(d.height - 1) * d.stride[0] + (size_t)d.width * decoded_bpp(d.format) : 0;
+}
+
+static int check_decoded(const pigo_decoded* src, int n) {
+  for (int i = 0; i < n; ++i) {
+    const pigo_decoded& d = src[i];
+    if (d.format < PIGO_DECODED_YCBCR || d.format > PIGO_DECODED_GRAY) return set_err(PIGO_E_INVALID, "source %d: unknown format %d", i, d.format);
+    if (d.width < 1 || d.height < 1) return set_err(PIGO_E_INVALID, "source %d: bad size %dx%d", i, d.width, d.height);
+    if ((uint64_t)d.width * (uint64_t)d.height > 0x7fffffffull) return set_err(PIGO_E_INVALID, "source %d: 2^31 pixels or more", i);
+    const bool ycc = d.format == PIGO_DECODED_YCBCR;
+    if (ycc && (d.subsample < 0 || d.subsample > 5))
+      return set_err(PIGO_E_INVALID, "source %d: unknown YCbCr subsample ratio %d (0..5 = 444, 422, 420, 440, 411, 410)", i, d.subsample);
+    if (ycc && (d.min_x < 0 || d.min_y < 0)) return set_err(PIGO_E_INVALID, "source %d: negative rectangle origin", i);
+    if (!d.plane[0] || (ycc && (!d.plane[1] || !d.plane[2]))) return set_err(PIGO_E_INVALID, "source %d: null plane", i);
+    if ((int64_t)d.stride[0] < (int64_t)d.width * decoded_bpp(d.format)) return set_err(PIGO_E_INVALID, "source %d: stride %d below the row", i, d.stride[0]);
+    if (ycc && d.stride[1] < ycbcr_extent(d.subsample, d.min_x, d.min_y, d.width, d.height, d.stride[0], d.stride[1]).c_cols)
+      return set_err(PIGO_E_INVALID, "source %d: chroma stride %d below the chroma row", i, d.stride[1]);
+  }
+  return PIGO_OK;
+}
+
 extern "C" {
 
 static int check_detect_args(const pigo_cascade* face, const pigo_puploc* puploc, const pigo_puploc* const* flp, int ncalls, const uint8_t* frames,
@@ -1703,13 +1760,10 @@ int pigo_ycbcr_to_nrgba(const uint8_t* y, const uint8_t* cb, const uint8_t* cr, 
   cudaStream_t st = stream_ ? (cudaStream_t)stream_ : w->stream;
   if ((rc = ws_enter(w, st))) return rc;
   const bool in_dev = flags & PIGO_FRAMES_DEVICE, out_dev = flags & PIGO_OUT_DEVICE;
-  // plane extents as image.YCbCr lays them out for Rect (min)-(min + size): COffset rows / columns per ratio
-  const int cw_div = (subsample == 1 || subsample == 2) ? 2 : ((subsample == 4 || subsample == 5) ? 4 : 1);
-  const int ch_div = (subsample == 2 || subsample == 3 || subsample == 5) ? 2 : 1;
-  const int c_rows = (min_y + height - 1) / ch_div - min_y / ch_div + 1, c_cols = (min_x + width - 1) / cw_div - min_x / cw_div + 1;
-  const size_t y_bytes = (size_t)(height - 1) * y_stride + width, c_bytes = (size_t)(c_rows - 1) * c_stride + c_cols;
   const uint8_t *d_y = y, *d_cb = cb, *d_cr = cr;
   if (!in_dev) {
+    const YCbCrExtent e = ycbcr_extent(subsample, min_x, min_y, width, height, y_stride, c_stride);
+    const size_t y_bytes = e.y_bytes, c_bytes = e.c_bytes;
     const size_t yo = (y_bytes + 255) & ~(size_t)255, co = (c_bytes + 255) & ~(size_t)255;
     if ((rc = w->frames.reserve(yo + 2 * co))) return rc;
     uint8_t* b = (uint8_t*)w->frames.p;
@@ -1733,6 +1787,88 @@ int pigo_ycbcr_to_nrgba(const uint8_t* y, const uint8_t* cb, const uint8_t* cr, 
   if (nrgba) CUDA_TRY(cudaMemcpyAsync(nrgba, d_rgba, npix * 4, cudaMemcpyDeviceToHost, st));
   if (gray) CUDA_TRY(cudaMemcpyAsync(gray, d_gray, npix, cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaStreamSynchronize(st));
+  return PIGO_OK;
+}
+
+// ---- RgbToGrayscale(ImgToNRGBA(img)) for a batch of decoded images, core/grayscale.go:8-23 + core/image.go:35-90 -----------
+// One slot per distinct source in the caller's device arena (arena_layout), one kernel launch for the whole batch.
+int pigo_gray_images(const pigo_decoded* src, int n, uint8_t* gray, size_t* gray_bytes, pigo_image* images, unsigned flags, void* stream_) {
+  if (n < 0 || n > 65535) return set_err(PIGO_E_INVALID, "%d sources: outside 0..65535", n);
+  if (!gray_bytes) return set_err(PIGO_E_INVALID, "null gray_bytes");
+  if (n > 0 && (!src || !images)) return set_err(PIGO_E_INVALID, "null src or images");
+  int rc = check_decoded(src, n);
+  if (rc) return rc;
+  std::vector<size_t> off;
+  std::vector<char> first;
+  const size_t total = arena_layout(src, n, off, first);
+  if (!gray || *gray_bytes < total) {
+    *gray_bytes = total;
+    if (total > 0) return set_err(PIGO_E_CAP, "the gray arena needs %zu bytes", total);
+  }
+  if (n == 0) return PIGO_OK;
+  if ((rc = ensure_device())) return rc;
+  if (stream_ && stream_capturing((cudaStream_t)stream_)) return set_err(PIGO_E_INVALID, "pigo_gray_images does not support stream capture");
+  for (int i = 0; i < n; ++i) images[i] = pigo_image{gray + off[i], src[i].height, src[i].width, src[i].width};
+  const int dev = default_device();
+  WsGuard g(g_misc_pool[dev]);
+  Workspace* w = g.w;
+  if (!w) return set_err(PIGO_E_CUDA, "could not create a CUDA stream");
+  cudaStream_t st = stream_ ? (cudaStream_t)stream_ : w->stream;
+  if ((rc = ws_enter(w, st))) return rc;
+  const bool in_dev = flags & PIGO_FRAMES_DEVICE;
+
+  // the distinct sources; host planes go to one staging buffer, each plane 256-byte aligned
+  std::vector<int> who;
+  for (int i = 0; i < n; ++i)
+    if (first[i]) who.push_back(i);
+  const int ns = (int)who.size();
+  std::vector<size_t> stage_off((size_t)ns * 3, 0);
+  size_t stage_bytes = 0;
+  if (!in_dev) {
+    for (int k = 0; k < ns; ++k)
+      for (int p = 0; p < 3; ++p) {
+        stage_off[(size_t)k * 3 + p] = stage_bytes;
+        stage_bytes += (decoded_plane_bytes(src[who[k]], p) + 255) & ~(size_t)255;
+      }
+    if ((rc = w->frames.reserve(stage_bytes + 256))) return rc;
+  }
+  std::vector<GraySrc> tab(ns);
+  std::vector<uint64_t> firsts(ns + 1, 0);
+  for (int k = 0; k < ns; ++k) {
+    const pigo_decoded& d = src[who[k]];
+    GraySrc& t = tab[k];
+    for (int p = 0; p < 3; ++p)
+      t.plane[p] = !in_dev && decoded_plane_bytes(d, p) ? (const uint8_t*)w->frames.p + stage_off[(size_t)k * 3 + p] : d.plane[p];
+    t.dst = gray + off[who[k]];
+    t.format = d.format; t.sub = d.subsample; t.min_x = d.min_x; t.min_y = d.min_y; t.width = d.width; t.height = d.height;
+    t.stride0 = d.stride[0]; t.stride1 = d.stride[1];
+    firsts[k + 1] = firsts[k] + (uint64_t)d.height * (uint64_t)((d.width + 15) / 16);
+  }
+  const size_t tab_bytes = ((size_t)ns * sizeof(GraySrc) + 255) & ~(size_t)255;
+  std::vector<uint8_t> blob(tab_bytes + firsts.size() * sizeof(uint64_t));
+  memcpy(blob.data(), tab.data(), (size_t)ns * sizeof(GraySrc));
+  memcpy(blob.data() + tab_bytes, firsts.data(), firsts.size() * sizeof(uint64_t));
+  if ((rc = w->img_tab.reserve(blob.size()))) return rc;
+  if (!in_dev) {
+    for (int k = 0; k < ns; ++k)
+      for (int p = 0; p < 3; ++p) {
+        const size_t b = decoded_plane_bytes(src[who[k]], p);
+        if (b) CUDA_TRY(cudaMemcpyAsync((uint8_t*)w->frames.p + stage_off[(size_t)k * 3 + p], src[who[k]].plane[p], b, cudaMemcpyHostToDevice, st));
+      }
+  }
+  cudaEvent_t copied = nullptr;
+  if (!in_dev && stream_) {   // host planes are the caller's again once their copies are done; the kernel may still run
+    if (!(copied = w->copy_event(0))) return set_err(PIGO_E_CUDA, "event creation failed");
+    CUDA_TRY(cudaEventRecord(copied, st));
+  }
+  CUDA_TRY(cudaMemcpyAsync(w->img_tab.p, blob.data(), blob.size(), cudaMemcpyHostToDevice, st));
+  timing_begin(T_GRAY_IMAGES, st);
+  launch_gray_images((const GraySrc*)w->img_tab.p, (const uint64_t*)((const uint8_t*)w->img_tab.p + tab_bytes), ns, firsts[ns], device_sms(dev) * 16, st);
+  timing_end(T_GRAY_IMAGES, st);
+  g_launches++;
+  CUDA_TRY(cudaGetLastError());
+  if (!stream_) CUDA_TRY(cudaStreamSynchronize(st));   // the library's own stream: the arena is complete on return
+  else if (copied) CUDA_TRY(cudaEventSynchronize(copied));
   return PIGO_OK;
 }
 

@@ -52,19 +52,29 @@ void launch_gray(const uint8_t* rgba, size_t npix, uint8_t* gray, int grid, cuda
 // make the round trip through HBM when only the detector's input is wanted.
 __device__ __forceinline__ uint32_t sat16(int v) { return (uint32_t)v & 0xff000000u ? (uint32_t)(~(v >> 31)) & 0xffu : (uint32_t)(v >> 16); }
 
+// color.YCbCrToRGB of one sample, as an NRGBA pixel with alpha 0xff.
+__device__ __forceinline__ uint32_t ycbcr_px(int y, int cb, int cr) {
+  const int yy1 = y * 0x10101, cb1 = cb - 128, cr1 = cr - 128;
+  const uint32_t r = sat16(yy1 + 91881 * cr1), gg = sat16(yy1 - 22554 * cb1 - 46802 * cr1), b = sat16(yy1 + 116130 * cb1);
+  return r | (b << 16) | (gg << 8) | 0xff000000u;   // (this operand order keeps ycbcr_kernel's SASS as it was before the factoring)
+}
+
+// image.YCbCr.COffset relative to the rectangle origin (min_x, min_y >= 0), split into its row and column parts.
+__device__ __forceinline__ size_t coffset_row(int sy, int min_y, int ys, int c_stride) { return (size_t)((sy >> ys) - (min_y >> ys)) * c_stride; }
+__device__ __forceinline__ size_t coffset_col(int sx, int min_x, int xs) { return (size_t)((sx >> xs) - (min_x >> xs)); }
+
 // One thread converts 4 consecutive pixels of a row (32-bit index arithmetic, one 16-byte store for the NRGBA output).
 __global__ void __launch_bounds__(256) ycbcr_kernel(const uint8_t* __restrict__ yp, const uint8_t* __restrict__ cbp, const uint8_t* __restrict__ crp,
                                                     int y_stride, int c_stride, int sub, int min_x, int min_y, int width, int height,
                                                     uint32_t* __restrict__ nrgba, uint8_t* __restrict__ gray, int vec_ok) {
-  const int xs = (sub == 1 || sub == 2) ? 1 : ((sub == 4 || sub == 5) ? 2 : 0);   // chroma x shift: 422/420 halve, 411/410 quarter
-  const int ys = (sub == 2 || sub == 3 || sub == 5) ? 1 : 0;                       // chroma y shift: 420/440/410 halve
+  const int xs = chroma_xshift(sub), ys = chroma_yshift(sub);
   const unsigned chunks = (unsigned)(width + 3) >> 2;
   const unsigned total = chunks * (unsigned)height;                                // < 2^31: width * height < 2^31 is checked by the host
   for (unsigned q = blockIdx.x * blockDim.x + threadIdx.x; q < total; q += gridDim.x * blockDim.x) {
     const int dy = (int)(q / chunks), dx0 = (int)(q - (unsigned)dy * chunks) * 4;
     const int sy = min_y + dy;                                                     // image.go:66-67
     const uint8_t* yrow = yp + (size_t)dy * y_stride;                             // YOffset: (y-Rect.Min.Y)*YStride + (x-Rect.Min.X)
-    const size_t crow = (size_t)((sy >> ys) - (min_y >> ys)) * c_stride;          // COffset row
+    const size_t crow = coffset_row(sy, min_y, ys, c_stride);
     uint32_t px[4], lum = 0;
     const int n = min(4, width - dx0);
 #pragma unroll
@@ -72,10 +82,8 @@ __global__ void __launch_bounds__(256) ycbcr_kernel(const uint8_t* __restrict__ 
       px[k] = 0;
       if (k < n) {
         const int dx = dx0 + k;
-        const size_t sic = crow + (size_t)(((min_x + dx) >> xs) - (min_x >> xs));
-        const int yy1 = (int)__ldg(yrow + dx) * 0x10101, cb1 = (int)__ldg(cbp + sic) - 128, cr1 = (int)__ldg(crp + sic) - 128;
-        const uint32_t r = sat16(yy1 + 91881 * cr1), gg = sat16(yy1 - 22554 * cb1 - 46802 * cr1), b = sat16(yy1 + 116130 * cb1);
-        px[k] = r | (gg << 8) | (b << 16) | 0xff000000u;
+        const size_t sic = crow + coffset_col(min_x + dx, min_x, xs);
+        px[k] = ycbcr_px(__ldg(yrow + dx), __ldg(cbp + sic), __ldg(crp + sic));
         if (gray) lum |= luma(px[k]) << (8 * k);
       }
     }
@@ -98,6 +106,106 @@ void launch_ycbcr(const uint8_t* y, const uint8_t* cb, const uint8_t* cr, int y_
   const int vec_ok = (width % 4 == 0) && (((uintptr_t)nrgba) % 16 == 0) && (((uintptr_t)gray) % 4 == 0);
   ycbcr_kernel<<<(int)std::max<size_t>(1, std::min<size_t>(want, (size_t)grid)), 256, 0, st>>>(y, cb, cr, y_stride, c_stride, subsample, min_x, min_y, width,
                                                                                              height, reinterpret_cast<uint32_t*>(nrgba), gray, vec_ok);
+}
+
+
+// ---- RgbToGrayscale(ImgToNRGBA(img)) for a batch of decoded images (pigo_gray_images) ---------------------------------------
+// ImgToNRGBA (core/image.go:35-90) then RgbToGrayscale (core/grayscale.go:8-23) per pixel, without the NRGBA image:
+//   *image.YCbCr  luma(YCbCrToRGB(Y, Cb, Cr)), the `gray` output of ycbcr_kernel;
+//   *image.NRGBA  luma of the pixel (the reference copies the rows);
+//   *image.RGBA   luma(color.NRGBAModel(pixel)) -- rgba_to_nrgba below;
+//   *image.Gray   luma(Y, Y, Y, 0xff) == Y for every Y (pinned by a CPU test), so the rows are copied.
+// color.nrgbaModel (image/color/color.go) of a color.RGBA pixel: its RGBA() channels c*0x101 (alpha-premultiplied) back to
+// straight 8-bit channels.  uint32 arithmetic as Go's: a == 0xffff -> c >> 8; a == 0 -> all zero; else (c*0xffff)/a >> 8,
+// truncated to uint8 (a channel above alpha -- invalid premultiplied input -- wraps like the reference's conversion).
+__device__ __forceinline__ uint32_t rgba_to_nrgba(uint32_t px) {
+  const uint32_t a = (px >> 24) * 0x101u;
+  if (a == 0xffffu) return px;
+  if (a == 0) return 0;
+  uint32_t out = px & 0xff000000u;                        // uint8(a >> 8)
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    const uint32_t v = ((px >> (8 * c)) & 0xffu) * 0x101u;
+    out |= (((v * 0xffffu) / a >> 8) & 0xffu) << (8 * c);   // v * 0xffff <= 0xfffe0001: no overflow
+  }
+  return out;
+}
+
+// Pixel k of a 16-pixel chunk of 4-byte pixels: one of four 16-byte loads when the chunk is aligned and full, else bytes.
+__device__ __forceinline__ uint32_t px32(const uint4* q, const uint8_t* p, bool vec, int k) {
+  if (vec) { const uint4 v = q[k >> 2]; return (k & 3) == 0 ? v.x : (k & 3) == 1 ? v.y : (k & 3) == 2 ? v.z : v.w; }
+  return (uint32_t)__ldg(p + 4 * k) | ((uint32_t)__ldg(p + 4 * k + 1) << 8) | ((uint32_t)__ldg(p + 4 * k + 2) << 16) | ((uint32_t)__ldg(p + 4 * k + 3) << 24);
+}
+
+// One thread per (source, row, 16-pixel chunk) work item over every distinct source of the call; the source is found by a
+// binary search over the sources' first work items.  16-byte stores where the slot row is aligned, bytes otherwise.
+__global__ void __launch_bounds__(256) gray_images_kernel(const GraySrc* __restrict__ src, const uint64_t* __restrict__ first, int nsrc, uint64_t total) {
+  for (uint64_t q = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; q < total; q += (uint64_t)gridDim.x * blockDim.x) {
+    int lo = 0, hi = nsrc - 1;
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (__ldg(first + mid) <= q) lo = mid; else hi = mid - 1;
+    }
+    const GraySrc& s = src[lo];
+    const int width = s.width, format = s.format;
+    const unsigned chunks = (unsigned)(width + 15) >> 4;
+    const unsigned local = (unsigned)(q - __ldg(first + lo));   // < width * height < 2^31
+    const int row = (int)(local / chunks), x0 = (int)(local - (unsigned)row * chunks) * 16;
+    const int n = min(16, width - x0);
+    const uint8_t* p = s.plane[0] + (size_t)row * s.stride0 + (size_t)x0 * (format == PIGO_DECODED_NRGBA || format == PIGO_DECODED_RGBA ? 4 : 1);
+    const bool vec = n == 16 && ((uintptr_t)p & 15) == 0;
+    uint32_t w[4] = {0, 0, 0, 0};
+    if (format == PIGO_DECODED_GRAY) {
+      if (vec) {
+        const uint4 v = __ldg(reinterpret_cast<const uint4*>(p));
+        w[0] = v.x; w[1] = v.y; w[2] = v.z; w[3] = v.w;
+      } else {
+#pragma unroll
+        for (int k = 0; k < 16; ++k)
+          if (k < n) w[k >> 2] |= (uint32_t)__ldg(p + k) << (8 * (k & 3));
+      }
+    } else if (format == PIGO_DECODED_YCBCR) {
+      const int xs = chroma_xshift(s.sub), ys = chroma_yshift(s.sub);
+      const size_t crow = coffset_row(s.min_y + row, s.min_y, ys, s.stride1);
+      uint4 yv = make_uint4(0, 0, 0, 0);
+      if (vec) yv = __ldg(reinterpret_cast<const uint4*>(p));
+#pragma unroll
+      for (int k = 0; k < 16; ++k) {
+        if (k < n) {
+          const uint32_t yw = (k >> 2) == 0 ? yv.x : (k >> 2) == 1 ? yv.y : (k >> 2) == 2 ? yv.z : yv.w;
+          const uint32_t y = vec ? (yw >> (8 * (k & 3))) & 0xffu : (uint32_t)__ldg(p + k);
+          const size_t sic = crow + coffset_col(s.min_x + x0 + k, s.min_x, xs);
+          w[k >> 2] |= luma(ycbcr_px(y, __ldg(s.plane[1] + sic), __ldg(s.plane[2] + sic))) << (8 * (k & 3));
+        }
+      }
+    } else {
+      const bool premul = format == PIGO_DECODED_RGBA;
+      uint4 v[4];
+      if (vec) {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) v[k] = __ldg(reinterpret_cast<const uint4*>(p) + k);
+      }
+#pragma unroll
+      for (int k = 0; k < 16; ++k) {
+        if (k < n) {
+          const uint32_t px = px32(v, p, vec, k);
+          w[k >> 2] |= luma(premul ? rgba_to_nrgba(px) : px) << (8 * (k & 3));
+        }
+      }
+    }
+    uint8_t* d = s.dst + (size_t)row * width + x0;
+    if (n == 16 && ((uintptr_t)d & 15) == 0) *reinterpret_cast<uint4*>(d) = make_uint4(w[0], w[1], w[2], w[3]);
+    else {
+#pragma unroll
+      for (int k = 0; k < 16; ++k)
+        if (k < n) d[k] = (uint8_t)(w[k >> 2] >> (8 * (k & 3)));
+    }
+  }
+}
+
+void launch_gray_images(const GraySrc* src, const uint64_t* first, int nsrc, uint64_t total, int grid, cudaStream_t st) {
+  const uint64_t want = (total + 255) / 256;
+  gray_images_kernel<<<(int)std::max<uint64_t>(1, std::min<uint64_t>(want, (uint64_t)grid)), 256, 0, st>>>(src, first, nsrc, total);
 }
 
 }  // namespace pigo

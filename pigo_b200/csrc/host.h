@@ -16,7 +16,7 @@ extern std::atomic<long long> g_launches;
 
 // Per-kernel CUDA-event timing (enabled by option "timing"): every launch of kernel class `slot` is bracketed by an
 // event pair on its stream; "t_<name>_ns" / "t_<name>_n" return the summed device time and the launch count.
-enum TimeSlot { T_TILED = 0, T_GATHER, T_DEEP, T_FINALIZE, T_CLUSTER, T_PUPLOC, T_GRAY, T_SEEDS, T_ROTTAB, T_YCBCR, T_NSLOTS };
+enum TimeSlot { T_TILED = 0, T_GATHER, T_DEEP, T_FINALIZE, T_CLUSTER, T_PUPLOC, T_GRAY, T_SEEDS, T_ROTTAB, T_YCBCR, T_GRAY_IMAGES, T_NSLOTS };
 void timing_reset();
 void walk_stats_reset();
 long long walk_stats_query(int which);
@@ -133,6 +133,18 @@ struct PupWork {
   const ImageDesc* images;     // mixed-size call: the image table the frame indices refer to (frames .. dim unused); nullptr = uniform frames
 };
 
+// Chroma subsampling of image.YCbCrSubsampleRatio `sub` (0..5 = 444, 422, 420, 440, 411, 410) as shifts of the luma
+// coordinates: 422/420 halve x, 411/410 quarter it; 420/440/410 halve y.
+__host__ __device__ __forceinline__ int chroma_xshift(int sub) { return (sub == 1 || sub == 2) ? 1 : ((sub == 4 || sub == 5) ? 2 : 0); }
+__host__ __device__ __forceinline__ int chroma_yshift(int sub) { return (sub == 2 || sub == 3 || sub == 5) ? 1 : 0; }
+
+// One distinct source of a pigo_gray_images call, all pointers on the device.  Work item q of the call's kernel is the
+// 16-pixel chunk q - first[k] (row-major, ceil(width/16) chunks per row) of the source k with first[k] <= q < first[k+1].
+struct GraySrc {
+  const uint8_t* plane[3];   // pigo_decoded.plane, at the rectangle's origin
+  uint8_t* dst;              // the source's slot in the arena: height rows of width bytes
+  int32_t format, sub, min_x, min_y, width, height, stride0, stride1;
+};
 
 // ---- workspace -----------------------------------------------------------------------------------------
 struct DevBuf {
@@ -312,6 +324,7 @@ void launch_ptab_build(const FaceTables& T, const ScaleEntry* plan, const TiledA
 void launch_gray(const uint8_t* rgba, size_t npix, uint8_t* gray, int grid, cudaStream_t st);
 void launch_ycbcr(const uint8_t* y, const uint8_t* cb, const uint8_t* cr, int y_stride, int c_stride, int subsample, int min_x, int min_y,
                   int width, int height, uint8_t* nrgba, uint8_t* gray, int grid, cudaStream_t st);
+void launch_gray_images(const GraySrc* src, const uint64_t* first, int nsrc, uint64_t total, int grid, cudaStream_t st);
 void launch_scan_gather2(const TiledArgs& A, int grid, size_t smem, cudaStream_t st);
 int gather2_ctas_per_sm(size_t smem, int ng, bool rot, bool img = false);
 void launch_rot_table(const FaceTables& T, const ScaleEntry* plan, int nscales, int slot, RotNode* out, int grid, cudaStream_t st);

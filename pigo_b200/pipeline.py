@@ -224,3 +224,19 @@ def _detect_images(clf, plc, flpcs, images, cp, iou, min_face, eye_perturbs, flp
     if raw:
         return faces, nfaces[:n], points
     return _faces_of(faces, nfaces, points, min_face)
+
+
+def detect_decoded(clf: Pigo, plc: PuplocCascade, flpcs: Dict[str, PuplocCascade], sources, cp: CascadeParams, angles=None, iou: float = 0.1,
+                   min_face: int = 50, eye_perturbs: int = 50, flp_perturbs: int = 63, face_cap: int = 32, randoms: Optional[np.ndarray] = None,
+                   rng_seed: int = 0, det_cap: int = 0, raw: bool = False, device_sources: bool = False):
+    """Go's DetectDecoded: RgbToGrayscale(ImgToNRGBA(img)) of every DecodedImage in one pigo_gray_images call, then
+    detect_images_angles_device on the device arena (angles None = every image at 0).  Returns what
+    detect_images_angles_device returns for the oracle-made gray images with Dim = Cols."""
+    from . import gray_images
+    arena, images = gray_images(sources, device_sources=device_sources)
+    angles = [0.0] * len(images) if angles is None else angles
+    out = detect_images_angles_device(clf, plc, flpcs, images, cp, angles, iou, min_face, eye_perturbs, flp_perturbs, face_cap, randoms,
+                                      rng_seed, det_cap, raw)
+    del arena   # the call above returns after its results are on the host
+    return out
+

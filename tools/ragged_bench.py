@@ -15,6 +15,12 @@ Usage: `python tools/ragged_bench.py [--frames 256]` on one GPU prints one JSON 
               asserted identical): (1) one 1080p frame at 0 and k/32 (k = 1..32) against 33 single-frame calls; (2) bench.py's
               configs[3] batch, 8 x 4K frames at the 32 rotated slots, against 32 batch calls; (3) 16 wide images x 8 angles
               through the pipeline, listed image-major and angle-major, against 8 pigo_detect_images calls
+  decoded : the same 256 images as 4:2:0 YCbCr (luma = the image, seeded chroma) in pinned host memory through face -> pupils
+              -> 15 landmarks, host clock around each whole way, median of 5, outputs asserted identical: (a) one
+              pigo_gray_images + one pigo_detect_images on the device images; (b) per image pigo_ycbcr_to_nrgba (gray only)
+              to the host, then one pigo_detect_images from host gray; (c) per image pigo_ycbcr_to_nrgba (NRGBA) +
+              pigo_rgba_to_gray, then one pigo_detect_images.  Also pigo_gray_images alone from device-resident planes
+              (CUDA events) and from pinned host planes (host clock).
 `--sections scan,pipeline` (the default) selects the sections; `--sections angles` runs the sweeps alone.  Writes nothing
 to the tree.
 """
@@ -485,11 +491,132 @@ def angles_bench(clf, dev: int, stream) -> dict:
     return res
 
 
+def decoded_bench(clf, dev: int, stream) -> dict:
+    """Decoded JPEG-like sources to detector results three ways, and the conversion alone; see the module docstring."""
+    import ctypes as C
+    import torch
+    import pigo_b200
+    from pigo_b200 import DecodedImage, pipeline
+    L = pigo_b200.lib()
+    st = C.c_void_p(stream.cuda_stream)
+    cuda = f"cuda:{dev}"
+    plc = pigo_b200.NewPuplocCascade().UnpackCascade(pigo_b200.load_cascade("puploc"))
+    names = sorted(set(pipeline.EYE_CASCADES + pipeline.MOUTH_CASCADES))
+    flp = {nm: pigo_b200.NewPuplocCascade().UnpackCascade(pigo_b200.load_cascade("lps/" + nm)) for nm in names}
+    hs, fl = pipeline.landmark_call_arrays(flp)
+    ncalls = len(fl)
+    face_cap = 128
+    prm = pigo_b200.PipelineParams(*PARAMS, 0.0, 0.1, 50, 50, 63, 4096)
+    rng = np.random.default_rng(77)
+    imgs = ragged_images()
+    n = len(imgs)
+
+    def check(rc):
+        if rc != 0:
+            raise RuntimeError(L.pigo_last_error().decode())
+
+    # 4:2:0 planes of every image in pinned host memory (YStride = the image's Dim, CStride = chroma width + 3)
+    planes, src_bytes = [], 0
+    for b, r, c, d in imgs:
+        cw, ch = (c + 1) // 2, (r + 1) // 2
+        y = torch.from_numpy(np.ascontiguousarray(b)).pin_memory()
+        cb = torch.from_numpy((128 + rng.integers(-20, 21, size=(ch, cw + 3))).astype(np.uint8)).pin_memory()
+        cr = torch.from_numpy((128 + rng.integers(-20, 21, size=(ch, cw + 3))).astype(np.uint8)).pin_memory()
+        planes.append((y, cb, cr))
+        src_bytes += r * c + 2 * ch * cw
+    gray_px = sum(r * c for _, r, c, _ in imgs)
+    host_src = [DecodedImage.ycbcr(y, cb, cr, 2, c, r, y_stride=d, c_stride=cb.shape[1]) for (y, cb, cr), (_, r, c, d) in zip(planes, imgs)]
+    dev_planes = [tuple(p.to(cuda) for p in pl) for pl in planes]
+    dev_src = [DecodedImage.ycbcr(y, cb, cr, 2, c, r, y_stride=d, c_stride=cb.shape[1]) for (y, cb, cr), (_, r, c, d) in zip(dev_planes, imgs)]
+    need = pigo_b200.gray_images_bytes(host_src)
+    arena = torch.empty(need, dtype=torch.uint8, device=cuda)
+    host_descs, dev_descs = pigo_b200.decoded_descs(host_src), pigo_b200.decoded_descs(dev_src)
+    out_imgs = (pigo_b200.PigoImage * n)()
+    size = C.c_size_t(need)
+
+    def outputs():
+        return (np.zeros((n, face_cap), dtype=pigo_b200.DET_DTYPE), np.zeros(n, dtype=np.int32),
+                np.zeros((n, face_cap, 2 + ncalls), dtype=pigo_b200.POINT_DTYPE))
+
+    def detect(descs, flags, o):
+        check(L.pigo_detect_images(clf._h, plc._h, hs, fl.ctypes.data, ncalls, descs, n, C.byref(prm), None, 7, o[0].ctypes.data, face_cap,
+                                   o[1].ctypes.data, o[2].ctypes.data, flags, st))
+
+    gray_host = [np.zeros((r, c), dtype=np.uint8) for _, r, c, _ in imgs]
+    nrgba_host = [np.zeros((r, c, 4), dtype=np.uint8) for _, r, c, _ in imgs]
+    gray_descs = pigo_b200.image_descs([(g.ctypes.data, r, c, c) for g, (_, r, c, _) in zip(gray_host, imgs)])
+
+    def way_a(o):
+        check(L.pigo_gray_images(host_descs, n, arena.data_ptr(), C.byref(size), out_imgs, pigo_b200.MEM_HOST, st))
+        detect(out_imgs, pigo_b200.FRAMES_DEVICE, o)
+
+    def ycc(i, nrgba, gray):
+        (y, cb, cr), (_, r, c, d) = planes[i], imgs[i]
+        check(L.pigo_ycbcr_to_nrgba(y.data_ptr(), cb.data_ptr(), cr.data_ptr(), d, cb.shape[1], 2, 0, 0, c, r, nrgba, gray, pigo_b200.MEM_HOST, st))
+
+    def way_b(o):
+        for i in range(n):
+            ycc(i, None, gray_host[i].ctypes.data)
+        detect(gray_descs, pigo_b200.MEM_HOST, o)
+
+    def way_c(o):
+        for i in range(n):
+            ycc(i, nrgba_host[i].ctypes.data, None)
+            check(L.pigo_rgba_to_gray(nrgba_host[i].ctypes.data, nrgba_host[i].size // 4, gray_host[i].ctypes.data, pigo_b200.MEM_HOST, st))
+        detect(gray_descs, pigo_b200.MEM_HOST, o)
+
+    res, outs = {}, {}
+    for name, fn in (("a_gray_images_then_detect", way_a), ("b_ycbcr_gray_per_image", way_b), ("c_nrgba_then_gray_per_image", way_c)):
+        o = outputs()
+        fn(o)   # warm-up
+        ts = []
+        for _ in range(5):
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            fn(o)
+            torch.cuda.synchronize()
+            ts.append(time.perf_counter() - t0)
+        res[name + "_ms"] = round(1e3 * float(np.median(ts)), 3)
+        outs[name] = o
+    ref = outs["a_gray_images_then_detect"]
+    for name, o in outs.items():
+        assert all(x.tobytes() == y.tobytes() for x, y in zip(o, ref)), f"{name} differs from the one-call way"
+    res["faces"] = int(ref[1].sum())
+
+    # the conversion alone: device-resident planes (CUDA events), pinned host planes (host clock)
+    ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
+    ks = []
+    for _ in range(6):
+        ev[0].record(stream)
+        check(L.pigo_gray_images(dev_descs, n, arena.data_ptr(), C.byref(size), out_imgs, pigo_b200.FRAMES_DEVICE, st))
+        ev[1].record(stream)
+        ev[1].synchronize()
+        ks.append(ev[0].elapsed_time(ev[1]))
+    k_ms = float(np.median(ks[1:]))
+    moved = src_bytes + gray_px
+    res["gray_images_device_ms"] = round(k_ms, 4)
+    res["gray_images_device_bytes"] = moved
+    res["gray_images_device_tb_s"] = round(moved / (k_ms * 1e-3) / 1e12, 3)
+    res["gray_images_device_of_3_35_tb_s"] = round(moved / (k_ms * 1e-3) / 3.35e12, 3)
+    hs_ = []
+    for _ in range(6):
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        check(L.pigo_gray_images(host_descs, n, arena.data_ptr(), C.byref(size), out_imgs, pigo_b200.MEM_HOST, st))
+        torch.cuda.synchronize()
+        hs_.append(time.perf_counter() - t0)
+    h_s = float(np.median(hs_[1:]))
+    res["gray_images_pinned_ms"] = round(1e3 * h_s, 3)
+    res["gray_images_pinned_source_gb_s"] = round(src_bytes / h_s / 1e9, 2)
+    res["source_bytes"], res["gray_pixels"], res["images"] = src_bytes, gray_px, n
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--frames", type=int, default=256, help="frames of the uniform 1080p comparison")
     ap.add_argument("--pipeline-frames", type=int, default=64, help="frames of the uniform 1080p pipeline comparison")
-    ap.add_argument("--sections", default="scan,pipeline", help="comma-separated: scan, pipeline, angles")
+    ap.add_argument("--sections", default="scan,pipeline", help="comma-separated: scan, pipeline, angles, decoded")
     args = ap.parse_args()
     sections = set(args.sections.split(","))
     import torch
@@ -504,6 +631,8 @@ def main():
         res["pipeline"] = pipeline_bench(clf, 0, stream, d_frames[:args.pipeline_frames], args.pipeline_frames)
     if "angles" in sections:
         res["angles"] = angles_bench(clf, 0, stream)
+    if "decoded" in sections:
+        res["decoded"] = decoded_bench(clf, 0, stream)
     res["gpu"] = torch.cuda.get_device_name(0)
     try:   # read-only query: the power limit belongs beside the numbers
         import subprocess

@@ -34,11 +34,16 @@ def main():
     ap.add_argument("--new", action="store_true", help="only the kernels added late in round 2 (offset tables, shared-memory deep, queue overflow)")
     ap.add_argument("--images", action="store_true", help="only the mixed-size pipeline and RunDetector (image-table kernel variants)")
     ap.add_argument("--angles", action="store_true", help="only the per-image angle calls (several node tables, unrotated and rotated passes)")
+    ap.add_argument("--decoded", action="store_true", help="only pigo_gray_images (every decoded format, host and device planes)")
     args = ap.parse_args()
     pigo_b200.init(0)
     clf = pigo_b200.NewPigo().Unpack(pigo_b200.load_cascade("facefinder"))
     sample = synth.sample_gray()
     counts = []
+    if args.decoded:
+        counts += decoded_case()
+        print("sanitize_run counts:", counts, "launches:", pigo_b200.launch_count())
+        return
     if args.images or args.angles:
         counts += angles_case(clf, sample) if args.angles else images_case(clf, sample)
         print("sanitize_run counts:", counts, "launches:", pigo_b200.launch_count())
@@ -109,6 +114,7 @@ def main():
         counts += [int(out.sum()), int(gy.sum())]
         counts += images_case(clf, sample)
         counts += angles_case(clf, sample)
+        counts += decoded_case()
     print("sanitize_run counts:", counts, "launches:", pigo_b200.launch_count() if hasattr(pigo_b200, "launch_count") else "n/a")
 
 
@@ -162,6 +168,53 @@ def angles_case(clf, sample):
         f, n, p = pipeline.detect_images_angles_device(clf, plc, flp, ims, cp, ang, face_cap=8, rng_seed=3, raw=True)
         counts += [int(n.sum()), int((p["row"] > 0).sum())]
     pigo_b200.set_option("puploc_stage", 1)
+    return counts
+
+
+def decoded_case():
+    """pigo_gray_images over every decoded format (odd sizes and origins, padded strides, 16-byte aligned and unaligned rows,
+    one repeated source) from host planes into a device arena, and again from device planes."""
+    import ctypes as C
+    rng = np.random.default_rng(6)
+    y, cb, cr = (rng.integers(0, 256, size=(21, 43), dtype=np.uint8) for _ in range(3))
+    px = rng.integers(0, 256, size=(9, 40 * 4 + 4), dtype=np.uint8)
+    g = rng.integers(0, 256, size=(5, 35), dtype=np.uint8)
+    src = [pigo_b200.DecodedImage.ycbcr(y, cb, cr, sub, 37, 20, min_x=1, min_y=1) for sub in range(6)]
+    src += [pigo_b200.DecodedImage.nrgba(px, 40, 9), pigo_b200.DecodedImage.rgba(px, 33, 9), pigo_b200.DecodedImage.gray(g, 32, 5),
+            pigo_b200.DecodedImage.gray(g, 35, 5), pigo_b200.DecodedImage.gray(g, 1, 1)]
+    src.append(src[2])
+    need = pigo_b200.gray_images_bytes(src)
+    L = pigo_b200.lib()
+    counts = []
+    for flags in (pigo_b200.MEM_HOST, pigo_b200.FRAMES_DEVICE):
+        gray = C.c_void_p()
+        pigo_b200._check(L.pigo_device_alloc(C.byref(gray), need))
+        bufs = []
+        cur = src
+        if flags == pigo_b200.FRAMES_DEVICE:   # the same planes uploaded with pigo_device_upload
+            cur, seen = [], {}
+            for s in src:
+                if id(s) in seen:   # a repeated source stays byte-identical
+                    cur.append(seen[id(s)])
+                    continue
+                pl = []
+                for p in s.planes:
+                    d = C.c_void_p()
+                    pigo_b200._check(L.pigo_device_alloc(C.byref(d), p.nbytes))
+                    pigo_b200._check(L.pigo_device_upload(d, p.ctypes.data, p.nbytes))
+                    bufs.append(d.value)
+                    pl.append(d.value)
+                seen[id(s)] = pigo_b200.DecodedImage(s.format, s.width, s.height, tuple(pl), s.strides, s.subsample, s.min_x, s.min_y)
+                cur.append(seen[id(s)])
+        imgs = (pigo_b200.PigoImage * len(cur))()
+        size = C.c_size_t(need)
+        pigo_b200._check(L.pigo_gray_images(pigo_b200.decoded_descs(cur), len(cur), gray.value, C.byref(size), imgs, flags, None))
+        out = np.zeros(need, dtype=np.uint8)
+        pigo_b200._check(L.pigo_device_download(out.ctypes.data, gray.value, need))
+        counts.append(int(out.astype(np.int64).sum()))
+        for b in bufs:
+            L.pigo_device_free(b)
+        L.pigo_device_free(gray.value)
     return counts
 
 
