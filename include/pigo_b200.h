@@ -346,6 +346,9 @@ int pigo_set_option(const char *name, int64_t value);
 int pigo_describe_plan(int rows, int cols, int min_size, int max_size, double shift_factor, double scale_factor,
                        char *json, size_t cap);
 int64_t pigo_get_option(const char *name);
+/* Copies the default device's block-interleaved copy of a depth-6 cascade (the table the unrotated deep kernel reads) to
+ * dst and sets *bytes to its size; dst == NULL only sets *bytes (0: depth != 6, no such table). */
+int pigo_cascade_block_table(pigo_cascade *c, uint8_t *dst, size_t *bytes);
 
 #if defined(__GNUC__)
 #pragma GCC visibility pop

@@ -45,7 +45,7 @@ ABI_SYMBOLS = [
     "pigo_device_free", "pigo_device_upload", "pigo_describe_plan", "pigo_init_devices", "pigo_device_count",
     "pigo_device_download", "pigo_run_cascade_batch_sharded", "pigo_detect_batch", "pigo_detect_batch_sharded",
     "pigo_ycbcr_to_nrgba", "pigo_run_cascade_images", "pigo_detect_images", "pigo_puploc_run_images",
-    "pigo_run_cascade_images_angles", "pigo_detect_images_angles", "pigo_gray_images",
+    "pigo_run_cascade_images_angles", "pigo_detect_images_angles", "pigo_gray_images", "pigo_cascade_block_table",
 ]
 
 
@@ -116,6 +116,7 @@ def lib() -> C.CDLL:
         L.pigo_set_option.argtypes = [C.c_char_p, C.c_int64]
         L.pigo_get_option.argtypes = [C.c_char_p]
         L.pigo_get_option.restype = C.c_int64
+        L.pigo_cascade_block_table.argtypes = [vp, vp, C.POINTER(sz)]
         _lib = L
     return _lib
 

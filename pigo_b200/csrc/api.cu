@@ -192,6 +192,8 @@ FaceReplica* face_replica(pigo_cascade* c, int dev, int* rc) {
   r->tab.codes = (const int8_t*)r->codes.p; r->tab.preds = (const float*)r->preds.p; r->tab.thresh = (const float*)r->thresh.p;
   r->tab.depth = (int)c->depth; r->tab.ntrees = (int)c->ntrees; r->tab.leaves = (int)c->leaves;
   if ((*rc = build_tiled_tables(r->tab, c->h_codes, c->h_preds, c->h_thr, r->tiled_tab))) { delete r; return nullptr; }
+  if ((*rc = build_block_tables(r->tab, c->h_codes, c->h_preds, c->h_thr, r->block_tab))) { delete r; return nullptr; }
+  r->tab.blocks = (const uint8_t*)r->block_tab.p;
   c->rep[dev] = r;
   return r;
 }
@@ -1067,6 +1069,21 @@ int pigo_set_option(const char* name, int64_t value) {
   return g_opt.set(name, value) ? PIGO_OK : set_err(PIGO_E_INVALID, "unknown option '%s'", name);
 }
 int64_t pigo_get_option(const char* name) { return name ? g_opt.get(name) : -1; }
+
+int pigo_cascade_block_table(pigo_cascade* c, uint8_t* dst, size_t* bytes) {
+  if (!c || !bytes) return set_err(PIGO_E_INVALID, "null argument");
+  int rc = ensure_device();
+  if (rc) return rc;
+  FaceReplica* R = face_replica(c, default_device(), &rc);
+  if (!R) return rc;
+  const size_t n = R->block_tab.p ? (size_t)((c->ntrees + kBlockTrees - 1) / kBlockTrees) * kBlockBytes : 0;
+  if (dst) {
+    if (*bytes < n) return set_err(PIGO_E_INVALID, "block table needs %zu bytes", n);
+    if (n) CUDA_TRY(cudaMemcpy(dst, R->block_tab.p, n, cudaMemcpyDeviceToHost));
+  }
+  *bytes = n;
+  return PIGO_OK;
+}
 
 // ---- (*Pigo).Unpack, core/pigo.go:51-110 ----------------------------------------------------------------
 static uint32_t rd_u32(const uint8_t* p) { return (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24); }

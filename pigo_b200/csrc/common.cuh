@@ -28,8 +28,21 @@ struct FaceTables {
   const int8_t* codes;   // [ntrees][4*leaves]
   const float* preds;    // [ntrees][leaves]
   const float* thresh;   // [ntrees]
+  const uint8_t* blocks; // depth 6: the block-interleaved copy read by the unrotated deep walk (kBlockBytes, below); else null
   int32_t depth, ntrees, leaves;
 };
+
+// Block-interleaved copy of a depth-6 cascade, for lane groups that walk 8 consecutive trees of one window.  Block b holds
+// trees 8b..8b+7, tree 8b+k in slot k (pad slots of the last block repeat the last tree):
+//   bytes 0..31          thresh of slot k at 4k
+//   bytes 32..63         root code word (node 1) of slot k at 32 + 4k
+//   bytes 64p..64p+63    p = 1..63: for slot k at 64p + 8k, the int2 of node p's two children -- code words 2p, 2p+1 for
+//                        p < 32, leaves preds[2p-64], preds[2p-63] for p >= 32
+// A 128-byte line holds the records of two nodes, so the 8 lanes of a group step read one line for the thresholds, the roots
+// and the first level, then at most 1, 2, 4, 8, 8 lines for the five other levels, where each load of the reference layout
+// (codes[t][256 B], preds[t][256 B]) touches 8 lines.  Thresholds and walks stay the reference's numbers, bit for bit.
+constexpr int kBlockTrees = 8;
+constexpr int kBlockBytes = 4096;
 
 // Unsorted detection as produced by the scan kernels: the in-frame window index doubles as the
 // sort key that restores the reference's emission order (scale, row, col).

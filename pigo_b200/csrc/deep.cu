@@ -9,6 +9,8 @@
 // Round 2: (1) queue items carry their ladder entry, so the consumer needs no binary search; (2) ROT variant:
 // classifyRotatedRegion (core/pigo.go:150-191) with the node's sample offsets read from the per-call table (RotNode,
 // common.cuh) instead of being recomputed per node; (3) a flat-loop variant (deep_flat=1), measured and left off.
+// The unrotated walk reads the cascade from its block-interleaved copy (FaceTables::blocks): the lane group's trees are
+// consecutive, so their records of one node share cache lines instead of sitting 256 bytes apart.
 #include <algorithm>
 
 #include "common.cuh"
@@ -21,9 +23,9 @@ namespace pigo {
 template <int ROT>
 __device__ __forceinline__ float deep_walk(const ScanArgs& A, const FaceTables& T, const uint8_t* __restrict__ pc, const RotNode* __restrict__ rt,
                                            int t, int r, int c, int s, int lim, int dim) {
-  const int2* tp2 = reinterpret_cast<const int2*>(T.preds + (size_t)t * 64);
   int idx = 1;
   if (ROT) {
+    const int2* tp2 = reinterpret_cast<const int2*>(T.preds + (size_t)t * 64);
     // children of node idx are nodes 2idx, 2idx+1: adjacent 8-byte records, fetched with one 16-byte load while
     // this node's two pixels are in flight
     const RotNode* tn = rt + (size_t)t * 64;
@@ -45,13 +47,14 @@ __device__ __forceinline__ float deep_walk(const ScanArgs& A, const FaceTables& 
     }
     return __int_as_float(leafbits);
   } else {
-    // child-pair prefetch: both children of node idx (codes: bytes 8*idx.., leaves: floats 2*idx-64..) are fetched
-    // with one 64-bit load that is in flight together with the two pixel gathers
-    const int2* tc2 = reinterpret_cast<const int2*>(T.codes + (size_t)t * 256);
-    int cw = __ldg(reinterpret_cast<const int*>(tc2) + 1);
+    // child-pair prefetch: both children of node idx (code words, or the two leaves after the last level) are fetched
+    // with one 64-bit load that is in flight together with the two pixel gathers.  The block-interleaved table puts the
+    // GROUP lanes' records of one node side by side (common.cuh), so the group's loads share cache lines.
+    const uint32_t blk = (uint32_t)(t >> 3) * kBlockBytes, rec = blk + 8 * (t & 7);   // 32-bit offsets: one register
+    int cw = __ldg(reinterpret_cast<const int*>(T.blocks + blk + 32) + (t & 7));
 #pragma unroll
     for (int j = 0; j < 6; ++j) {
-      const int2 kids = j < 5 ? __ldg(tc2 + idx) : __ldg(tp2 + (idx - 32));
+      const int2 kids = __ldg(reinterpret_cast<const int2*>(T.blocks + rec + 64 * idx));
       const int o1 = (((int)(int8_t)(cw) * s) >> 8) * dim + (((int)(int8_t)(cw >> 8) * s) >> 8);
       const int o2 = (((int)(int8_t)(cw >> 16) * s) >> 8) * dim + (((cw >> 24) * s) >> 8);
       const unsigned p1 = __ldg(pc + o1), p2 = __ldg(pc + o2);
@@ -61,6 +64,13 @@ __device__ __forceinline__ float deep_walk(const ScanArgs& A, const FaceTables& 
     }
     return __int_as_float(cw);
   }
+}
+
+// Tree t's threshold: unrotated from the block table that deep_walk<0> reads (the group's 8 thresholds are one 32-byte run).
+template <int ROT>
+__device__ __forceinline__ float deep_thresh(const FaceTables& T, int t) {
+  if (ROT) return __ldg(T.thresh + t);
+  return __ldg(reinterpret_cast<const float*>(T.blocks + (size_t)(t >> 3) * kBlockBytes) + (t & 7));
 }
 
 // Where a queue item's window lies: frame (IMG = 1: the image of the group), ladder entry, size and centre (r, c), from the
@@ -169,7 +179,7 @@ __global__ void __launch_bounds__(CHUNK ? kDeepOrdThreads : 256, CHUNK ? 2048 / 
     float thr_prev = 0.f;
     while (t0 < T.ntrees && !rejected) {
       const int t = min(t0 + sub, T.ntrees - 1);      // lanes past the last tree redo it harmlessly
-      const float thr = __ldg(T.thresh + t);
+      const float thr = deep_thresh<ROT>(T, t);
       const float pred = deep_walk<ROT>(A, T, w.pc, w.rt, t, w.r, w.c, w.s, IMG ? w.lim : lim, IMG ? w.dim : A.dim);
       const int nvalid = min(GROUP, T.ntrees - t0);
       for (int j = 0; j < nvalid; ++j) {              // the reference's sequential accumulation, :137-141

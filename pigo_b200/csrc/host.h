@@ -280,10 +280,10 @@ std::vector<int> shard_devices();   // devices of the mask given to pigo_init_de
 
 struct FaceReplica {            // device copy of one face cascade
   int device = 0, num_sms = 132;
-  DevBuf codes, preds, thresh, tiled_tab;
+  DevBuf codes, preds, thresh, tiled_tab, block_tab;
   FaceTables tab{};
   WorkspacePool pool;
-  ~FaceReplica() { cudaSetDevice(device); codes.release(); preds.release(); thresh.release(); tiled_tab.release(); }
+  ~FaceReplica() { cudaSetDevice(device); codes.release(); preds.release(); thresh.release(); tiled_tab.release(); block_tab.release(); }
 };
 struct PuplocReplica {
   int device = 0, num_sms = 132;
@@ -348,6 +348,8 @@ void launch_eye_seeds(const pigo_det* clusters, const int32_t* ncl, int cl_cap, 
                       int eye_perturbs, pigo_det* faces, int32_t* nfaces, pigo_point* seeds, cudaStream_t st);
 void launch_landmark_seeds(const pigo_point* points, pigo_point* seeds, int nslots, int stride, int ncalls, int flp_perturbs, cudaStream_t st);
 int build_tiled_tables(const FaceTables& tab, const std::vector<int8_t>& codes, const std::vector<float>& preds,
+                       const std::vector<float>& thr, DevBuf& out);
+int build_block_tables(const FaceTables& tab, const std::vector<int8_t>& codes, const std::vector<float>& preds,
                        const std::vector<float>& thr, DevBuf& out);
 int describe_plan(const std::vector<ScaleEntry>& plan, uint64_t wins, int ntrees, char* buf, size_t cap);
 int run_scan(FaceReplica* c, Workspace* w, int lane, ScanArgs& A, unsigned long long* d_work, cudaStream_t st, int num_sms);

@@ -37,6 +37,33 @@ int build_tiled_tables(const FaceTables& tab, const std::vector<int8_t>& codes, 
   return PIGO_OK;
 }
 
+// Builds the block-interleaved table the unrotated deep walk reads (depth 6 only; layout: kBlockBytes in common.cuh).
+int build_block_tables(const FaceTables& tab, const std::vector<int8_t>& codes, const std::vector<float>& preds,
+                       const std::vector<float>& thr, DevBuf& out) {
+  if (tab.depth != 6 || tab.ntrees <= 0) return PIGO_OK;
+  const int n = tab.ntrees, nblk = (n + kBlockTrees - 1) / kBlockTrees;
+  std::vector<uint8_t> blk((size_t)nblk * kBlockBytes, 0);
+  for (int i = 0; i < nblk * kBlockTrees; ++i) {
+    const int t = std::min(i, n - 1);   // pad slots: a copy of the last tree
+    uint8_t* b = blk.data() + (size_t)(i / kBlockTrees) * kBlockBytes;
+    const int k = i % kBlockTrees;
+    memcpy(b + 4 * k, thr.data() + t, 4);
+    memcpy(b + 32 + 4 * k, codes.data() + (size_t)t * 256 + 4, 4);                         // node 1
+    for (int p = 1; p < 64; ++p) {
+      const void* kids = p < 32 ? (const void*)(codes.data() + (size_t)t * 256 + 8 * p)       // code words 2p, 2p+1
+                                : (const void*)(preds.data() + (size_t)t * 64 + 2 * p - 64);  // leaves 2p-64, 2p-63
+      memcpy(b + 64 * p + 8 * k, kids, 8);
+    }
+  }
+  int rc = out.reserve(blk.size());
+  if (rc) return rc;
+  if (cudaMemcpy(out.p, blk.data(), blk.size(), cudaMemcpyHostToDevice) != cudaSuccess) {
+    cudaGetLastError();
+    return set_err(PIGO_E_CUDA, "block table upload failed");
+  }
+  return PIGO_OK;
+}
+
 struct TilePlan {
   int nbands = 0;
   TileBand band[kMaxBands];
