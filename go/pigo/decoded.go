@@ -13,6 +13,7 @@ import "C"
 
 import (
 	"image"
+	"image/color"
 	"reflect"
 	"sync/atomic"
 	"unsafe"
@@ -26,8 +27,10 @@ type decodedPart struct {
 	strides                                      [2]int
 }
 
-// partOf describes img in its own pixel format: *image.YCbCr with Rect.Min >= 0, *image.NRGBA, *image.RGBA and *image.Gray
-// as they are; every other type, and a YCbCr image with a negative origin, through the shim's ImgToNRGBA as NRGBA.
+// partOf describes img in its own pixel format: *image.YCbCr with Rect.Min >= 0, *image.NRGBA, *image.RGBA, *image.Gray,
+// *image.Gray16, *image.RGBA64, *image.NRGBA64, *image.CMYK and *image.Paletted with a non-empty palette as they are (every
+// type image/jpeg and image/png return); other types (*image.NYCbCrA, *image.Alpha, *image.Alpha16, user types), a YCbCr
+// image with a negative origin and an empty palette (which panics like the reference) through the shim's ImgToNRGBA as NRGBA.
 func partOf(img image.Image) decodedPart {
 	b := img.Bounds()
 	w, h := b.Dx(), b.Dy()
@@ -58,6 +61,38 @@ func partOf(img image.Image) decodedPart {
 		p.format, p.planes[0], p.strides[0] = C.PIGO_DECODED_GRAY, src.Pix[src.PixOffset(b.Min.X, b.Min.Y):src.PixOffset(last.X, last.Y)+1], src.Stride
 		p.minX, p.minY = 0, 0
 		return p
+	case *image.Gray16:
+		p.format, p.planes[0], p.strides[0] = C.PIGO_DECODED_GRAY16, src.Pix[src.PixOffset(b.Min.X, b.Min.Y):src.PixOffset(last.X, last.Y)+2], src.Stride
+		p.minX, p.minY = 0, 0
+		return p
+	case *image.RGBA64:
+		p.format, p.planes[0], p.strides[0] = C.PIGO_DECODED_RGBA64, src.Pix[src.PixOffset(b.Min.X, b.Min.Y):src.PixOffset(last.X, last.Y)+8], src.Stride
+		p.minX, p.minY = 0, 0
+		return p
+	case *image.NRGBA64:
+		p.format, p.planes[0], p.strides[0] = C.PIGO_DECODED_NRGBA64, src.Pix[src.PixOffset(b.Min.X, b.Min.Y):src.PixOffset(last.X, last.Y)+8], src.Stride
+		p.minX, p.minY = 0, 0
+		return p
+	case *image.CMYK:
+		p.format, p.planes[0], p.strides[0] = C.PIGO_DECODED_CMYK, src.Pix[src.PixOffset(b.Min.X, b.Min.Y):src.PixOffset(last.X, last.Y)+4], src.Stride
+		p.minX, p.minY = 0, 0
+		return p
+	case *image.Paletted:
+		if len(src.Palette) > 0 {
+			// an index is a byte: entries past 255 are unreachable.  Each entry is converted the way ImgToNRGBA converts
+			// the pixel that uses it, so the result is exact by construction.
+			k := min(len(src.Palette), 256)
+			pal := make([]uint8, 4*k)
+			for i, c := range src.Palette[:k] {
+				n := color.NRGBAModel.Convert(c).(color.NRGBA)
+				pal[4*i], pal[4*i+1], pal[4*i+2], pal[4*i+3] = n.R, n.G, n.B, n.A
+			}
+			p.format = C.PIGO_DECODED_PALETTED
+			p.planes = [3][]uint8{src.Pix[src.PixOffset(b.Min.X, b.Min.Y) : src.PixOffset(last.X, last.Y)+1], pal}
+			p.strides = [2]int{src.Stride, k}
+			p.minX, p.minY = 0, 0
+			return p
+		}
 	}
 	n := ImgToNRGBA(img)
 	return decodedPart{format: C.PIGO_DECODED_NRGBA, width: w, height: h, planes: [3][]uint8{n.Pix[:(h-1)*n.Stride+4*w]}, strides: [2]int{n.Stride, 0}}

@@ -305,6 +305,10 @@ int pigo_ycbcr_to_nrgba(const uint8_t *y, const uint8_t *cb, const uint8_t *cr, 
  *   PIGO_DECODED_NRGBA  *image.NRGBA: plane[0] = Pix[PixOffset(Rect.Min):], stride[0] = Stride
  *   PIGO_DECODED_RGBA   *image.RGBA (alpha-premultiplied), laid out as NRGBA
  *   PIGO_DECODED_GRAY   *image.Gray: plane[0] = Pix[PixOffset(Rect.Min):], stride[0] = Stride
+ *   PIGO_DECODED_GRAY16, _RGBA64, _NRGBA64, _CMYK, _PALETTED  *image.Gray16, RGBA64, NRGBA64, CMYK, Paletted:
+ *                       plane[0] = Pix[PixOffset(Rect.Min):], stride[0] = Stride; 2, 8, 8, 4 and 1 bytes per pixel
+ *                       (16-bit samples big-endian, as Go stores them).  Paletted only: plane[1] = the palette as
+ *                       stride[1] (1..256) NRGBA entries of 4 bytes, entry i = color.NRGBAModel.Convert(Palette[i]).
  * width, height = Rect size.  Fields a format does not use are ignored, but take part in the repeat test below.
  * Output: `gray` is a device buffer of *gray_bytes bytes.  Source i gets a 256-byte-aligned slot of height rows of exactly
  * width bytes and images[i] = {slot, height, width, width} (dim == width: the rotated scan's column clamp,
@@ -312,14 +316,21 @@ int pigo_ycbcr_to_nrgba(const uint8_t *y, const uint8_t *cb, const uint8_t *cr, 
  * with PIGO_FRAMES_DEVICE, to pigo_run_cascade_images[_angles], pigo_detect_images[_angles] or pigo_puploc_run_images.
  * Slot bytes: YCbCr = the fused `gray` output of pigo_ycbcr_to_nrgba; NRGBA = pigo_rgba_to_gray of the pixels; RGBA =
  * the same after color.NRGBAModel (c*0xffff/a >> 8 in uint32, a == 0 -> 0; a channel above alpha wraps as in Go);
- * Gray = Y (luma(Y, Y, Y, 0xff) == Y for every Y).
+ * Gray = Y (luma(Y, Y, Y, 0xff) == Y for every Y).  The other types go through color.NRGBAModel (go1.22 image/color, all
+ * arithmetic uint32; nrgbaModel(r, g, b, a) = a == 0xffff: c >> 8; a == 0: all zero; else uint8((c*0xffff/a) >> 8),
+ * alpha uint8(a >> 8)) and then luma: Gray16 = the high byte of Y (nrgbaModel(Y, Y, Y, 0xffff)); RGBA64 =
+ * nrgbaModel(R, G, B, A) of the stored channels (a channel above alpha wraps as in Go); NRGBA64 = nrgbaModel(C*A/0xffff
+ * for each colour channel, A), keeping the precision that premultiplying loses; CMYK = w = 0xffff - K*0x101,
+ * R = (0xffff - C*0x101)*w/0xffff (G from M, B from Y), alpha 0xffff; Paletted = luma(palette[index]).
+ * One difference from the reference: a palette index at or past stride[1] gives gray 0 here, where Go's Paletted.At
+ * would panic; Go's PNG decoder never makes such an index, since it extends a short palette with opaque black (gray 0).
  * Descriptors that are byte-identical share one slot and are converted once (an angle sweep of one photo costs one
  * conversion).  Required size = sum over distinct descriptors of round256(width*height).  If `gray` is NULL or
  * *gray_bytes is smaller, the call sets *gray_bytes to the required size and returns PIGO_E_CAP; that query, every
  * argument check and a call with n == 0 (PIGO_OK, required size 0) need no device.  PIGO_E_INVALID: n outside 0..65535, an unknown
- * format, subsample outside 0..5, a negative YCbCr origin, width or height < 1, width*height >= 2^31, a stride below
- * width * bytes per pixel (CStride: below the rectangle's chroma width), a null plane, a null src / images / gray_bytes,
- * or a stream that is being captured into a CUDA graph.
+ * format (4 is not assigned), subsample outside 0..5, a negative YCbCr origin, width or height < 1, width*height >= 2^31,
+ * a stride below width * bytes per pixel (CStride: below the rectangle's chroma width), a null plane, a null palette or a
+ * palette length outside 1..256, a null src / images / gray_bytes, or a stream that is being captured into a CUDA graph.
  * flags: PIGO_FRAMES_DEVICE = the planes are device pointers; on a caller's stream the call then returns without
  * synchronising.  Host planes are read only during the call: one copy per plane per distinct source, of the bytes the
  * rectangle covers.  With stream NULL the call synchronises before it returns. */
@@ -327,6 +338,11 @@ int pigo_ycbcr_to_nrgba(const uint8_t *y, const uint8_t *cb, const uint8_t *cr, 
 #define PIGO_DECODED_NRGBA 1
 #define PIGO_DECODED_RGBA 2
 #define PIGO_DECODED_GRAY 3
+#define PIGO_DECODED_GRAY16 5
+#define PIGO_DECODED_RGBA64 6
+#define PIGO_DECODED_NRGBA64 7
+#define PIGO_DECODED_CMYK 8
+#define PIGO_DECODED_PALETTED 9
 typedef struct {
   int32_t format, subsample, min_x, min_y, width, height;
   const uint8_t *plane[3];

@@ -31,6 +31,7 @@ CASCADE_DIR = os.path.join(DATA_DIR, "cascade")
 PIGO_OK, PIGO_E_INVALID, PIGO_E_CUDA, PIGO_E_CAP, PIGO_E_NOMEM, PIGO_E_NODEVICE = 0, -1, -2, -3, -4, -5
 MEM_HOST, FRAMES_DEVICE, OUT_DEVICE = 0, 1, 2
 DECODED_YCBCR, DECODED_NRGBA, DECODED_RGBA, DECODED_GRAY = 0, 1, 2, 3
+DECODED_GRAY16, DECODED_RGBA64, DECODED_NRGBA64, DECODED_CMYK, DECODED_PALETTED = 5, 6, 7, 8, 9
 
 DET_DTYPE = np.dtype([("row", "<i4"), ("col", "<i4"), ("scale", "<i4"), ("q", "<f4")])
 POINT_DTYPE = np.dtype([("row", "<i4"), ("col", "<i4"), ("scale", "<f4"), ("perturbs", "<i4")])
@@ -696,6 +697,34 @@ class DecodedImage:
     def gray(cls, pix, width: int, height: int, stride: Optional[int] = None) -> "DecodedImage":
         """*image.Gray: Pix[PixOffset(Rect.Min):] and Stride."""
         return cls(DECODED_GRAY, width, height, (pix,), (stride if stride is not None else _row_bytes(pix, width), 0))
+
+    @classmethod
+    def gray16(cls, pix, width: int, height: int, stride: Optional[int] = None) -> "DecodedImage":
+        """*image.Gray16: Pix[PixOffset(Rect.Min):] (2 bytes per pixel, big-endian) and Stride."""
+        return cls(DECODED_GRAY16, width, height, (pix,), (stride if stride is not None else _row_bytes(pix, 2 * width), 0))
+
+    @classmethod
+    def rgba64(cls, pix, width: int, height: int, stride: Optional[int] = None) -> "DecodedImage":
+        """*image.RGBA64 (alpha-premultiplied): Pix[PixOffset(Rect.Min):] (R, G, B, A big-endian uint16) and Stride."""
+        return cls(DECODED_RGBA64, width, height, (pix,), (stride if stride is not None else _row_bytes(pix, 8 * width), 0))
+
+    @classmethod
+    def nrgba64(cls, pix, width: int, height: int, stride: Optional[int] = None) -> "DecodedImage":
+        """*image.NRGBA64: Pix[PixOffset(Rect.Min):] (R, G, B, A big-endian uint16) and Stride."""
+        return cls(DECODED_NRGBA64, width, height, (pix,), (stride if stride is not None else _row_bytes(pix, 8 * width), 0))
+
+    @classmethod
+    def cmyk(cls, pix, width: int, height: int, stride: Optional[int] = None) -> "DecodedImage":
+        """*image.CMYK: Pix[PixOffset(Rect.Min):] (C, M, Y, K bytes) and Stride."""
+        return cls(DECODED_CMYK, width, height, (pix,), (stride if stride is not None else _row_bytes(pix, 4 * width), 0))
+
+    @classmethod
+    def paletted(cls, pix, palette, width: int, height: int, stride: Optional[int] = None) -> "DecodedImage":
+        """*image.Paletted: Pix[PixOffset(Rect.Min):] (palette indices) and Stride; `palette` is [k][4] uint8 NRGBA entries,
+        entry i = color.NRGBAModel.Convert(Palette[i]), k in 1..256 (host array, or a CUDA tensor with device_sources)."""
+        if isinstance(palette, np.ndarray):
+            palette = np.ascontiguousarray(palette, dtype=np.uint8).reshape(-1, 4)
+        return cls(DECODED_PALETTED, width, height, (pix, palette), (stride if stride is not None else _row_bytes(pix, width), len(palette)))
 
     def desc(self) -> PigoDecoded:
         d = PigoDecoded()

@@ -1584,21 +1584,22 @@ static YCbCrExtent ycbcr_extent(int subsample, int min_x, int min_y, int width, 
   return YCbCrExtent{(size_t)(height - 1) * y_stride + width, (size_t)(c_rows - 1) * c_stride + c_cols, c_cols};
 }
 
-static int decoded_bpp(int format) { return format == PIGO_DECODED_NRGBA || format == PIGO_DECODED_RGBA ? 4 : 1; }
-
 // Host bytes of plane k of a decoded source from its rectangle's origin to its last sample (0: the format has no plane k).
+// A Paletted source's plane 1 is its palette of stride[1] 4-byte entries.
 static size_t decoded_plane_bytes(const pigo_decoded& d, int k) {
   if (d.format == PIGO_DECODED_YCBCR) {
     const YCbCrExtent e = ycbcr_extent(d.subsample, d.min_x, d.min_y, d.width, d.height, d.stride[0], d.stride[1]);
     return k == 0 ? e.y_bytes : e.c_bytes;
   }
+  if (d.format == PIGO_DECODED_PALETTED && k == 1) return (size_t)4 * d.stride[1];
   return k == 0 ? (size_t)(d.height - 1) * d.stride[0] + (size_t)d.width * decoded_bpp(d.format) : 0;
 }
 
 static int check_decoded(const pigo_decoded* src, int n) {
   for (int i = 0; i < n; ++i) {
     const pigo_decoded& d = src[i];
-    if (d.format < PIGO_DECODED_YCBCR || d.format > PIGO_DECODED_GRAY) return set_err(PIGO_E_INVALID, "source %d: unknown format %d", i, d.format);
+    if (d.format < PIGO_DECODED_YCBCR || d.format > PIGO_DECODED_PALETTED || d.format == 4)
+      return set_err(PIGO_E_INVALID, "source %d: unknown format %d", i, d.format);
     if (d.width < 1 || d.height < 1) return set_err(PIGO_E_INVALID, "source %d: bad size %dx%d", i, d.width, d.height);
     if ((uint64_t)d.width * (uint64_t)d.height > 0x7fffffffull) return set_err(PIGO_E_INVALID, "source %d: 2^31 pixels or more", i);
     const bool ycc = d.format == PIGO_DECODED_YCBCR;
@@ -1609,6 +1610,9 @@ static int check_decoded(const pigo_decoded* src, int n) {
     if ((int64_t)d.stride[0] < (int64_t)d.width * decoded_bpp(d.format)) return set_err(PIGO_E_INVALID, "source %d: stride %d below the row", i, d.stride[0]);
     if (ycc && d.stride[1] < ycbcr_extent(d.subsample, d.min_x, d.min_y, d.width, d.height, d.stride[0], d.stride[1]).c_cols)
       return set_err(PIGO_E_INVALID, "source %d: chroma stride %d below the chroma row", i, d.stride[1]);
+    if (d.format == PIGO_DECODED_PALETTED && !d.plane[1]) return set_err(PIGO_E_INVALID, "source %d: null palette", i);
+    if (d.format == PIGO_DECODED_PALETTED && (d.stride[1] < 1 || d.stride[1] > 256))
+      return set_err(PIGO_E_INVALID, "source %d: palette length %d outside 1..256", i, d.stride[1]);
   }
   return PIGO_OK;
 }
@@ -1808,7 +1812,8 @@ int pigo_ycbcr_to_nrgba(const uint8_t* y, const uint8_t* cb, const uint8_t* cr, 
 }
 
 // ---- RgbToGrayscale(ImgToNRGBA(img)) for a batch of decoded images, core/grayscale.go:8-23 + core/image.go:35-90 -----------
-// One slot per distinct source in the caller's device arena (arena_layout), one kernel launch for the whole batch.
+// One slot per distinct source in the caller's device arena (arena_layout); one kernel launch for the YCbCr, NRGBA, RGBA
+// and Gray sources and one for the other formats, each made only when the call has such sources.
 int pigo_gray_images(const pigo_decoded* src, int n, uint8_t* gray, size_t* gray_bytes, pigo_image* images, unsigned flags, void* stream_) {
   if (n < 0 || n > 65535) return set_err(PIGO_E_INVALID, "%d sources: outside 0..65535", n);
   if (!gray_bytes) return set_err(PIGO_E_INVALID, "null gray_bytes");
@@ -1834,11 +1839,15 @@ int pigo_gray_images(const pigo_decoded* src, int n, uint8_t* gray, size_t* gray
   if ((rc = ws_enter(w, st))) return rc;
   const bool in_dev = flags & PIGO_FRAMES_DEVICE;
 
-  // the distinct sources; host planes go to one staging buffer, each plane 256-byte aligned
+  // the distinct sources, the ones gray_images_kernel<false> converts first (nnarrow of them); host planes go to one
+  // staging buffer, each plane 256-byte aligned
   std::vector<int> who;
-  for (int i = 0; i < n; ++i)
-    if (first[i]) who.push_back(i);
+  for (int wide = 0; wide < 2; ++wide)
+    for (int i = 0; i < n; ++i)
+      if (first[i] && decoded_wide(src[i].format) == (wide == 1)) who.push_back(i);
   const int ns = (int)who.size();
+  int nnarrow = 0;
+  while (nnarrow < ns && !decoded_wide(src[who[nnarrow]].format)) ++nnarrow;
   std::vector<size_t> stage_off((size_t)ns * 3, 0);
   size_t stage_bytes = 0;
   if (!in_dev) {
@@ -1850,7 +1859,8 @@ int pigo_gray_images(const pigo_decoded* src, int n, uint8_t* gray, size_t* gray
     if ((rc = w->frames.reserve(stage_bytes + 256))) return rc;
   }
   std::vector<GraySrc> tab(ns);
-  std::vector<uint64_t> firsts(ns + 1, 0);
+  // each kernel's work range starts at 0: firsts[0..nnarrow] for the first kernel, firsts[nnarrow+1..ns+1] for the second
+  std::vector<uint64_t> firsts(ns + 2, 0);
   for (int k = 0; k < ns; ++k) {
     const pigo_decoded& d = src[who[k]];
     GraySrc& t = tab[k];
@@ -1859,7 +1869,8 @@ int pigo_gray_images(const pigo_decoded* src, int n, uint8_t* gray, size_t* gray
     t.dst = gray + off[who[k]];
     t.format = d.format; t.sub = d.subsample; t.min_x = d.min_x; t.min_y = d.min_y; t.width = d.width; t.height = d.height;
     t.stride0 = d.stride[0]; t.stride1 = d.stride[1];
-    firsts[k + 1] = firsts[k] + (uint64_t)d.height * (uint64_t)((d.width + 15) / 16);
+    const int at = k < nnarrow ? k : k + 1;
+    firsts[at + 1] = firsts[at] + (uint64_t)d.height * (uint64_t)((d.width + 15) / 16);
   }
   const size_t tab_bytes = ((size_t)ns * sizeof(GraySrc) + 255) & ~(size_t)255;
   std::vector<uint8_t> blob(tab_bytes + firsts.size() * sizeof(uint64_t));
@@ -1879,10 +1890,18 @@ int pigo_gray_images(const pigo_decoded* src, int n, uint8_t* gray, size_t* gray
     CUDA_TRY(cudaEventRecord(copied, st));
   }
   CUDA_TRY(cudaMemcpyAsync(w->img_tab.p, blob.data(), blob.size(), cudaMemcpyHostToDevice, st));
+  const GraySrc* d_tab = (const GraySrc*)w->img_tab.p;
+  const uint64_t* d_first = (const uint64_t*)((const uint8_t*)w->img_tab.p + tab_bytes);
   timing_begin(T_GRAY_IMAGES, st);
-  launch_gray_images((const GraySrc*)w->img_tab.p, (const uint64_t*)((const uint8_t*)w->img_tab.p + tab_bytes), ns, firsts[ns], device_sms(dev) * 16, st);
+  if (nnarrow > 0) {
+    launch_gray_images(d_tab, d_first, nnarrow, firsts[nnarrow], false, device_sms(dev) * 16, st);
+    g_launches++;
+  }
+  if (ns > nnarrow) {
+    launch_gray_images(d_tab + nnarrow, d_first + nnarrow + 1, ns - nnarrow, firsts[ns + 1], true, device_sms(dev) * 16, st);
+    g_launches++;
+  }
   timing_end(T_GRAY_IMAGES, st);
-  g_launches++;
   CUDA_TRY(cudaGetLastError());
   if (!stream_) CUDA_TRY(cudaStreamSynchronize(st));   // the library's own stream: the arena is complete on return
   else if (copied) CUDA_TRY(cudaEventSynchronize(copied));

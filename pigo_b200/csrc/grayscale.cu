@@ -114,7 +114,8 @@ void launch_ycbcr(const uint8_t* y, const uint8_t* cb, const uint8_t* cr, int y_
 //   *image.YCbCr  luma(YCbCrToRGB(Y, Cb, Cr)), the `gray` output of ycbcr_kernel;
 //   *image.NRGBA  luma of the pixel (the reference copies the rows);
 //   *image.RGBA   luma(color.NRGBAModel(pixel)) -- rgba_to_nrgba below;
-//   *image.Gray   luma(Y, Y, Y, 0xff) == Y for every Y (pinned by a CPU test), so the rows are copied.
+//   *image.Gray   luma(Y, Y, Y, 0xff) == Y for every Y (pinned by a CPU test), so the rows are copied;
+//   *image.Gray16, RGBA64, NRGBA64, CMYK, Paletted   luma(color.NRGBAModel(pixel)) -- wide_chunk below.
 // color.nrgbaModel (image/color/color.go) of a color.RGBA pixel: its RGBA() channels c*0x101 (alpha-premultiplied) back to
 // straight 8-bit channels.  uint32 arithmetic as Go's: a == 0xffff -> c >> 8; a == 0 -> all zero; else (c*0xffff)/a >> 8,
 // truncated to uint8 (a channel above alpha -- invalid premultiplied input -- wraps like the reference's conversion).
@@ -131,14 +132,106 @@ __device__ __forceinline__ uint32_t rgba_to_nrgba(uint32_t px) {
   return out;
 }
 
+// color.nrgbaModel of the 16-bit alpha-premultiplied channels a Color.RGBA() returns, as an NRGBA pixel (uint32 like Go;
+// c * 0xffff <= 0xfffe0001 cannot overflow, and a channel above alpha wraps through the uint8 conversion).
+__device__ __forceinline__ uint32_t nrgba_model(uint32_t r, uint32_t g, uint32_t b, uint32_t a) {
+  if (a == 0xffffu) return (r >> 8) | ((g >> 8) << 8) | ((b >> 8) << 16) | 0xff000000u;
+  if (a == 0) return 0;
+  return (((r * 0xffffu) / a >> 8) & 0xffu) | ((((g * 0xffffu) / a >> 8) & 0xffu) << 8) | ((((b * 0xffffu) / a >> 8) & 0xffu) << 16) |
+         ((a >> 8) << 24);
+}
+
+// One *image.RGBA64 / *image.NRGBA64 pixel, R G B A as big-endian uint16: `rg` and `ba` are its two 4-byte halves as
+// loaded (little-endian words).  NRGBA64.RGBA() premultiplies first (c*a/0xffff); the precision that loses is kept.
+__device__ __forceinline__ uint32_t px64_to_nrgba(uint32_t rg, uint32_t ba, bool premul) {
+  uint32_t r = __byte_perm(rg, 0, 0x4401), g = __byte_perm(rg, 0, 0x4423), b = __byte_perm(ba, 0, 0x4401);
+  const uint32_t a = __byte_perm(ba, 0, 0x4423);
+  if (!premul) { r = r * a / 0xffffu; g = g * a / 0xffffu; b = b * a / 0xffffu; }
+  return nrgba_model(r, g, b, a);
+}
+
+// color.CMYK.RGBA() of one pixel (bytes C, M, Y, K), opaque, then nrgbaModel's a == 0xffff case.
+__device__ __forceinline__ uint32_t cmyk_to_nrgba(uint32_t px) {
+  const uint32_t w = 0xffffu - (px >> 24) * 0x101u;
+  const uint32_t r = (0xffffu - (px & 0xffu) * 0x101u) * w / 0xffffu;
+  const uint32_t g = (0xffffu - ((px >> 8) & 0xffu) * 0x101u) * w / 0xffffu;
+  const uint32_t b = (0xffffu - ((px >> 16) & 0xffu) * 0x101u) * w / 0xffffu;
+  return (r >> 8) | ((g >> 8) << 8) | ((b >> 8) << 16) | 0xff000000u;
+}
+
 // Pixel k of a 16-pixel chunk of 4-byte pixels: one of four 16-byte loads when the chunk is aligned and full, else bytes.
 __device__ __forceinline__ uint32_t px32(const uint4* q, const uint8_t* p, bool vec, int k) {
   if (vec) { const uint4 v = q[k >> 2]; return (k & 3) == 0 ? v.x : (k & 3) == 1 ? v.y : (k & 3) == 2 ? v.z : v.w; }
   return (uint32_t)__ldg(p + 4 * k) | ((uint32_t)__ldg(p + 4 * k + 1) << 8) | ((uint32_t)__ldg(p + 4 * k + 2) << 16) | ((uint32_t)__ldg(p + 4 * k + 3) << 24);
 }
 
+// Palette entry i (an NRGBA pixel) of a Paletted source; a device palette need not be 4-byte aligned.
+__device__ __forceinline__ uint32_t palette_px(const uint8_t* pal, uint32_t i) {
+  return ((uintptr_t)pal & 3) == 0 ? __ldg(reinterpret_cast<const uint32_t*>(pal) + i) : px32(nullptr, pal + 4 * i, false, 0);
+}
+
+// The 16 gray bytes w[] of one chunk of a Gray16, RGBA64, NRGBA64, CMYK or Paletted source: p = the chunk's first pixel,
+// n <= 16 pixels, vec = full and 16-byte aligned (2, 8, 4 and 1 16-byte loads; the 64-bit formats in two halves of four).
+__device__ __forceinline__ void wide_chunk(const GraySrc& s, const uint8_t* p, int n, bool vec, uint32_t w[4]) {
+  const uint4* q = reinterpret_cast<const uint4*>(p);
+  if (s.format == PIGO_DECODED_GRAY16) {   // luma(Y>>8, Y>>8, Y>>8, 0xff) == Y>>8: the high (first) byte of each sample
+    if (vec) {
+      const uint4 a = __ldg(q), b = __ldg(q + 1);
+      w[0] = __byte_perm(a.x, a.y, 0x6420); w[1] = __byte_perm(a.z, a.w, 0x6420);
+      w[2] = __byte_perm(b.x, b.y, 0x6420); w[3] = __byte_perm(b.z, b.w, 0x6420);
+    } else {
+#pragma unroll
+      for (int k = 0; k < 16; ++k)
+        if (k < n) w[k >> 2] |= (uint32_t)__ldg(p + 2 * k) << (8 * (k & 3));
+    }
+  } else if (s.format == PIGO_DECODED_PALETTED) {
+    const uint32_t len = (uint32_t)s.stride1;
+    uint4 iv = make_uint4(0, 0, 0, 0);
+    if (vec) iv = __ldg(q);
+#pragma unroll
+    for (int k = 0; k < 16; ++k) {
+      if (k < n) {
+        const uint32_t iw = (k >> 2) == 0 ? iv.x : (k >> 2) == 1 ? iv.y : (k >> 2) == 2 ? iv.z : iv.w;
+        const uint32_t i = vec ? (iw >> (8 * (k & 3))) & 0xffu : (uint32_t)__ldg(p + k);
+        if (i < len) w[k >> 2] |= luma(palette_px(s.plane[1], i)) << (8 * (k & 3));   // past the palette: gray 0
+      }
+    }
+  } else if (s.format == PIGO_DECODED_CMYK) {
+    uint4 v[4];
+    if (vec) {
+#pragma unroll
+      for (int k = 0; k < 4; ++k) v[k] = __ldg(q + k);
+    }
+#pragma unroll
+    for (int k = 0; k < 16; ++k)
+      if (k < n) w[k >> 2] |= luma(cmyk_to_nrgba(px32(v, p, vec, k))) << (8 * (k & 3));
+  } else {
+    const bool premul = s.format == PIGO_DECODED_RGBA64;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      uint4 v[4];
+      if (vec) {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) v[k] = __ldg(q + 4 * h + k);
+      }
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const int k = 8 * h + j;
+        if (k < n) {
+          // pixel j of the half is words 2j and 2j+1 of its four loads
+          const uint32_t rg = px32(v, p + 64 * h, vec, 2 * j), ba = px32(v, p + 64 * h, vec, 2 * j + 1);
+          w[k >> 2] |= luma(px64_to_nrgba(rg, ba, premul)) << (8 * (k & 3));
+        }
+      }
+    }
+  }
+}
+
 // One thread per (source, row, 16-pixel chunk) work item over every distinct source of the call; the source is found by a
 // binary search over the sources' first work items.  16-byte stores where the slot row is aligned, bytes otherwise.
+// Wide = the Gray16, RGBA64, NRGBA64, CMYK and Paletted sources: their conversions need about 90 registers where the
+// YCbCr, NRGBA, RGBA and Gray ones need 57, so they run in an instantiation of their own over their own work range.
+template <bool Wide>
 __global__ void __launch_bounds__(256) gray_images_kernel(const GraySrc* __restrict__ src, const uint64_t* __restrict__ first, int nsrc, uint64_t total) {
   for (uint64_t q = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; q < total; q += (uint64_t)gridDim.x * blockDim.x) {
     int lo = 0, hi = nsrc - 1;
@@ -152,10 +245,12 @@ __global__ void __launch_bounds__(256) gray_images_kernel(const GraySrc* __restr
     const unsigned local = (unsigned)(q - __ldg(first + lo));   // < width * height < 2^31
     const int row = (int)(local / chunks), x0 = (int)(local - (unsigned)row * chunks) * 16;
     const int n = min(16, width - x0);
-    const uint8_t* p = s.plane[0] + (size_t)row * s.stride0 + (size_t)x0 * (format == PIGO_DECODED_NRGBA || format == PIGO_DECODED_RGBA ? 4 : 1);
+    const uint8_t* p = s.plane[0] + (size_t)row * s.stride0 + (size_t)x0 * (Wide ? decoded_bpp(format) : format == PIGO_DECODED_NRGBA || format == PIGO_DECODED_RGBA ? 4 : 1);
     const bool vec = n == 16 && ((uintptr_t)p & 15) == 0;
     uint32_t w[4] = {0, 0, 0, 0};
-    if (format == PIGO_DECODED_GRAY) {
+    if (Wide) {
+      wide_chunk(s, p, n, vec, w);
+    } else if (format == PIGO_DECODED_GRAY) {
       if (vec) {
         const uint4 v = __ldg(reinterpret_cast<const uint4*>(p));
         w[0] = v.x; w[1] = v.y; w[2] = v.z; w[3] = v.w;
@@ -203,9 +298,11 @@ __global__ void __launch_bounds__(256) gray_images_kernel(const GraySrc* __restr
   }
 }
 
-void launch_gray_images(const GraySrc* src, const uint64_t* first, int nsrc, uint64_t total, int grid, cudaStream_t st) {
+void launch_gray_images(const GraySrc* src, const uint64_t* first, int nsrc, uint64_t total, bool wide, int grid, cudaStream_t st) {
   const uint64_t want = (total + 255) / 256;
-  gray_images_kernel<<<(int)std::max<uint64_t>(1, std::min<uint64_t>(want, (uint64_t)grid)), 256, 0, st>>>(src, first, nsrc, total);
+  const int blocks = (int)std::max<uint64_t>(1, std::min<uint64_t>(want, (uint64_t)grid));
+  if (wide) gray_images_kernel<true><<<blocks, 256, 0, st>>>(src, first, nsrc, total);
+  else gray_images_kernel<false><<<blocks, 256, 0, st>>>(src, first, nsrc, total);
 }
 
 }  // namespace pigo

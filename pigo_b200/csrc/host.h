@@ -146,6 +146,19 @@ struct GraySrc {
   int32_t format, sub, min_x, min_y, width, height, stride0, stride1;
 };
 
+// The formats gray_images_kernel<true> converts: Gray16, RGBA64, NRGBA64, CMYK and Paletted.
+__host__ __device__ __forceinline__ bool decoded_wide(int format) { return format >= PIGO_DECODED_GRAY16; }
+
+// Bytes per pixel of plane 0 of a pigo_decoded format.
+__host__ __device__ __forceinline__ int decoded_bpp(int format) {
+  switch (format) {
+    case PIGO_DECODED_NRGBA: case PIGO_DECODED_RGBA: case PIGO_DECODED_CMYK: return 4;
+    case PIGO_DECODED_RGBA64: case PIGO_DECODED_NRGBA64: return 8;
+    case PIGO_DECODED_GRAY16: return 2;
+    default: return 1;
+  }
+}
+
 // ---- workspace -----------------------------------------------------------------------------------------
 struct DevBuf {
   void* p = nullptr;
@@ -324,7 +337,8 @@ void launch_ptab_build(const FaceTables& T, const ScaleEntry* plan, const TiledA
 void launch_gray(const uint8_t* rgba, size_t npix, uint8_t* gray, int grid, cudaStream_t st);
 void launch_ycbcr(const uint8_t* y, const uint8_t* cb, const uint8_t* cr, int y_stride, int c_stride, int subsample, int min_x, int min_y,
                   int width, int height, uint8_t* nrgba, uint8_t* gray, int grid, cudaStream_t st);
-void launch_gray_images(const GraySrc* src, const uint64_t* first, int nsrc, uint64_t total, int grid, cudaStream_t st);
+// wide: the sources are all Gray16, RGBA64, NRGBA64, CMYK or Paletted (else all YCbCr, NRGBA, RGBA or Gray).
+void launch_gray_images(const GraySrc* src, const uint64_t* first, int nsrc, uint64_t total, bool wide, int grid, cudaStream_t st);
 void launch_scan_gather2(const TiledArgs& A, int grid, size_t smem, cudaStream_t st);
 int gather2_ctas_per_sm(size_t smem, int ng, bool rot, bool img = false);
 void launch_rot_table(const FaceTables& T, const ScaleEntry* plan, int nscales, int slot, RotNode* out, int grid, cudaStream_t st);

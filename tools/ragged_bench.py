@@ -21,6 +21,9 @@ Usage: `python tools/ragged_bench.py [--frames 256]` on one GPU prints one JSON 
               to the host, then one pigo_detect_images from host gray; (c) per image pigo_ycbcr_to_nrgba (NRGBA) +
               pigo_rgba_to_gray, then one pigo_detect_images.  Also pigo_gray_images alone from device-resident planes
               (CUDA events) and from pinned host planes (host clock).
+  formats : the same 256 images as NRGBA, Gray16, RGBA64, NRGBA64, CMYK and Paletted sources whose gray is exactly the
+              image, detections asserted equal: pigo_gray_images alone (device and pinned planes) and with
+              pigo_detect_images end to end (formats_bench)
 `--sections scan,pipeline` (the default) selects the sections; `--sections angles` runs the sweeps alone.  Writes nothing
 to the tree.
 """
@@ -612,11 +615,144 @@ def decoded_bench(clf, dev: int, stream) -> dict:
     return res
 
 
+FORMATS = {"nrgba": (1, 4), "gray16": (5, 2), "rgba64": (6, 8), "nrgba64": (7, 8), "cmyk": (8, 4), "paletted": (9, 1)}   # code, bytes/px
+
+
+def encode_gray(fmt: str, b: np.ndarray, noise: np.ndarray, inv: np.ndarray, out: np.ndarray) -> None:
+    """Writes into out [rows][dim * bytes/px] the Pix rows of gray image b [rows][dim] in format fmt such that
+    RgbToGrayscale(ImgToNRGBA(img)) is b: NRGBA opaque (g, g, g); Gray16 g<<8 | noise; RGBA64 and NRGBA64 opaque with each
+    channel g<<8 | noise; CMYK (0, 0, 0, 255-g); Paletted the index inv[g] of a permuted gray palette."""
+    r, d = b.shape
+    bpp = FORMATS[fmt][1]
+    px = out.reshape(r, d, bpp)
+    if fmt == "nrgba":
+        px[..., :3] = b[..., None]
+        px[..., 3] = 255
+    elif fmt == "gray16":
+        px[..., 0], px[..., 1] = b, noise
+    elif fmt in ("rgba64", "nrgba64"):
+        px[..., 0:6:2] = b[..., None]
+        px[..., 1:6:2] = noise[..., None]
+        px[..., 6:] = 255
+    elif fmt == "cmyk":
+        px[..., :3] = 0
+        px[..., 3] = 255 - b
+    else:
+        px[..., 0] = inv[b]
+
+
+def formats_bench(clf, dev: int, stream) -> dict:
+    """The 256 ragged images encoded in each format pigo_gray_images takes beyond YCbCr and Gray, each such that its gray
+    is exactly the image (encode_gray): detections asserted equal to those of the plain gray images; pigo_gray_images alone
+    from device-resident planes (CUDA events) and from pinned host planes (host clock), and pigo_gray_images +
+    pigo_detect_images end to end from pinned planes (host clock), medians of 5.  NRGBA is what a caller converting on
+    the CPU first (the Go shim's ImgToNRGBA for these types) sends; that CPU pass itself is not measured here."""
+    import ctypes as C
+    import torch
+    import pigo_b200
+    from pigo_b200 import DecodedImage, pipeline
+    L = pigo_b200.lib()
+    st = C.c_void_p(stream.cuda_stream)
+    cuda = f"cuda:{dev}"
+    plc = pigo_b200.NewPuplocCascade().UnpackCascade(pigo_b200.load_cascade("puploc"))
+    names = sorted(set(pipeline.EYE_CASCADES + pipeline.MOUTH_CASCADES))
+    flp = {nm: pigo_b200.NewPuplocCascade().UnpackCascade(pigo_b200.load_cascade("lps/" + nm)) for nm in names}
+    hs, fl = pipeline.landmark_call_arrays(flp)
+    ncalls, face_cap = len(fl), 128
+    prm = pigo_b200.PipelineParams(*PARAMS, 0.0, 0.1, 50, 50, 63, 4096)
+    imgs = ragged_images()
+    n = len(imgs)
+    gray_px = sum(r * c for _, r, c, _ in imgs)
+
+    def check(rc):
+        if rc != 0:
+            raise RuntimeError(L.pigo_last_error().decode())
+
+    def outputs():
+        return (np.zeros((n, face_cap), dtype=pigo_b200.DET_DTYPE), np.zeros(n, dtype=np.int32),
+                np.zeros((n, face_cap, 2 + ncalls), dtype=pigo_b200.POINT_DTYPE))
+
+    def detect(descs, flags, o):
+        check(L.pigo_detect_images(clf._h, plc._h, hs, fl.ctypes.data, ncalls, descs, n, C.byref(prm), None, 7, o[0].ctypes.data, face_cap,
+                                   o[1].ctypes.data, o[2].ctypes.data, flags, st))
+
+    def host_ms(fn, reps=5):
+        fn()
+        ts = []
+        for _ in range(reps):
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            fn()
+            torch.cuda.synchronize()
+            ts.append(time.perf_counter() - t0)
+        return 1e3 * float(np.median(ts))
+
+    gray = [np.ascontiguousarray(b[:, :c]) for b, _, c, _ in imgs]
+    ref = outputs()
+    detect(pigo_b200.image_descs([(g.ctypes.data, r, c, c) for g, (_, r, c, _) in zip(gray, imgs)]), pigo_b200.MEM_HOST, ref)
+    rng = np.random.default_rng(78)
+    perm = rng.permutation(256)
+    palette = torch.from_numpy(np.stack([perm, perm, perm, np.full(256, 255)], axis=-1).astype(np.uint8)).pin_memory()
+    inv = np.argsort(perm).astype(np.uint8)
+    res = {}
+    for fmt, (code, bpp) in FORMATS.items():
+        pinned = []
+        for b, r, c, d in imgs:
+            t = torch.empty((r, d * bpp), dtype=torch.uint8, pin_memory=True)
+            encode_gray(fmt, b, rng.integers(0, 256, size=(r, d), dtype=np.uint8), inv, t.numpy())
+            pinned.append(t)
+        dev_planes = [t.to(cuda) for t in pinned]
+        d_palette = palette.to(cuda)
+
+        def src(planes, pal):
+            return [DecodedImage(code, c, r, (p, pal) if fmt == "paletted" else (p,), (d * bpp, len(pal) if fmt == "paletted" else 0))
+                    for p, (_, r, c, d) in zip(planes, imgs)]
+        host_descs, dev_descs = pigo_b200.decoded_descs(src(pinned, palette)), pigo_b200.decoded_descs(src(dev_planes, d_palette))
+        need = pigo_b200.gray_images_bytes(src(pinned, palette))
+        arena = torch.empty(need, dtype=torch.uint8, device=cuda)
+        out_imgs = (pigo_b200.PigoImage * n)()
+        size = C.c_size_t(need)
+
+        def convert(descs, flags):
+            check(L.pigo_gray_images(descs, n, arena.data_ptr(), C.byref(size), out_imgs, flags, st))
+
+        o = outputs()
+
+        def e2e():
+            convert(host_descs, pigo_b200.MEM_HOST)
+            detect(out_imgs, pigo_b200.FRAMES_DEVICE, o)
+        row = {"e2e_ms": round(host_ms(e2e), 3)}
+        assert all(x.tobytes() == y.tobytes() for x, y in zip(o, ref)), f"{fmt}: detections differ from the gray images'"
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
+        ks = []
+        for _ in range(6):
+            ev[0].record(stream)
+            convert(dev_descs, pigo_b200.FRAMES_DEVICE)
+            ev[1].record(stream)
+            ev[1].synchronize()
+            ks.append(ev[0].elapsed_time(ev[1]))
+        k_ms = float(np.median(ks[1:]))
+        src_bytes = gray_px * bpp + (1024 if fmt == "paletted" else 0)
+        row["gray_images_device_ms"] = round(k_ms, 4)
+        row["gray_images_device_tb_s"] = round((src_bytes + gray_px) / (k_ms * 1e-3) / 1e12, 3)
+        row["gray_images_device_of_3_35_tb_s"] = round((src_bytes + gray_px) / (k_ms * 1e-3) / 3.35e12, 3)
+        p_ms = host_ms(lambda: convert(host_descs, pigo_b200.MEM_HOST))
+        row["gray_images_pinned_ms"] = round(p_ms, 3)
+        row["gray_images_pinned_source_gb_s"] = round(src_bytes / (p_ms * 1e-3) / 1e9, 2)
+        row["source_bytes"] = src_bytes
+        res[fmt] = row
+        del pinned, dev_planes, arena
+        torch.cuda.empty_cache()
+    res["faces"], res["gray_pixels"], res["images"] = int(ref[1].sum()), gray_px, n
+    res["go_cpu_pass"] = "not measured"
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--frames", type=int, default=256, help="frames of the uniform 1080p comparison")
     ap.add_argument("--pipeline-frames", type=int, default=64, help="frames of the uniform 1080p pipeline comparison")
-    ap.add_argument("--sections", default="scan,pipeline", help="comma-separated: scan, pipeline, angles, decoded")
+    ap.add_argument("--sections", default="scan,pipeline", help="comma-separated: scan, pipeline, angles, decoded, formats")
     args = ap.parse_args()
     sections = set(args.sections.split(","))
     import torch
@@ -633,6 +769,8 @@ def main():
         res["angles"] = angles_bench(clf, 0, stream)
     if "decoded" in sections:
         res["decoded"] = decoded_bench(clf, 0, stream)
+    if "formats" in sections:
+        res["formats"] = formats_bench(clf, 0, stream)
     res["gpu"] = torch.cuda.get_device_name(0)
     try:   # read-only query: the power limit belongs beside the numbers
         import subprocess

@@ -173,7 +173,7 @@ def angles_case(clf, sample):
 
 def decoded_case():
     """pigo_gray_images over every decoded format (odd sizes and origins, padded strides, 16-byte aligned and unaligned rows,
-    one repeated source) from host planes into a device arena, and again from device planes."""
+    a short palette, one repeated source) from host planes into a device arena, and again from device planes."""
     import ctypes as C
     rng = np.random.default_rng(6)
     y, cb, cr = (rng.integers(0, 256, size=(21, 43), dtype=np.uint8) for _ in range(3))
@@ -182,6 +182,11 @@ def decoded_case():
     src = [pigo_b200.DecodedImage.ycbcr(y, cb, cr, sub, 37, 20, min_x=1, min_y=1) for sub in range(6)]
     src += [pigo_b200.DecodedImage.nrgba(px, 40, 9), pigo_b200.DecodedImage.rgba(px, 33, 9), pigo_b200.DecodedImage.gray(g, 32, 5),
             pigo_b200.DecodedImage.gray(g, 35, 5), pigo_b200.DecodedImage.gray(g, 1, 1)]
+    pal = rng.integers(0, 256, size=(7, 4), dtype=np.uint8)   # indices past it give 0
+    flat = px.reshape(-1)
+    src += [pigo_b200.DecodedImage.gray16(px, 82, 9), pigo_b200.DecodedImage.gray16(flat[3:], 75, 9, stride=164),
+            pigo_b200.DecodedImage.rgba64(px, 20, 9), pigo_b200.DecodedImage.nrgba64(flat[5:], 19, 9, stride=164),
+            pigo_b200.DecodedImage.cmyk(px, 40, 9), pigo_b200.DecodedImage.paletted(g, pal, 35, 5)]
     src.append(src[2])
     need = pigo_b200.gray_images_bytes(src)
     L = pigo_b200.lib()
