@@ -240,19 +240,41 @@ func (pg *Pigo) RunCascadeDecoded(imgs []image.Image, cp CascadeParams, angles [
 	}
 }
 
+// RunCascadeDecodedSharded is RunCascadeDecoded over the GPUs of InitDevices (pigo_run_cascade_decoded_sharded): the
+// images, packed once to pinned memory in their own pixel format, are cut into contiguous shards of about equal modelled
+// cost, and each device copies, converts and scans its own shard.  The result equals RunCascadeDecoded's.
+func (pg *Pigo) RunCascadeDecodedSharded(imgs []image.Image, cp CascadeParams, angles []float64) [][]Detection {
+	n := len(imgs)
+	angles = decodedAngles("RunCascadeDecodedSharded", angles, n)
+	if n == 0 {
+		return nil
+	}
+	desc, free := packDecoded(imgs)
+	defer free()
+	return runCapped(n, func(buf *C.pigo_det, capacity C.int, cnt *C.int) C.int {
+		return C.pigo_run_cascade_decoded_sharded(pg.h, &desc[0], C.int(n), anglesPtr(angles), C.int(cp.MinSize), C.int(cp.MaxSize),
+			C.double(cp.ShiftFactor), C.double(cp.ScaleFactor), buf, capacity, cnt)
+	})
+}
+
 // DetectDecoded is DetectImagesAngles on RgbToGrayscale(ImgToNRGBA(img)) of every decoded image: one conversion into device
 // memory, then the whole face -> pupils -> landmarks sequence there.  angles is nil (every image at 0) or has one entry per
-// image; pp.Angle is not used.  There is no sharded form: pp.Sharded panics.
+// image; pp.Angle is not used.  With pp.Sharded the packed images are spread over the GPUs of InitDevices
+// (pigo_detect_decoded_sharded): each device copies, converts and runs its own shard, with the same result.
 func (pg *Pigo) DetectDecoded(plc *PuplocCascade, calls []LandmarkCall, imgs []image.Image, cp CascadeParams, pp PipelineParams, angles []float64) [][]FaceResult {
-	if pp.Sharded {
-		panic("pigo: DetectDecoded has no sharded form")
-	}
 	n := len(imgs)
 	angles = decodedAngles("DetectDecoded", angles, n)
 	if n == 0 {
 		return nil
 	}
-	images, free := grayDecoded(imgs)
+	var images []C.pigo_image
+	var desc []C.pigo_decoded
+	var free func()
+	if pp.Sharded {
+		desc, free = packDecoded(imgs) // the host planes, read by the call
+	} else {
+		images, free = grayDecoded(imgs)
+	}
 	defer free()
 	ncalls := len(calls)
 	hs, fl := callArrays(calls)
@@ -267,6 +289,10 @@ func (pg *Pigo) DetectDecoded(plc *PuplocCascade, calls []LandmarkCall, imgs []i
 		nfaces := make([]C.int, n)
 		points := make([]C.pigo_point, n*faceCap*(2+ncalls))
 		rc, err := call(func() C.int {
+			if pp.Sharded {
+				return C.pigo_detect_decoded_sharded(pg.h, plc.h, hs, &fl[0], C.int(ncalls), &desc[0], C.int(n), (*C.double)(unsafe.Pointer(&angles[0])),
+					&prm, nil, C.uint64_t(key), &faces[0], C.int(faceCap), &nfaces[0], &points[0])
+			}
 			return C.pigo_detect_images_angles(pg.h, plc.h, hs, &fl[0], C.int(ncalls), &images[0], C.int(n), (*C.double)(unsafe.Pointer(&angles[0])),
 				&prm, nil, C.uint64_t(key), &faces[0], C.int(faceCap), &nfaces[0], &points[0], C.PIGO_FRAMES_DEVICE, nil)
 		})

@@ -352,6 +352,60 @@ func (pg *Pigo) RunCascadeImagesAngles(images []ImageParams, cp CascadeParams, a
 	}
 }
 
+// RunCascadeImagesSharded is RunCascadeImagesAngles over the GPUs of InitDevices (pigo_run_cascade_images_sharded): the
+// images are cut into contiguous shards of about equal modelled cost, one per device, and the result equals the single-GPU
+// call's.  angles is nil (every image at 0) or has one entry per image; any other length panics.
+func (pg *Pigo) RunCascadeImagesSharded(images []ImageParams, cp CascadeParams, angles []float64) [][]Detection {
+	n := len(images)
+	if angles != nil && len(angles) != n {
+		panic("pigo: RunCascadeImagesSharded needs nil angles or one angle per image")
+	}
+	if n == 0 {
+		return nil
+	}
+	desc, free := packImages(images)
+	defer free()
+	return runCapped(n, func(buf *C.pigo_det, capacity C.int, cnt *C.int) C.int {
+		return C.pigo_run_cascade_images_sharded(pg.h, &desc[0], C.int(n), anglesPtr(angles), C.int(cp.MinSize), C.int(cp.MaxSize),
+			C.double(cp.ShiftFactor), C.double(cp.ScaleFactor), buf, capacity, cnt)
+	})
+}
+
+// anglesPtr is the C view of angles (nil stays NULL).
+func anglesPtr(angles []float64) *C.double {
+	if len(angles) == 0 {
+		return nil
+	}
+	return (*C.double)(unsafe.Pointer(&angles[0]))
+}
+
+// runCapped calls f(out [n][capacity], capacity, counts [n]) until the capacity is enough (PIGO_E_CAP retries with the
+// largest reported count) and returns the detections of every entry.
+func runCapped(n int, f func(buf *C.pigo_det, capacity C.int, cnt *C.int) C.int) [][]Detection {
+	capacity := 1024
+	for {
+		buf := make([]C.pigo_det, capacity*n)
+		cnt := make([]C.int, n)
+		rc, err := call(func() C.int { return f(&buf[0], C.int(capacity), &cnt[0]) })
+		if rc == C.PIGO_E_CAP {
+			for _, c := range cnt {
+				if int(c) > capacity {
+					capacity = int(c)
+				}
+			}
+			continue
+		}
+		if err != nil {
+			panic(err)
+		}
+		out := make([][]Detection, n)
+		for i := range out {
+			out[i] = toGo(buf[i*capacity:(i+1)*capacity], int(cnt[i]))
+		}
+		return out
+	}
+}
+
 // ClusterDetections mirrors core/pigo.go:262-308, including the in-place sort of the caller's slice by Q.
 func (pg *Pigo) ClusterDetections(detections []Detection, iouThreshold float64) []Detection {
 	n := len(detections)

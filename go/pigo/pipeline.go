@@ -146,11 +146,9 @@ func faceResults(faces []C.pigo_det, nfaces []C.int, points []C.pigo_point, face
 
 // DetectImages runs the whole sequence for images of different sizes in one call (pigo_detect_images); result[i] lists
 // image i's clusters in the reference's order.  cp's MinSize, MaxSize, ShiftFactor and ScaleFactor are shared by every image
-// (cp's own ImageParams is not used).  There is no sharded mixed-size form: pp.Sharded panics.
+// (cp's own ImageParams is not used).  With pp.Sharded the images are spread over the GPUs of InitDevices
+// (pigo_detect_images_sharded) in contiguous shards of about equal modelled cost; the result is the same.
 func (pg *Pigo) DetectImages(plc *PuplocCascade, calls []LandmarkCall, images []ImageParams, cp CascadeParams, pp PipelineParams) [][]FaceResult {
-	if pp.Sharded {
-		panic("pigo: DetectImages has no sharded form; use DetectBatch with Sharded for frames of one geometry")
-	}
 	n := len(images)
 	if n == 0 {
 		return nil
@@ -188,6 +186,10 @@ func (pg *Pigo) DetectImages(plc *PuplocCascade, calls []LandmarkCall, images []
 		nfaces := make([]C.int, n)
 		points := make([]C.pigo_point, n*faceCap*(2+ncalls))
 		rc, err := call(func() C.int {
+			if pp.Sharded {
+				return C.pigo_detect_images_sharded(pg.h, plc.h, hs, &fl[0], C.int(ncalls), &desc[0], C.int(n), nil, &prm, nil, C.uint64_t(key),
+					&faces[0], C.int(faceCap), &nfaces[0], &points[0])
+			}
 			return C.pigo_detect_images(pg.h, plc.h, hs, &fl[0], C.int(ncalls), &desc[0], C.int(n), &prm, nil, C.uint64_t(key), &faces[0],
 				C.int(faceCap), &nfaces[0], &points[0], C.PIGO_MEM_HOST, nil)
 		})
@@ -212,11 +214,9 @@ func (pg *Pigo) DetectImages(plc *PuplocCascade, calls []LandmarkCall, images []
 
 // DetectImagesAngles is DetectImages with image i scanned and its eyes refined at angles[i] (pigo_detect_images_angles);
 // pp.Angle is not used and the landmark calls stay at angle 0, as GetLandmarkPoint does.  A pixel slice listed several
-// times (an angle sweep) is copied once.  It panics unless there is one angle per image, and on pp.Sharded.
+// times (an angle sweep) is copied once (once per device with pp.Sharded, which spreads the images over the GPUs of
+// InitDevices like DetectImages).  It panics unless there is one angle per image.
 func (pg *Pigo) DetectImagesAngles(plc *PuplocCascade, calls []LandmarkCall, images []ImageParams, cp CascadeParams, pp PipelineParams, angles []float64) [][]FaceResult {
-	if pp.Sharded {
-		panic("pigo: DetectImagesAngles has no sharded form")
-	}
 	if len(angles) != len(images) {
 		panic("pigo: DetectImagesAngles needs one angle per image")
 	}
@@ -239,6 +239,10 @@ func (pg *Pigo) DetectImagesAngles(plc *PuplocCascade, calls []LandmarkCall, ima
 		nfaces := make([]C.int, n)
 		points := make([]C.pigo_point, n*faceCap*(2+ncalls))
 		rc, err := call(func() C.int {
+			if pp.Sharded {
+				return C.pigo_detect_images_sharded(pg.h, plc.h, hs, &fl[0], C.int(ncalls), &desc[0], C.int(n), (*C.double)(unsafe.Pointer(&angles[0])),
+					&prm, nil, C.uint64_t(key), &faces[0], C.int(faceCap), &nfaces[0], &points[0])
+			}
 			return C.pigo_detect_images_angles(pg.h, plc.h, hs, &fl[0], C.int(ncalls), &desc[0], C.int(n), (*C.double)(unsafe.Pointer(&angles[0])),
 				&prm, nil, C.uint64_t(key), &faces[0], C.int(faceCap), &nfaces[0], &points[0], C.PIGO_MEM_HOST, nil)
 		})

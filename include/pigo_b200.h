@@ -352,6 +352,44 @@ typedef struct {
 int pigo_gray_images(const pigo_decoded *src, int n, uint8_t *gray, size_t *gray_bytes, pigo_image *images, unsigned flags,
                      void *stream);
 
+/* ---- Multi-GPU forms of the mixed-size and decoded calls: HOST inputs and HOST outputs, over the devices of
+ * pigo_init_devices (the default device if none were selected), one host thread per shard, no data-path collective.
+ * The entries are cut into contiguous ranges of the caller's order (an entry is never split) that balance a modelled
+ * cost, count_windows x (rotated ? 1.4 : 1) + 4096 per entry, not the entry count (pigo_shard_plan); shard s writes its
+ * entries' slices of the output arrays.  For any split, entry i's slices are byte for byte what the single-device call
+ * returns:
+ *   pigo_run_cascade_images_sharded  = pigo_run_cascade_images_angles (pigo_run_cascade_images at angle 0 when angles is NULL)
+ *   pigo_detect_images_sharded       = pigo_detect_images_angles (angles NULL: params->angle for every image), with the same
+ *                                      randoms ([nimages][face_cap][2+ncalls][63][3]) or the same rng_seed: a shard that
+ *                                      starts at image lo keys its generator and reads its randoms as image lo of the call
+ *   pigo_*_decoded_sharded           = pigo_gray_images of the sources, then the matching call above on its images; each
+ *                                      device copies and converts its own sources (repeats within a shard share a slot)
+ * Host images listed several times in a shard are copied to that shard's device once.  Argument checks are those of the
+ * single-device calls (the decoded forms: pigo_gray_images' checks first) and need no device.  PIGO_E_CAP: the first
+ * other error of a shard wins; otherwise, after every shard ran, every n_out[i] / n_faces[i] holds the required count.
+ * Developer option "shard_split" = k > 0 cuts these calls into k shards, shard s on the (s mod G)-th device. */
+int pigo_run_cascade_images_sharded(const pigo_cascade *c, const pigo_image *images, int nimages, const double *angles,
+                                    int min_size, int max_size, double shift_factor, double scale_factor, pigo_det *out,
+                                    int cap_per_image, int *n_out);
+int pigo_detect_images_sharded(const pigo_cascade *face, const pigo_puploc *puploc, const pigo_puploc *const *flp,
+                               const uint8_t *flp_flip, int ncalls, const pigo_image *images, int nimages,
+                               const double *angles, const pigo_pipeline_params *params, const float *randoms,
+                               uint64_t rng_seed, pigo_det *faces, int face_cap, int *n_faces, pigo_point *points);
+int pigo_run_cascade_decoded_sharded(const pigo_cascade *c, const pigo_decoded *src, int n, const double *angles,
+                                     int min_size, int max_size, double shift_factor, double scale_factor, pigo_det *out,
+                                     int cap_per_image, int *n_out);
+int pigo_detect_decoded_sharded(const pigo_cascade *face, const pigo_puploc *puploc, const pigo_puploc *const *flp,
+                                const uint8_t *flp_flip, int ncalls, const pigo_decoded *src, int n, const double *angles,
+                                const pigo_pipeline_params *params, const float *randoms, uint64_t rng_seed, pigo_det *faces,
+                                int face_cap, int *n_faces, pigo_point *points);
+/* The split the four calls above make (no device needed): first[0..n_used] are the shards' first entries, first[n_used] ==
+ * nimages, n_used = min(shards, nimages) non-empty shards.  The largest shard's cost is the least any contiguous split
+ * into that many shards reaches.  nshards = 0: the count the calls use (option shard_split, else one per selected
+ * device); `first` may be NULL (n_used only) and otherwise holds n_used + 1 entries (nimages + 1 always suffice).
+ * `angles` NULL: every entry unrotated.  Images are checked as in pigo_run_cascade_images; pixels are not read. */
+int pigo_shard_plan(const pigo_image *images, int nimages, const double *angles, int min_size, int max_size,
+                    double shift_factor, double scale_factor, int nshards, int *first, int *n_used);
+
 /* ---- tuning / introspection (not part of the reference surface) ------------------------- */
 /* Process-global developer knobs (kernel variants, group sizes, per-kernel timing): debugging and
  * benchmarking only, NOT per handle -- set them before the first compute call and leave them alone while

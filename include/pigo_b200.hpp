@@ -111,6 +111,20 @@ class Pigo {                    // core/pigo.go:37-43
   std::vector<std::vector<Detection>> RunCascadeImagesAngles(const std::vector<ImageParams>& images, const CascadeParams& cp,
                                                              const std::vector<double>& angles) const {
     if (angles.size() != images.size()) throw std::invalid_argument("RunCascadeImagesAngles needs one angle per image");
+    return runImages(images, cp, angles, false);
+  }
+  // additive: RunCascadeImagesAngles over the GPUs of InitDevices (host pixels, contiguous shards of about equal modelled
+  // cost); the result equals the single-GPU call's
+  std::vector<std::vector<Detection>> RunCascadeImagesSharded(const std::vector<ImageParams>& images, const CascadeParams& cp,
+                                                              const std::vector<double>& angles) const {
+    if (angles.size() != images.size()) throw std::invalid_argument("RunCascadeImagesSharded needs one angle per image");
+    return runImages(images, cp, angles, true);
+  }
+  const pigo_cascade* handle() const { return h_.get(); }
+
+ private:
+  std::vector<std::vector<Detection>> runImages(const std::vector<ImageParams>& images, const CascadeParams& cp, const std::vector<double>& angles,
+                                                bool sharded) const {
     const int n = (int)images.size();
     std::vector<pigo_image> desc((size_t)n);
     for (int i = 0; i < n; ++i) desc[i] = pigo_image{images[i].Pixels, images[i].Rows, images[i].Cols, images[i].Dim};
@@ -118,8 +132,10 @@ class Pigo {                    // core/pigo.go:37-43
     for (;;) {
       std::vector<pigo_det> buf((size_t)cap * (n > 0 ? n : 1));
       std::vector<int> cnt((size_t)(n > 0 ? n : 1));
-      const int rc = pigo_run_cascade_images_angles(h_.get(), desc.data(), n, angles.data(), cp.MinSize, cp.MaxSize, cp.ShiftFactor, cp.ScaleFactor,
-                                                    buf.data(), cap, cnt.data(), PIGO_MEM_HOST, nullptr);
+      const int rc = sharded ? pigo_run_cascade_images_sharded(h_.get(), desc.data(), n, angles.data(), cp.MinSize, cp.MaxSize, cp.ShiftFactor,
+                                                               cp.ScaleFactor, buf.data(), cap, cnt.data())
+                             : pigo_run_cascade_images_angles(h_.get(), desc.data(), n, angles.data(), cp.MinSize, cp.MaxSize, cp.ShiftFactor,
+                                                              cp.ScaleFactor, buf.data(), cap, cnt.data(), PIGO_MEM_HOST, nullptr);
       if (rc == PIGO_E_CAP) { for (int c : cnt) cap = c > cap ? c : cap; continue; }
       check(rc);
       std::vector<std::vector<Detection>> out((size_t)n);
@@ -128,9 +144,6 @@ class Pigo {                    // core/pigo.go:37-43
       return out;
     }
   }
-  const pigo_cascade* handle() const { return h_.get(); }
-
- private:
   std::shared_ptr<pigo_cascade> h_;
 };
 inline Pigo NewPigo() { return Pigo(); }   // core/pigo.go:46
@@ -217,15 +230,12 @@ inline std::vector<std::vector<FaceResult>> DetectBatch(const Pigo& face, const 
     }
   return out;
 }
-// additive: DetectImages with image i scanned and its eyes refined at angles[i] (one angle per image; the landmark calls stay
-// at angle 0).  result[i] lists image i's clusters; on PIGO_E_CAP the call is retried with the reported face count (or a
-// larger det_cap).
-inline std::vector<std::vector<FaceResult>> DetectImagesAngles(const Pigo& face, const PuplocCascade& plc,
-                                                               const std::vector<std::pair<const PuplocCascade*, bool>>& calls,
-                                                               const std::vector<ImageParams>& images, const CascadeParams& cp, double iou,
-                                                               int min_face_scale, int eye_perturbs, int flp_perturbs, uint64_t rng_seed,
-                                                               const std::vector<double>& angles, int face_cap = 32) {
-  if (angles.size() != images.size()) throw std::invalid_argument("DetectImagesAngles needs one angle per image");
+namespace detail {
+inline std::vector<std::vector<FaceResult>> detectImages(const Pigo& face, const PuplocCascade& plc,
+                                                         const std::vector<std::pair<const PuplocCascade*, bool>>& calls,
+                                                         const std::vector<ImageParams>& images, const CascadeParams& cp, double iou,
+                                                         int min_face_scale, int eye_perturbs, int flp_perturbs, uint64_t rng_seed,
+                                                         const std::vector<double>& angles, int face_cap, bool sharded) {
   const int ncalls = (int)calls.size(), n = (int)images.size();
   std::vector<const pigo_puploc*> hs;
   std::vector<uint8_t> fl;
@@ -239,8 +249,10 @@ inline std::vector<std::vector<FaceResult>> DetectImagesAngles(const Pigo& face,
     std::vector<pigo_det> faces((size_t)(n > 0 ? n : 1) * face_cap);
     std::vector<int> nfaces((size_t)(n > 0 ? n : 1));
     std::vector<pigo_point> pts((size_t)(n > 0 ? n : 1) * face_cap * (2 + ncalls));
-    const int rc = pigo_detect_images_angles(face.handle(), plc.handle(), hs.data(), fl.data(), ncalls, desc.data(), n, angles.data(), &prm, nullptr,
-                                             rng_seed, faces.data(), face_cap, nfaces.data(), pts.data(), PIGO_MEM_HOST, nullptr);
+    const int rc = sharded ? pigo_detect_images_sharded(face.handle(), plc.handle(), hs.data(), fl.data(), ncalls, desc.data(), n, angles.data(), &prm,
+                                                        nullptr, rng_seed, faces.data(), face_cap, nfaces.data(), pts.data())
+                           : pigo_detect_images_angles(face.handle(), plc.handle(), hs.data(), fl.data(), ncalls, desc.data(), n, angles.data(), &prm,
+                                                       nullptr, rng_seed, faces.data(), face_cap, nfaces.data(), pts.data(), PIGO_MEM_HOST, nullptr);
     if (rc == PIGO_E_CAP) {
       bool grown = false;
       for (int i = 0; i < n; ++i)
@@ -265,6 +277,29 @@ inline std::vector<std::vector<FaceResult>> DetectImagesAngles(const Pigo& face,
       }
     return out;
   }
+}
+}  // namespace detail
+
+// additive: DetectImages with image i scanned and its eyes refined at angles[i] (one angle per image; the landmark calls stay
+// at angle 0).  result[i] lists image i's clusters; on PIGO_E_CAP the call is retried with the reported face count (or a
+// larger det_cap).
+inline std::vector<std::vector<FaceResult>> DetectImagesAngles(const Pigo& face, const PuplocCascade& plc,
+                                                               const std::vector<std::pair<const PuplocCascade*, bool>>& calls,
+                                                               const std::vector<ImageParams>& images, const CascadeParams& cp, double iou,
+                                                               int min_face_scale, int eye_perturbs, int flp_perturbs, uint64_t rng_seed,
+                                                               const std::vector<double>& angles, int face_cap = 32) {
+  if (angles.size() != images.size()) throw std::invalid_argument("DetectImagesAngles needs one angle per image");
+  return detail::detectImages(face, plc, calls, images, cp, iou, min_face_scale, eye_perturbs, flp_perturbs, rng_seed, angles, face_cap, false);
+}
+// additive: DetectImagesAngles over the GPUs of InitDevices (host pixels, contiguous shards of about equal modelled cost); the
+// result, generator keys included, equals the single-GPU call's
+inline std::vector<std::vector<FaceResult>> DetectImagesSharded(const Pigo& face, const PuplocCascade& plc,
+                                                                const std::vector<std::pair<const PuplocCascade*, bool>>& calls,
+                                                                const std::vector<ImageParams>& images, const CascadeParams& cp, double iou,
+                                                                int min_face_scale, int eye_perturbs, int flp_perturbs, uint64_t rng_seed,
+                                                                const std::vector<double>& angles, int face_cap = 32) {
+  if (angles.size() != images.size()) throw std::invalid_argument("DetectImagesSharded needs one angle per image");
+  return detail::detectImages(face, plc, calls, images, cp, iou, min_face_scale, eye_perturbs, flp_perturbs, rng_seed, angles, face_cap, true);
 }
 // additive: DetectBatch for images of different sizes in one library call (host pixels; cp.Image is not used), every image at
 // `angle`.  result[i] lists image i's clusters; PIGO_E_CAP is retried as in DetectImagesAngles.

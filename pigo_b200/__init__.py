@@ -47,6 +47,8 @@ ABI_SYMBOLS = [
     "pigo_device_download", "pigo_run_cascade_batch_sharded", "pigo_detect_batch", "pigo_detect_batch_sharded",
     "pigo_ycbcr_to_nrgba", "pigo_run_cascade_images", "pigo_detect_images", "pigo_puploc_run_images",
     "pigo_run_cascade_images_angles", "pigo_detect_images_angles", "pigo_gray_images", "pigo_cascade_block_table",
+    "pigo_run_cascade_images_sharded", "pigo_detect_images_sharded", "pigo_run_cascade_decoded_sharded", "pigo_detect_decoded_sharded",
+    "pigo_shard_plan",
 ]
 
 
@@ -118,6 +120,11 @@ def lib() -> C.CDLL:
         L.pigo_get_option.argtypes = [C.c_char_p]
         L.pigo_get_option.restype = C.c_int64
         L.pigo_cascade_block_table.argtypes = [vp, vp, C.POINTER(sz)]
+        L.pigo_run_cascade_images_sharded.argtypes = [vp, vp, i, vp, i, i, d, d, vp, i, vp]
+        L.pigo_detect_images_sharded.argtypes = [vp, vp, vp, vp, i, vp, i, vp, vp, vp, u64, vp, i, vp, vp]
+        L.pigo_run_cascade_decoded_sharded.argtypes = [vp, vp, i, vp, i, i, d, d, vp, i, vp]
+        L.pigo_detect_decoded_sharded.argtypes = [vp, vp, vp, vp, i, vp, i, vp, vp, vp, u64, vp, i, vp, vp]
+        L.pigo_shard_plan.argtypes = [vp, i, vp, i, i, d, d, i, vp, C.POINTER(i)]
         _lib = L
     return _lib
 
@@ -230,6 +237,31 @@ def image_descs(items) -> C.Array:
     for k, (p, r, c, d) in enumerate(items):
         arr[k] = PigoImage(p, r, c, d)
     return arr
+
+
+def _angles_array(angles, n: int) -> Optional[np.ndarray]:
+    """float64 array of one angle per entry, or None."""
+    if angles is None:
+        return None
+    if len(angles) != n:
+        raise ValueError("angles must have one entry per image")
+    return np.ascontiguousarray(angles, dtype=np.float64)
+
+
+def shard_plan(images, min_size: int, max_size: int, shift_factor: float, scale_factor: float, angles: Optional[Sequence[float]] = None,
+               nshards: int = 0) -> List[int]:
+    """The split the sharded mixed-size calls make (pigo_shard_plan; no device needed): the first entry of every shard, then
+    len(images).  images: ImageParams or (pixels, rows, cols, dim) tuples (pixels are not read); nshards 0 = the count the
+    calls use (option shard_split, else one per selected device)."""
+    items = [(0, im.Rows, im.Cols, im.Dim) if isinstance(im, ImageParams) else (0, im[1], im[2], im[3]) for im in images]
+    n = len(items)
+    desc = image_descs(items)
+    ang = _angles_array(angles, n)
+    first = np.zeros(n + 1, dtype=np.int32)
+    used = C.c_int()
+    _check(lib().pigo_shard_plan(desc, n, ang.ctypes.data if ang is not None else None, min_size, max_size, shift_factor, scale_factor, nshards,
+                                 first.ctypes.data, C.byref(used)))
+    return first[:used.value + 1].tolist()
 
 
 def _pixels(img: ImageParams) -> np.ndarray:
@@ -399,6 +431,43 @@ class Pigo:
         ang = np.ascontiguousarray(angles, dtype=np.float64)
         _check(lib().pigo_run_cascade_images_angles(self._h, image_descs(images), len(images), ang.ctypes.data, min_size, max_size, shift, scale,
                                                     out_ptr, cap_per_image, counts_ptr, FRAMES_DEVICE | OUT_DEVICE, stream or None))
+
+    def run_cascade_images_sharded(self, images: Sequence[ImageParams], cp: CascadeParams, angles: Optional[Sequence[float]] = None,
+                                   cap_per_image: int = 1024):
+        """RunCascadeImagesAngles over the devices of init_devices (pigo_run_cascade_images_sharded): host images, cut into
+        contiguous shards of about equal modelled cost; angles None = every image at 0.  The result equals the single-device
+        call byte for byte.  Returns (dets[N, cap] DET_DTYPE, counts[N])."""
+        self._need()
+        n = len(images)
+        keep = [_pixels(im) for im in images]   # host pixels stay alive for the call
+        desc = image_descs([(p.ctypes.data, im.Rows, im.Cols, im.Dim) for im, p in zip(images, keep)])
+        ang = _angles_array(angles, n)
+        return self._retry_cap(n, cap_per_image, lambda out, cap, cnt: lib().pigo_run_cascade_images_sharded(
+            self._h, desc, n, ang.ctypes.data if ang is not None else None, cp.MinSize, cp.MaxSize, cp.ShiftFactor, cp.ScaleFactor, out, cap, cnt))
+
+    def run_cascade_decoded_sharded(self, sources: Sequence["DecodedImage"], cp: CascadeParams, angles: Optional[Sequence[float]] = None,
+                                    cap_per_image: int = 1024):
+        """gray_images of host DecodedImage sources, then RunCascadeImagesAngles, over the devices of init_devices
+        (pigo_run_cascade_decoded_sharded): each device converts its own shard.  Returns (dets[N, cap] DET_DTYPE, counts[N])."""
+        self._need()
+        n = len(sources)
+        desc = decoded_descs(sources)
+        ang = _angles_array(angles, n)
+        return self._retry_cap(n, cap_per_image, lambda out, cap, cnt: lib().pigo_run_cascade_decoded_sharded(
+            self._h, desc, n, ang.ctypes.data if ang is not None else None, cp.MinSize, cp.MaxSize, cp.ShiftFactor, cp.ScaleFactor, out, cap, cnt))
+
+    @staticmethod
+    def _retry_cap(n: int, cap: int, fn):
+        """Calls fn(out, cap, counts) until the output capacity is enough (PIGO_E_CAP retries with the reported count)."""
+        while True:
+            out = np.zeros((n, max(cap, 1)), dtype=DET_DTYPE)
+            cnt = np.zeros(max(n, 1), dtype=np.int32)
+            rc = fn(out.ctypes.data, cap, cnt.ctypes.data)
+            if rc == PIGO_E_CAP:
+                cap = int(cnt.max())
+                continue
+            _check(rc)
+            return out, cnt[:n]
 
     # -- ClusterDetections -----------------------------------------------------------------------------------
     def cluster_array(self, dets: np.ndarray, iou: float):

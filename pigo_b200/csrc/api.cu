@@ -104,6 +104,18 @@ static int ws_leave_async(Workspace* w, cudaStream_t st) {
   return PIGO_OK;
 }
 
+void raise_dyn_smem(const void* fn, int bytes) {
+  static std::mutex mu;
+  static std::map<std::pair<int, const void*>, int> granted;   // (device, kernel) -> the attribute's value
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) { cudaGetLastError(); return; }
+  std::lock_guard<std::mutex> g(mu);
+  int& cur = granted[{dev, fn}];
+  if (bytes <= cur) return;
+  if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes) == cudaSuccess) cur = bytes;
+  else cudaGetLastError();   // the launch that needs it fails and reports
+}
+
 int set_err(int code, const char* fmt, ...) {
   char buf[512];
   va_list ap;
@@ -799,37 +811,109 @@ static int scan_images_on(pigo_cascade* c, int dev, const pigo_image* images, in
   return copy_results_to_host(d_out, d_nout, cap, nimages, out, cap_per_image, n_out, st);
 }
 
-// Runs fn(shard index, device, first frame, frame count) on one host thread per device of the mask; frames are split
-// [g*ceil(N/G), (g+1)*ceil(N/G)) like SURVEY.md section 8e.  Returns the first error, PIGO_E_CAP last (so that every
-// shard's required counts are valid when the caller retries).
-template <typename F>
-static int for_each_shard(int nframes, F fn) {
+// The devices of the sharded calls: those of pigo_init_devices, or the default device.  Empty if there is none.
+static std::vector<int> sharded_devices() {
   std::vector<int> devs = shard_devices();
   if (devs.empty()) {
     const int d = default_device();
-    if (d < 0) return PIGO_E_NODEVICE;
-    devs.push_back(d);
+    if (d >= 0) devs.push_back(d);
   }
-  const int G = (int)devs.size();
-  const int per = (nframes + G - 1) / G;
-  std::vector<int> rcs(G, PIGO_OK);
-  std::vector<std::string> msgs(G);
+  return devs;
+}
+
+// Runs fn(shard index, device, first entry, entry count) for shard s = entries [first[s], first[s+1]) on devs[s % G], one
+// host thread per non-empty shard.  Returns the first error, PIGO_E_CAP last (so that every shard's required counts are
+// valid when the caller retries).
+template <typename F>
+static int for_each_shard(const std::vector<int>& devs, const std::vector<int>& first, F fn) {
+  const int S = (int)first.size() - 1, G = (int)devs.size();
+  std::vector<int> rcs(std::max(S, 0), PIGO_OK);
+  std::vector<std::string> msgs(std::max(S, 0));
   std::vector<std::thread> th;
-  for (int gidx = 0; gidx < G; ++gidx) {
-    const int lo = std::min(nframes, gidx * per), hi = std::min(nframes, lo + per);
+  for (int s = 0; s < S; ++s) {
+    const int lo = first[s], hi = first[s + 1];
     if (hi <= lo) continue;
-    th.emplace_back([&, gidx, lo, hi]() {
-      rcs[gidx] = fn(gidx, devs[gidx], lo, hi - lo);
-      if (rcs[gidx] != PIGO_OK) msgs[gidx] = g_err;   // g_err is thread-local: carry the worker's message back
+    th.emplace_back([&, s, lo, hi]() {
+      rcs[s] = fn(s, devs[s % G], lo, hi - lo);
+      if (rcs[s] != PIGO_OK) msgs[s] = g_err;   // g_err is thread-local: carry the worker's message back
     });
   }
   for (auto& t : th) t.join();
   int rc = PIGO_OK;
-  for (int gidx = 0; gidx < G; ++gidx) {
-    if (rcs[gidx] == PIGO_OK) continue;
-    if (rc == PIGO_OK || (rc == PIGO_E_CAP && rcs[gidx] != PIGO_E_CAP)) { rc = rcs[gidx]; g_err = msgs[gidx]; }
+  for (int s = 0; s < S; ++s) {
+    if (rcs[s] == PIGO_OK) continue;
+    if (rc == PIGO_OK || (rc == PIGO_E_CAP && rcs[s] != PIGO_E_CAP)) { rc = rcs[s]; g_err = msgs[s]; }
   }
   return rc;
+}
+
+// The frame batches' split: one shard per device of the mask, frames [g*ceil(N/G), (g+1)*ceil(N/G)) like SURVEY.md section 8e.
+template <typename F>
+static int for_each_shard(int nframes, F fn) {
+  const std::vector<int> devs = sharded_devices();
+  if (devs.empty()) return PIGO_E_NODEVICE;
+  const int G = (int)devs.size();
+  const int per = (nframes + G - 1) / G;
+  std::vector<int> first(G + 1);
+  for (int g = 0; g <= G; ++g) first[g] = std::min(nframes, g * per);
+  return for_each_shard(devs, first, fn);
+}
+
+// ---- the split of a sharded mixed-size call (pigo_shard_plan) -----------------------------------------------------------
+// Modelled cost of an entry, in tenths of a window: count_windows x (rotated ? kRotCost : 10) + kImgCost.
+// kRotCost / 10 = 1.4 is the ratio of the unrotated to the rotated windows/s of DESIGN.md section 5.  Those two rates come
+// from different workloads and were never measured as a cost ratio; tools/ragged_bench.py --sections sharded sets modelled
+// shard costs against measured shard times.  kImgCost stands for the fixed cost of an entry (descriptor, finalize, its
+// share of the launches): 4096 windows, a guess of the same standing.
+static constexpr uint64_t kRotCost = 14, kImgCost = 4096 * 10;
+
+// first[0..S] of the cut of cost[] into S = min(nshards, n) contiguous non-empty ranges whose largest cost is the least
+// any contiguous split into at most S ranges reaches (binary search on that bottleneck, then a greedy cut that also
+// leaves one entry for every shard still to come).
+static std::vector<int> cut_shards(const std::vector<uint64_t>& cost, int nshards) {
+  const int n = (int)cost.size(), S = std::min(nshards, n);
+  std::vector<int> first{0};
+  if (S <= 0) return first;
+  uint64_t lo = 0, hi = 0;
+  for (uint64_t c : cost) { lo = std::max(lo, c); hi += c; }
+  auto ranges_at = [&](uint64_t B) {   // ranges a greedy cut at bottleneck B needs
+    int k = 1;
+    uint64_t sum = 0;
+    for (uint64_t c : cost) {
+      if (sum + c > B) { ++k; sum = 0; }
+      sum += c;
+    }
+    return k;
+  };
+  while (lo < hi) {
+    const uint64_t mid = lo + (hi - lo) / 2;
+    if (ranges_at(mid) <= S) hi = mid; else lo = mid + 1;
+  }
+  uint64_t sum = 0;
+  for (int i = 0; i < n; ++i) {
+    const int shards_left = S - (int)first.size();   // ranges still to start after the current one
+    // cut before entry i when it does not fit under the bottleneck, or when entries i.. are just enough for those ranges
+    if (i > 0 && shards_left > 0 && (sum + cost[i] > lo || n - i <= shards_left)) {
+      first.push_back(i);
+      sum = 0;
+    }
+    sum += cost[i];
+  }
+  first.push_back(n);
+  return first;
+}
+
+// Shards of a sharded mixed-size call on G devices: option shard_split, or one per device.
+static int shard_count(int G) {
+  const long long k = g_opt.shard_split.load();
+  return k > 0 ? (int)std::min<long long>(k, 65535) : G;
+}
+
+// The split of entries with window counts wins[] at angles[] (nullptr: all unrotated) into at most nshards shards.
+static std::vector<int> plan_shards(const std::vector<uint64_t>& wins, const double* angles, int nshards) {
+  std::vector<uint64_t> cost(wins.size());
+  for (size_t i = 0; i < wins.size(); ++i) cost[i] = wins[i] * (angles && rot_slot_of(angles[i]) >= 0 ? kRotCost : 10) + kImgCost;
+  return cut_shards(cost, nshards);
 }
 
 // ---- RunDetector over uniform frames or over an image table (pigo_puploc_run_frames / pigo_puploc_run_images) -----------
@@ -1554,11 +1638,12 @@ static int detect_batch_on(int dev, pigo_cascade* face, pigo_puploc* puploc, pig
 
 // Mixed-size form: the images' pixels are staged once (stage_images) and both the images scan and the RunDetector stages
 // read them; `plans` / `wins` / `longest` are the call's ladders (build_image_plans).  Image i is scanned and its eyes are
-// refined at angles[i] (P.angle is not used).
+// refined at angles[i] (P.angle is not used).  slot_base offsets the generator key as in detect_batch_on (a shard that
+// starts at image lo of a larger call passes lo*face_cap*(2+ncalls)).
 static int detect_images_on(int dev, pigo_cascade* face, pigo_puploc* puploc, pigo_puploc* const* flp, const uint8_t* flp_flip, int ncalls,
                             const pigo_image* images, int nimages, const double* angles, const std::vector<std::vector<ScaleEntry>>& plans,
                             const std::vector<uint64_t>& wins, int longest, const pigo_pipeline_params& P, const float* randoms, uint64_t rng_seed,
-                            pigo_det* faces, int face_cap, int* n_faces, pigo_point* points, unsigned flags, void* stream_) {
+                            uint64_t slot_base, pigo_det* faces, int face_cap, int* n_faces, pigo_point* points, unsigned flags, void* stream_) {
   const bool frames_dev = flags & PIGO_FRAMES_DEVICE;
   auto scan = [&](Workspace* w, cudaStream_t st, pigo_det* d_dets, int det_cap, int32_t* d_cnt, PupWork& W) {
     std::vector<pigo_image> staged;
@@ -1568,8 +1653,8 @@ static int detect_images_on(int dev, pigo_cascade* face, pigo_puploc* puploc, pi
     return scan_images_on(face, dev, staged.data(), nimages, plans, wins, longest, P.min_size, P.max_size, P.shift_factor, P.scale_factor,
                           angles, d_dets, det_cap, d_cnt, PIGO_FRAMES_DEVICE | PIGO_OUT_DEVICE, st);
   };
-  return detect_on(dev, face, puploc, flp, flp_flip, ncalls, nimages, "image", P, randoms, rng_seed, 0, faces, face_cap, n_faces, points, flags,
-                   stream_, scan);
+  return detect_on(dev, face, puploc, flp, flp_flip, ncalls, nimages, "image", P, randoms, rng_seed, slot_base, faces, face_cap, n_faces, points,
+                   flags, stream_, scan);
 }
 
 // Extent of the planes image.YCbCr holds for Rect (min)-(min + size), min >= 0: bytes from the rectangle's origin to its
@@ -1705,7 +1790,7 @@ static int detect_images(const char* fn, const pigo_cascade* face, const pigo_pu
   std::vector<double> uniform;
   if (!angles) { uniform.assign(nimages, prm->angle); angles = uniform.data(); }
   return detect_images_on(default_device(), const_cast<pigo_cascade*>(face), const_cast<pigo_puploc*>(puploc), (pigo_puploc* const*)flp, flp_flip,
-                          ncalls, images, nimages, angles, plans, wins, longest, *prm, randoms, rng_seed, faces, face_cap, n_faces, points, flags,
+                          ncalls, images, nimages, angles, plans, wins, longest, *prm, randoms, rng_seed, 0, faces, face_cap, n_faces, points, flags,
                           stream);
 }
 
@@ -1811,27 +1896,16 @@ int pigo_ycbcr_to_nrgba(const uint8_t* y, const uint8_t* cb, const uint8_t* cr, 
   return PIGO_OK;
 }
 
+}  // extern "C"
+
 // ---- RgbToGrayscale(ImgToNRGBA(img)) for a batch of decoded images, core/grayscale.go:8-23 + core/image.go:35-90 -----------
-// One slot per distinct source in the caller's device arena (arena_layout); one kernel launch for the YCbCr, NRGBA, RGBA
-// and Gray sources and one for the other formats, each made only when the call has such sources.
-int pigo_gray_images(const pigo_decoded* src, int n, uint8_t* gray, size_t* gray_bytes, pigo_image* images, unsigned flags, void* stream_) {
-  if (n < 0 || n > 65535) return set_err(PIGO_E_INVALID, "%d sources: outside 0..65535", n);
-  if (!gray_bytes) return set_err(PIGO_E_INVALID, "null gray_bytes");
-  if (n > 0 && (!src || !images)) return set_err(PIGO_E_INVALID, "null src or images");
-  int rc = check_decoded(src, n);
+// The distinct sources of src (first[i], arena_layout) into their slots gray + off[i] on device dev: one kernel launch for
+// the YCbCr, NRGBA, RGBA and Gray sources and one for the other formats, each made only when the call has such sources.
+// With stream_ NULL the slots are complete on return; on a caller's stream only the host planes' copies are.
+static int gray_images_on(int dev, const pigo_decoded* src, int n, const std::vector<size_t>& off, const std::vector<char>& first, uint8_t* gray,
+                          unsigned flags, void* stream_) {
+  int rc = use_device(dev);
   if (rc) return rc;
-  std::vector<size_t> off;
-  std::vector<char> first;
-  const size_t total = arena_layout(src, n, off, first);
-  if (!gray || *gray_bytes < total) {
-    *gray_bytes = total;
-    if (total > 0) return set_err(PIGO_E_CAP, "the gray arena needs %zu bytes", total);
-  }
-  if (n == 0) return PIGO_OK;
-  if ((rc = ensure_device())) return rc;
-  if (stream_ && stream_capturing((cudaStream_t)stream_)) return set_err(PIGO_E_INVALID, "pigo_gray_images does not support stream capture");
-  for (int i = 0; i < n; ++i) images[i] = pigo_image{gray + off[i], src[i].height, src[i].width, src[i].width};
-  const int dev = default_device();
   WsGuard g(g_misc_pool[dev]);
   Workspace* w = g.w;
   if (!w) return set_err(PIGO_E_CUDA, "could not create a CUDA stream");
@@ -1905,6 +1979,212 @@ int pigo_gray_images(const pigo_decoded* src, int n, uint8_t* gray, size_t* gray
   CUDA_TRY(cudaGetLastError());
   if (!stream_) CUDA_TRY(cudaStreamSynchronize(st));   // the library's own stream: the arena is complete on return
   else if (copied) CUDA_TRY(cudaEventSynchronize(copied));
+  return PIGO_OK;
+}
+
+extern "C" {
+
+// One slot per distinct source in the caller's device arena (arena_layout), converted by gray_images_on.
+int pigo_gray_images(const pigo_decoded* src, int n, uint8_t* gray, size_t* gray_bytes, pigo_image* images, unsigned flags, void* stream_) {
+  if (n < 0 || n > 65535) return set_err(PIGO_E_INVALID, "%d sources: outside 0..65535", n);
+  if (!gray_bytes) return set_err(PIGO_E_INVALID, "null gray_bytes");
+  if (n > 0 && (!src || !images)) return set_err(PIGO_E_INVALID, "null src or images");
+  int rc = check_decoded(src, n);
+  if (rc) return rc;
+  std::vector<size_t> off;
+  std::vector<char> first;
+  const size_t total = arena_layout(src, n, off, first);
+  if (!gray || *gray_bytes < total) {
+    *gray_bytes = total;
+    if (total > 0) return set_err(PIGO_E_CAP, "the gray arena needs %zu bytes", total);
+  }
+  if (n == 0) return PIGO_OK;
+  if ((rc = ensure_device())) return rc;
+  if (stream_ && stream_capturing((cudaStream_t)stream_)) return set_err(PIGO_E_INVALID, "pigo_gray_images does not support stream capture");
+  for (int i = 0; i < n; ++i) images[i] = pigo_image{gray + off[i], src[i].height, src[i].width, src[i].width};
+  return gray_images_on(default_device(), src, n, off, first, gray, flags, stream_);
+}
+
+}  // extern "C"
+
+// ---- sharded mixed-size calls: contiguous ranges of entries over the devices (pigo_*_images_sharded, pigo_*_decoded_sharded) ----
+// Geometry-only images of decoded sources (Dim = width, as pigo_gray_images gives them): the argument checks and ladders
+// read no pixels, so every descriptor points at one placeholder byte.
+static const uint8_t kNoPixels = 0;
+static std::vector<pigo_image> decoded_geometry(const pigo_decoded* src, int n) {
+  std::vector<pigo_image> v(n);
+  for (int i = 0; i < n; ++i) v[i] = pigo_image{&kNoPixels, src[i].height, src[i].width, src[i].width};
+  return v;
+}
+
+// The ladders of entries [lo, lo+n) of a call (a shard plans and schedules its own entries).
+struct ShardPlans {
+  std::vector<std::vector<ScaleEntry>> plans;
+  std::vector<uint64_t> wins;
+  int longest = 0;
+};
+static int shard_plans(const pigo_image* images, int n, int min_size, int max_size, double shift, double scale_factor, ShardPlans& sp) {
+  return build_image_plans(images, n, min_size, max_size, shift, scale_factor, sp.plans, sp.wins, sp.longest);
+}
+
+// Converts a shard's decoded sources into the gray arena of workspace `wa` on device dev, on wa's stream, and fills
+// images[0..n) with the device images (the layout pigo_gray_images gives the same sources).
+static int gray_shard(int dev, Workspace* wa, const pigo_decoded* src, int n, std::vector<pigo_image>& images) {
+  std::vector<size_t> off;
+  std::vector<char> first;
+  const size_t total = arena_layout(src, n, off, first);
+  int rc = wa->gray_arena.reserve(total + 256);
+  if (rc) return rc;
+  uint8_t* gray = (uint8_t*)wa->gray_arena.p;
+  images.resize(n);
+  for (int i = 0; i < n; ++i) images[i] = pigo_image{gray + off[i], src[i].height, src[i].width, src[i].width};
+  return gray_images_on(dev, src, n, off, first, gray, PIGO_MEM_HOST, wa->stream);
+}
+
+// Runs fn(device, workspace holding the shard's gray arena, device images) for a decoded shard.  Everything of the shard
+// is ordered on the workspace's stream: the copies and conversion, then the scan or pipeline that reads the arena.
+template <typename F>
+static int with_gray_shard(int dev, const pigo_decoded* src, int n, F fn) {
+  int rc = use_device(dev);
+  if (rc) return rc;
+  WsGuard ga(g_misc_pool[dev]);
+  Workspace* wa = ga.w;
+  if (!wa) return set_err(PIGO_E_CUDA, "could not create a CUDA stream");
+  if ((rc = ws_enter(wa, wa->stream))) return rc;   // behind the last asynchronous user of this workspace
+  std::vector<pigo_image> images;
+  if ((rc = gray_shard(dev, wa, src, n, images))) return rc;
+  return fn(wa, images);
+}
+
+static int run_cascade_sharded(const pigo_cascade* cc, const pigo_image* images, const pigo_decoded* src, int nimages, const double* angles,
+                               int min_size, int max_size, double shift_factor, double scale_factor, pigo_det* out, int cap_per_image, int* n_out) {
+  // images: the call's images (host pixels), or (src != nullptr) the geometry of the decoded sources
+  std::vector<std::vector<ScaleEntry>> plans;
+  std::vector<uint64_t> wins;
+  int longest = 0;
+  int rc = build_image_plans(images, nimages, min_size, max_size, shift_factor, scale_factor, plans, wins, longest);
+  if (rc) return rc;
+  if (nimages == 0) return ensure_device();
+  const std::vector<double> zeros(angles ? 0 : nimages, 0.0);
+  if (!angles) angles = zeros.data();
+  const std::vector<int> devs = sharded_devices();
+  if (devs.empty()) return PIGO_E_NODEVICE;   // message set by pigo_init
+  const std::vector<int> first = plan_shards(wins, angles, shard_count((int)devs.size()));
+  pigo_cascade* c = const_cast<pigo_cascade*>(cc);
+  return for_each_shard(devs, first, [&](int, int dev, int lo, int n) {
+    ShardPlans sp;
+    int rc = shard_plans(images + lo, n, min_size, max_size, shift_factor, scale_factor, sp);
+    if (rc) return rc;
+    pigo_det* o = out ? out + (size_t)lo * cap_per_image : nullptr;
+    if (!src)
+      return scan_images_on(c, dev, images + lo, n, sp.plans, sp.wins, sp.longest, min_size, max_size, shift_factor, scale_factor, angles + lo, o,
+                            cap_per_image, n_out + lo, PIGO_MEM_HOST, nullptr);
+    return with_gray_shard(dev, src + lo, n, [&](Workspace* wa, const std::vector<pigo_image>& dimg) {
+      return scan_images_on(c, dev, dimg.data(), n, sp.plans, sp.wins, sp.longest, min_size, max_size, shift_factor, scale_factor, angles + lo, o,
+                            cap_per_image, n_out + lo, PIGO_FRAMES_DEVICE, wa->stream);
+    });
+  });
+}
+
+static int detect_sharded(const pigo_cascade* face, const pigo_puploc* puploc, const pigo_puploc* const* flp, const uint8_t* flp_flip, int ncalls,
+                          const pigo_image* images, const pigo_decoded* src, int nimages, const double* angles, const pigo_pipeline_params* prm,
+                          const float* randoms, uint64_t rng_seed, pigo_det* faces, int face_cap, int* n_faces, pigo_point* points) {
+  std::vector<std::vector<ScaleEntry>> plans;
+  std::vector<uint64_t> wins;
+  int longest = 0;
+  int rc = build_image_plans(images, nimages, prm->min_size, prm->max_size, prm->shift_factor, prm->scale_factor, plans, wins, longest);
+  if (rc) return rc;
+  if (nimages == 0) return ensure_device();
+  const std::vector<double> uniform(angles ? 0 : nimages, prm->angle);
+  if (!angles) angles = uniform.data();
+  const std::vector<int> devs = sharded_devices();
+  if (devs.empty()) return PIGO_E_NODEVICE;
+  const std::vector<int> first = plan_shards(wins, angles, shard_count((int)devs.size()));
+  const size_t per_image = (size_t)face_cap * (2 + ncalls);
+  pigo_cascade* fc = const_cast<pigo_cascade*>(face);
+  pigo_puploc* pc = const_cast<pigo_puploc*>(puploc);
+  return for_each_shard(devs, first, [&](int, int dev, int lo, int n) {
+    ShardPlans sp;
+    int rc = shard_plans(images + lo, n, prm->min_size, prm->max_size, prm->shift_factor, prm->scale_factor, sp);
+    if (rc) return rc;
+    // the shard's generator keys and injected randoms are those of images lo.. in the whole call
+    const float* rnd = randoms ? randoms + (size_t)lo * per_image * 189 : nullptr;
+    pigo_det* f = faces + (size_t)lo * face_cap;
+    pigo_point* p = points + (size_t)lo * per_image;
+    if (!src)
+      return detect_images_on(dev, fc, pc, (pigo_puploc* const*)flp, flp_flip, ncalls, images + lo, n, angles + lo, sp.plans, sp.wins, sp.longest,
+                              *prm, rnd, rng_seed, (uint64_t)lo * per_image, f, face_cap, n_faces + lo, p, PIGO_MEM_HOST, nullptr);
+    return with_gray_shard(dev, src + lo, n, [&](Workspace* wa, const std::vector<pigo_image>& dimg) {
+      return detect_images_on(dev, fc, pc, (pigo_puploc* const*)flp, flp_flip, ncalls, dimg.data(), n, angles + lo, sp.plans, sp.wins, sp.longest,
+                              *prm, rnd, rng_seed, (uint64_t)lo * per_image, f, face_cap, n_faces + lo, p, PIGO_FRAMES_DEVICE, wa->stream);
+    });
+  });
+}
+
+// Arguments of the decoded forms: what pigo_gray_images checks, before the checks of the matching mixed-size call.
+static int check_decoded_args(const pigo_decoded* src, int n) {
+  if (n < 0 || n > 65535) return set_err(PIGO_E_INVALID, "%d sources: outside 0..65535", n);
+  if (n > 0 && !src) return set_err(PIGO_E_INVALID, "null src");
+  return check_decoded(src, n);
+}
+
+extern "C" {
+
+int pigo_run_cascade_images_sharded(const pigo_cascade* c, const pigo_image* images, int nimages, const double* angles, int min_size, int max_size,
+                                    double shift_factor, double scale_factor, pigo_det* out, int cap_per_image, int* n_out) {
+  const int rc = check_images_args(c, images, nimages, out, cap_per_image, n_out);
+  if (rc) return rc;
+  return run_cascade_sharded(c, images, nullptr, nimages, angles, min_size, max_size, shift_factor, scale_factor, out, cap_per_image, n_out);
+}
+
+int pigo_detect_images_sharded(const pigo_cascade* face, const pigo_puploc* puploc, const pigo_puploc* const* flp, const uint8_t* flp_flip,
+                               int ncalls, const pigo_image* images, int nimages, const double* angles, const pigo_pipeline_params* prm,
+                               const float* randoms, uint64_t rng_seed, pigo_det* faces, int face_cap, int* n_faces, pigo_point* points) {
+  const int rc = check_detect_images_args(face, puploc, flp, ncalls, images, nimages, prm, faces, face_cap, n_faces, points);
+  if (rc) return rc;
+  return detect_sharded(face, puploc, flp, flp_flip, ncalls, images, nullptr, nimages, angles, prm, randoms, rng_seed, faces, face_cap, n_faces,
+                        points);
+}
+
+int pigo_run_cascade_decoded_sharded(const pigo_cascade* c, const pigo_decoded* src, int n, const double* angles, int min_size, int max_size,
+                                     double shift_factor, double scale_factor, pigo_det* out, int cap_per_image, int* n_out) {
+  int rc = check_decoded_args(src, n);
+  if (rc) return rc;
+  const std::vector<pigo_image> geo = decoded_geometry(src, n);
+  if ((rc = check_images_args(c, geo.data(), n, out, cap_per_image, n_out))) return rc;
+  return run_cascade_sharded(c, geo.data(), src, n, angles, min_size, max_size, shift_factor, scale_factor, out, cap_per_image, n_out);
+}
+
+int pigo_detect_decoded_sharded(const pigo_cascade* face, const pigo_puploc* puploc, const pigo_puploc* const* flp, const uint8_t* flp_flip,
+                                int ncalls, const pigo_decoded* src, int n, const double* angles, const pigo_pipeline_params* prm,
+                                const float* randoms, uint64_t rng_seed, pigo_det* faces, int face_cap, int* n_faces, pigo_point* points) {
+  int rc = check_decoded_args(src, n);
+  if (rc) return rc;
+  const std::vector<pigo_image> geo = decoded_geometry(src, n);
+  if ((rc = check_detect_images_args(face, puploc, flp, ncalls, geo.data(), n, prm, faces, face_cap, n_faces, points))) return rc;
+  return detect_sharded(face, puploc, flp, flp_flip, ncalls, geo.data(), src, n, angles, prm, randoms, rng_seed, faces, face_cap, n_faces, points);
+}
+
+int pigo_shard_plan(const pigo_image* images, int nimages, const double* angles, int min_size, int max_size, double shift_factor,
+                    double scale_factor, int nshards, int* first, int* n_used) {
+  if (nimages < 0 || nimages > 65535) return set_err(PIGO_E_INVALID, "nimages must be 0..65535");
+  if (nimages > 0 && !images) return set_err(PIGO_E_INVALID, "null images");
+  if (!n_used) return set_err(PIGO_E_INVALID, "null n_used");
+  if (nshards < 0) return set_err(PIGO_E_INVALID, "negative nshards");
+  for (int i = 0; i < nimages; ++i) {
+    const pigo_image& im = images[i];
+    if (im.rows < 0 || im.cols < 0 || im.dim < im.cols)
+      return set_err(PIGO_E_INVALID, "image %d: bad geometry rows=%d cols=%d dim=%d", i, im.rows, im.cols, im.dim);
+  }
+  std::vector<std::vector<ScaleEntry>> plans;
+  std::vector<uint64_t> wins;
+  int longest = 0;
+  int rc = build_image_plans(images, nimages, min_size, max_size, shift_factor, scale_factor, plans, wins, longest);
+  if (rc) return rc;
+  if (nshards == 0) nshards = shard_count(std::max(1, (int)shard_devices().size()));
+  const std::vector<int> cut = plan_shards(wins, angles, nshards);
+  *n_used = (int)cut.size() - 1;
+  if (first) std::copy(cut.begin(), cut.end(), first);
   return PIGO_OK;
 }
 

@@ -300,7 +300,7 @@ void launch_deep_smem(const ScanArgs& A, unsigned long long* counter, const uint
   const size_t smem = kDeepRecOff + (size_t)k * kTreeRec;
 #define PIGO_DEEP_SMEM(G)                                                                                              \
   do {                                                                                                                 \
-    cudaFuncSetAttribute(deep_smem_kernel<G>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);                 \
+    raise_dyn_smem((const void*)deep_smem_kernel<G>, (int)smem);                                                     \
     int per_sm = 1;                                                                                                    \
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, deep_smem_kernel<G>, threads, smem) != cudaSuccess || per_sm < 1) { \
       cudaGetLastError();                                                                                              \

@@ -13,6 +13,10 @@ namespace pigo {
 
 int set_err(int code, const char* fmt, ...);
 extern std::atomic<long long> g_launches;
+// Makes kernel `fn` on the current device accept launches of `bytes` of dynamic shared memory.  The attribute is shared
+// by every host thread, so it only ever grows: calls that run concurrently on one device (several threads on one handle,
+// several shards of a sharded call) never lower it below another launch's request.
+void raise_dyn_smem(const void* fn, int bytes);
 
 // Per-kernel CUDA-event timing (enabled by option "timing"): every launch of kernel class `slot` is bracketed by an
 // event pair on its stream; "t_<name>_ns" / "t_<name>_n" return the summed device time and the launch count.
@@ -69,6 +73,8 @@ struct Options {
   std::atomic<long long> tile_tail_min{6};  // tail policy threshold
   std::atomic<long long> tile_band_ratio{0};    // a band spans scales up to ratio/100 x its first scale; 0 = auto (200, or 140 for calls of <= 2 M windows)
   std::atomic<long long> timing{0};         // 1 = bracket every kernel with CUDA events (bench.py roofline pass)
+  std::atomic<long long> shard_split{0};    // sharded mixed-size / decoded calls: 0 = one shard per selected device, k > 0 = k shards,
+                                            // shard s on device s mod G (several shards share a device: the multi-shard path on one GPU)
   std::atomic<long long>* find(const std::string& k) {
     struct Entry { const char* name; std::atomic<long long> Options::*field; };
     static const Entry table[] = {
@@ -80,7 +86,7 @@ struct Options {
          {"gather_block", &Options::gather_block}, {"deep_group", &Options::deep_group},
         {"sub_batch", &Options::sub_batch}, {"lanes", &Options::lanes}, {"tile_tail_min", &Options::tile_tail_min},
         {"tile_band_ratio", &Options::tile_band_ratio}, {"timing", &Options::timing}, {"host_stream", &Options::host_stream}, {"copy_chunk", &Options::copy_chunk}, {"stream_taper", &Options::stream_taper},
-        {"deep_flat", &Options::deep_flat}, {"tile_head", &Options::tile_head}, {"tile_ptab", &Options::tile_ptab}, {"queue_cap", &Options::queue_cap}, {"ptab_kt", &Options::ptab_kt}, {"ptab_ks", &Options::ptab_ks}, {"tile_core_cap", &Options::tile_core_cap}, {"walk_stats", &Options::walk_stats}, {"tile_tmap", &Options::tile_tmap}, {"gather_limit", &Options::gather_limit}, {"deep_smem", &Options::deep_smem}, {"deep_smem_threads", &Options::deep_smem_threads}, {"deep_smem_lo", &Options::deep_smem_lo}, {"deep_smem_k", &Options::deep_smem_k}, {"head_back", &Options::head_back}, {"rot_mode", &Options::rot_mode}, {"puploc_mode", &Options::puploc_mode}, {"puploc_stage", &Options::puploc_stage}};
+        {"deep_flat", &Options::deep_flat}, {"tile_head", &Options::tile_head}, {"tile_ptab", &Options::tile_ptab}, {"queue_cap", &Options::queue_cap}, {"ptab_kt", &Options::ptab_kt}, {"ptab_ks", &Options::ptab_ks}, {"tile_core_cap", &Options::tile_core_cap}, {"walk_stats", &Options::walk_stats}, {"tile_tmap", &Options::tile_tmap}, {"gather_limit", &Options::gather_limit}, {"deep_smem", &Options::deep_smem}, {"deep_smem_threads", &Options::deep_smem_threads}, {"deep_smem_lo", &Options::deep_smem_lo}, {"deep_smem_k", &Options::deep_smem_k}, {"head_back", &Options::head_back}, {"rot_mode", &Options::rot_mode}, {"puploc_mode", &Options::puploc_mode}, {"puploc_stage", &Options::puploc_stage}, {"shard_split", &Options::shard_split}};
     for (const Entry& e : table)
       if (k == e.name) return &(this->*e.field);
     return nullptr;
@@ -224,7 +230,8 @@ struct Workspace {
   // mixed-size calls keep their own device plan / image table and rotated node tables, so that they never disturb the
   // cached uniform plan above (plan_host, pad_first_untiled, rot_slot + rot_tab, ptab_sig)
   DevBuf img_tab, img_rot;
-  std::vector<int> img_rot_slots;                            // what img_rot was built for: one table per slot, in order (empty = nothing)
+  DevBuf gray_arena;                           // a sharded decoded call's converted images on this device (pigo_*_decoded_sharded)
+  std::vector<int> img_rot_slots;                           // what img_rot was built for: one table per slot, in order (empty = nothing)
   int img_rot_len = 0, img_rot_min = 0;
   double img_rot_scale = 0;
   void* pinned = nullptr;
@@ -242,7 +249,7 @@ struct Workspace {
     for (auto e : copy_events) cudaEventDestroy(e);
     if (copy_stream) cudaStreamDestroy(copy_stream);
     tiles.release(); scratch_a.release(); scratch_b.release(); scratch_c.release(); rot_tab.release(); ptab.release();
-    img_tab.release(); img_rot.release();
+    img_tab.release(); img_rot.release(); gray_arena.release();
     if (pinned) cudaFreeHost(pinned);
     if (seq) cudaFreeHost(seq);
     if (stream) cudaStreamDestroy(stream);

@@ -380,9 +380,9 @@ __global__ void __launch_bounds__(kPairThreads, PATCH ? 2 : 3) puploc_pair_kerne
 
 template <bool IMG>
 static void set_pair_smem(int bytes) {
-  cudaFuncSetAttribute(puploc_pair_kernel<true, true, IMG>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  cudaFuncSetAttribute(puploc_pair_kernel<true, false, IMG>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  cudaFuncSetAttribute(puploc_pair_kernel<false, false, IMG>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  raise_dyn_smem((const void*)puploc_pair_kernel<true, true, IMG>, bytes);
+  raise_dyn_smem((const void*)puploc_pair_kernel<true, false, IMG>, bytes);
+  raise_dyn_smem((const void*)puploc_pair_kernel<false, false, IMG>, bytes);
 }
 // codes_bytes > 0: the stage's node codes are staged; patch_cap > 0 (with them): so is the stage's pixel patch
 template <bool IMG>

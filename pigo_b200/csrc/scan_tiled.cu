@@ -1381,7 +1381,7 @@ __global__ void __launch_bounds__(MAXT, 1) scan_head_kernel(const TiledArgs A, c
 
 template <int NI, int MAXT>
 static void launch_tiled_ni(const TiledArgs& A, const TileMaps& TM, int grid, int threads, size_t smem, cudaStream_t st) {
-  cudaFuncSetAttribute(scan_tiled_kernel<NI, MAXT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  raise_dyn_smem((const void*)scan_tiled_kernel<NI, MAXT>, (int)smem);
   scan_tiled_kernel<NI, MAXT><<<grid, threads, smem, st>>>(A, TM);
 }
 
@@ -1401,14 +1401,14 @@ static const void* gather2_fn(int ng, bool rot, bool img = false) {
 }
 void launch_scan_gather2(const TiledArgs& A, int grid, size_t smem, cudaStream_t st) {
   const void* fn = gather2_fn(A.gather_ni, A.scan.rot_slot >= 0, A.scan.images != nullptr);
-  cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  raise_dyn_smem(fn, (int)smem);
   void* args[] = {(void*)&A};
   cudaLaunchKernel(fn, dim3(grid), dim3(256), args, smem, st);
 }
 int gather2_ctas_per_sm(size_t smem, int ng, bool rot, bool img) {
   int n = 0;
   const void* fn = gather2_fn(ng, rot, img);
-  cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  raise_dyn_smem(fn, (int)smem);
   if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, fn, 256, smem) != cudaSuccess || n < 1) { cudaGetLastError(); n = 1; }
   return n;
 }
@@ -1428,12 +1428,12 @@ void launch_ptab_build(const FaceTables& T, const ScaleEntry* plan, const TiledA
 
 void launch_scan_tiled(const TiledArgs& A, const TileMaps& TM, int grid, int threads, size_t smem, int ni, cudaStream_t st) {
   if (A.kt > 0) {
-    cudaFuncSetAttribute(scan_ptab_kernel<1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    raise_dyn_smem((const void*)scan_ptab_kernel<1024>, (int)smem);
     scan_ptab_kernel<1024><<<grid, threads, smem, st>>>(A, TM);
     return;
   }
   if (A.head_trees > 0) {
-    cudaFuncSetAttribute(scan_head_kernel<1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    raise_dyn_smem((const void*)scan_head_kernel<1024>, (int)smem);
     scan_head_kernel<1024><<<grid, threads, smem, st>>>(A, TM);
     return;
   }

@@ -194,16 +194,34 @@ def detect_images_angles_device(clf: Pigo, plc: PuplocCascade, flpcs: Dict[str, 
                           det_cap, raw)
 
 
+def detect_images_sharded(clf: Pigo, plc: PuplocCascade, flpcs: Dict[str, PuplocCascade], images, cp: CascadeParams, angles=None,
+                          iou: float = 0.1, min_face: int = 50, eye_perturbs: int = 50, flp_perturbs: int = 63, face_cap: int = 32,
+                          angle: float = 0.0, randoms: Optional[np.ndarray] = None, rng_seed: int = 0, det_cap: int = 0, raw: bool = False):
+    """detect_images_angles_device over the devices of init_devices (pigo_detect_images_sharded): host images cut into
+    contiguous shards of about equal modelled cost; angles None = every image at `angle`.  Results, generator keys and
+    injected randoms are those of the single-device call, byte for byte."""
+    if angles is not None and len(angles) != len(images):
+        raise ValueError("angles must have one entry per image")
+    return _detect_images(clf, plc, flpcs, images, cp, iou, min_face, eye_perturbs, flp_perturbs, face_cap, angle, angles, randoms, rng_seed,
+                          det_cap, raw, sharded=True)
+
+
 def _detect_images(clf, plc, flpcs, images, cp, iou, min_face, eye_perturbs, flp_perturbs, face_cap, angle, angles, randoms, rng_seed, det_cap,
-                   raw):
+                   raw, sharded=False, sources=None):
     import ctypes as C
     from . import DET_DTYPE, POINT_DTYPE, FRAMES_DEVICE, MEM_HOST, PipelineParams, _check, _pixels, image_descs, lib
+    from . import decoded_descs
     hs, fl = landmark_call_arrays(flpcs)
     ncalls = len(fl)
-    n = len(images)
-    on_dev = n > 0 and all(isinstance(im.Pixels, int) for im in images)
-    keep = [None if on_dev else _pixels(im) for im in images]   # host pixels stay alive for the call
-    desc = image_descs([(im.Pixels if on_dev else p.ctypes.data, im.Rows, im.Cols, im.Dim) for im, p in zip(images, keep)])
+    if sources is not None:   # decoded sources (host planes): converted on the devices by the call
+        n = len(sources)
+        desc = decoded_descs(sources)
+        on_dev = False
+    else:
+        n = len(images)
+        on_dev = n > 0 and all(isinstance(im.Pixels, int) for im in images)
+        keep = [None if on_dev else _pixels(im) for im in images]   # host pixels stay alive for the call
+        desc = image_descs([(im.Pixels if on_dev else p.ctypes.data, im.Rows, im.Cols, im.Dim) for im, p in zip(images, keep)])
     prm = PipelineParams(cp.MinSize, cp.MaxSize, cp.ShiftFactor, cp.ScaleFactor, angle, iou, min_face, eye_perturbs, flp_perturbs, det_cap)
     rnd = None
     if randoms is not None:
@@ -214,7 +232,14 @@ def _detect_images(clf, plc, flpcs, images, cp, iou, min_face, eye_perturbs, flp
     points = np.zeros((n, face_cap, 2 + ncalls), dtype=POINT_DTYPE)
     flags = FRAMES_DEVICE if on_dev else MEM_HOST
     rptr = rnd.ctypes.data if rnd is not None else None
-    if angles is None:
+    if sharded:
+        if on_dev:
+            raise ValueError("the sharded calls take host images")
+        ang = np.ascontiguousarray(angles, dtype=np.float64) if angles is not None else None
+        fn = lib().pigo_detect_decoded_sharded if sources is not None else lib().pigo_detect_images_sharded
+        _check(fn(clf._h, plc._h, hs, fl.ctypes.data, ncalls, desc, n, ang.ctypes.data if ang is not None else None, C.byref(prm), rptr, rng_seed,
+                  faces.ctypes.data, face_cap, nfaces.ctypes.data, points.ctypes.data))
+    elif angles is None:
         _check(lib().pigo_detect_images(clf._h, plc._h, hs, fl.ctypes.data, ncalls, desc, n, C.byref(prm), rptr, rng_seed, faces.ctypes.data,
                                         face_cap, nfaces.ctypes.data, points.ctypes.data, flags, None))
     else:
@@ -228,10 +253,20 @@ def _detect_images(clf, plc, flpcs, images, cp, iou, min_face, eye_perturbs, flp
 
 def detect_decoded(clf: Pigo, plc: PuplocCascade, flpcs: Dict[str, PuplocCascade], sources, cp: CascadeParams, angles=None, iou: float = 0.1,
                    min_face: int = 50, eye_perturbs: int = 50, flp_perturbs: int = 63, face_cap: int = 32, randoms: Optional[np.ndarray] = None,
-                   rng_seed: int = 0, det_cap: int = 0, raw: bool = False, device_sources: bool = False):
+                   rng_seed: int = 0, det_cap: int = 0, raw: bool = False, device_sources: bool = False, sharded: bool = False):
     """Go's DetectDecoded: RgbToGrayscale(ImgToNRGBA(img)) of every DecodedImage in one pigo_gray_images call, then
     detect_images_angles_device on the device arena (angles None = every image at 0).  Returns what
-    detect_images_angles_device returns for the oracle-made gray images with Dim = Cols."""
+    detect_images_angles_device returns for the oracle-made gray images with Dim = Cols.  sharded=True: the same result
+    from pigo_detect_decoded_sharded, every device of init_devices converting and detecting its own shard of the (host)
+    sources."""
+    if sharded:
+        if device_sources:
+            raise ValueError("the sharded call takes host sources")
+        if angles is not None and len(angles) != len(sources):
+            raise ValueError("angles must have one entry per image")
+        angles = [0.0] * len(sources) if angles is None else angles
+        return _detect_images(clf, plc, flpcs, None, cp, iou, min_face, eye_perturbs, flp_perturbs, face_cap, 0.0, angles, randoms, rng_seed,
+                              det_cap, raw, sharded=True, sources=sources)
     from . import gray_images
     arena, images = gray_images(sources, device_sources=device_sources)
     angles = [0.0] * len(images) if angles is None else angles

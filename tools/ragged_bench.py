@@ -24,6 +24,9 @@ Usage: `python tools/ragged_bench.py [--frames 256]` on one GPU prints one JSON 
   formats : the same 256 images as NRGBA, Gray16, RGBA64, NRGBA64, CMYK and Paletted sources whose gray is exactly the
               image, detections asserted equal: pigo_gray_images alone (device and pinned planes) and with
               pigo_detect_images end to end (formats_bench)
+  sharded : the same 256 images (a quarter of the wide ones rotated) from host memory: one single-device call against the
+              sharded calls with shard_split 1, 2, 4, 8, outputs asserted identical; per-shard modelled cost against
+              measured time (sharded_bench)
 `--sections scan,pipeline` (the default) selects the sections; `--sections angles` runs the sweeps alone.  Writes nothing
 to the tree.
 """
@@ -748,11 +751,92 @@ def formats_bench(clf, dev: int, stream) -> dict:
     return res
 
 
+def sharded_bench(clf, dev: int) -> dict:
+    """The sharded mixed-size calls on the 256 images, host inputs and outputs, host clock, median of 5 alternated rounds:
+    one pigo_run_cascade_images_angles / pigo_detect_images_angles call against pigo_run_cascade_images_sharded /
+    pigo_detect_images_sharded with shard_split 1, 2, 4 and 8 on the visible devices (outputs asserted identical).  On one
+    GPU every shard shares the card: the difference is the cost of splitting, not scaling.  Then the cost model: every
+    shard of the 4- and 8-way splits timed alone as a single-device call against its modelled cost, and a least-squares fit
+    of time = a * unrotated windows + b * rotated windows + c * images over those shards (k_rot = b / a, k_img = c / a)."""
+    import torch
+    import pigo_b200
+    from pigo_b200 import CascadeParams, ImageParams, pipeline
+    imgs = ragged_images()
+    n = len(imgs)
+    rng = np.random.default_rng(7)
+    # a quarter of the wide images rotated (tall images stay unrotated: see tests/test_angles_gpu.py)
+    angles = [float(rng.choice([0.1, 0.25, 0.5])) if c >= r and rng.random() < 0.25 else 0.0 for _, r, c, _ in imgs]
+    images = [ImageParams(b, r, c, d) for b, r, c, d in imgs]
+    cp = CascadeParams(ImageParams(), *PARAMS)
+    plc = pigo_b200.NewPuplocCascade().UnpackCascade(pigo_b200.load_cascade("puploc"))
+    flp = {k: pigo_b200.NewPuplocCascade().UnpackCascade(pigo_b200.load_cascade("lps/" + k))
+           for k in sorted(set(pipeline.EYE_CASCADES + pipeline.MOUTH_CASCADES))}
+    splits = [1, 2, 4, 8]
+    ways = {"one_call": None, **{f"sharded_{k}": k for k in splits}}
+    old = pigo_b200.get_option("shard_split")
+
+    def scan(k):
+        if k is None:
+            return clf.RunCascadeImagesAngles(images, cp, angles, 4096)
+        pigo_b200.set_option("shard_split", k)
+        return clf.run_cascade_images_sharded(images, cp, angles, 4096)
+
+    def detect(k):
+        if k is None:
+            return pipeline.detect_images_angles_device(clf, plc, flp, images, cp, angles, face_cap=64, rng_seed=5, raw=True)
+        pigo_b200.set_option("shard_split", k)
+        return pipeline.detect_images_sharded(clf, plc, flp, images, cp, angles, face_cap=64, rng_seed=5, raw=True)
+
+    def timed(fn):
+        torch.cuda.synchronize(dev)
+        t = time.perf_counter()
+        r = fn()
+        return r, (time.perf_counter() - t) * 1e3
+
+    res = {"images": n, "rotated": int(sum(a > 0 for a in angles)), "devices": torch.cuda.device_count()}
+    try:
+        for name, fn in (("scan", scan), ("pipeline", detect)):
+            ref = fn(None)
+            for k in splits:   # warm-up, and the outputs
+                got = fn(k)
+                assert all(a.tobytes() == b.tobytes() for a, b in zip(got, ref)), (name, k)
+            ms = {w: [] for w in ways}
+            for _ in range(5):
+                for w, k in ways.items():
+                    ms[w].append(timed(lambda: fn(k))[1])
+            res[name] = {w: round(float(np.median(v)), 2) for w, v in ms.items()}
+        # cost model against per-shard times (each shard alone, one device, host in and out)
+        wins = [pigo_b200.count_windows(r, c, *PARAMS) for _, r, c, _ in imgs]
+        rows, times, model = [], [], []
+        for k in (4, 8):
+            first = pigo_b200.shard_plan(images, *PARAMS, angles=angles, nshards=k)
+            for s in range(len(first) - 1):
+                lo, hi = first[s], first[s + 1]
+                sub, sa = images[lo:hi], angles[lo:hi]
+                clf.RunCascadeImagesAngles(sub, cp, sa, 4096)
+                t = float(np.median([timed(lambda: clf.RunCascadeImagesAngles(sub, cp, sa, 4096))[1] for _ in range(5)]))
+                un = sum(wins[i] for i in range(lo, hi) if not angles[i] > 0)
+                ro = sum(wins[i] for i in range(lo, hi) if angles[i] > 0)
+                rows.append([un, ro, hi - lo])
+                times.append(t)
+                model.append((10 * un + 14 * ro + 40960 * (hi - lo)) / 10)
+        ratio = np.array(times) / np.array(model)
+        a, b, c = np.linalg.lstsq(np.array(rows, dtype=np.float64), np.array(times), rcond=None)[0]
+        res["shards"] = [{"model_windows": int(m), "ms": round(t, 3)} for m, t in zip(model, times)]
+        res["ms_per_model_window_spread"] = round(float(ratio.max() / ratio.min()), 3)
+        res["fit"] = {"k_rot": round(float(b / a), 3) if a > 0 else None, "k_img_windows": round(float(c / a), 1) if a > 0 else None,
+                      "ns_per_unrotated_window": round(float(a * 1e6), 5)}
+    finally:
+        pigo_b200.set_option("shard_split", old)
+    res["multi_gpu_scaling"] = "measured" if res["devices"] > 1 else "not measured (one visible GPU: every shard shares it)"
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--frames", type=int, default=256, help="frames of the uniform 1080p comparison")
     ap.add_argument("--pipeline-frames", type=int, default=64, help="frames of the uniform 1080p pipeline comparison")
-    ap.add_argument("--sections", default="scan,pipeline", help="comma-separated: scan, pipeline, angles, decoded, formats")
+    ap.add_argument("--sections", default="scan,pipeline", help="comma-separated: scan, pipeline, angles, decoded, formats, sharded")
     args = ap.parse_args()
     sections = set(args.sections.split(","))
     import torch
@@ -771,6 +855,8 @@ def main():
         res["decoded"] = decoded_bench(clf, 0, stream)
     if "formats" in sections:
         res["formats"] = formats_bench(clf, 0, stream)
+    if "sharded" in sections:
+        res["sharded"] = sharded_bench(clf, 0)
     res["gpu"] = torch.cuda.get_device_name(0)
     try:   # read-only query: the power limit belongs beside the numbers
         import subprocess
