@@ -396,9 +396,13 @@ int pigo_shard_plan(const pigo_image *images, int nimages, const double *angles,
  * other threads are inside the library.  Names: pigo_b200/csrc/host.h (struct Options). */
 int pigo_set_option(const char *name, int64_t value);
 /* Host-only: JSON description of how RunCascade would be scheduled for this geometry (scale ladder, tile bands and
- * their shared-memory tile geometry, first ladder entry left to the gather role).  Needs no device. */
+ * their shared-memory tile geometry, first ladder entry left to the gather role, tile role of the fused kernel, band
+ * ratio), for a call of many frames.  Needs no device. */
 int pigo_describe_plan(int rows, int cols, int min_size, int max_size, double shift_factor, double scale_factor,
                        char *json, size_t cap);
+/* The same for a call of `nframes` frames of this geometry (>= 1): small calls plan narrower tile bands. */
+int pigo_describe_plan_frames(int rows, int cols, int min_size, int max_size, double shift_factor, double scale_factor,
+                              int nframes, char *json, size_t cap);
 int64_t pigo_get_option(const char *name);
 /* Copies the default device's block-interleaved copy of a depth-6 cascade (the table the unrotated deep kernel reads) to
  * dst and sets *bytes to its size; dst == NULL only sets *bytes (0: depth != 6, no such table). */

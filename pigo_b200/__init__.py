@@ -48,7 +48,7 @@ ABI_SYMBOLS = [
     "pigo_ycbcr_to_nrgba", "pigo_run_cascade_images", "pigo_detect_images", "pigo_puploc_run_images",
     "pigo_run_cascade_images_angles", "pigo_detect_images_angles", "pigo_gray_images", "pigo_cascade_block_table",
     "pigo_run_cascade_images_sharded", "pigo_detect_images_sharded", "pigo_run_cascade_decoded_sharded", "pigo_detect_decoded_sharded",
-    "pigo_shard_plan",
+    "pigo_shard_plan", "pigo_describe_plan_frames",
 ]
 
 
@@ -104,6 +104,7 @@ def lib() -> C.CDLL:
         L.pigo_device_free.argtypes = [vp]
         L.pigo_device_upload.argtypes = [vp, vp, sz]
         L.pigo_describe_plan.argtypes = [i, i, i, i, d, d, C.c_char_p, sz]
+        L.pigo_describe_plan_frames.argtypes = [i, i, i, i, d, d, i, C.c_char_p, sz]
         L.pigo_init_devices.argtypes = [C.c_uint]
         L.pigo_device_download.argtypes = [vp, vp, sz]
         L.pigo_run_cascade_batch_sharded.argtypes = [vp, vp, i, sz, i, i, i, i, i, d, d, d, vp, i, vp]
@@ -159,11 +160,15 @@ def launch_count() -> int:
     return int(lib().pigo_launch_count())
 
 
-def describe_plan(rows, cols, min_size, max_size, shift_factor, scale_factor) -> dict:
-    """Host-only view of the scan schedule (tile bands, tile geometry, gather scales) for this geometry."""
+def describe_plan(rows, cols, min_size, max_size, shift_factor, scale_factor, nframes: Optional[int] = None) -> dict:
+    """Host-only view of the scan schedule (tile bands, tile geometry, gather scales, tile role, band ratio) for this
+    geometry, in a call of `nframes` frames (None: a call of many frames)."""
     import json
     buf = C.create_string_buffer(1 << 20)
-    _check(lib().pigo_describe_plan(rows, cols, min_size, max_size, shift_factor, scale_factor, buf, len(buf)))
+    if nframes is None:
+        _check(lib().pigo_describe_plan(rows, cols, min_size, max_size, shift_factor, scale_factor, buf, len(buf)))
+    else:
+        _check(lib().pigo_describe_plan_frames(rows, cols, min_size, max_size, shift_factor, scale_factor, nframes, buf, len(buf)))
     return json.loads(buf.value.decode())
 
 

@@ -1232,13 +1232,18 @@ int64_t pigo_count_windows(int rows, int cols, int min_size, int max_size, doubl
   return (int64_t)total;
 }
 
-int pigo_describe_plan(int rows, int cols, int min_size, int max_size, double shift_factor, double scale_factor, char* json, size_t cap) {
+int pigo_describe_plan_frames(int rows, int cols, int min_size, int max_size, double shift_factor, double scale_factor, int nframes,
+                              char* json, size_t cap) {
   if (!json) return set_err(PIGO_E_INVALID, "null buffer");
+  if (nframes < 1) return set_err(PIGO_E_INVALID, "nframes must be at least 1");
   std::vector<ScaleEntry> plan;
   uint64_t total = 0;
   int rc = build_plan(rows, cols, min_size, max_size, shift_factor, scale_factor, plan, total);
   if (rc) return rc;
-  return describe_plan(plan, total, 468, json, cap);   // geometry of the stock 468-tree facefinder cascade
+  return describe_plan(plan, total, 468, nframes, json, cap);   // geometry of the stock 468-tree facefinder cascade
+}
+int pigo_describe_plan(int rows, int cols, int min_size, int max_size, double shift_factor, double scale_factor, char* json, size_t cap) {
+  return pigo_describe_plan_frames(rows, cols, min_size, max_size, shift_factor, scale_factor, 1 << 20, json, cap);
 }
 
 // ---- RunCascade ------------------------------------------------------------------------------------------

@@ -372,7 +372,7 @@ int build_tiled_tables(const FaceTables& tab, const std::vector<int8_t>& codes, 
                        const std::vector<float>& thr, DevBuf& out);
 int build_block_tables(const FaceTables& tab, const std::vector<int8_t>& codes, const std::vector<float>& preds,
                        const std::vector<float>& thr, DevBuf& out);
-int describe_plan(const std::vector<ScaleEntry>& plan, uint64_t wins, int ntrees, char* buf, size_t cap);
+int describe_plan(const std::vector<ScaleEntry>& plan, uint64_t wins, int ntrees, int batch_frames, char* buf, size_t cap);
 int run_scan(FaceReplica* c, Workspace* w, int lane, ScanArgs& A, unsigned long long* d_work, cudaStream_t st, int num_sms);
 struct ImagesSchedule {
   int gb_shift;       // log2 of the gather block edge in windows

@@ -157,6 +157,7 @@ struct FusedPlan {
   int W = 0, ks = 0, ni = 1;
   int head = 0;   // trees of the dense head (0 = classic tile role)
   int kt = 0;     // trees of the per-scale offset tables (0 = classic tile role)
+  int band_ratio = 0;   // a band spans scales up to band_ratio/100 x its first scale
 };
 static FusedPlan plan_fused(const std::vector<ScaleEntry>& plan, int ntrees, int batch_frames = 1 << 20) {
   FusedPlan P;
@@ -188,6 +189,7 @@ static FusedPlan plan_fused(const std::vector<ScaleEntry>& plan, int ntrees, int
   long long ratio_opt = g_opt.tile_band_ratio.load();
   if (ratio_opt <= 0) ratio_opt = call_windows <= 2000000ull ? 140 : 200;
   const int band_ratio = (int)std::max<long long>(100, ratio_opt);
+  P.band_ratio = band_ratio;
   auto plan_with = [&](int head) {
     P.L = fused_layout(P.W, P.ks, (size_t)std::max<long long>(0, g_opt.fused_smem_kb.load()) * 1024, head, P.kt);
     P.tp = TilePlan();
@@ -244,10 +246,12 @@ static int upload_block_prefix(Workspace* w, int lo, int hi, int gb_shift, cudaS
 }
 
 // Host-only introspection of the scan plan (no device needed): which ladder entries go to per-warp tiles (and with what
-// tile geometry), which go to the gather role.  JSON text; used by tests/test_plan_cpu.py to check on the CPU that the
-// tiles partition the windows of their scales exactly and that every sample stays inside its tile.
-int describe_plan(const std::vector<ScaleEntry>& plan, uint64_t wins, int ntrees, char* buf, size_t cap) {
-  const FusedPlan P = plan_fused(plan, ntrees);
+// tile geometry), which go to the gather role, and which tile role the fused kernel runs (head > 0: dense head, ptab_kt > 0:
+// per-scale offset tables, both 0: classic), for a call of `batch_frames` frames of this geometry (the frame count decides
+// the band ratio, as in run_scan).  JSON text; used by tests/test_plan_cpu.py to check on the CPU that the tiles partition
+// the windows of their scales exactly and that every sample stays inside its tile.
+int describe_plan(const std::vector<ScaleEntry>& plan, uint64_t wins, int ntrees, int batch_frames, char* buf, size_t cap) {
+  const FusedPlan P = plan_fused(plan, ntrees, batch_frames);
   const TilePlan& tp = P.tp;
   const uint32_t tile_bytes = P.L.ok ? P.L.tile_bytes : 0;
   std::string s = "{";
@@ -255,7 +259,8 @@ int describe_plan(const std::vector<ScaleEntry>& plan, uint64_t wins, int ntrees
   snprintf(tmp, sizeof(tmp), "\"nscales\": %d, \"windows\": %llu, \"tile_warps\": %d, \"tiles_off\": %zu, ", (int)plan.size(),
            (unsigned long long)wins, P.W, P.L.tiles_off);
   s += tmp;
-  snprintf(tmp, sizeof(tmp), "\"tile_bytes\": %u, \"first_untiled\": %d, \"ptab_kt\": %d, \"bands\": [", tile_bytes, tp.first_untiled, P.kt);
+  snprintf(tmp, sizeof(tmp), "\"tile_bytes\": %u, \"first_untiled\": %d, \"ptab_kt\": %d, \"head\": %d, \"ks\": %d, \"band_ratio\": %d, \"bands\": [",
+           tile_bytes, tp.first_untiled, P.kt, P.head, P.ks, P.band_ratio);
   s += tmp;
   for (int b = 0; b < tp.nbands; ++b) {
     const TileBand& B = tp.band[b];

@@ -14,6 +14,7 @@ import pytest
 import oracle_lib as O
 import pigo_b200
 from pigo_b200 import CascadeParams, ImageParams, pipeline, synth
+from option_guard import options, options_at_defaults   # noqa: F401 (autouse: every test ends with the options at their defaults)
 from test_images_gpu import CLI_PARAMS, DOC_PARAMS, KNOBS, MIXED, TEST_PARAMS, assert_slices, cp_of, lone, make_image
 
 pytestmark = pytest.mark.gpu
@@ -120,14 +121,8 @@ def test_repeated_host_descriptors_device_and_stream_forms_agree(gpu_face, sweep
 @pytest.mark.parametrize("knobs", KNOBS)
 def test_options_leave_the_outputs_unchanged(gpu_face, mixed, mixed_angles, knobs):
     ed, ec = run(gpu_face, mixed, mixed_angles)
-    saved = {k: pigo_b200.get_option(k) for k in knobs}
-    try:
-        for k, v in knobs.items():
-            pigo_b200.set_option(k, v)
+    with options(**knobs):
         d, c = run(gpu_face, mixed, mixed_angles)
-    finally:
-        for k, v in saved.items():
-            pigo_b200.set_option(k, v)
     assert np.array_equal(c, ec)
     for i in range(len(mixed)):
         assert d[i, :c[i]].tobytes() == ed[i, :ec[i]].tobytes(), i
@@ -150,12 +145,9 @@ def test_tables_past_the_bound_run_in_passes(gpu_face):
     angles = [0.0, 1 / 64] + [k / 32 for k in range(1, 33)]
     lst = [im for im in ims for _ in angles]
     ang = [a for _ in ims for a in angles]
-    pigo_b200.set_option("timing", 1)
-    try:
+    with options(timing=1):
         d, c = run(gpu_face, lst, ang, params)
         builds = pigo_b200.get_option("t_rottab_n")
-    finally:
-        pigo_b200.set_option("timing", 0)
     assert builds == 2, builds
     assert_slices(d, c, [lone(gpu_face, im, params, a) for im, a in zip(lst, ang)])
     assert c.sum() > 0
@@ -251,9 +243,7 @@ def same(a, b):
 @pytest.mark.parametrize("stage", [1, 2])
 def test_pipeline_each_image_equals_a_lone_detect_images(gpu_face, cascades, images, image_angles, face_cap, stage):
     plc, flp, _, _ = cascades
-    saved = pigo_b200.get_option("puploc_stage")
-    pigo_b200.set_option("puploc_stage", stage)
-    try:
+    with options(puploc_stage=stage):
         rnd = randoms_for(len(images), face_cap, 41)
         got = pipeline.detect_images_angles_device(gpu_face, plc, flp, images, cp_of(TEST_PARAMS), image_angles, face_cap=face_cap,
                                                    randoms=rnd, raw=True)
@@ -262,8 +252,6 @@ def test_pipeline_each_image_equals_a_lone_detect_images(gpu_face, cascades, ima
                                                 angle=a, raw=True)
             assert int(got[1][i]) == int(one[1][0]), i
             assert got[0][i].tobytes() == one[0][0].tobytes() and got[2][i].tobytes() == one[2][0].tobytes(), (i, a)
-    finally:
-        pigo_b200.set_option("puploc_stage", saved)
     faces, nfaces, _ = got
     rotated_refined = [i for i, a in enumerate(image_angles) if a > 0 and (faces[i, :nfaces[i]]["scale"] > 50).any()]
     assert len(rotated_refined) >= 2, rotated_refined

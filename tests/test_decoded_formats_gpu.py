@@ -11,6 +11,7 @@ import torch
 import decoded_formats_oracle as F
 import pigo_b200
 from pigo_b200 import CascadeParams, ImageParams, pipeline, synth
+from option_guard import options_at_defaults   # noqa: F401 (autouse: every test ends with the options at their defaults)
 from test_decoded_gpu import Src, face_gray, gray_src, host_images, premultiplied_alpha, rgba_src, slot, ycbcr_src
 
 pytestmark = pytest.mark.gpu

@@ -11,6 +11,7 @@ import decoded_oracle as D
 import oracle_lib as O
 import pigo_b200
 from pigo_b200 import CascadeParams, DecodedImage, ImageParams, pipeline, synth
+from option_guard import options_at_defaults   # noqa: F401 (autouse: every test ends with the options at their defaults)
 
 pytestmark = pytest.mark.gpu
 

@@ -9,6 +9,7 @@ import pytest
 
 import pigo_b200
 from pigo_b200 import CascadeParams, ImageParams, synth
+from option_guard import options, options_at_defaults   # noqa: F401 (autouse: every test ends with the options at their defaults)
 from oracle.np_oracle import FaceCascade
 
 pytestmark = pytest.mark.gpu
@@ -55,14 +56,6 @@ def test_block_table_matches_host_packing(gpu_face, facefinder_bytes):
     assert got == pack_blocks(cas)
 
 
-@pytest.fixture
-def restore_knobs():
-    saved = {k: pigo_b200.get_option(k) for k in KNOBS}
-    yield
-    for k, v in saved.items():
-        pigo_b200.set_option(k, v)
-
-
 @pytest.fixture(scope="module")
 def frames():
     return synth.make_batch(NF, R, C_, "USF", seed0=31)
@@ -86,22 +79,25 @@ CASES = [
 
 
 @pytest.mark.parametrize("gather_limit,tile_ks,tile_tail_min,deep_group,queue_cap", CASES)
-def test_deep_blocks_batch_matches_oracle_and_single_frames(gpu_face, frames, oracle_dets, restore_knobs,
+def test_deep_blocks_batch_matches_oracle_and_single_frames(gpu_face, frames, oracle_dets,
                                                             gather_limit, tile_ks, tile_tail_min, deep_group, queue_cap):
-    for k, v in zip(KNOBS, (gather_limit, tile_ks, tile_tail_min, deep_group, queue_cap)):
-        pigo_b200.set_option(k, v)
     cp = CascadeParams(ImageParams(None, R, C_, C_), *PARAMS)
-    dets, cnt = gpu_face.RunCascadeBatch(frames, cp, 0.0)
-    for f in range(NF):
-        one = gpu_face.run_cascade_array(CascadeParams(ImageParams(frames[f], R, C_, C_), *PARAMS), 0.0)
-        assert cnt[f] == len(one) and dets[f, :cnt[f]].tobytes() == one.tobytes(), f"frame {f}"
-        assert one.tobytes() == oracle_dets[f].tobytes(), f"frame {f}"
+    with options(**dict(zip(KNOBS, (gather_limit, tile_ks, tile_tail_min, deep_group, queue_cap)))):
+        dets, cnt = gpu_face.RunCascadeBatch(frames, cp, 0.0)
+        for f in range(NF):
+            one = gpu_face.run_cascade_array(CascadeParams(ImageParams(frames[f], R, C_, C_), *PARAMS), 0.0)
+            assert cnt[f] == len(one) and dets[f, :cnt[f]].tobytes() == one.tobytes(), f"frame {f}"
+            assert one.tobytes() == oracle_dets[f].tobytes(), f"frame {f}"
     assert sum(len(o) for o in oracle_dets) > 0
 
 
 @pytest.mark.parametrize("deep_group", [8, 32])
-def test_deep_blocks_ragged_images_match_single_image_calls(gpu_face, frames, restore_knobs, deep_group):
-    pigo_b200.set_option("deep_group", deep_group)
+def test_deep_blocks_ragged_images_match_single_image_calls(gpu_face, frames, deep_group):
+    with options(deep_group=deep_group):
+        _ragged_images_match_single_image_calls(gpu_face, frames)
+
+
+def _ragged_images_match_single_image_calls(gpu_face, frames):
     cp = CascadeParams(ImageParams(None, R, C_, C_), *PARAMS)
     sizes = [(R, C_), (720, 1280), (1000, 1900), (480, 640), (1080, 1500), (333, 517), (900, 1920), (1079, 1919)]
     imgs = [ImageParams(np.ascontiguousarray(frames[i % NF][:r, :c]), r, c, c) for i, (r, c) in enumerate(sizes)]

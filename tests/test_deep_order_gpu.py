@@ -5,18 +5,12 @@ import pytest
 
 import pigo_b200
 from pigo_b200 import CascadeParams, ImageParams, synth
+from option_guard import options, options_at_defaults   # noqa: F401 (autouse: every test ends with the options at their defaults)
 
 pytestmark = pytest.mark.gpu
 
 PARAMS = (20, 1000, 0.2, 1.1)
 R, C = 1080, 1920
-
-
-@pytest.fixture
-def restore_queue_cap():
-    saved = pigo_b200.get_option("queue_cap")
-    yield
-    pigo_b200.set_option("queue_cap", saved)
 
 
 def _one(gpu_face, img: ImageParams, angle: float):
@@ -29,8 +23,12 @@ def _check(dets, cnt, singles):
 
 
 @pytest.mark.parametrize("queue_cap", [0, 50])
-def test_ordered_deep_queue_equals_per_frame_calls(gpu_face, oracle_face, restore_queue_cap, queue_cap):
-    pigo_b200.set_option("queue_cap", queue_cap)
+def test_ordered_deep_queue_equals_per_frame_calls(gpu_face, oracle_face, queue_cap):
+    with options(queue_cap=queue_cap):
+        _ordered_deep_queue_equals_per_frame_calls(gpu_face, oracle_face)
+
+
+def _ordered_deep_queue_equals_per_frame_calls(gpu_face, oracle_face):
     nf = 8   # 7.2 M windows
     frames = synth.make_batch(nf, R, C, "USF", seed0=7)
     cp = CascadeParams(ImageParams(None, R, C, C), *PARAMS)

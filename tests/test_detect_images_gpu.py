@@ -12,6 +12,7 @@ import pytest
 import oracle_lib as O
 import pigo_b200
 from pigo_b200 import CascadeParams, ImageParams, Puploc, pipeline, synth
+from option_guard import options, options_at_defaults   # noqa: F401 (autouse: every test ends with the options at their defaults)
 
 pytestmark = pytest.mark.gpu
 
@@ -64,15 +65,6 @@ def face_cap(gpu_face, cascades, images):
     _, n, _ = pipeline.detect_images_device(gpu_face, plc, flp, images, cp_of(CLI_PARAMS), face_cap=256, raw=True)
     _, n2, _ = pipeline.detect_images_device(gpu_face, plc, flp, images, cp_of(TEST_PARAMS), face_cap=256, raw=True)
     return int(max(n.max(), n2.max(), 1))
-
-
-@pytest.fixture
-def restore_options():
-    keys = ["puploc_stage", "puploc_mode", "scan_mode", "rot_mode"]
-    saved = {k: pigo_b200.get_option(k) for k in keys}
-    yield
-    for k, v in saved.items():
-        pigo_b200.set_option(k, v)
 
 
 def cp_of(params):
@@ -134,15 +126,15 @@ def replay_on_oracle(got, images, params, angle, randoms, eye, oracle_face, casc
 @pytest.mark.parametrize("stage", [1, 2])
 @pytest.mark.parametrize("angle", [0.0, 0.03])
 @pytest.mark.parametrize("params", [TEST_PARAMS, CLI_PARAMS])
-def test_each_image_equals_a_lone_detect_batch(gpu_face, oracle_face, cascades, images, face_cap, restore_options, params, angle, stage):
-    pigo_b200.set_option("puploc_stage", stage)
+def test_each_image_equals_a_lone_detect_batch(gpu_face, oracle_face, cascades, images, face_cap, params, angle, stage):
     plc, flp, _, _ = cascades
     eye = EYE[params]
     rnd = randoms_for(len(images), face_cap, 17)
-    got = pipeline.detect_images_device(gpu_face, plc, flp, images, cp_of(params), face_cap=face_cap, randoms=rnd, angle=angle,
-                                        eye_perturbs=eye, raw=True)
-    for i, im in enumerate(images):
-        assert_same_outputs(got, lone(gpu_face, cascades, im, params, face_cap, rnd[i:i + 1], angle, eye), [i], [0])
+    with options(puploc_stage=stage):
+        got = pipeline.detect_images_device(gpu_face, plc, flp, images, cp_of(params), face_cap=face_cap, randoms=rnd, angle=angle,
+                                            eye_perturbs=eye, raw=True)
+        for i, im in enumerate(images):
+            assert_same_outputs(got, lone(gpu_face, cascades, im, params, face_cap, rnd[i:i + 1], angle, eye), [i], [0])
     faces, nfaces, _ = got
     refined = {GEOMS[i][:3] for i in range(len(images)) if (faces[i, :nfaces[i]]["scale"] > 50).any()}
     assert len(refined) >= 3, refined
@@ -253,25 +245,27 @@ def test_concurrent_calls_get_the_sequential_results(gpu_face, cascades, images,
 
 
 @pytest.mark.parametrize("knobs,angle", [({"scan_mode": 1}, 0.0), ({"rot_mode": 1}, 0.03)])
-def test_universal_scan_options_give_the_same_results(gpu_face, cascades, images, face_cap, restore_options, knobs, angle):
+def test_universal_scan_options_give_the_same_results(gpu_face, cascades, images, face_cap, knobs, angle):
     """The images scan's own per-image fallback (universal gather kernel) under the pipeline."""
     plc, flp, _, _ = cascades
     some = [im for im in images if im.Rows * im.Cols <= 1080 * 1920]
     rnd = randoms_for(len(some), face_cap, 37)
     expect = pipeline.detect_images_device(gpu_face, plc, flp, some, cp_of(TEST_PARAMS), face_cap=face_cap, randoms=rnd, angle=angle, raw=True)
-    for k, v in knobs.items():
-        pigo_b200.set_option(k, v)
-    got = pipeline.detect_images_device(gpu_face, plc, flp, some, cp_of(TEST_PARAMS), face_cap=face_cap, randoms=rnd, angle=angle, raw=True)
+    with options(**knobs):
+        got = pipeline.detect_images_device(gpu_face, plc, flp, some, cp_of(TEST_PARAMS), face_cap=face_cap, randoms=rnd, angle=angle, raw=True)
     assert_same_outputs(got, expect)
     assert expect[1].sum() > 0
 
 
 @pytest.mark.parametrize("mode,stage", [(0, 0), (0, 1), (0, 2), (1, 0)])
-def test_puploc_run_images_matches_the_oracle(restore_options, mode, stage):
+def test_puploc_run_images_matches_the_oracle(mode, stage):
     """Both RunDetector kernels' image-table variants: seeds inside and past the borders of tall, wide and padded images,
     flips, Perturbs 0..63, rotated and not."""
-    pigo_b200.set_option("puploc_mode", mode)
-    pigo_b200.set_option("puploc_stage", stage)
+    with options(puploc_mode=mode, puploc_stage=stage):
+        _puploc_run_images_matches_the_oracle()
+
+
+def _puploc_run_images_matches_the_oracle():
     ims = [make_image(700, 260, 272, "F", 3), make_image(300, 900, 912, "F", 4), make_image(333, 517, 531, "F", 5),
            ImageParams(synth.sample_gray(), 400, 320, 320), make_image(96, 128, 144, "S", 6)]
     rng = np.random.default_rng(77)

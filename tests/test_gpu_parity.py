@@ -7,6 +7,7 @@ import pytest
 import oracle_lib as O
 import pigo_b200
 from pigo_b200 import CascadeParams, ImageParams, Puploc, synth
+from option_guard import options, options_at_defaults   # noqa: F401 (autouse: every test ends with the options at their defaults)
 
 pytestmark = pytest.mark.gpu
 
@@ -241,73 +242,91 @@ def test_get_landmark_point_vs_oracle(sample_gray):
 
 
 # ---- scan implementation variants (tiled shared-memory kernel vs gather kernel) ------------------------------
+# Each variant names the kernels it runs on one 720p frame (TEST_PARAMS), and the test asserts them: a variant whose kernel
+# falls back on this geometry fails rather than testing another path.  "universal": the standalone gather kernel alone;
+# "classic" / "head" / "ptab": the fused kernel with that tile role (classic lane refill, dense head, per-scale offset
+# tables); "gather": the gather-v2 kernel; "deep": the deep kernel.
 VARIANTS = [
-    {"scan_mode": 1},                                                     # gather kernel only
-    {"scan_mode": 0},                                                     # default: tiled + gather + resume
-    {"scan_mode": 0, "tile_ni": 1, "tile_warps": 4, "tile_ks": 16, "tile_tail_min": 33},   # everything spills early
-    {"scan_mode": 0, "tile_ni": 4, "tile_warps": 12, "tile_ks": 128, "tile_tail_min": 0},  # nothing spills at tails
-    {"scan_mode": 0, "tile_ni": 3, "tile_warps": 16, "tile_ks": 468, "tile_band_ratio": 130},
-    {"scan_mode": 0, "tile_max_scale": 30, "chunk": 64},
-    {"scan_mode": 0, "gather_warps": 0, "tile_warps": 8, "tile_ni": 2},               # tiles fused kernel + separate gather launch
-    {"scan_mode": 0, "gather_warps": 24, "tile_warps": 8, "tile_ni": 1, "tile_ks": 32},
-    {"scan_mode": 3, "gather_ks": 32, "gather_ni": 1, "sub_batch": 2, "lanes": 2},      # gather-v2 + deep kernel only
-    {"scan_mode": 0, "gather_ni": 3, "sub_batch": 1, "lanes": 3},
-    {"scan_mode": 0, "deep_group": 32, "tile_ks": 8, "gather_ks": 8},
-    {"scan_mode": 0, "tile_tail_min": 33, "tile_ks": 5, "gather_ks": 7},
-    {"scan_mode": 0, "gather_block": 8, "tile_prefetch": 1, "deep_group": 16},
-    {"scan_mode": 0, "fused_smem_kb": 160, "tile_warps": 14, "gather_warps": 18},
-    {"scan_mode": 0, "tile_warps": 4, "gather_warps": 28, "tile_max_scale": 24},
-    {"scan_mode": 3, "gather_block": 16, "gather_ni": 2},
-    {"scan_mode": 3, "gather_ks": 4},                                                   # nearly everything through the deep kernel
-    {"scan_mode": 0, "gather_ks": 468, "tile_ks": 468, "tile_warps": 4, "gather_warps": 0},   # whole cascade resident: no Q2
-    {"scan_mode": 0, "deep_flat": 1, "deep_group": 8, "tile_ks": 6},                          # flat deep loop, lots of Q2 traffic
-    {"scan_mode": 3, "deep_flat": 1, "deep_group": 16, "gather_ks": 3},
-    {"scan_mode": 0, "tile_head": 2, "tile_warps": 22},                                       # dense head over trees 0..1, ring + generic tail
-    {"scan_mode": 0, "tile_head": 1, "tile_warps": 24, "head_back": 1},
-    {"scan_mode": 0, "tile_ptab": 1},                                                         # per-scale offset tables, scale-synchronous rounds
-    {"scan_mode": 0, "tile_ptab": 1, "ptab_kt": 4, "ptab_ks": 6, "tile_warps": 7, "gather_warps": 3},
-    {"scan_mode": 0, "tile_ptab": 1, "ptab_kt": 468, "tile_tail_min": 33, "tile_warps": 12},  # capped at 60 trees; every drained tile spills
-    {"scan_mode": 0, "tile_ptab": 1, "ptab_kt": 5, "tile_tail_min": 0, "gather_warps": 0, "tile_warps": 16},
-    {"scan_mode": 0, "tile_ptab": 1, "ptab_kt": 1, "tile_max_scale": 30, "tile_band_ratio": 110},   # many narrow bands
-    {"scan_mode": 0, "queue_cap": 40, "tile_ks": 4, "gather_ks": 6, "tile_tail_min": 33},     # both queues overflow: producers finish their windows in place
-    {"scan_mode": 0, "queue_cap": 7, "tile_ptab": 1, "ptab_kt": 3, "ptab_ks": 5, "tile_tail_min": 33},
-    {"scan_mode": 3, "queue_cap": 16, "gather_ks": 2},
-    {"scan_mode": 0, "deep_smem": 1, "deep_smem_k": 468, "deep_smem_lo": 0},                                                         # deep kernel, tree records in shared memory
-    {"scan_mode": 0, "deep_smem": 1, "deep_group": 4, "gather_limit": 4, "tile_ks": 6, "deep_smem_threads": 512, "deep_smem_k": 30, "deep_smem_lo": 11},   # + entries below its first resident tree
-    {"scan_mode": 3, "deep_smem": 1, "deep_group": 32, "gather_ks": 3, "deep_smem_threads": 256},
-    {"scan_mode": 0, "tile_head": 3, "tile_warps": 6, "tile_ks": 5, "head_back": 16, "tile_tail_min": 33},   # everything spills, tiny prefix
-    {"scan_mode": 0, "tile_head": 4, "tile_warps": 12, "tile_ks": 63, "gather_warps": 0, "tile_tail_min": 0},
-    {"scan_mode": 0, "tile_head": 2, "tile_ks": 2},                                           # prefix not longer than the head: classic kernel
+    ({"scan_mode": 1}, "universal"),
+    ({"scan_mode": 0}, "classic deep"),                                  # default: fused kernel (tile + gather warps) + deep
+    ({"scan_mode": 0, "tile_ni": 1, "tile_warps": 4, "tile_ks": 16, "tile_tail_min": 33}, "classic deep"),   # everything spills early
+    ({"scan_mode": 0, "tile_ni": 4, "tile_warps": 12, "tile_ks": 128, "tile_tail_min": 0}, "classic deep"),  # nothing spills at tails
+    ({"scan_mode": 0, "tile_ni": 3, "tile_warps": 16, "tile_ks": 200, "tile_band_ratio": 130}, "classic gather deep"),   # no room for gather warps
+    ({"scan_mode": 0, "tile_max_scale": 30, "chunk": 64}, "classic deep"),
+    ({"scan_mode": 0, "gather_warps": 0, "tile_warps": 8, "tile_ni": 2}, "classic gather deep"),   # tiles fused kernel + separate gather launch
+    ({"scan_mode": 0, "gather_warps": 24, "tile_warps": 8, "tile_ni": 1, "tile_ks": 32}, "classic deep"),
+    ({"scan_mode": 3, "gather_ks": 32, "gather_ni": 1, "sub_batch": 2, "lanes": 2}, "gather deep"),   # gather-v2 + deep kernel only
+    ({"scan_mode": 0, "gather_ni": 3, "sub_batch": 1, "lanes": 3}, "classic deep"),
+    ({"scan_mode": 0, "deep_group": 32, "tile_ks": 8, "gather_ks": 8}, "classic deep"),
+    ({"scan_mode": 0, "tile_tail_min": 33, "tile_ks": 5, "gather_ks": 7}, "classic deep"),
+    ({"scan_mode": 0, "gather_block": 8, "tile_prefetch": 1, "deep_group": 16}, "classic deep"),
+    ({"scan_mode": 0, "fused_smem_kb": 160, "tile_warps": 14, "gather_warps": 18}, "classic deep"),
+    ({"scan_mode": 0, "tile_warps": 4, "gather_warps": 28, "tile_max_scale": 24}, "classic deep"),
+    ({"scan_mode": 3, "gather_block": 16, "gather_ni": 2}, "gather deep"),
+    ({"scan_mode": 3, "gather_ks": 4}, "gather deep"),                                                  # nearly everything through the deep kernel
+    # no room for tiles beside a 446-tree prefix: gather-v2 alone keeps 446 trees resident, the deep kernel walks the last 22
+    ({"scan_mode": 0, "gather_ks": 468, "gather_limit": 468, "tile_ks": 468, "tile_warps": 4, "gather_warps": 0}, "gather deep"),
+    ({"scan_mode": 0, "deep_flat": 1, "deep_group": 8, "tile_ks": 6}, "classic deep"),                   # flat deep loop, lots of Q2 traffic
+    ({"scan_mode": 3, "deep_flat": 1, "deep_group": 16, "gather_ks": 3}, "gather deep"),
+    ({"scan_mode": 0, "tile_head": 2, "tile_warps": 22}, "head deep"),                                   # dense head over trees 0..1, ring + generic tail
+    ({"scan_mode": 0, "tile_head": 1, "tile_warps": 24, "head_back": 1}, "head deep"),
+    ({"scan_mode": 0, "tile_ptab": 1}, "ptab deep"),                                                     # per-scale offset tables, scale-synchronous rounds
+    ({"scan_mode": 0, "tile_ptab": 1, "ptab_kt": 4, "ptab_ks": 6, "tile_warps": 7, "gather_warps": 3}, "ptab deep"),
+    ({"scan_mode": 0, "tile_ptab": 1, "ptab_kt": 468, "tile_tail_min": 33, "tile_warps": 12}, "ptab deep"),   # capped at 60 trees; every drained tile spills
+    ({"scan_mode": 0, "tile_ptab": 1, "ptab_kt": 5, "tile_tail_min": 0, "gather_warps": 0, "tile_warps": 16}, "ptab gather deep"),
+    ({"scan_mode": 0, "tile_ptab": 1, "ptab_kt": 1, "tile_max_scale": 30, "tile_band_ratio": 110}, "ptab deep"),   # many narrow bands
+    ({"scan_mode": 0, "queue_cap": 40, "tile_ks": 4, "gather_ks": 6, "tile_tail_min": 33}, "classic deep"),   # both queues overflow: producers finish their windows in place
+    ({"scan_mode": 0, "queue_cap": 7, "tile_ptab": 1, "ptab_kt": 3, "ptab_ks": 5, "tile_tail_min": 33}, "ptab deep"),
+    ({"scan_mode": 3, "queue_cap": 16, "gather_ks": 2}, "gather deep"),
+    ({"scan_mode": 0, "deep_smem": 1, "deep_smem_k": 468, "deep_smem_lo": 0}, "classic deep"),          # deep kernel, tree records in shared memory
+    ({"scan_mode": 0, "deep_smem": 1, "deep_group": 4, "gather_limit": 4, "tile_ks": 6, "deep_smem_threads": 512, "deep_smem_k": 30, "deep_smem_lo": 11},
+     "classic deep"),                                                                                    # + entries below its first resident tree
+    ({"scan_mode": 3, "deep_smem": 1, "deep_group": 32, "gather_ks": 3, "deep_smem_threads": 256}, "gather deep"),
+    # everything spills, tiny prefix (tile_max_scale keeps the tiled ladder within the head's 16 table slots)
+    ({"scan_mode": 0, "tile_head": 3, "tile_warps": 6, "tile_ks": 5, "head_back": 16, "tile_tail_min": 33, "tile_max_scale": 60}, "head deep"),
+    ({"scan_mode": 0, "tile_head": 4, "tile_warps": 12, "tile_ks": 63, "gather_warps": 0, "tile_tail_min": 0}, "head gather deep"),
+    ({"scan_mode": 0, "tile_head": 2, "tile_ks": 2}, "classic deep"),                                   # prefix not longer than the head: classic kernel
 ]
 
 
-@pytest.fixture
-def restore_options():
-    keys = ["scan_mode", "tile_ni", "tile_warps", "tile_ks", "tile_tail_min", "tile_band_ratio", "tile_max_scale", "chunk",
-            "gather_warps", "gather_ks", "gather_ni", "sub_batch", "lanes", "deep_group", "gather_block", "fused_smem_kb", "tile_prefetch", "deep_flat", "tile_head", "head_back"]
-    saved = {k: pigo_b200.get_option(k) for k in keys}
-    yield
-    for k, v in saved.items():
-        pigo_b200.set_option(k, v)
+def run_timed(fn):
+    """fn() with per-kernel timing on; returns its result and the launch counts of the fused, gather and deep kernel slots."""
+    with options(timing=1):
+        out = fn()
+        launches = {k: pigo_b200.get_option(k) for k in ("t_tiled_n", "t_gather_n", "t_deep_n")}
+    return out, launches
 
 
-@pytest.mark.parametrize("variant", VARIANTS)
-def test_scan_variants_agree_with_oracle(gpu_face, oracle_face, sample_gray, restore_options, variant):
-    for k, v in variant.items():
-        pigo_b200.set_option(k, v)
+def assert_kernels(expect: str, launches: dict, rows, cols, prm, nframes, groups=1):
+    """The launches of one call (of `groups` pipeline groups) are the kernels `expect` names, and the fused kernel's tile role
+    is the one the planner picks for the call (describe_plan with the call's frame count)."""
+    k = expect.split()
+    role = next((r for r in k if r in ("classic", "head", "ptab")), None)
+    want = {"t_tiled_n": groups * (role is not None), "t_gather_n": groups * ("gather" in k or "universal" in k), "t_deep_n": groups * ("deep" in k)}
+    assert launches == want, f"expected {expect}"
+    if role is not None:
+        p = pigo_b200.describe_plan(rows, cols, *prm, nframes=nframes)
+        assert ("head" if p["head"] else "ptab" if p["ptab_kt"] else "classic") == role, p
+
+
+@pytest.mark.parametrize("variant,expect", VARIANTS, ids=[f"variant{i}" for i in range(len(VARIANTS))])
+def test_scan_variants_agree_with_oracle(gpu_face, oracle_face, sample_gray, variant, expect):
     frames = synth.make_batch(3, 720, 1280, "SFU", seed0=21)
     cases = [(frames[0], 720, 1280, 1280, TEST_PARAMS), (frames[1], 720, 1280, 1280, DOC_PARAMS),
              (frames[2], 720, 1280, 1280, CLI_PARAMS), (sample_gray, 400, 320, 320, (20, 1000, 0.05, 1.05))]
-    for img, r, c, d, prm in cases:
-        g = gpu_face.run_cascade_array(cp_of(img, r, c, d, prm), 0.0)
-        assert_same(g, oracle_face.run_cascade(img, r, c, d, *prm, 0.0))
-    # unaligned stride (Dim % 16 != 0) takes the byte-wise tile fill
-    buf = np.zeros((301, 523), dtype=np.uint8)
-    buf[:, :500] = synth.frame_faces(None, 301, 500, shift=(3, 1), noise_seed=8)
-    g = gpu_face.run_cascade_array(cp_of(buf, 301, 500, 523, TEST_PARAMS), 0.0)
-    assert_same(g, oracle_face.run_cascade(buf, 301, 500, 523, *TEST_PARAMS, 0.0))
-    # batch with the deep queue shared by several frames
-    dets, cnt = gpu_face.RunCascadeBatch(frames, cp_of(None, 720, 1280, 1280, TEST_PARAMS), 0.0, cap_per_frame=512)
+    with options(**variant):
+        _, launches = run_timed(lambda: gpu_face.run_cascade_array(cp_of(frames[0], 720, 1280, 1280, TEST_PARAMS), 0.0))
+        assert_kernels(expect, launches, 720, 1280, TEST_PARAMS, 1)
+        for img, r, c, d, prm in cases:
+            g = gpu_face.run_cascade_array(cp_of(img, r, c, d, prm), 0.0)
+            assert_same(g, oracle_face.run_cascade(img, r, c, d, *prm, 0.0))
+        # unaligned stride (Dim % 16 != 0) takes the byte-wise tile fill
+        buf = np.zeros((301, 523), dtype=np.uint8)
+        buf[:, :500] = synth.frame_faces(None, 301, 500, shift=(3, 1), noise_seed=8)
+        g = gpu_face.run_cascade_array(cp_of(buf, 301, 500, 523, TEST_PARAMS), 0.0)
+        assert_same(g, oracle_face.run_cascade(buf, 301, 500, 523, *TEST_PARAMS, 0.0))
+        # batch with the deep queue shared by several frames
+        dets, cnt = gpu_face.RunCascadeBatch(frames, cp_of(None, 720, 1280, 1280, TEST_PARAMS), 0.0, cap_per_frame=512)
     for f in range(3):
         o = oracle_face.run_cascade(frames[f], 720, 1280, 1280, *TEST_PARAMS, 0.0)
         assert cnt[f] == len(o) and dets[f, :cnt[f]].tobytes() == o.tobytes()
@@ -443,7 +462,7 @@ def _synthetic_cascade(depth: int, ntrees: int, seed: int) -> bytes:
 
 
 @pytest.mark.parametrize("depth,ntrees", [(6, 3), (6, 70), (4, 9), (1, 2), (8, 5), (6, 1)])
-def test_synthetic_cascades_other_depths_and_sizes(depth, ntrees, restore_options):
+def test_synthetic_cascades_other_depths_and_sizes(depth, ntrees):
     """Generic tree depth (universal gather kernel) and tiny / odd-sized depth-6 cascades (resident prefix larger than the
     cascade, Q2 never used, ...), unrotated and rotated."""
     pk = _synthetic_cascade(depth, ntrees, seed=depth * 100 + ntrees)
@@ -485,29 +504,29 @@ def test_4k_rotated_every_table_slot(gpu_face, oracle_face, frame_4k, k):
     assert_same(g, oracle_face.run_cascade(frame_4k, 2160, 3840, 3840, *TEST_PARAMS, k / 32.0))
 
 
-@pytest.fixture
-def restore_round2_options():
-    keys = ["rot_mode", "puploc_mode", "puploc_stage", "deep_group", "deep_flat", "gather_ks", "gather_ni", "host_stream", "copy_chunk", "sub_batch", "gather_block", "tile_warps", "scan_mode"]
-    saved = {k: pigo_b200.get_option(k) for k in keys}
-    yield
-    for k, v in saved.items():
-        pigo_b200.set_option(k, v)
+ROTATED_VARIANTS = [
+    ({"rot_mode": 1}, "universal"),
+    ({"rot_mode": 0, "gather_ks": 4, "deep_group": 8}, "gather deep"),
+    ({"rot_mode": 0, "gather_ni": 2, "deep_group": 16}, "gather deep"),
+    ({"rot_mode": 0, "gather_ks": 468, "gather_limit": 468, "deep_group": 32}, "gather deep"),   # 446 trees resident, the deep kernel walks the last 22
+    ({"rot_mode": 0, "gather_block": 8, "sub_batch": 1}, "gather deep"),
+]
 
 
-@pytest.mark.parametrize("variant", [{"rot_mode": 1}, {"rot_mode": 0, "gather_ks": 4, "deep_group": 8}, {"rot_mode": 0, "gather_ni": 2, "deep_group": 16},
-                                     {"rot_mode": 0, "gather_ks": 468, "deep_group": 32}, {"rot_mode": 0, "gather_block": 8, "sub_batch": 1}])
-def test_rotated_kernel_variants(gpu_face, oracle_face, sample_gray, restore_round2_options, variant):
-    """Universal gather kernel vs table-driven kernels, tiny / whole resident prefix (everything / nothing through the deep kernel)."""
-    for k, v in variant.items():
-        pigo_b200.set_option(k, v)
+@pytest.mark.parametrize("variant,expect", ROTATED_VARIANTS, ids=[f"variant{i}" for i in range(len(ROTATED_VARIANTS))])
+def test_rotated_kernel_variants(gpu_face, oracle_face, sample_gray, variant, expect):
+    """Universal gather kernel vs table-driven kernels (gather-v2 + deep), tiny / longest resident prefix."""
     wide = synth.frame_faces(sample_gray, 300, 900, noise_seed=1)       # cols > rows: the nrows-1 column clamp bites
     tall = synth.frame_faces(sample_gray, 700, 260, noise_seed=2)
-    for img, r, c in ((sample_gray, 400, 320), (wide, 300, 900), (tall, 700, 260)):
-        for a in (1 / 32.0, 0.26, 0.5, 0.77, 1.0):
-            g = gpu_face.run_cascade_array(cp_of(img, r, c, c, TEST_PARAMS), a)
-            assert_same(g, oracle_face.run_cascade(img, r, c, c, *TEST_PARAMS, a))
     frames = synth.make_batch(3, 360, 640, "FSU", seed0=41)
-    dets, cnt = gpu_face.RunCascadeBatch(frames, cp_of(None, 360, 640, 640, DOC_PARAMS), 0.4, cap_per_frame=64)
+    with options(**variant):
+        _, launches = run_timed(lambda: gpu_face.run_cascade_array(cp_of(sample_gray, 400, 320, 320, TEST_PARAMS), 0.26))
+        assert_kernels(expect, launches, 400, 320, TEST_PARAMS, 1)
+        for img, r, c in ((sample_gray, 400, 320), (wide, 300, 900), (tall, 700, 260)):
+            for a in (1 / 32.0, 0.26, 0.5, 0.77, 1.0):
+                g = gpu_face.run_cascade_array(cp_of(img, r, c, c, TEST_PARAMS), a)
+                assert_same(g, oracle_face.run_cascade(img, r, c, c, *TEST_PARAMS, a))
+        dets, cnt = gpu_face.RunCascadeBatch(frames, cp_of(None, 360, 640, 640, DOC_PARAMS), 0.4, cap_per_frame=64)
     for f in range(3):
         o = oracle_face.run_cascade(frames[f], 360, 640, 640, *DOC_PARAMS, 0.4)
         assert cnt[f] == len(o) and dets[f, :cnt[f]].tobytes() == o.tobytes()
@@ -553,32 +572,46 @@ def test_host_frames_with_tight_stride_and_short_last_frame(gpu_face, oracle_fac
         assert cnt[f] == len(o) and out[f, :cnt[f]].tobytes() == o.tobytes()
 
 
-@pytest.mark.parametrize("variant", [{"host_stream": 0}, {"host_stream": 1, "copy_chunk": 1, "sub_batch": 4}, {"host_stream": 1, "copy_chunk": 3},
-                                     {"host_stream": 1, "copy_chunk": 100, "deep_flat": 1}, {"host_stream": 1, "scan_mode": 3}, {"host_stream": 1, "tile_warps": 0}])
-def test_host_frames_streamed_behind_the_copy(gpu_face, oracle_face, restore_round2_options, variant):
+# (options, kernels of the unrotated 11-frame call, pipeline groups of that call)
+HOST_STREAM_VARIANTS = [
+    ({"host_stream": 0}, "classic deep", 1),
+    ({"host_stream": 1, "copy_chunk": 1, "sub_batch": 4}, "classic deep", 3),
+    ({"host_stream": 1, "copy_chunk": 3}, "classic deep", 1),
+    ({"host_stream": 1, "copy_chunk": 100, "deep_flat": 1}, "classic deep", 1),
+    ({"host_stream": 1, "scan_mode": 3}, "gather deep", 1),
+    ({"host_stream": 1, "tile_warps": 0}, "gather deep", 1),    # no tile warps: the fused kernel does not run
+]
+
+
+@pytest.mark.parametrize("variant,expect,groups", HOST_STREAM_VARIANTS, ids=[f"variant{i}" for i in range(len(HOST_STREAM_VARIANTS))])
+def test_host_frames_streamed_behind_the_copy(gpu_face, oracle_face, variant, expect, groups):
     """Host frames: the scan kernels start at once and wait in-kernel for each frame's copy chunk (ready counter); the result
     must not depend on the chunking, the grouping, or on whether the polling fused kernel runs at all for the geometry."""
-    for k, v in variant.items():
-        pigo_b200.set_option(k, v)
     frames = synth.make_batch(11, 270, 480, "USF", seed0=77)
-    for ang in (0.0, 0.3):
-        dets, cnt = gpu_face.RunCascadeBatch(frames, cp_of(None, 270, 480, 480, TEST_PARAMS), ang, cap_per_frame=128)
-        for f in range(11):
-            o = oracle_face.run_cascade(frames[f], 270, 480, 480, *TEST_PARAMS, ang)
-            assert cnt[f] == len(o) and dets[f, :cnt[f]].tobytes() == o.tobytes()
     tiny = synth.make_batch(3, 30, 40, "UUU", seed0=2)      # no tileable band: the fused kernel does not run
-    dets, cnt = gpu_face.RunCascadeBatch(tiny, cp_of(None, 30, 40, 40, (20, 30, 0.1, 1.1)), 0.0, cap_per_frame=64)
+    with options(**variant):
+        for ang in (0.0, 0.3):
+            (dets, cnt), launches = run_timed(lambda: gpu_face.RunCascadeBatch(frames, cp_of(None, 270, 480, 480, TEST_PARAMS), ang, cap_per_frame=128))
+            if ang == 0.0:
+                assert_kernels(expect, launches, 270, 480, TEST_PARAMS, 11, groups)
+            for f in range(11):
+                o = oracle_face.run_cascade(frames[f], 270, 480, 480, *TEST_PARAMS, ang)
+                assert cnt[f] == len(o) and dets[f, :cnt[f]].tobytes() == o.tobytes()
+        dets, cnt = gpu_face.RunCascadeBatch(tiny, cp_of(None, 30, 40, 40, (20, 30, 0.1, 1.1)), 0.0, cap_per_frame=64)
     for f in range(3):
         o = oracle_face.run_cascade(tiny[f], 30, 40, 40, 20, 30, 0.1, 1.1, 0.0)
         assert cnt[f] == len(o) and dets[f, :cnt[f]].tobytes() == o.tobytes()
 
 
 @pytest.mark.parametrize("mode,stage", [(0, 2), (0, 1), (0, 0), (1, 0)])
-def test_puploc_kernels_agree_with_oracle(sample_gray, restore_round2_options, mode, stage):
+def test_puploc_kernels_agree_with_oracle(sample_gray, mode, stage):
     """Both RunDetector kernels ((perturbation, tree)-pair kernel and warp-per-perturbation kernel), rotated and not,
     flips, Perturbs 0..63, seeds near and beyond the image border, on a frame batch."""
-    pigo_b200.set_option("puploc_mode", mode)
-    pigo_b200.set_option("puploc_stage", stage)
+    with options(puploc_mode=mode, puploc_stage=stage):
+        _puploc_kernels_agree_with_oracle(sample_gray)
+
+
+def _puploc_kernels_agree_with_oracle(sample_gray):
     rng = np.random.default_rng(123)
     frames = np.stack([sample_gray, np.roll(sample_gray, 13, axis=1), 255 - sample_gray])
     for pkname in ("puploc", "lps/lp93"):
@@ -637,28 +670,28 @@ def _check_pipeline_against_oracle(got, frames, rows, cols, oracle_face, oplc, o
 
 
 @pytest.mark.parametrize("angle,stage", [(0.0, 1), (0.03, 1), (0.0, 2), (0.03, 2)])
-def test_device_pipeline_vs_oracle(gpu_face, oracle_face, sample_gray, restore_round2_options, angle, stage):
+def test_device_pipeline_vs_oracle(gpu_face, oracle_face, sample_gray, angle, stage):
     """pigo_detect_batch (SURVEY.md 8f N1): the whole face -> cluster -> eye seeds -> RunDetector x2 -> landmark seeds ->
     15 x RunDetector sequence on the device in one call, replayed step by step on the CPU oracle with the same injected
     randoms (core/flploc_test.go:75-154; angle > 0 like cmd/pigo/main.go:422 passes det.angle to the eye RunDetector)."""
     from pigo_b200 import pipeline
-    pigo_b200.set_option("puploc_stage", stage)
     plc, flp, oplc, oflp = _pipeline_cascades()
     frames = np.stack([synth.frame_faces(sample_gray, 540, 960, shift=(40 * i, 25 * i), noise_seed=30 + i) for i in range(3)] +
                       [synth.frame_noise(540, 960, 5)])
     cp = cp_of(None, 540, 960, 960, TEST_PARAMS)
     face_cap = 24
     randoms = np.random.default_rng(8).random((4, face_cap, 17, 63, 3), dtype=np.float32)
-    got = pipeline.detect_batch_device(gpu_face, plc, flp, frames, cp, iou=0.1, face_cap=face_cap, randoms=randoms, angle=angle)
+    with options(puploc_stage=stage):
+        got = pipeline.detect_batch_device(gpu_face, plc, flp, frames, cp, iou=0.1, face_cap=face_cap, randoms=randoms, angle=angle)
+        # resident frames give the same answer
+        df = pigo_b200.DeviceFrames(frames)
+        try:
+            got2 = pipeline.detect_batch_device(gpu_face, plc, flp, df, cp, iou=0.1, face_cap=face_cap, randoms=randoms, angle=angle)
+        finally:
+            df.free()
     n = _check_pipeline_against_oracle(got, frames, 540, 960, oracle_face, oplc, oflp, randoms, face_cap, angle=angle)
     assert n >= 3 or angle > 0
     assert got[3] == [] or all(fc.left_eye is None or fc.det[2] > 50 for fc in got[3])
-    # resident frames give the same answer
-    df = pigo_b200.DeviceFrames(frames)
-    try:
-        got2 = pipeline.detect_batch_device(gpu_face, plc, flp, df, cp, iou=0.1, face_cap=face_cap, randoms=randoms, angle=angle)
-    finally:
-        df.free()
     assert got2 == got
 
 

@@ -9,6 +9,7 @@ import pytest
 
 import pigo_b200
 from pigo_b200 import CascadeParams, ImageParams, synth
+from option_guard import options, options_at_defaults   # noqa: F401 (autouse: every test ends with the options at their defaults)
 
 pytestmark = pytest.mark.gpu
 
@@ -136,18 +137,12 @@ KNOBS = [{"queue_cap": 1}, {"queue_cap": 16, "gather_ks": 2}, {"gather_ks": 8}, 
 @pytest.mark.parametrize("knobs", KNOBS)
 def test_options_leave_the_outputs_unchanged(gpu_face, wide, knobs):
     expect = {a: gpu_face.RunCascadeImages(wide, cp_of(TEST_PARAMS), a) for a in (0.0, 0.5)}
-    saved = {k: pigo_b200.get_option(k) for k in knobs}
-    try:
-        for k, v in knobs.items():
-            pigo_b200.set_option(k, v)
+    with options(**knobs):
         for a, (ed, ec) in expect.items():
             d, c = gpu_face.RunCascadeImages(wide, cp_of(TEST_PARAMS), a)
             assert np.array_equal(c, ec), a
             for i in range(len(wide)):
                 assert d[i, :c[i]].tobytes() == ed[i, :ec[i]].tobytes(), (a, i)
-    finally:
-        for k, v in saved.items():
-            pigo_b200.set_option(k, v)
 
 
 def test_cascade_of_another_depth_takes_the_single_image_path(mixed):

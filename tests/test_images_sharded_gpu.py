@@ -13,6 +13,7 @@ import pytest
 import oracle_lib as O
 import pigo_b200
 from pigo_b200 import CascadeParams, ImageParams, pipeline, synth
+from option_guard import options, options_at_defaults   # noqa: F401 (autouse: every test ends with the options at their defaults)
 from test_decoded_formats_gpu import PALETTED, face_sources, narrow_sources, sources, wide_src  # noqa: F401 (fixtures)
 from test_decoded_gpu import host_images, ycbcr_src
 from test_images_gpu import MIXED, make_image
@@ -35,10 +36,9 @@ def cp_of(params=TEST_PARAMS):
 
 @pytest.fixture(autouse=True)
 def shard_split():
-    """Sets option shard_split for a test and restores it afterwards."""
-    old = pigo_b200.get_option("shard_split")
-    yield lambda k: pigo_b200.set_option("shard_split", k)
-    pigo_b200.set_option("shard_split", old)
+    """Sets option shard_split within a test; every option is restored afterwards."""
+    with options():
+        yield lambda k: pigo_b200.set_option("shard_split", k)
 
 
 @pytest.fixture(scope="module")

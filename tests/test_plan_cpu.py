@@ -6,10 +6,11 @@ import numpy as np
 import pytest
 
 import pigo_b200
+from option_guard import options, options_at_defaults   # noqa: F401 (autouse: every test ends with the options at their defaults)
 
 
-def _check(rows, cols, prm):
-    p = pigo_b200.describe_plan(rows, cols, *prm)
+def _check(rows, cols, prm, nframes=None):
+    p = pigo_b200.describe_plan(rows, cols, *prm, nframes=nframes)
     scales = p["scales"]
     assert sum(e[3] * e[4] for e in scales) == p["windows"] == pigo_b200.count_windows(rows, cols, *prm)
     covered = 0
@@ -45,30 +46,20 @@ def test_tiles_partition_windows_and_contain_all_samples(geom, prm):
 def test_plan_follows_the_tuning_options():
     base = _check(1080, 1920, (20, 1000, 0.2, 1.1))
     assert base["bands"] and base["bands"][0]["scale_lo"] == 0
-    saved = {k: pigo_b200.get_option(k) for k in ("tile_warps", "tile_max_scale", "tile_ks")}
-    try:
-        pigo_b200.set_option("tile_warps", 8)
+    with options(tile_warps=8):
         big = _check(1080, 1920, (20, 1000, 0.2, 1.1))
         assert big["tile_bytes"] > base["tile_bytes"] and big["first_untiled"] >= base["first_untiled"]
-        pigo_b200.set_option("tile_max_scale", 24)
-        small = _check(1080, 1920, (20, 1000, 0.2, 1.1))
+        with options(tile_max_scale=24):
+            small = _check(1080, 1920, (20, 1000, 0.2, 1.1))
         assert small["first_untiled"] == 3      # scales 20, 22, 24
-    finally:
-        for k, v in saved.items():
-            pigo_b200.set_option(k, v)
 
 
 def test_offset_table_kernel_plan_keeps_the_tile_invariants():
     """tile_ptab=1 (scan_ptab_kernel) moves the tiles behind two table buffers: same partition / containment invariants, a smaller
     tile budget, offsets that fit 16 bits, at most 32 tiled ladder entries."""
-    saved = {k: pigo_b200.get_option(k) for k in ("tile_ptab", "ptab_kt", "ptab_ks", "tile_warps")}
-    try:
-        base = _check(1080, 1920, (20, 1000, 0.2, 1.1))
-        pigo_b200.set_option("tile_ptab", 1)
-        for kt, ks, warps in ((16, 24, 24), (4, 6, 7), (60, 48, 12), (1, 1, 24)):
-            pigo_b200.set_option("ptab_kt", kt)
-            pigo_b200.set_option("ptab_ks", ks)
-            pigo_b200.set_option("tile_warps", warps)
+    base = _check(1080, 1920, (20, 1000, 0.2, 1.1))
+    for kt, ks, warps in ((16, 24, 24), (4, 6, 7), (60, 48, 12), (1, 1, 24)):
+        with options(tile_ptab=1, ptab_kt=kt, ptab_ks=ks, tile_warps=warps):
             for geom, prm in (((1080, 1920), (20, 1000, 0.2, 1.1)), ((2160, 3840), (20, 1000, 0.1, 1.1)), ((97, 131), (12, 90, 0.05, 1.05))):
                 p = _check(geom[0], geom[1], prm)
                 if p["ptab_kt"] == 0:        # more than 32 tiled ladder entries: the planner falls back to the classic kernel
@@ -79,6 +70,43 @@ def test_offset_table_kernel_plan_keeps_the_tile_invariants():
                     assert b["rows_t"] * (b["pitch"] + 1) < 65536
                 if warps == 24 and geom == (1080, 1920) and kt == 16:
                     assert p["tiles_off"] > base["tiles_off"] and p["tile_bytes"] <= base["tile_bytes"]
-    finally:
-        for k, v in saved.items():
-            pigo_b200.set_option(k, v)
+
+
+GEOMS = [(1080, 1920), (2160, 3840), (400, 320), (97, 131), (720, 1280), (33, 4000)]
+PARAMS = [(20, 1000, 0.2, 1.1), (20, 1000, 0.1, 1.1), (20, 1000, 0.15, 1.15), (12, 90, 0.05, 1.05), (64, 400, 0.3, 1.3)]
+
+
+@pytest.mark.parametrize("geom", GEOMS)
+@pytest.mark.parametrize("ratio", [0, 110, 130, 400])
+@pytest.mark.parametrize("head", [1, 2, 3, 4])
+def test_single_frame_plans_keep_the_invariants_and_the_dense_head_rules(geom, ratio, head):
+    """What one-frame calls run: the band ratio the library picks for them (0 = auto: 140 up to 2 M windows per call, else
+    200) or a forced one, with the dense head asked for.  The tiles keep the partition / containment invariants, and
+    where the planner keeps the head, the geometry satisfies what the head kernel needs: a resident prefix longer than
+    the head and short enough for a ring entry's 6-bit tree field, at most 16 tiled ladder entries (its table slots),
+    window sizes that fit the ring entry's 8-bit field, and int16 tile offsets."""
+    for prm in PARAMS:
+        with options(tile_head=head, tile_band_ratio=ratio):
+            p = _check(geom[0], geom[1], prm, nframes=1)
+        assert p["band_ratio"] == (ratio if ratio else (140 if p["windows"] <= 2000000 else 200))
+        assert p["head"] in (0, head) and p["ptab_kt"] == 0
+        if p["head"]:
+            assert head < p["ks"] <= 63
+            assert p["bands"] and p["first_untiled"] <= 16
+            for b in p["bands"]:
+                assert p["scales"][b["scale_lo"] + b["nscales"] - 1][0] <= 255
+                assert (b["halo_lo"] + 1) * (b["pitch"] + 1) < 32768
+
+
+def test_describe_plan_plans_for_the_call_s_frame_count():
+    """A call of <= 2 M windows plans bands of 1.4x its first scale, a larger one 2x (run_scan's rule); the default
+    description is that of a call of many frames."""
+    one = pigo_b200.describe_plan(1080, 1920, 20, 1000, 0.2, 1.1, nframes=1)     # 0.9 M windows
+    two = pigo_b200.describe_plan(1080, 1920, 20, 1000, 0.2, 1.1, nframes=2)     # 1.8 M
+    three = pigo_b200.describe_plan(1080, 1920, 20, 1000, 0.2, 1.1, nframes=3)   # 2.7 M
+    many = pigo_b200.describe_plan(1080, 1920, 20, 1000, 0.2, 1.1)
+    assert (one["band_ratio"], two["band_ratio"], three["band_ratio"], many["band_ratio"]) == (140, 140, 200, 200)
+    assert three["bands"] == many["bands"] and one["bands"] == two["bands"] != many["bands"]
+    assert one["head"] == 0 and one["ptab_kt"] == 0 and one["ks"] == pigo_b200.get_option("tile_ks")
+    with pytest.raises(pigo_b200.PigoError):
+        pigo_b200.describe_plan(1080, 1920, 20, 1000, 0.2, 1.1, nframes=0)
