@@ -550,3 +550,56 @@ func (plc *PuplocCascade) ReadCascadeDir(path string) (map[string][]*FlpCascade,
 	}
 	return flpcs, err
 }
+
+// SweepDetection is one merged face of an angle sweep and the angle it was found at: Angle is the value the caller listed.
+type SweepDetection struct {
+	Detection
+	Angle float64
+}
+
+// RunCascadeImagesSweep scans every image at every angle of angles and merges each image's lists
+// (pigo_run_cascade_images_sweep): result[i] is ClusterDetections(iou) of image i's RunCascade lists over the angles,
+// concatenated in angle order, each cluster with the listed angle of its largest-Q member.  Listing two values of one
+// orientation (0 and 1) counts every face found there twice.  A pixel slice is copied to the device once.
+func (pg *Pigo) RunCascadeImagesSweep(images []ImageParams, cp CascadeParams, angles []float64, iou float64) [][]SweepDetection {
+	n := len(images)
+	if n == 0 || len(angles) == 0 {
+		return make([][]SweepDetection, n)
+	}
+	desc, free := packImages(images)
+	defer free()
+	capacity, detCap := 64, 0
+	for {
+		buf := make([]C.pigo_det, capacity*n)
+		idx := make([]C.int32_t, capacity*n)
+		cnt := make([]C.int, n)
+		rc, err := call(func() C.int {
+			return C.pigo_run_cascade_images_sweep(pg.h, &desc[0], C.int(n), (*C.double)(unsafe.Pointer(&angles[0])), C.int(len(angles)),
+				C.int(cp.MinSize), C.int(cp.MaxSize), C.double(cp.ShiftFactor), C.double(cp.ScaleFactor), C.double(iou), C.int(detCap), &buf[0],
+				&idx[0], C.int(capacity), &cnt[0], C.PIGO_MEM_HOST, nil)
+		})
+		if rc == C.PIGO_E_CAP {
+			grown := false
+			for _, c := range cnt {
+				if int(c) > capacity {
+					capacity, grown = int(c), true
+				}
+			}
+			if !grown {
+				detCap = 4 * (detCap + 512) // raw detections of an (image, angle) entry exceeded det_cap
+			}
+			continue
+		}
+		if err != nil {
+			panic(err)
+		}
+		out := make([][]SweepDetection, n)
+		for i := range out {
+			dets := toGo(buf[i*capacity:(i+1)*capacity], int(cnt[i]))
+			for k, d := range dets {
+				out[i] = append(out[i], SweepDetection{d, angles[int(idx[i*capacity+k])]})
+			}
+		}
+		return out
+	}
+}

@@ -264,3 +264,63 @@ func (pg *Pigo) DetectImagesAngles(plc *PuplocCascade, calls []LandmarkCall, ima
 		return faceResults(faces, nfaces, points, faceCap, ncalls, pp.MinFaceScale)
 	}
 }
+
+// SweepFace is one merged face of DetectImagesSweep and the angle it was found at (the value the caller listed); its eyes
+// were refined at that angle.
+type SweepFace struct {
+	FaceResult
+	Angle float64
+}
+
+// DetectImagesSweep scans every image at every angle of angles, merges each image's lists as RunCascadeImagesSweep does
+// (pp.IoU) and refines every merged face with its eyes at its own angle (pigo_detect_images_sweep); pp.Angle and
+// pp.Sharded are not used and the landmark calls stay at angle 0, as GetLandmarkPoint does.
+func (pg *Pigo) DetectImagesSweep(plc *PuplocCascade, calls []LandmarkCall, images []ImageParams, cp CascadeParams, pp PipelineParams, angles []float64) [][]SweepFace {
+	n := len(images)
+	if n == 0 || len(angles) == 0 {
+		return make([][]SweepFace, n)
+	}
+	desc, free := packImages(images)
+	defer free()
+	ncalls := len(calls)
+	hs, fl := callArrays(calls)
+	defer C.free(unsafe.Pointer(hs))
+	prm := C.pigo_pipeline_params{min_size: C.int32_t(cp.MinSize), max_size: C.int32_t(cp.MaxSize), shift_factor: C.double(cp.ShiftFactor),
+		scale_factor: C.double(cp.ScaleFactor), iou_threshold: C.double(pp.IoU), min_face_scale: C.int32_t(pp.MinFaceScale),
+		eye_perturbs: C.int32_t(pp.EyePerturbs), flp_perturbs: C.int32_t(pp.FlpPerturbs)}
+	key := atomic.AddUint64(&plc.seed, 1)
+	faceCap := 32
+	for {
+		faces := make([]C.pigo_det, n*faceCap)
+		fangle := make([]C.int32_t, n*faceCap)
+		nfaces := make([]C.int, n)
+		points := make([]C.pigo_point, n*faceCap*(2+ncalls))
+		rc, err := call(func() C.int {
+			return C.pigo_detect_images_sweep(pg.h, plc.h, hs, &fl[0], C.int(ncalls), &desc[0], C.int(n), (*C.double)(unsafe.Pointer(&angles[0])),
+				C.int(len(angles)), &prm, nil, C.uint64_t(key), &faces[0], &fangle[0], C.int(faceCap), &nfaces[0], &points[0], C.PIGO_MEM_HOST, nil)
+		})
+		if rc == C.PIGO_E_CAP {
+			grown := false
+			for _, c := range nfaces {
+				if int(c) > faceCap {
+					faceCap, grown = int(c), true
+				}
+			}
+			if !grown {
+				prm.det_cap = 4 * (prm.det_cap + 512) // raw detections of an (image, angle) entry exceeded det_cap
+			}
+			continue
+		}
+		if err != nil {
+			panic(err)
+		}
+		res := faceResults(faces, nfaces, points, faceCap, ncalls, pp.MinFaceScale)
+		out := make([][]SweepFace, n)
+		for i := range res {
+			for k, fr := range res[i] {
+				out[i] = append(out[i], SweepFace{fr, angles[int(fangle[i*faceCap+k])]})
+			}
+		}
+		return out
+	}
+}

@@ -281,6 +281,40 @@ int pigo_detect_images_angles(const pigo_cascade *face, const pigo_puploc *puplo
                               uint64_t rng_seed, pigo_det *faces, int face_cap, int *n_faces, pigo_point *points,
                               unsigned flags, void *stream);
 
+/* ---- Angle sweep merged per image (additive).  A caller who does not know a photo's tilt scans it at several angles and
+ * wants one face list, each face with the angle it was found at.  Every image is scanned at every angle of the host
+ * array angles[nangles] (rules as pigo_run_cascade_images_angles).  For image i:
+ *   D_i = RunCascade(image i, angles[0]) ++ ... ++ RunCascade(image i, angles[nangles-1])   (each list in emission order)
+ *   clusters of image i = ClusterDetections(D_i, iou_threshold)   (stable sort by Q: ties keep their order in D_i)
+ *   angle_index[i][k] = index into `angles` of the member of cluster k with the largest Q (among equal Q the earliest in
+ *                       D_i, so the angle listed first wins).
+ * Listing two values of one orientation (0 and 1, say, or 0 and -0.5) scans it twice, and every face it finds is counted
+ * twice in D_i; the clusters then weigh that orientation double.
+ * det_cap (0 = 2048) bounds the raw detections of each (image, angle) entry: PIGO_E_CAP names the entry that exceeds it.
+ * out[nimages][cap_per_image] / n_out[nimages] as pigo_run_cascade_images (PIGO_E_CAP with the required counts in n_out);
+ * angle_index[nimages][cap_per_image] may be NULL.  With PIGO_OUT_DEVICE, out, angle_index and n_out are device pointers
+ * and the call is asynchronous.  Host pixels of an image are copied to the device once.  Invalid arguments fail with
+ * PIGO_E_INVALID before any device work: a null `angles`, nangles < 1, nimages*nangles > 65535,
+ * nimages*nangles*det_cap > 2^31-1, and the checks of pigo_run_cascade_images; a stream that is being captured into a
+ * CUDA graph is rejected with PIGO_E_INVALID. */
+int pigo_run_cascade_images_sweep(const pigo_cascade *c, const pigo_image *images, int nimages, const double *angles, int nangles,
+                                  int min_size, int max_size, double shift_factor, double scale_factor, double iou_threshold,
+                                  int det_cap, pigo_det *out, int32_t *angle_index, int cap_per_image, int *n_out,
+                                  unsigned flags, void *stream);
+
+/* Pipeline form: the clusters of pigo_run_cascade_images_sweep (params->iou_threshold, params->det_cap per (image, angle)
+ * entry; params->angle is ignored), then pigo_detect_images' per-face sequence on them, with the eye RunDetector of face k
+ * of image i at angles[face_angle[i][k]] and the landmark calls at angle 0, as GetLandmarkPoint does.  Outputs, randoms
+ * layout, generator key, face_cap, PIGO_E_CAP (n_faces then holds the required counts), flags and stream as
+ * pigo_detect_images with nimages images; face_angle[nimages][face_cap] may be NULL.  With nangles == 1 the call returns
+ * byte for byte what pigo_detect_images_angles returns with every angle equal to angles[0], and every face_angle is 0.
+ * Invalid arguments as pigo_run_cascade_images_sweep and pigo_detect_images (nimages*face_cap*(2+ncalls) <= 2^31-1). */
+int pigo_detect_images_sweep(const pigo_cascade *face, const pigo_puploc *puploc, const pigo_puploc *const *flp,
+                             const uint8_t *flp_flip, int ncalls, const pigo_image *images, int nimages, const double *angles,
+                             int nangles, const pigo_pipeline_params *params, const float *randoms, uint64_t rng_seed,
+                             pigo_det *faces, int32_t *face_angle, int face_cap, int *n_faces, pigo_point *points,
+                             unsigned flags, void *stream);
+
 /* ---- RgbToGrayscale(src image.Image) []uint8, core/grayscale.go:8-23, for *image.NRGBA input (what GetImage returns,
  * core/image.go:13-33): gray = uint8((0.299 r + 0.587 g + 0.114 b) / 256) in float64 on the 16-bit, alpha-premultiplied
  * channels color.NRGBA.RGBA() yields.  rgba is [npixels][4] (R,G,B,A), gray is [npixels].  flags: PIGO_FRAMES_DEVICE /

@@ -34,6 +34,10 @@ struct Detection {              // core/pigo.go:195-200
   int Row = 0, Col = 0, Scale = 0;
   float Q = 0;
 };
+struct SweepDetection {         // additive: a cluster of an angle sweep and the listed angle it was found at
+  Detection Det;
+  double Angle = 0.0;
+};
 struct Puploc {                 // core/puploc.go:14-19
   int Row = 0, Col = 0;
   float Scale = 0;
@@ -119,6 +123,37 @@ class Pigo {                    // core/pigo.go:37-43
                                                               const std::vector<double>& angles) const {
     if (angles.size() != images.size()) throw std::invalid_argument("RunCascadeImagesSharded needs one angle per image");
     return runImages(images, cp, angles, true);
+  }
+  // additive: every image scanned at every angle of `angles`, one merged list per image: the clusters of the concatenation
+  // of its RunCascade lists over the angles, each with the listed angle of its largest-Q member (pigo_run_cascade_images_sweep).
+  // PIGO_E_CAP is retried with the reported counts (or a larger det_cap).
+  std::vector<std::vector<SweepDetection>> RunCascadeImagesSweep(const std::vector<ImageParams>& images, const CascadeParams& cp,
+                                                                 const std::vector<double>& angles, double iou) const {
+    const int n = (int)images.size();
+    std::vector<pigo_image> desc((size_t)n);
+    for (int i = 0; i < n; ++i) desc[i] = pigo_image{images[i].Pixels, images[i].Rows, images[i].Cols, images[i].Dim};
+    int cap = 64, det_cap = 0;
+    for (;;) {
+      std::vector<pigo_det> buf((size_t)cap * (n > 0 ? n : 1));
+      std::vector<int32_t> idx(buf.size());
+      std::vector<int> cnt((size_t)(n > 0 ? n : 1));
+      const int rc = pigo_run_cascade_images_sweep(h_.get(), desc.data(), n, angles.data(), (int)angles.size(), cp.MinSize, cp.MaxSize, cp.ShiftFactor,
+                                                   cp.ScaleFactor, iou, det_cap, buf.data(), idx.data(), cap, cnt.data(), PIGO_MEM_HOST, nullptr);
+      if (rc == PIGO_E_CAP) {
+        bool grown = false;
+        for (int c : cnt) if (c > cap) { cap = c; grown = true; }
+        if (!grown) det_cap = 4 * (det_cap + 512);   // raw detections of an (image, angle) entry exceeded det_cap
+        continue;
+      }
+      check(rc);
+      std::vector<std::vector<SweepDetection>> out((size_t)n);
+      for (int f = 0; f < n; ++f)
+        for (int i = 0; i < cnt[f]; ++i) {
+          const size_t k = (size_t)f * cap + i;
+          out[f].push_back(SweepDetection{Detection{buf[k].row, buf[k].col, buf[k].scale, buf[k].q}, angles[(size_t)idx[k]]});
+        }
+      return out;
+    }
   }
   const pigo_cascade* handle() const { return h_.get(); }
 
@@ -309,6 +344,62 @@ inline std::vector<std::vector<FaceResult>> DetectImages(const Pigo& face, const
                                                          int eye_perturbs, int flp_perturbs, uint64_t rng_seed, double angle = 0.0, int face_cap = 32) {
   return DetectImagesAngles(face, plc, calls, images, cp, iou, min_face_scale, eye_perturbs, flp_perturbs, rng_seed,
                             std::vector<double>(images.size(), angle), face_cap);
+}
+// additive: DetectImages over an angle sweep (pigo_detect_images_sweep): every image scanned at every angle of `angles`, one
+// merged face list per image, each face refined with its eyes at the angle it was found at (Angle, the listed value); the
+// landmark calls stay at angle 0.  PIGO_E_CAP is retried as in DetectImagesAngles.
+struct SweepFace {
+  FaceResult Face;
+  double Angle = 0.0;
+};
+inline std::vector<std::vector<SweepFace>> DetectImagesSweep(const Pigo& face, const PuplocCascade& plc,
+                                                             const std::vector<std::pair<const PuplocCascade*, bool>>& calls,
+                                                             const std::vector<ImageParams>& images, const CascadeParams& cp, double iou,
+                                                             int min_face_scale, int eye_perturbs, int flp_perturbs, uint64_t rng_seed,
+                                                             const std::vector<double>& angles, int face_cap = 32) {
+  const int ncalls = (int)calls.size(), n = (int)images.size();
+  std::vector<const pigo_puploc*> hs;
+  std::vector<uint8_t> fl;
+  for (auto& c : calls) { hs.push_back(c.first->handle()); fl.push_back(c.second ? 1 : 0); }
+  std::vector<pigo_image> desc((size_t)n);
+  for (int i = 0; i < n; ++i) desc[i] = pigo_image{images[i].Pixels, images[i].Rows, images[i].Cols, images[i].Dim};
+  pigo_pipeline_params prm{};
+  prm.min_size = cp.MinSize; prm.max_size = cp.MaxSize; prm.shift_factor = cp.ShiftFactor; prm.scale_factor = cp.ScaleFactor; prm.angle = 0.0;
+  prm.iou_threshold = iou; prm.min_face_scale = min_face_scale; prm.eye_perturbs = eye_perturbs; prm.flp_perturbs = flp_perturbs; prm.det_cap = 0;
+  for (;;) {
+    std::vector<pigo_det> faces((size_t)(n > 0 ? n : 1) * face_cap);
+    std::vector<int32_t> fangle(faces.size());
+    std::vector<int> nfaces((size_t)(n > 0 ? n : 1));
+    std::vector<pigo_point> pts((size_t)(n > 0 ? n : 1) * face_cap * (2 + ncalls));
+    const int rc = pigo_detect_images_sweep(face.handle(), plc.handle(), hs.data(), fl.data(), ncalls, desc.data(), n, angles.data(), (int)angles.size(),
+                                            &prm, nullptr, rng_seed, faces.data(), fangle.data(), face_cap, nfaces.data(), pts.data(), PIGO_MEM_HOST,
+                                            nullptr);
+    if (rc == PIGO_E_CAP) {
+      bool grown = false;
+      for (int i = 0; i < n; ++i)
+        if (nfaces[i] > face_cap) { face_cap = nfaces[i]; grown = true; }
+      if (!grown) prm.det_cap = 4 * (prm.det_cap + 512);   // raw detections of an (image, angle) entry exceeded det_cap
+      continue;
+    }
+    check(rc);
+    std::vector<std::vector<SweepFace>> out((size_t)n);
+    for (int f = 0; f < n; ++f)
+      for (int k = 0; k < nfaces[f]; ++k) {
+        const size_t s = (size_t)f * face_cap + k;
+        const pigo_det& d = faces[s];
+        SweepFace r;
+        r.Face.Face = Detection{d.row, d.col, d.scale, d.q};
+        r.Angle = angles[(size_t)fangle[s]];
+        if (d.scale > min_face_scale) {
+          const pigo_point* p = &pts[s * (2 + ncalls)];
+          r.Face.Refined = true;
+          r.Face.LeftEye = Puploc{p[0].row, p[0].col, p[0].scale, 0}; r.Face.RightEye = Puploc{p[1].row, p[1].col, p[1].scale, 0};
+          for (int c = 0; c < ncalls; ++c) r.Face.Landmarks.push_back(Puploc{p[2 + c].row, p[2 + c].col, p[2 + c].scale, 0});
+        }
+        out[f].push_back(r);
+      }
+    return out;
+  }
 }
 inline PuplocCascade NewPuplocCascade() { return PuplocCascade(); }   // core/puploc.go:33
 

@@ -48,7 +48,7 @@ ABI_SYMBOLS = [
     "pigo_ycbcr_to_nrgba", "pigo_run_cascade_images", "pigo_detect_images", "pigo_puploc_run_images",
     "pigo_run_cascade_images_angles", "pigo_detect_images_angles", "pigo_gray_images", "pigo_cascade_block_table",
     "pigo_run_cascade_images_sharded", "pigo_detect_images_sharded", "pigo_run_cascade_decoded_sharded", "pigo_detect_decoded_sharded",
-    "pigo_shard_plan", "pigo_describe_plan_frames",
+    "pigo_shard_plan", "pigo_describe_plan_frames", "pigo_run_cascade_images_sweep", "pigo_detect_images_sweep",
 ]
 
 
@@ -126,6 +126,8 @@ def lib() -> C.CDLL:
         L.pigo_run_cascade_decoded_sharded.argtypes = [vp, vp, i, vp, i, i, d, d, vp, i, vp]
         L.pigo_detect_decoded_sharded.argtypes = [vp, vp, vp, vp, i, vp, i, vp, vp, vp, u64, vp, i, vp, vp]
         L.pigo_shard_plan.argtypes = [vp, i, vp, i, i, d, d, i, vp, C.POINTER(i)]
+        L.pigo_run_cascade_images_sweep.argtypes = [vp, vp, i, vp, i, i, i, d, d, d, i, vp, vp, i, vp, C.c_uint, vp]
+        L.pigo_detect_images_sweep.argtypes = [vp, vp, vp, vp, i, vp, i, vp, i, vp, vp, u64, vp, vp, i, vp, vp, C.c_uint, vp]
         _lib = L
     return _lib
 
@@ -436,6 +438,45 @@ class Pigo:
         ang = np.ascontiguousarray(angles, dtype=np.float64)
         _check(lib().pigo_run_cascade_images_angles(self._h, image_descs(images), len(images), ang.ctypes.data, min_size, max_size, shift, scale,
                                                     out_ptr, cap_per_image, counts_ptr, FRAMES_DEVICE | OUT_DEVICE, stream or None))
+
+    def RunCascadeImagesSweep(self, images: Sequence[ImageParams], cp: CascadeParams, angles: Sequence[float], iou: float, det_cap: int = 0,
+                              cap_per_image: int = 256):
+        """Every image scanned at every angle of `angles`, merged per image (pigo_run_cascade_images_sweep): image i's clusters
+        of the concatenation of its RunCascade lists over the angles, with the index into `angles` of each cluster's largest-Q
+        member.  Pixels as RunCascadeImages.  PIGO_E_CAP is retried (a larger det_cap for raw lists, else the reported counts).
+        Returns (clusters[N, cap] DET_DTYPE, angle_index[N, cap] int32, counts[N])."""
+        self._need()
+        n = len(images)
+        on_dev = n > 0 and all(isinstance(im.Pixels, int) for im in images)
+        keep = [None if on_dev else _pixels(im) for im in images]   # host pixels stay alive for the call
+        desc = image_descs([(im.Pixels if on_dev else p.ctypes.data, im.Rows, im.Cols, im.Dim) for im, p in zip(images, keep)])
+        ang = np.ascontiguousarray(angles, dtype=np.float64)
+        while True:
+            out = np.zeros((n, max(cap_per_image, 1)), dtype=DET_DTYPE)
+            tag = np.full((n, max(cap_per_image, 1)), -1, dtype=np.int32)
+            cnt = np.zeros(max(n, 1), dtype=np.int32)
+            rc = lib().pigo_run_cascade_images_sweep(self._h, desc, n, ang.ctypes.data, len(ang), cp.MinSize, cp.MaxSize, cp.ShiftFactor,
+                                                     cp.ScaleFactor, iou, det_cap, out.ctypes.data, tag.ctypes.data, cap_per_image,
+                                                     cnt.ctypes.data, FRAMES_DEVICE if on_dev else MEM_HOST, None)
+            if rc == PIGO_E_CAP:
+                if "raw detections" in lib().pigo_last_error().decode():
+                    det_cap = 4 * (det_cap or 2048)
+                else:
+                    cap_per_image = int(cnt.max())
+                continue
+            _check(rc)
+            return out, tag, cnt[:n]
+
+    def run_cascade_images_sweep_device(self, images, angles: Sequence[float], min_size: int, max_size: int, shift: float, scale: float,
+                                        iou: float, det_cap: int, out_ptr: int, angle_index_ptr: int, cap_per_image: int, counts_ptr: int,
+                                        stream: int = 0):
+        """Device-resident, asynchronous form of RunCascadeImagesSweep: images = [(device pointer, rows, cols, dim)], angles a host
+        sequence, out [N][cap], angle_index [N][cap] (0 = not wanted) and counts [N] device pointers; no host sync."""
+        self._need()
+        ang = np.ascontiguousarray(angles, dtype=np.float64)
+        _check(lib().pigo_run_cascade_images_sweep(self._h, image_descs(images), len(images), ang.ctypes.data, len(ang), min_size, max_size, shift,
+                                                   scale, iou, det_cap, out_ptr, angle_index_ptr or None, cap_per_image, counts_ptr,
+                                                   FRAMES_DEVICE | OUT_DEVICE, stream or None))
 
     def run_cascade_images_sharded(self, images: Sequence[ImageParams], cp: CascadeParams, angles: Optional[Sequence[float]] = None,
                                    cap_per_image: int = 1024):

@@ -34,7 +34,7 @@ struct TimingSlot {
 };
 static TimingSlot g_tslot[T_NSLOTS];
 static std::mutex g_tmu;
-static const char* kSlotNames[T_NSLOTS] = {"tiled", "gather", "deep", "finalize", "cluster", "puploc", "gray", "seeds", "rottab", "ycbcr", "gray_images"};
+static const char* kSlotNames[T_NSLOTS] = {"tiled", "gather", "deep", "finalize", "cluster", "puploc", "gray", "seeds", "rottab", "ycbcr", "gray_images", "merge"};
 
 void timing_reset() {
   std::lock_guard<std::mutex> g(g_tmu);
@@ -1507,11 +1507,26 @@ int pigo_get_landmark_point(const pigo_puploc* p, const pigo_point* left_eye, co
 // one D2H copy of the results at the end.  Only the pixel source differs between the uniform batch and the mixed-size
 // call: `scan(w, st, dets, det_cap, cnt, W)` stages the pixels, runs RunCascade into dets[nframes][det_cap] / cnt[nframes]
 // on `st`, points W's pixel fields (uniform frames, or the image table) at the pixels the RunDetector stages read and sets
-// W.rot_slot to the eye stage's rotation (the call's slot, or kRotSlotPerImage).  `unit` names a frame in the capacity messages.
-template <typename ScanFn>
+// W.rot_slot to the eye stage's rotation (the call's slot, kRotSlotPerImage or kRotSlotPerFace).  `unit` names a frame in
+// the capacity messages.  An angle sweep scans every frame at `nangles` angles: the scan writes nframes*nangles lists
+// (frame-major), and `cluster(w, st, dets, det_cap, cnt, clusters, ncl, W, &tags)` turns them into clusters[nframes][face_cap]
+// / ncl[nframes]; it may point `tags` at per-face device values that are copied to `face_tags` with the other results.
+// ClusterFrames is the one-list-per-frame clustering.
+struct ClusterFrames {
+  int dev, nframes;
+  double iou;
+  int face_cap;
+  int operator()(Workspace*, cudaStream_t st, pigo_det* d_dets, int det_cap, int32_t* d_cnt, pigo_det* d_clusters, int32_t* d_ncl, PupWork&,
+                 int32_t**) const {
+    return cluster_batch_on(dev, d_dets, d_cnt, nframes, det_cap, iou, d_clusters, face_cap, d_ncl, PIGO_OUT_DEVICE, st);
+  }
+};
+
+template <typename ScanFn, typename ClusterFn>
 static int detect_on(int dev, pigo_cascade* face, pigo_puploc* puploc, pigo_puploc* const* flp, const uint8_t* flp_flip, int ncalls, int nframes,
-                     const char* unit, const pigo_pipeline_params& P, const float* randoms, uint64_t rng_seed, uint64_t slot_base, pigo_det* faces,
-                     int face_cap, int* n_faces, pigo_point* points, unsigned flags, void* stream_, ScanFn scan) {
+                     int nangles, const char* unit, const pigo_pipeline_params& P, const float* randoms, uint64_t rng_seed, uint64_t slot_base,
+                     pigo_det* faces, int face_cap, int* n_faces, pigo_point* points, int32_t* face_tags, unsigned flags, void* stream_,
+                     ScanFn scan, ClusterFn cluster) {
   int rc = PIGO_OK;
   FaceReplica* R = face_replica(face, dev, &rc);
   if (!R) return rc;
@@ -1543,18 +1558,18 @@ static int detect_on(int dev, pigo_cascade* face, pigo_puploc* puploc, pigo_pupl
   cudaStream_t st = stream_ ? (cudaStream_t)stream_ : w->stream;
   if ((rc = ws_enter(w, st))) return rc;
 
-  const size_t nslots = (size_t)nframes * face_cap * stride;
+  const size_t nslots = (size_t)nframes * face_cap * stride, nscan = (size_t)nframes * nangles;
   // scratch: raw detections + counts, clusters + counts, seeds, points, faces, work counters
-  const size_t b_dets = (size_t)nframes * det_cap * sizeof(pigo_det), b_cl = (size_t)nframes * face_cap * sizeof(pigo_det);
+  const size_t b_dets = nscan * det_cap * sizeof(pigo_det), b_cl = (size_t)nframes * face_cap * sizeof(pigo_det);
   const size_t b_pts = nslots * sizeof(pigo_point);
-  if ((rc = w->raw.reserve(b_dets)) || (rc = w->out.reserve(b_cl + b_cl)) || (rc = w->nout.reserve((size_t)nframes * 16 + 256)) ||
+  if ((rc = w->raw.reserve(b_dets)) || (rc = w->out.reserve(b_cl + b_cl)) || (rc = w->nout.reserve((nscan + 3 * (size_t)nframes) * 4 + 256)) ||
       (rc = w->scratch_a.reserve(b_pts)) || (rc = w->scratch_b.reserve(b_pts)) || (rc = w->counters.reserve(256))) return rc;
   pigo_det* d_dets = (pigo_det*)w->raw.p;
   pigo_det* d_clusters = (pigo_det*)w->out.p;
   pigo_det* d_faces = out_dev ? faces : (pigo_det*)((char*)w->out.p + b_cl);
   int32_t* d_cnt = (int32_t*)w->nout.p;
-  int32_t* d_ncl = d_cnt + nframes;
-  int32_t* d_nfaces = out_dev ? n_faces : d_cnt + 2 * (size_t)nframes;
+  int32_t* d_ncl = d_cnt + nscan;
+  int32_t* d_nfaces = out_dev ? n_faces : d_ncl + nframes;
   pigo_point* d_seeds = (pigo_point*)w->scratch_a.p;
   pigo_point* d_points = out_dev ? points : (pigo_point*)w->scratch_b.p;
   const float* d_rnd = randoms;
@@ -1568,8 +1583,8 @@ static int detect_on(int dev, pigo_cascade* face, pigo_puploc* puploc, pigo_pupl
   CUDA_TRY(cudaMemsetAsync(d_points, 0, b_pts, st));
 
   if ((rc = scan(w, st, d_dets, det_cap, d_cnt, W))) return rc;
-  rc = cluster_batch_on(dev, d_dets, d_cnt, nframes, det_cap, P.iou_threshold, d_clusters, face_cap, d_ncl, PIGO_OUT_DEVICE, st);
-  if (rc) return rc;
+  int32_t* d_tags = nullptr;
+  if ((rc = cluster(w, st, d_dets, det_cap, d_cnt, d_clusters, d_ncl, W, &d_tags))) return rc;
   timing_begin(T_SEEDS, st);
   launch_eye_seeds(d_clusters, d_ncl, face_cap, nframes, face_cap, stride, P.min_face_scale, P.eye_perturbs, d_faces, d_nfaces, d_seeds, st);
   timing_end(T_SEEDS, st);
@@ -1579,7 +1594,7 @@ static int detect_on(int dev, pigo_cascade* face, pigo_puploc* puploc, pigo_pupl
   W.slot_frame = nullptr; W.flipv = nullptr;
   W.slots_per_frame = face_cap * stride;
   W.stride = stride;
-  // (a) both eyes of every face slot, at the scan's angle: RunDetector(puploc, img, det.angle, false), main.go:422
+  // (a) both eyes of every face slot, at the scan's angle (a sweep: the face's own angle): RunDetector(puploc, img, det.angle, false), main.go:422
   PupWork E = W;
   E.first = 0; E.span = 2; E.nwork = nframes * face_cap * 2;
   E.tab_of[0] = E.tab_of[1] = 0; E.flip_of[0] = E.flip_of[1] = 0;
@@ -1603,15 +1618,20 @@ static int detect_on(int dev, pigo_cascade* face, pigo_puploc* puploc, pigo_pupl
   CUDA_TRY(cudaGetLastError());
   if (out_dev) return ws_leave_async(w, st);
 
-  // one D2H round: counts (raw detections, clusters), faces, points
-  std::vector<int32_t> cnt(2 * (size_t)nframes);
+  // one D2H round: counts (raw detections, clusters), faces, points (and the faces' tags)
+  std::vector<int32_t> cnt(nscan + nframes);
   CUDA_TRY(cudaMemcpyAsync(cnt.data(), d_cnt, cnt.size() * 4, cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaMemcpyAsync(n_faces, d_nfaces, (size_t)nframes * 4, cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaMemcpyAsync(faces, d_faces, b_cl, cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaMemcpyAsync(points, d_points, b_pts, cudaMemcpyDeviceToHost, st));
+  if (face_tags && d_tags) CUDA_TRY(cudaMemcpyAsync(face_tags, d_tags, (size_t)nframes * face_cap * 4, cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaStreamSynchronize(st));
-  for (int f = 0; f < nframes; ++f)
-    if (cnt[f] > det_cap) return set_err(PIGO_E_CAP, "%s %d has %d raw detections, det_cap is %d: raise pigo_pipeline_params.det_cap", unit, f, cnt[f], det_cap);
+  for (size_t e = 0; e < nscan; ++e) {
+    if (cnt[e] <= det_cap) continue;
+    if (nangles == 1) return set_err(PIGO_E_CAP, "%s %d has %d raw detections, det_cap is %d: raise pigo_pipeline_params.det_cap", unit, (int)e, cnt[e], det_cap);
+    return set_err(PIGO_E_CAP, "%s %d at angle %d has %d raw detections, det_cap is %d: raise pigo_pipeline_params.det_cap", unit, (int)(e / nangles),
+                   (int)(e % nangles), cnt[e], det_cap);
+  }
   for (int f = 0; f < nframes; ++f)
     if (n_faces[f] > face_cap) return set_err(PIGO_E_CAP, "%s %d has %d faces, face_cap is %d", unit, f, n_faces[f], face_cap);
   return PIGO_OK;
@@ -1637,8 +1657,8 @@ static int detect_batch_on(int dev, pigo_cascade* face, pigo_puploc* puploc, pig
     return scan_batch_on(face, dev, frames, nframes, frame_stride, rows, cols, dim, P.min_size, P.max_size, P.shift_factor, P.scale_factor,
                          P.angle, d_dets, det_cap, d_cnt, PIGO_OUT_DEVICE, st, (uint8_t*)w->frames.p);
   };
-  return detect_on(dev, face, puploc, flp, flp_flip, ncalls, nframes, "frame", P, randoms, rng_seed, slot_base, faces, face_cap, n_faces, points,
-                   flags, stream_, scan);
+  return detect_on(dev, face, puploc, flp, flp_flip, ncalls, nframes, 1, "frame", P, randoms, rng_seed, slot_base, faces, face_cap, n_faces, points,
+                   nullptr, flags, stream_, scan, ClusterFrames{dev, nframes, P.iou_threshold, face_cap});
 }
 
 // Mixed-size form: the images' pixels are staged once (stage_images) and both the images scan and the RunDetector stages
@@ -1658,8 +1678,149 @@ static int detect_images_on(int dev, pigo_cascade* face, pigo_puploc* puploc, pi
     return scan_images_on(face, dev, staged.data(), nimages, plans, wins, longest, P.min_size, P.max_size, P.shift_factor, P.scale_factor,
                           angles, d_dets, det_cap, d_cnt, PIGO_FRAMES_DEVICE | PIGO_OUT_DEVICE, st);
   };
-  return detect_on(dev, face, puploc, flp, flp_flip, ncalls, nimages, "image", P, randoms, rng_seed, slot_base, faces, face_cap, n_faces, points,
-                   flags, stream_, scan);
+  return detect_on(dev, face, puploc, flp, flp_flip, ncalls, nimages, 1, "image", P, randoms, rng_seed, slot_base, faces, face_cap, n_faces, points,
+                   nullptr, flags, stream_, scan, ClusterFrames{dev, nimages, P.iou_threshold, face_cap});
+}
+
+// ---- angle sweep: every image at every angle, merged per image (pigo_run_cascade_images_sweep, pigo_detect_images_sweep) ----
+// Entry e = i*nangles + a of a sweep's expanded list is images[i] at angles[a]; the scan writes one raw list per entry.
+static void sweep_entries(const pigo_image* images, int nimages, const double* angles, int nangles, std::vector<pigo_image>& ex,
+                          std::vector<double>& ex_angles) {
+  ex.clear(); ex_angles.clear();
+  for (int i = 0; i < nimages; ++i)
+    for (int a = 0; a < nangles; ++a) { ex.push_back(images[i]); ex_angles.push_back(angles[a]); }
+}
+
+// Image i's clusters of D_i = list(i, 0) ++ ... ++ list(i, nangles-1) (raw lists dets[e][det_cap], cnt[e]), as ClusterDetections
+// computes them with a stable sort by Q: out[nimages][out_cap], n_out[nimages] (the required counts), and per cluster the index
+// into `angles` of its largest-Q member (*tags: tags_dst if given, else scratch) and that angle's rotation slot (*rot).  All
+// on the device, on `st`; the scratch is w->sweep.
+static int sweep_merge(Workspace* w, cudaStream_t st, const pigo_det* d_dets, const int32_t* d_cnt, int nimages, const double* angles, int nangles,
+                       int det_cap, double iou, pigo_det* d_out, int out_cap, int32_t* d_nout, int32_t* tags_dst, int32_t** tags, int32_t** rot) {
+  const int seg_cap = nangles * det_cap;
+  const size_t N = (size_t)nimages * seg_cap, nf = (size_t)nimages * out_cap;
+  const size_t sort_bytes = sweep_sort_bytes(nimages, seg_cap);
+  size_t total = 0;
+  auto carve = [&](size_t bytes) { const size_t o = total; total += (bytes + 255) & ~(size_t)255; return o; };
+  const size_t o_slot = carve((size_t)nangles * 4), o_seg = carve((size_t)nimages * 12), o_merged = carve(N * sizeof(pigo_det)),
+               o_tmp = carve(N * sizeof(pigo_det)), o_tag = carve(N * 4), o_seeds = carve(N * 4), o_flags = carve(N), o_kin = carve(N * 8),
+               o_kout = carve(N * 8), o_ftag = carve(nf * 4), o_rot = carve(nf * 4), o_sort = carve(sort_bytes);
+  int rc = w->sweep.reserve(total);
+  if (rc) return rc;
+  uint8_t* b = (uint8_t*)w->sweep.p;
+  std::vector<int32_t> slot_of(nangles);
+  for (int a = 0; a < nangles; ++a) slot_of[a] = rot_slot_of(angles[a]);
+  CUDA_TRY(cudaMemcpyAsync(b + o_slot, slot_of.data(), (size_t)nangles * 4, cudaMemcpyHostToDevice, st));
+  SweepScratch S{};
+  S.merged = (pigo_det*)(b + o_merged); S.tmp = (pigo_det*)(b + o_tmp); S.tag = (int32_t*)(b + o_tag); S.seeds = (int32_t*)(b + o_seeds);
+  S.flags = b + o_flags; S.keys_in = (uint64_t*)(b + o_kin); S.keys_out = (uint64_t*)(b + o_kout);
+  S.seg_begin = (int32_t*)(b + o_seg); S.seg_end = S.seg_begin + nimages; S.n_merged = S.seg_end + nimages;
+  S.sort_temp = b + o_sort; S.sort_bytes = sort_bytes;
+  *tags = tags_dst ? tags_dst : (int32_t*)(b + o_ftag);
+  *rot = (int32_t*)(b + o_rot);
+  timing_begin(T_MERGE, st);
+  if (launch_sweep_merge(d_dets, d_cnt, nimages, nangles, det_cap, iou, S, (const int32_t*)(b + o_slot), d_out, out_cap, d_nout, *tags, *rot, st))
+    return set_err(PIGO_E_CUDA, "segmented sort of the sweep failed");
+  timing_end(T_MERGE, st);
+  g_launches += 3;
+  CUDA_TRY(cudaGetLastError());
+  return PIGO_OK;
+}
+
+// Raw-list capacity of a sweep: entry e = i*nangles + a holds more than det_cap detections.
+static int sweep_raw_cap(const int32_t* cnt, int nimages, int nangles, int det_cap, const char* what) {
+  for (int e = 0; e < nimages * nangles; ++e)
+    if (cnt[e] > det_cap)
+      return set_err(PIGO_E_CAP, "image %d at angle %d has %d raw detections, det_cap is %d: raise %s", e / nangles, e % nangles, cnt[e], det_cap, what);
+  return PIGO_OK;
+}
+
+static int sweep_scan_on(pigo_cascade* c, int dev, const pigo_image* images, int nimages, const double* angles, int nangles,
+                         const std::vector<std::vector<ScaleEntry>>& plans, const std::vector<uint64_t>& wins, int longest, int min_size, int max_size,
+                         double shift_factor, double scale_factor, double iou, int det_cap, pigo_det* out, int32_t* angle_index, int cap_per_image,
+                         int* n_out, unsigned flags, void* stream_) {
+  int rc = PIGO_OK;
+  FaceReplica* R = face_replica(c, dev, &rc);
+  if (!R) return rc;
+  if ((rc = use_device(dev))) return rc;
+  const bool out_dev = flags & PIGO_OUT_DEVICE;
+  WsGuard g(R->pool);
+  Workspace* w = g.w;
+  if (!w) return set_err(PIGO_E_CUDA, "could not create a CUDA stream");
+  cudaStream_t st = stream_ ? (cudaStream_t)stream_ : w->stream;
+  if ((rc = ws_enter(w, st))) return rc;
+  const int E = nimages * nangles, ocap = std::max(cap_per_image, 1);
+  if ((rc = w->raw.reserve((size_t)E * det_cap * sizeof(pigo_det))) || (rc = w->nout.reserve(((size_t)E + nimages) * 4))) return rc;
+  pigo_det* d_raw = (pigo_det*)w->raw.p;
+  int32_t* d_cnt = (int32_t*)w->nout.p;
+  std::vector<pigo_image> ex;
+  std::vector<double> ex_angles;
+  sweep_entries(images, nimages, angles, nangles, ex, ex_angles);
+  if ((rc = scan_images_on(c, dev, ex.data(), E, plans, wins, longest, min_size, max_size, shift_factor, scale_factor, ex_angles.data(), d_raw, det_cap,
+                           d_cnt, (flags & PIGO_FRAMES_DEVICE) | PIGO_OUT_DEVICE, st)))
+    return rc;
+  pigo_det* d_out = out;
+  int32_t* d_nout = n_out;
+  if (!out_dev) {
+    if ((rc = w->out.reserve((size_t)nimages * ocap * sizeof(pigo_det)))) return rc;
+    d_out = (pigo_det*)w->out.p;
+    d_nout = d_cnt + E;
+    CUDA_TRY(cudaMemsetAsync(d_out, 0, (size_t)nimages * ocap * sizeof(pigo_det), st));   // defined padding in the host copy
+  }
+  int32_t *d_tags = nullptr, *d_rot = nullptr;
+  if ((rc = sweep_merge(w, st, d_raw, d_cnt, nimages, angles, nangles, det_cap, iou, d_out, ocap, d_nout, out_dev ? angle_index : nullptr, &d_tags,
+                        &d_rot)))
+    return rc;
+  if (out_dev) return ws_leave_async(w, st);
+  std::vector<int32_t> cnt((size_t)E + nimages);
+  CUDA_TRY(cudaMemcpyAsync(cnt.data(), d_cnt, cnt.size() * 4, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  size_t max_n = 0;
+  for (int i = 0; i < nimages; ++i) {
+    n_out[i] = cnt[(size_t)E + i];
+    max_n = std::max(max_n, (size_t)std::min(n_out[i], cap_per_image));
+  }
+  if (max_n > 0) {
+    CUDA_TRY(cudaMemcpy2DAsync(out, (size_t)cap_per_image * sizeof(pigo_det), d_out, (size_t)ocap * sizeof(pigo_det), max_n * sizeof(pigo_det),
+                               nimages, cudaMemcpyDeviceToHost, st));
+    if (angle_index)
+      CUDA_TRY(cudaMemcpy2DAsync(angle_index, (size_t)cap_per_image * 4, d_tags, (size_t)ocap * 4, max_n * 4, nimages, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+  }
+  if ((rc = sweep_raw_cap(cnt.data(), nimages, nangles, det_cap, "det_cap"))) return rc;
+  for (int i = 0; i < nimages; ++i)
+    if (n_out[i] > cap_per_image) return set_err(PIGO_E_CAP, "image %d has %d clusters, cap_per_image is %d", i, n_out[i], cap_per_image);
+  return PIGO_OK;
+}
+
+// Pipeline form: the images' pixels are staged once (stage_images); the scan reads them at every angle and the eye and
+// landmark stages through the call's ImageDesc table.  The eyes of face k of image i are refined at angles[tag], tag being
+// the face's angle index (kRotSlotPerFace); the generator key and randoms layout are pigo_detect_images'.
+static int detect_sweep_on(int dev, pigo_cascade* face, pigo_puploc* puploc, pigo_puploc* const* flp, const uint8_t* flp_flip, int ncalls,
+                           const pigo_image* images, int nimages, const double* angles, int nangles, const std::vector<std::vector<ScaleEntry>>& plans,
+                           const std::vector<uint64_t>& wins, int longest, const pigo_pipeline_params& P, const float* randoms, uint64_t rng_seed,
+                           pigo_det* faces, int face_cap, int* n_faces, pigo_point* points, int32_t* face_angle, unsigned flags, void* stream_) {
+  const bool frames_dev = flags & PIGO_FRAMES_DEVICE, out_dev = flags & PIGO_OUT_DEVICE;
+  auto scan = [&](Workspace* w, cudaStream_t st, pigo_det* d_dets, int det_cap, int32_t* d_cnt, PupWork& W) {
+    std::vector<pigo_image> staged, ex;
+    std::vector<double> ex_angles;
+    int rc = stage_images(w, images, nimages, nullptr, frames_dev, st, &W.images, staged);
+    if (rc) return rc;
+    W.rot_slot = kRotSlotPerFace;
+    sweep_entries(staged.data(), nimages, angles, nangles, ex, ex_angles);
+    return scan_images_on(face, dev, ex.data(), nimages * nangles, plans, wins, longest, P.min_size, P.max_size, P.shift_factor, P.scale_factor,
+                          ex_angles.data(), d_dets, det_cap, d_cnt, PIGO_FRAMES_DEVICE | PIGO_OUT_DEVICE, st);
+  };
+  auto cluster = [&](Workspace* w, cudaStream_t st, pigo_det* d_dets, int det_cap, int32_t* d_cnt, pigo_det* d_clusters, int32_t* d_ncl, PupWork& W,
+                     int32_t** d_tags) {
+    int32_t* rot = nullptr;
+    const int rc = sweep_merge(w, st, d_dets, d_cnt, nimages, angles, nangles, det_cap, P.iou_threshold, d_clusters, face_cap, d_ncl,
+                               out_dev ? face_angle : nullptr, d_tags, &rot);
+    W.face_rot = rot;
+    return rc;
+  };
+  return detect_on(dev, face, puploc, flp, flp_flip, ncalls, nimages, nangles, "image", P, randoms, rng_seed, 0, faces, face_cap, n_faces, points,
+                   face_angle, flags, stream_, scan, cluster);
 }
 
 // Extent of the planes image.YCbCr holds for Rect (min)-(min + size), min >= 0: bytes from the rectangle's origin to its
@@ -1813,6 +1974,67 @@ int pigo_detect_images_angles(const pigo_cascade* face, const pigo_puploc* puplo
   if (nimages > 0 && !angles) return set_err(PIGO_E_INVALID, "null angles");
   return detect_images("pigo_detect_images_angles", face, puploc, flp, flp_flip, ncalls, images, nimages, angles, prm, randoms, rng_seed, faces,
                        face_cap, n_faces, points, flags, stream);
+}
+
+// Sweep arguments checked before the per-image ones: the angle list and the size of the expanded list (det_cap > 0).
+static int check_sweep_args(int nimages, const double* angles, int nangles) {
+  if (!angles) return set_err(PIGO_E_INVALID, "null angles");
+  if (nangles < 1) return set_err(PIGO_E_INVALID, "nangles must be >= 1");
+  if (nimages > 0 && (uint64_t)nimages * (uint64_t)nangles > 65535)
+    return set_err(PIGO_E_INVALID, "nimages*nangles = %llu scan entries exceeds 65535", (unsigned long long)nimages * nangles);
+  return PIGO_OK;
+}
+static int check_sweep_merge(int nimages, int nangles, int det_cap) {
+  if (nimages > 0 && (uint64_t)nimages * (uint64_t)nangles * (uint64_t)det_cap > 0x7fffffffull)
+    return set_err(PIGO_E_INVALID, "nimages*nangles*det_cap exceeds 2^31-1 merged detections");
+  return PIGO_OK;
+}
+
+int pigo_run_cascade_images_sweep(const pigo_cascade* cc, const pigo_image* images, int nimages, const double* angles, int nangles, int min_size,
+                                  int max_size, double shift_factor, double scale_factor, double iou_threshold, int det_cap, pigo_det* out,
+                                  int32_t* angle_index, int cap_per_image, int* n_out, unsigned flags, void* stream_) {
+  int rc = check_sweep_args(nimages, angles, nangles);
+  if (rc) return rc;
+  if (det_cap < 0) return set_err(PIGO_E_INVALID, "negative det_cap");
+  const int dcap = det_cap > 0 ? det_cap : 2048;
+  if ((rc = check_sweep_merge(nimages, nangles, dcap))) return rc;
+  if ((rc = check_images_args(cc, images, nimages, out, cap_per_image, n_out))) return rc;
+  std::vector<pigo_image> ex;
+  std::vector<double> ex_angles;
+  sweep_entries(images, nimages, angles, nangles, ex, ex_angles);
+  std::vector<std::vector<ScaleEntry>> plans;
+  std::vector<uint64_t> wins;
+  int longest = 0;
+  if ((rc = build_image_plans(ex.data(), (int)ex.size(), min_size, max_size, shift_factor, scale_factor, plans, wins, longest))) return rc;
+  if ((rc = ensure_device())) return rc;
+  if (stream_ && stream_capturing((cudaStream_t)stream_)) return set_err(PIGO_E_INVALID, "pigo_run_cascade_images_sweep does not support stream capture");
+  if (nimages == 0) return PIGO_OK;
+  return sweep_scan_on(const_cast<pigo_cascade*>(cc), default_device(), images, nimages, angles, nangles, plans, wins, longest, min_size, max_size,
+                       shift_factor, scale_factor, iou_threshold, dcap, out, angle_index, cap_per_image, n_out, flags, stream_);
+}
+
+int pigo_detect_images_sweep(const pigo_cascade* face, const pigo_puploc* puploc, const pigo_puploc* const* flp, const uint8_t* flp_flip, int ncalls,
+                             const pigo_image* images, int nimages, const double* angles, int nangles, const pigo_pipeline_params* prm,
+                             const float* randoms, uint64_t rng_seed, pigo_det* faces, int32_t* face_angle, int face_cap, int* n_faces,
+                             pigo_point* points, unsigned flags, void* stream) {
+  int rc = check_sweep_args(nimages, angles, nangles);
+  if (rc) return rc;
+  if (prm && (rc = check_sweep_merge(nimages, nangles, prm->det_cap > 0 ? prm->det_cap : 2048))) return rc;
+  if ((rc = check_detect_images_args(face, puploc, flp, ncalls, images, nimages, prm, faces, face_cap, n_faces, points))) return rc;
+  std::vector<pigo_image> ex;
+  std::vector<double> ex_angles;
+  sweep_entries(images, nimages, angles, nangles, ex, ex_angles);
+  std::vector<std::vector<ScaleEntry>> plans;
+  std::vector<uint64_t> wins;
+  int longest = 0;
+  if ((rc = build_image_plans(ex.data(), (int)ex.size(), prm->min_size, prm->max_size, prm->shift_factor, prm->scale_factor, plans, wins, longest)))
+    return rc;
+  if ((rc = ensure_device())) return rc;
+  if (stream && stream_capturing((cudaStream_t)stream)) return set_err(PIGO_E_INVALID, "pigo_detect_images_sweep does not support stream capture");
+  if (nimages == 0) return PIGO_OK;
+  return detect_sweep_on(default_device(), const_cast<pigo_cascade*>(face), const_cast<pigo_puploc*>(puploc), (pigo_puploc* const*)flp, flp_flip,
+                         ncalls, images, nimages, angles, nangles, plans, wins, longest, *prm, randoms, rng_seed, faces, face_cap, n_faces, points,
+                         face_angle, flags, stream);
 }
 
 // ---- RgbToGrayscale, core/grayscale.go:8-23 ----------------------------------------------------------------

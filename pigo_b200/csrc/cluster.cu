@@ -7,6 +7,13 @@
 //  3. per-seed accumulation, one thread per seed, j ascending so that the float32 q-sum (:298) has the
 //     reference's addition order; integer sums and the truncating division (:303) as in Go.
 // IoU is float64 with the reference's operation order (:268-278); the library is built with -fmad=false.
+//
+// The angle sweep (pigo_*_images_sweep) merges the lists of one image at several angles into one list D_i and clusters
+// it with the same kernel: sweep_compact_kernel concatenates the lists with an angle tag per detection, a segmented radix
+// sort orders each image's list by (Q, position in D_i) -- the stable sort of step 1 without its O(n^2) ranks -- and
+// cluster_kernel<true> takes that order instead of step 1 and also reports, per cluster, the tag of its largest-Q member.
+#include <cub/device/device_segmented_radix_sort.cuh>
+
 #include "common.cuh"
 #include "host.h"
 
@@ -22,10 +29,14 @@ __device__ __forceinline__ double calc_iou(const pigo_det& a, const pigo_det& b)
 }
 
 // scratch per frame: tmp[cap] (pigo_det), flags[cap] (u8: assigned), seeds[cap] (i32)
+// TAGGED (sweep merge): step 1 takes the order of the segmented sort (SweepTags.keys: position in the low 32 bits) instead
+// of ranking, and every cluster also gets the tag of its member with the largest Q (the first such member in sorted order,
+// i.e. the earliest in D_i among equal Q) and that tag's rotation slot.
+template <bool TAGGED>
 __global__ void __launch_bounds__(256) cluster_kernel(pigo_det* __restrict__ dets, const int32_t* __restrict__ n_in, int cap,
                                                       double thr, pigo_det* __restrict__ tmp, uint8_t* flags,
                                                       int32_t* __restrict__ seeds, pigo_det* __restrict__ out, int out_cap,
-                                                      int32_t* __restrict__ n_out) {
+                                                      int32_t* __restrict__ n_out, const SweepTags tg) {
   const int frame = blockIdx.x;
   const int n = max(0, min(n_in[frame], cap));
   pigo_det* d = dets + (size_t)frame * cap;
@@ -36,14 +47,19 @@ __global__ void __launch_bounds__(256) cluster_kernel(pigo_det* __restrict__ det
   __shared__ int s_nseeds;
 
   // ---- 1. stable rank sort by q ascending
+  const uint64_t* order = TAGGED ? tg.keys + (size_t)frame * cap : nullptr;
   for (int i = tid; i < n; i += nt) {
-    const float qi = d[i].q;
-    int rank = 0;
-    for (int j = 0; j < n; ++j) {
-      const float qj = d[j].q;
-      rank += (qj < qi || (qj == qi && j < i)) ? 1 : 0;
+    if (TAGGED) {
+      tp[i] = d[(uint32_t)order[i]];
+    } else {
+      const float qi = d[i].q;
+      int rank = 0;
+      for (int j = 0; j < n; ++j) {
+        const float qj = d[j].q;
+        rank += (qj < qi || (qj == qi && j < i)) ? 1 : 0;
+      }
+      tp[rank] = d[i];
     }
-    tp[rank] = d[i];
     asg[i] = 0;
   }
   __syncthreads();
@@ -72,11 +88,13 @@ __global__ void __launch_bounds__(256) cluster_kernel(pigo_det* __restrict__ det
     const pigo_det di = d[sd[k]];
     long long r = 0, c = 0, s = 0, cnt = 0;
     float q = 0.f;
+    int best = -1;   // TAGGED: sorted position of the first member with the largest Q
     for (int j = 0; j < n; ++j) {
       const pigo_det dj = d[j];
       if (calc_iou(di, dj) > thr) {
         r += dj.row; c += dj.col; s += dj.scale;
         q = __fadd_rn(q, dj.q);
+        if (TAGGED && (cnt == 0 || dj.q > d[best].q)) best = j;
         ++cnt;
       }
     }
@@ -84,6 +102,7 @@ __global__ void __launch_bounds__(256) cluster_kernel(pigo_det* __restrict__ det
     if (cnt > 0) { o.row = (int)(r / cnt); o.col = (int)(c / cnt); o.scale = (int)(s / cnt); o.q = q; }
     else { o.row = o.col = 0; o.scale = -1; o.q = 0.f; }  // scale -1 marks "n == 0" (:302), dropped below
     tp[k] = o;
+    if (TAGGED) sd[k] = best >= 0 ? tg.tag[(size_t)frame * cap + (uint32_t)order[best]] : -1;   // this thread's seed is read above
   }
   __syncthreads();
   if (tid == 0) {
@@ -95,16 +114,81 @@ __global__ void __launch_bounds__(256) cluster_kernel(pigo_det* __restrict__ det
         // input scales are >= 0 (always true for RunCascade output)
         continue;
       }
-      if (m < out_cap) of[m] = tp[k];
+      if (m < out_cap) {
+        of[m] = tp[k];
+        if (TAGGED && tg.out_tag) tg.out_tag[(size_t)frame * out_cap + m] = sd[k];
+        if (TAGGED && tg.out_rot) tg.out_rot[(size_t)frame * out_cap + m] = tg.slot_of[sd[k]];
+      }
       ++m;
     }
     n_out[frame] = m;
+    for (int k = m; TAGGED && k < out_cap; ++k) {   // unused face slots: defined values
+      if (tg.out_tag) tg.out_tag[(size_t)frame * out_cap + k] = -1;
+      if (tg.out_rot) tg.out_rot[(size_t)frame * out_cap + k] = -1;
+    }
   }
 }
 
 void launch_cluster(pigo_det* dets, const int32_t* n_in, int cap, double thr, pigo_det* tmp, uint8_t* flags, int32_t* seeds,
                     pigo_det* out, int out_cap, int32_t* n_out, int nframes, cudaStream_t st) {
-  cluster_kernel<<<nframes, 256, 0, st>>>(dets, n_in, cap, thr, tmp, flags, seeds, out, out_cap, n_out);
+  cluster_kernel<false><<<nframes, 256, 0, st>>>(dets, n_in, cap, thr, tmp, flags, seeds, out, out_cap, n_out, SweepTags{});
+}
+
+// ---- angle sweep merge -----------------------------------------------------------------------------------------------
+// Q as an unsigned key that orders like the float (-0 and +0 equal, as the reference's < compares them).
+__device__ __forceinline__ uint32_t q_key(float q) {
+  const uint32_t b = q == 0.f ? 0u : __float_as_uint(q);
+  return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+}
+
+// One CTA per image: D_i = the lists of entries i*nangles .. i*nangles+nangles-1 (angle a's list raw[e][0..min(cnt, det_cap)))
+// concatenated in angle order into merged[i][0..n_i), with tag[i][p] = a and key[i][p] = (q_key, p).
+__global__ void __launch_bounds__(256) sweep_compact_kernel(const pigo_det* __restrict__ raw, const int32_t* __restrict__ raw_count,
+                                                            int nangles, int det_cap, int seg_cap, pigo_det* __restrict__ merged,
+                                                            int32_t* __restrict__ tag, uint64_t* __restrict__ keys,
+                                                            int32_t* __restrict__ seg_begin, int32_t* __restrict__ seg_end,
+                                                            int32_t* __restrict__ n_merged) {
+  const int img = blockIdx.x, tid = threadIdx.x;
+  const size_t base = (size_t)img * seg_cap;
+  int pos = 0;   // prefix over this image's counts (every thread walks the same prefix)
+  for (int a = 0; a < nangles; ++a) {
+    const size_t e = (size_t)img * nangles + a;
+    const int n = max(0, min(raw_count[e], det_cap));
+    for (int j = tid; j < n; j += blockDim.x) {
+      const pigo_det d = raw[e * det_cap + j];
+      const int p = pos + j;
+      merged[base + p] = d;
+      tag[base + p] = a;
+      keys[base + p] = ((uint64_t)q_key(d.q) << 32) | (uint32_t)p;
+    }
+    pos += n;
+  }
+  if (tid == 0) {
+    seg_begin[img] = (int32_t)base;
+    seg_end[img] = (int32_t)base + pos;
+    n_merged[img] = pos;
+  }
+}
+
+size_t sweep_sort_bytes(int nimages, int seg_cap) {
+  size_t bytes = 0;
+  cub::DeviceSegmentedRadixSort::SortKeys(nullptr, bytes, (const uint64_t*)nullptr, (uint64_t*)nullptr, nimages * seg_cap, nimages,
+                                          (const int32_t*)nullptr, (const int32_t*)nullptr);
+  return bytes;
+}
+
+int launch_sweep_merge(const pigo_det* raw, const int32_t* raw_count, int nimages, int nangles, int det_cap, double thr, const SweepScratch& S,
+                       const int32_t* slot_of, pigo_det* out, int out_cap, int32_t* n_out, int32_t* out_tag, int32_t* out_rot, cudaStream_t st) {
+  const int seg_cap = nangles * det_cap;
+  sweep_compact_kernel<<<nimages, 256, 0, st>>>(raw, raw_count, nangles, det_cap, seg_cap, S.merged, S.tag, S.keys_in, S.seg_begin, S.seg_end,
+                                                S.n_merged);
+  size_t bytes = S.sort_bytes;
+  if (cub::DeviceSegmentedRadixSort::SortKeys(S.sort_temp, bytes, S.keys_in, S.keys_out, nimages * seg_cap, nimages, S.seg_begin, S.seg_end,
+                                              0, 64, st) != cudaSuccess)
+    return -1;
+  const SweepTags tg{S.keys_out, S.tag, slot_of, out_tag, out_rot};
+  cluster_kernel<true><<<nimages, 256, 0, st>>>(S.merged, S.n_merged, seg_cap, thr, S.tmp, S.flags, S.seeds, out, out_cap, n_out, tg);
+  return 0;
 }
 
 }  // namespace pigo

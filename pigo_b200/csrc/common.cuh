@@ -84,6 +84,7 @@ struct ImageDesc {
 
 // PupWork.rot_slot / puploc_kernel's rot_slot of a call whose images each carry their own angle (ImageDesc.rot_slot).
 constexpr int kRotSlotPerImage = -2;
+constexpr int kRotSlotPerFace = -3;    // angle sweep: RunDetector with PupWork.face_rot[slot / stride]
 
 struct ScanArgs {
   FaceTables tab;

@@ -20,7 +20,7 @@ void raise_dyn_smem(const void* fn, int bytes);
 
 // Per-kernel CUDA-event timing (enabled by option "timing"): every launch of kernel class `slot` is bracketed by an
 // event pair on its stream; "t_<name>_ns" / "t_<name>_n" return the summed device time and the launch count.
-enum TimeSlot { T_TILED = 0, T_GATHER, T_DEEP, T_FINALIZE, T_CLUSTER, T_PUPLOC, T_GRAY, T_SEEDS, T_ROTTAB, T_YCBCR, T_GRAY_IMAGES, T_NSLOTS };
+enum TimeSlot { T_TILED = 0, T_GATHER, T_DEEP, T_FINALIZE, T_CLUSTER, T_PUPLOC, T_GRAY, T_SEEDS, T_ROTTAB, T_YCBCR, T_GRAY_IMAGES, T_MERGE, T_NSLOTS };
 void timing_reset();
 void walk_stats_reset();
 long long walk_stats_query(int which);
@@ -132,11 +132,34 @@ struct PupWork {
   const int32_t* slot_frame;   // frame of each slot (nullptr = frame 0) unless slots_per_frame > 0
   const uint8_t* flipv;        // per-slot flip flags (nullptr: use flip_of[j])
   int32_t slots_per_frame;     // > 0: frame = slot / slots_per_frame
-  int32_t nrows, ncols, dim, rot_slot;   // rot_slot: -1 unrotated; kRotSlotPerImage: images[frame].rot_slot
+  int32_t nrows, ncols, dim, rot_slot;   // rot_slot: -1 unrotated; kRotSlotPerImage: images[frame].rot_slot; kRotSlotPerFace: face_rot[slot / stride]
   int32_t first, span, stride, nwork, ntabs;
   PuplocTables tab[kMaxPupTabs];
   uint8_t tab_of[32], flip_of[32];
   const ImageDesc* images;     // mixed-size call: the image table the frame indices refer to (frames .. dim unused); nullptr = uniform frames
+  const int32_t* face_rot;     // angle sweep (rot_slot == kRotSlotPerFace, with images): rotation slot of face slot `slot / stride`
+};
+
+// Angle sweep merge (cluster.cu).  cluster_kernel<true> reads the sorted keys (position in D_i in the low 32 bits) and the
+// per-position angle tags, and writes each cluster's tag and slot_of[tag] (either output may be nullptr).
+struct SweepTags {
+  const uint64_t* keys;
+  const int32_t* tag;
+  const int32_t* slot_of;
+  int32_t* out_tag;
+  int32_t* out_rot;
+};
+// Device scratch of launch_sweep_merge, per image a segment of nangles*det_cap entries.
+struct SweepScratch {
+  pigo_det* merged;
+  pigo_det* tmp;
+  int32_t* tag;
+  int32_t* seeds;
+  uint8_t* flags;
+  uint64_t *keys_in, *keys_out;
+  int32_t *seg_begin, *seg_end, *n_merged;
+  void* sort_temp;
+  size_t sort_bytes;
 };
 
 // Chroma subsampling of image.YCbCrSubsampleRatio `sub` (0..5 = 444, 422, 420, 440, 411, 410) as shifts of the luma
@@ -231,6 +254,7 @@ struct Workspace {
   // cached uniform plan above (plan_host, pad_first_untiled, rot_slot + rot_tab, ptab_sig)
   DevBuf img_tab, img_rot;
   DevBuf gray_arena;                           // a sharded decoded call's converted images on this device (pigo_*_decoded_sharded)
+  DevBuf sweep;                                // an angle sweep's merge scratch and per-face outputs (pigo_*_images_sweep)
   std::vector<int> img_rot_slots;                           // what img_rot was built for: one table per slot, in order (empty = nothing)
   int img_rot_len = 0, img_rot_min = 0;
   double img_rot_scale = 0;
@@ -249,7 +273,7 @@ struct Workspace {
     for (auto e : copy_events) cudaEventDestroy(e);
     if (copy_stream) cudaStreamDestroy(copy_stream);
     tiles.release(); scratch_a.release(); scratch_b.release(); scratch_c.release(); rot_tab.release(); ptab.release();
-    img_tab.release(); img_rot.release(); gray_arena.release();
+    img_tab.release(); img_rot.release(); gray_arena.release(); sweep.release();
     if (pinned) cudaFreeHost(pinned);
     if (seq) cudaFreeHost(seq);
     if (stream) cudaStreamDestroy(stream);
@@ -361,6 +385,9 @@ void launch_finalize_images(const RawDet* raw, const int32_t* raw_count, int cap
                             pigo_det* out, int32_t* n_out, int nimages, cudaStream_t st);
 void launch_cluster(pigo_det* dets, const int32_t* n_in, int cap, double thr, pigo_det* tmp, uint8_t* flags, int32_t* seeds,
                     pigo_det* out, int out_cap, int32_t* n_out, int nframes, cudaStream_t st);
+size_t sweep_sort_bytes(int nimages, int seg_cap);
+int launch_sweep_merge(const pigo_det* raw, const int32_t* raw_count, int nimages, int nangles, int det_cap, double thr, const SweepScratch& S,
+                       const int32_t* slot_of, pigo_det* out, int out_cap, int32_t* n_out, int32_t* out_tag, int32_t* out_rot, cudaStream_t st);
 void launch_puploc(const PuplocTables& T, const pigo_point* seeds, int nseeds, const float* randoms, uint64_t rng_seed,
                    const uint8_t* frames, const int32_t* seed_frame, size_t frame_stride, int rows, int cols, int dim, int rot_slot,
                    const uint8_t* flipv, pigo_point* out, const ImageDesc* images, cudaStream_t st);

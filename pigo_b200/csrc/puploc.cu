@@ -188,7 +188,8 @@ __device__ __forceinline__ int clamp_coord(float v) { return max(-(1 << 30), min
 // scale shrinks by 0.7-0.8 per stage, so the later stages of a landmark call fit).  Stages that do not fit gather from global memory.
 // IMG (mixed-size call): the slot's frame index selects an entry of the image table W.images, which gives the pixels, the
 // clamps rows-1 / cols-1 and the row pitch (the patch's 16-byte path then needs that image's pitch and base aligned), and
-// with W.rot_slot == kRotSlotPerImage the rotation table slot.
+// with W.rot_slot == kRotSlotPerImage the rotation table slot; with W.rot_slot == kRotSlotPerFace (angle sweep) the slot
+// comes from W.face_rot of the slot's face, slot / W.stride.
 template <bool STAGED, bool PATCH, bool IMG = false>
 __global__ void __launch_bounds__(kPairThreads, PATCH ? 2 : 3) puploc_pair_kernel(const PupWork W, unsigned int* __restrict__ counter, int leaf_bytes,
                                                                                  int codes_bytes, int patch_cap) {
@@ -221,7 +222,8 @@ __global__ void __launch_bounds__(kPairThreads, PATCH ? 2 : 3) puploc_pair_kerne
     const uint8_t* __restrict__ pixels = IMG ? W.images[frame].base : W.frames + (size_t)frame * W.frame_stride;
     auto dim = [&]() { return IMG ? W.images[frame].dim : W.dim; };   // row pitch (read at each use, as W.dim was before IMG)
     const int L = T.leaves, tree_codes = 4 * L, rlim = (IMG ? W.images[frame].rows : W.nrows) - 1, clim = (IMG ? W.images[frame].cols : W.ncols) - 1;   // padded device layout, see PuplocTables
-    const int rot_slot = (IMG && W.rot_slot == kRotSlotPerImage) ? W.images[frame].rot_slot : W.rot_slot;
+    const int rot_slot = (IMG && W.rot_slot == kRotSlotPerImage) ? W.images[frame].rot_slot
+                         : (IMG && W.rot_slot == kRotSlotPerFace) ? W.face_rot[slot / W.stride] : W.rot_slot;
     const bool rot = rot_slot >= 0;
     const int sstride = tree_codes + 8;                    // shared-memory tree stride (bank skew)
     auto stage_codes = [&](int st) {

@@ -194,6 +194,53 @@ def detect_images_angles_device(clf: Pigo, plc: PuplocCascade, flpcs: Dict[str, 
                           det_cap, raw)
 
 
+def detect_images_sweep_device(clf: Pigo, plc: PuplocCascade, flpcs: Dict[str, PuplocCascade], images, cp: CascadeParams, angles,
+                               iou: float = 0.1, min_face: int = 50, eye_perturbs: int = 50, flp_perturbs: int = 63, face_cap: int = 32,
+                               randoms: Optional[np.ndarray] = None, rng_seed: int = 0, det_cap: int = 0, raw: bool = False):
+    """Every image scanned at every angle of `angles`, one merged face list per image (pigo_detect_images_sweep): each face is
+    refined with its eyes at the angle it was found at (the landmark calls stay at angle 0).  images as detect_images_device;
+    randoms: optional [N][face_cap][17][63][3] float32.  Returns List[List[(Face, angle)]] with `angle` the listed value
+    (raw=True: the (faces, n_faces, points, face_angle) arrays, face_angle indexing `angles`)."""
+    import ctypes as C
+    from . import DET_DTYPE, POINT_DTYPE, FRAMES_DEVICE, MEM_HOST, PipelineParams, _check, _pixels, image_descs, lib
+    hs, fl = landmark_call_arrays(flpcs)
+    ncalls = len(fl)
+    n = len(images)
+    on_dev = n > 0 and all(isinstance(im.Pixels, int) for im in images)
+    keep = [None if on_dev else _pixels(im) for im in images]   # host pixels stay alive for the call
+    desc = image_descs([(im.Pixels if on_dev else p.ctypes.data, im.Rows, im.Cols, im.Dim) for im, p in zip(images, keep)])
+    ang = np.ascontiguousarray(angles, dtype=np.float64)
+    prm = PipelineParams(cp.MinSize, cp.MaxSize, cp.ShiftFactor, cp.ScaleFactor, 0.0, iou, min_face, eye_perturbs, flp_perturbs, det_cap)
+    rnd = None
+    if randoms is not None:
+        rnd = np.ascontiguousarray(randoms, dtype=np.float32)
+        assert rnd.size == n * face_cap * (2 + ncalls) * 189, "randoms must be [N][face_cap][2+ncalls][63][3]"
+    faces = np.zeros((n, face_cap), dtype=DET_DTYPE)
+    nfaces = np.zeros(max(n, 1), dtype=np.int32)
+    points = np.zeros((n, face_cap, 2 + ncalls), dtype=POINT_DTYPE)
+    face_angle = np.full((n, face_cap), -1, dtype=np.int32)
+    _check(lib().pigo_detect_images_sweep(clf._h, plc._h, hs, fl.ctypes.data, ncalls, desc, n, ang.ctypes.data, len(ang), C.byref(prm),
+                                          rnd.ctypes.data if rnd is not None else None, rng_seed, faces.ctypes.data, face_angle.ctypes.data,
+                                          face_cap, nfaces.ctypes.data, points.ctypes.data, FRAMES_DEVICE if on_dev else MEM_HOST, None))
+    if raw:
+        return faces, nfaces[:n], points, face_angle
+    return [[(fc, float(ang[face_angle[i, k]])) for k, fc in enumerate(row)] for i, row in enumerate(_faces_of(faces, nfaces, points, min_face))]
+
+
+def detect_images_sweep_device_ptrs(clf: Pigo, plc: PuplocCascade, flpcs: Dict[str, PuplocCascade], images, angles, prm, faces_ptr: int,
+                                    face_angle_ptr: int, face_cap: int, nfaces_ptr: int, points_ptr: int, randoms_ptr: int = 0,
+                                    rng_seed: int = 0, stream: int = 0):
+    """Fully device-resident, asynchronous pigo_detect_images_sweep: images = [(device pointer, rows, cols, dim)], prm a
+    PipelineParams, every output a device pointer (face_angle_ptr 0 = not wanted); no host sync."""
+    from . import FRAMES_DEVICE, OUT_DEVICE, _check, image_descs, lib
+    import ctypes as C
+    hs, fl = landmark_call_arrays(flpcs)
+    ang = np.ascontiguousarray(angles, dtype=np.float64)
+    _check(lib().pigo_detect_images_sweep(clf._h, plc._h, hs, fl.ctypes.data, len(fl), image_descs(images), len(images), ang.ctypes.data, len(ang),
+                                          C.byref(prm), randoms_ptr or None, rng_seed, faces_ptr, face_angle_ptr or None, face_cap, nfaces_ptr,
+                                          points_ptr, FRAMES_DEVICE | OUT_DEVICE, stream or None))
+
+
 def detect_images_sharded(clf: Pigo, plc: PuplocCascade, flpcs: Dict[str, PuplocCascade], images, cp: CascadeParams, angles=None,
                           iou: float = 0.1, min_face: int = 50, eye_perturbs: int = 50, flp_perturbs: int = 63, face_cap: int = 32,
                           angle: float = 0.0, randoms: Optional[np.ndarray] = None, rng_seed: int = 0, det_cap: int = 0, raw: bool = False):

@@ -27,6 +27,9 @@ Usage: `python tools/ragged_bench.py [--frames 256]` on one GPU prints one JSON 
   sharded : the same 256 images (a quarter of the wide ones rotated) from host memory: one single-device call against the
               sharded calls with shard_split 1, 2, 4, 8, outputs asserted identical; per-shard modelled cost against
               measured time (sharded_bench)
+  sweep   : one 1080p frame and 16 wide images of the mix, each x 32 angles: one pigo_detect_images_sweep against
+              pigo_detect_images_angles over the expanded list plus a merge through host memory; the merge kernels' own time
+              (sweep_bench)
 `--sections scan,pipeline` (the default) selects the sections; `--sections angles` runs the sweeps alone.  Writes nothing
 to the tree.
 """
@@ -497,6 +500,113 @@ def angles_bench(clf, dev: int, stream) -> dict:
     return res
 
 
+def sweep_bench(clf, dev: int, stream) -> dict:
+    """An angle sweep merged per image: one pigo_detect_images_sweep call against pigo_detect_images_angles over the expanded
+    (image x angle) list followed by a merge through host memory (D2H of its faces, then pigo_cluster_batch of each image's
+    concatenated faces).  Host clock around each way ending in a synchronise, median of 5 after 2; the merge kernels' own
+    time from the library's CUDA-event timing (option "timing") in a separate run."""
+    import ctypes as C
+    import time
+    import torch
+    import pigo_b200
+    from pigo_b200 import pipeline, synth
+    L = pigo_b200.lib()
+    st = stream.cuda_stream
+    cuda = f"cuda:{dev}"
+    plc = pigo_b200.NewPuplocCascade().UnpackCascade(pigo_b200.load_cascade("puploc"))
+    names = sorted(set(pipeline.EYE_CASCADES + pipeline.MOUTH_CASCADES))
+    flp = {nm: pigo_b200.NewPuplocCascade().UnpackCascade(pigo_b200.load_cascade("lps/" + nm)) for nm in names}
+    hs, fl = pipeline.landmark_call_arrays(flp)
+    ncalls = len(fl)
+    angles = [k / 32 for k in range(32)]
+    ang = np.array(angles, dtype=np.float64)
+    na = len(angles)
+    flags = pigo_b200.FRAMES_DEVICE | pigo_b200.OUT_DEVICE
+
+    def check(rc):
+        if rc != 0:
+            raise RuntimeError(L.pigo_last_error().decode())
+
+    def wall(fn, reps=5, warm=2):
+        for _ in range(warm):
+            fn()
+        torch.cuda.synchronize()
+        ts = []
+        for _ in range(reps):
+            t0 = time.perf_counter()
+            fn()
+            torch.cuda.synchronize()
+            ts.append((time.perf_counter() - t0) * 1e3)
+        return float(np.median(ts))
+
+    def workload(base, face_cap):
+        n = len(base)
+        prm = pigo_b200.PipelineParams(*PARAMS, 0.0, 0.1, 50, 50, 63, 4096)
+        desc = pigo_b200.image_descs(base)
+        f = torch.zeros((n, face_cap, 4), dtype=torch.int32, device=cuda)
+        fa = torch.zeros((n, face_cap), dtype=torch.int32, device=cuda)
+        nf = torch.zeros(n, dtype=torch.int32, device=cuda)
+        pts = torch.zeros((n, face_cap, 2 + ncalls, 4), dtype=torch.int32, device=cuda)
+
+        def sweep():
+            check(L.pigo_detect_images_sweep(clf._h, plc._h, hs, fl.ctypes.data, ncalls, desc, n, ang.ctypes.data, na, C.byref(prm), None, 7,
+                                             f.data_ptr(), fa.data_ptr(), face_cap, nf.data_ptr(), pts.data_ptr(), flags, C.c_void_p(st)))
+
+        ex = pigo_b200.image_descs([b for b in base for _ in angles])
+        exa = np.array([a for _ in base for a in angles], dtype=np.float64)
+        m = n * na
+        ef = torch.zeros((m, face_cap, 4), dtype=torch.int32, device=cuda)
+        enf = torch.zeros(m, dtype=torch.int32, device=cuda)
+        epts = torch.zeros((m, face_cap, 2 + ncalls, 4), dtype=torch.int32, device=cuda)
+        merged = {}
+
+        def per_entry():
+            check(L.pigo_detect_images_angles(clf._h, plc._h, hs, fl.ctypes.data, ncalls, ex, m, exa.ctypes.data, C.byref(prm), None, 7,
+                                              ef.data_ptr(), face_cap, enf.data_ptr(), epts.data_ptr(), flags, C.c_void_p(st)))
+            faces = ef.cpu().numpy().view(pigo_b200.DET_DTYPE).reshape(n, na * face_cap)
+            cnt = enf.cpu().numpy().reshape(n, na)
+            cat = np.zeros((n, na * face_cap), dtype=pigo_b200.DET_DTYPE)
+            k = np.zeros(n, dtype=np.int32)
+            for i in range(n):
+                parts = [faces[i, a * face_cap:a * face_cap + cnt[i, a]] for a in range(na)]
+                k[i] = sum(len(p) for p in parts)
+                cat[i, :k[i]] = np.concatenate(parts)
+            merged["clusters"], merged["n"] = clf.cluster_batch_array(cat, k, 0.1)
+            merged["refined"] = int((cat["scale"] > 50).sum())
+
+        ms_sweep = wall(sweep)
+        ms_entry = wall(per_entry)
+        pigo_b200.set_option("timing", 1)
+        sweep()
+        torch.cuda.synchronize()
+        merge_ms = pigo_b200.get_option("t_merge_ns") / 1e6
+        merge_n = pigo_b200.get_option("t_merge_n")
+        pigo_b200.set_option("timing", 0)
+        nfh, fh = nf.cpu().numpy(), f.cpu().numpy().view(pigo_b200.DET_DTYPE).reshape(n, face_cap)
+        assert int(nfh.max()) <= face_cap and int(enf.max()) <= face_cap, (int(nfh.max()), int(enf.max()), face_cap)
+        refined = int(sum((fh[i, :nfh[i]]["scale"] > 50).sum() for i in range(n)))
+        return {"images": n, "angles": na, "ms_sweep": ms_sweep, "ms_angles_plus_host_merge": ms_entry, "speedup": ms_entry / ms_sweep,
+                "merge_kernels_ms": merge_ms, "merge_launches": merge_n, "faces_sweep": int(nfh.sum()), "refined_sweep": refined,
+                "faces_host_merge": int(merged["n"].sum()), "refined_per_entry": merged["refined"]}
+
+    res = {}
+    fr = torch.from_numpy(synth.frame_faces(None, 1080, 1920, noise_seed=3)).to(cuda)
+    res["frame_1080p"] = workload([(fr.data_ptr(), 1080, 1920, 1920)], 1024)
+    imgs = [im for im in ragged_images(64, seed=7) if im[2] >= im[1]][:16]   # wide images: the rotated column clamp stays inside
+    offs, total = [], 0
+    for b, r, c, d in imgs:
+        offs.append(total)
+        total += (r * d + 255) & ~255
+    host = np.zeros(total, dtype=np.uint8)
+    for (b, r, c, d), o in zip(imgs, offs):
+        host[o:o + r * d] = b.reshape(-1)
+    dev_all = torch.from_numpy(host).to(cuda)
+    res["mixed_16"] = workload([(dev_all.data_ptr() + o, r, c, d) for (b, r, c, d), o in zip(imgs, offs)], 1024)
+    res["note"] = ("k/32, k = 0..31; test parameters, IoU 0.1, eye Perturbs 50, 15 landmark calls, device images; host clock, median of 5 "
+                   "after 2; merge_kernels_ms = compaction + segmented sort + tagged clustering of one sweep call (CUDA events)")
+    return res
+
+
 def decoded_bench(clf, dev: int, stream) -> dict:
     """Decoded JPEG-like sources to detector results three ways, and the conversion alone; see the module docstring."""
     import ctypes as C
@@ -836,7 +946,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--frames", type=int, default=256, help="frames of the uniform 1080p comparison")
     ap.add_argument("--pipeline-frames", type=int, default=64, help="frames of the uniform 1080p pipeline comparison")
-    ap.add_argument("--sections", default="scan,pipeline", help="comma-separated: scan, pipeline, angles, decoded, formats, sharded")
+    ap.add_argument("--sections", default="scan,pipeline", help="comma-separated: scan, pipeline, angles, decoded, formats, sharded, sweep")
     args = ap.parse_args()
     sections = set(args.sections.split(","))
     import torch
@@ -857,6 +967,8 @@ def main():
         res["formats"] = formats_bench(clf, 0, stream)
     if "sharded" in sections:
         res["sharded"] = sharded_bench(clf, 0)
+    if "sweep" in sections:
+        res["sweep"] = sweep_bench(clf, 0, stream)
     res["gpu"] = torch.cuda.get_device_name(0)
     try:   # read-only query: the power limit belongs beside the numbers
         import subprocess
