@@ -278,6 +278,15 @@ def _pixels(img: ImageParams) -> np.ndarray:
     return p
 
 
+def _image_table(images):
+    """(descriptor array, pixel flag, keep) of a mixed-size call's images: FRAMES_DEVICE when every image's Pixels is a device
+    pointer (int), else MEM_HOST with host arrays, which `keep` holds alive for the call."""
+    on_dev = len(images) > 0 and all(isinstance(im.Pixels, int) for im in images)
+    keep = [None if on_dev else _pixels(im) for im in images]
+    desc = image_descs([(im.Pixels if on_dev else p.ctypes.data, im.Rows, im.Cols, im.Dim) for im, p in zip(images, keep)])
+    return desc, (FRAMES_DEVICE if on_dev else MEM_HOST), keep
+
+
 class Pigo:
     """pigo.Pigo (core/pigo.go:37-43): the face classifier; tables live on the device."""
 
@@ -384,19 +393,9 @@ class Pigo:
         or for every image alike device pointers (int) holding Rows*Dim bytes.  Returns (dets[N, cap] DET_DTYPE, counts[N])."""
         self._need()
         n = len(images)
-        on_dev = n > 0 and all(isinstance(im.Pixels, int) for im in images)
-        keep = [None if on_dev else _pixels(im) for im in images]   # host pixels stay alive for the call
-        desc = image_descs([(im.Pixels if on_dev else p.ctypes.data, im.Rows, im.Cols, im.Dim) for im, p in zip(images, keep)])
-        while True:
-            out = np.zeros((n, max(cap_per_image, 1)), dtype=DET_DTYPE)
-            cnt = np.zeros(max(n, 1), dtype=np.int32)
-            rc = lib().pigo_run_cascade_images(self._h, desc, n, cp.MinSize, cp.MaxSize, cp.ShiftFactor, cp.ScaleFactor, angle,
-                                               out.ctypes.data, cap_per_image, cnt.ctypes.data, FRAMES_DEVICE if on_dev else MEM_HOST, None)
-            if rc == PIGO_E_CAP:
-                cap_per_image = int(cnt.max())
-                continue
-            _check(rc)
-            return out, cnt[:n]
+        desc, flags, keep = _image_table(images)
+        return self._retry_cap(n, cap_per_image, lambda out, cap, cnt: lib().pigo_run_cascade_images(
+            self._h, desc, n, cp.MinSize, cp.MaxSize, cp.ShiftFactor, cp.ScaleFactor, angle, out, cap, cnt, flags, None))
 
     def run_cascade_images_device(self, images, min_size: int, max_size: int, shift: float, scale: float, angle: float, out_ptr: int,
                                   cap_per_image: int, counts_ptr: int, stream: int = 0):
@@ -413,20 +412,10 @@ class Pigo:
         n = len(images)
         if len(angles) != n:
             raise ValueError("angles must have one entry per image")
-        on_dev = n > 0 and all(isinstance(im.Pixels, int) for im in images)
-        keep = [None if on_dev else _pixels(im) for im in images]   # host pixels stay alive for the call
-        desc = image_descs([(im.Pixels if on_dev else p.ctypes.data, im.Rows, im.Cols, im.Dim) for im, p in zip(images, keep)])
+        desc, flags, keep = _image_table(images)
         ang = np.ascontiguousarray(angles, dtype=np.float64)
-        while True:
-            out = np.zeros((n, max(cap_per_image, 1)), dtype=DET_DTYPE)
-            cnt = np.zeros(max(n, 1), dtype=np.int32)
-            rc = lib().pigo_run_cascade_images_angles(self._h, desc, n, ang.ctypes.data, cp.MinSize, cp.MaxSize, cp.ShiftFactor, cp.ScaleFactor,
-                                                      out.ctypes.data, cap_per_image, cnt.ctypes.data, FRAMES_DEVICE if on_dev else MEM_HOST, None)
-            if rc == PIGO_E_CAP:
-                cap_per_image = int(cnt.max())
-                continue
-            _check(rc)
-            return out, cnt[:n]
+        return self._retry_cap(n, cap_per_image, lambda out, cap, cnt: lib().pigo_run_cascade_images_angles(
+            self._h, desc, n, ang.ctypes.data, cp.MinSize, cp.MaxSize, cp.ShiftFactor, cp.ScaleFactor, out, cap, cnt, flags, None))
 
     def run_cascade_images_angles_device(self, images, angles: Sequence[float], min_size: int, max_size: int, shift: float, scale: float,
                                          out_ptr: int, cap_per_image: int, counts_ptr: int, stream: int = 0):
@@ -447,9 +436,7 @@ class Pigo:
         Returns (clusters[N, cap] DET_DTYPE, angle_index[N, cap] int32, counts[N])."""
         self._need()
         n = len(images)
-        on_dev = n > 0 and all(isinstance(im.Pixels, int) for im in images)
-        keep = [None if on_dev else _pixels(im) for im in images]   # host pixels stay alive for the call
-        desc = image_descs([(im.Pixels if on_dev else p.ctypes.data, im.Rows, im.Cols, im.Dim) for im, p in zip(images, keep)])
+        desc, flags, keep = _image_table(images)
         ang = np.ascontiguousarray(angles, dtype=np.float64)
         while True:
             out = np.zeros((n, max(cap_per_image, 1)), dtype=DET_DTYPE)
@@ -457,7 +444,7 @@ class Pigo:
             cnt = np.zeros(max(n, 1), dtype=np.int32)
             rc = lib().pigo_run_cascade_images_sweep(self._h, desc, n, ang.ctypes.data, len(ang), cp.MinSize, cp.MaxSize, cp.ShiftFactor,
                                                      cp.ScaleFactor, iou, det_cap, out.ctypes.data, tag.ctypes.data, cap_per_image,
-                                                     cnt.ctypes.data, FRAMES_DEVICE if on_dev else MEM_HOST, None)
+                                                     cnt.ctypes.data, flags, None)
             if rc == PIGO_E_CAP:
                 if "raw detections" in lib().pigo_last_error().decode():
                     det_cap = 4 * (det_cap or 2048)
@@ -661,12 +648,10 @@ class PuplocCascade:
         out = np.zeros(n, dtype=POINT_DTYPE)
         rnd = np.ascontiguousarray(randoms, dtype=np.float32) if randoms is not None else None
         fl = np.ascontiguousarray(np.asarray(flipv, dtype=np.uint8)) if flipv is not None else None
-        on_dev = len(images) > 0 and all(isinstance(im.Pixels, int) for im in images)
-        keep = [None if on_dev else _pixels(im) for im in images]   # host pixels stay alive for the call
-        desc = image_descs([(im.Pixels if on_dev else p.ctypes.data, im.Rows, im.Cols, im.Dim) for im, p in zip(images, keep)])
+        desc, flags, keep = _image_table(images)
         _check(lib().pigo_puploc_run_images(self._h, s.ctypes.data, n, si.ctypes.data, rnd.ctypes.data if rnd is not None else None, rng_seed,
                                             desc, len(images), angle, fl.ctypes.data if fl is not None else None, out.ctypes.data,
-                                            FRAMES_DEVICE if on_dev else MEM_HOST, None))
+                                            flags, None))
         return [Puploc(int(o["row"]), int(o["col"]), float(np.float32(o["scale"])), int(o["perturbs"])) for o in out]
 
     def RunDetector(self, pl: Puploc, img: ImageParams, angle: float, flipV: bool, randoms: Optional[np.ndarray] = None,

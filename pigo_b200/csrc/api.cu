@@ -104,6 +104,23 @@ static int ws_leave_async(Workspace* w, cudaStream_t st) {
   return PIGO_OK;
 }
 
+// One call's borrow of a workspace of `pool`, used as that Workspace*.  st = the caller's stream (or, stream_ NULL, the
+// workspace's own), already ordered behind the workspace's last asynchronous use (ws_enter); rc = the borrow's result.
+struct Borrow {
+  WsGuard guard;
+  Workspace* w = nullptr;
+  cudaStream_t st = nullptr;
+  int rc = PIGO_OK;
+  Borrow(WorkspacePool& pool, void* stream_) : guard(pool), w(guard.w) {
+    if (!w) { rc = set_err(PIGO_E_CUDA, "could not create a CUDA stream"); return; }
+    st = stream_ ? (cudaStream_t)stream_ : w->stream;
+    rc = ws_enter(w, st);
+  }
+  Workspace* operator->() const { return w; }
+  operator Workspace*() const { return w; }
+  void keep() { guard.w = nullptr; }   // the workspace never goes back to the pool (it belongs to a captured graph)
+};
+
 void raise_dyn_smem(const void* fn, int bytes) {
   static std::mutex mu;
   static std::map<std::pair<int, const void*>, int> granted;   // (device, kernel) -> the attribute's value
@@ -312,12 +329,16 @@ static std::vector<int> group_schedule(int nframes, bool resident, bool streamed
   return g;
 }
 
-// Host outputs of a RunCascade batch: the counts, then only the used prefix of every frame's slice of d_out
-// ([nframes][cap]); PIGO_E_CAP if a frame has more detections than cap_per_frame.
-static int copy_results_to_host(const pigo_det* d_out, const int32_t* d_nout, int cap, int nframes, pigo_det* out, int cap_per_frame,
-                                int* n_out, cudaStream_t st) {
-  CUDA_TRY(cudaMemcpyAsync(n_out, d_nout, (size_t)nframes * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+// Host outputs of a scan: the counts, then only the used prefix of every frame's slice of d_out ([nframes][cap]) and, given
+// `tags`, of the per-slot int32 d_tags ([nframes][cap]); PIGO_E_CAP if a frame has more detections than cap_per_frame.
+// The counts are the lead + nframes int32 at d_cnt, copied at once: the frame counts come last, after `lead` others (an
+// angle sweep's raw-list counts), and with lead > 0 all of them go to cnt and n_out receives the frame counts.
+static int copy_results_to_host(const pigo_det* d_out, const int32_t* d_cnt, int cap, int nframes, pigo_det* out, int cap_per_frame,
+                                int* n_out, cudaStream_t st, const int32_t* d_tags = nullptr, int32_t* tags = nullptr, int lead = 0,
+                                int32_t* cnt = nullptr) {
+  CUDA_TRY(cudaMemcpyAsync(lead > 0 ? cnt : n_out, d_cnt, (size_t)(lead + nframes) * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaStreamSynchronize(st));
+  if (lead > 0) std::copy(cnt + lead, cnt + lead + nframes, n_out);
   int need_more = 0;
   size_t max_n = 0;
   for (int f = 0; f < nframes; ++f) {
@@ -328,11 +349,21 @@ static int copy_results_to_host(const pigo_det* d_out, const int32_t* d_nout, in
   if (cap_per_frame > 0 && max_n > 0) {
     CUDA_TRY(cudaMemcpy2DAsync(out, (size_t)cap_per_frame * sizeof(pigo_det), d_out, (size_t)cap * sizeof(pigo_det),
                                max_n * sizeof(pigo_det), nframes, cudaMemcpyDeviceToHost, st));
+    if (tags)
+      CUDA_TRY(cudaMemcpy2DAsync(tags, (size_t)cap_per_frame * 4, d_tags, (size_t)cap * 4, max_n * 4, nframes, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
   }
   if (need_more) return set_err(PIGO_E_CAP, "output capacity %d per frame too small", cap_per_frame);
   return PIGO_OK;
 }
+
+// Bytes of a host image the reference may index, (rows-1)*dim + cols (core/pigo.go:126 with Dim >= Cols): never read more
+// than that from the caller's buffer.
+static size_t readable_bytes(int rows, int cols, int dim) { return rows > 0 ? (size_t)(rows - 1) * dim + cols : 0; }
+
+// Table slot of a rotated scan, core/pigo.go:159,:232-236: angle > 0 rotates, angle > 1 is clamped to 1, and angle <= 0
+// or NaN scans unrotated (-1).
+static int rot_slot_of(double angle) { return angle > 0.0 ? (int)(32.0 * (angle > 1.0 ? 1.0 : angle)) : -1; }
 
 // ---- RunCascade on one device -----------------------------------------------------------------------------------
 static int scan_batch_on(pigo_cascade* c, int dev, const uint8_t* frames, int nframes, size_t frame_stride, int rows, int cols, int dim,
@@ -346,26 +377,26 @@ static int scan_batch_on(pigo_cascade* c, int dev, const uint8_t* frames, int nf
   if ((rc = use_device(dev))) return rc;
   const bool frames_dev = flags & PIGO_FRAMES_DEVICE, out_dev = flags & PIGO_OUT_DEVICE;
 
-  WsGuard g(R->pool);
-  Workspace* w = g.w;
-  if (!w) return set_err(PIGO_E_CUDA, "could not create a CUDA stream");
-  cudaStream_t st = stream_ ? (cudaStream_t)stream_ : w->stream;
-  if ((rc = ws_enter(w, st))) return rc;
+  Borrow w(R->pool, stream_);
+  if (w.rc) return w.rc;
+  cudaStream_t st = w.st;
+  auto plan_cached = [&] {
+    return w->p_rows == rows && w->p_cols == cols && w->p_min == min_size && w->p_max == max_size && w->p_shift == shift_factor &&
+           w->p_scale == scale_factor;
+  };
   // CUDA-graph capture (device frames + device outputs on the caller's capturing stream, after one un-captured warm-up call
   // with the same arguments): the captured kernels keep using this workspace's scratch on every replay, so the workspace
   // is taken out of the pool for good -- it belongs to the graph from now on.
   const bool capturing = stream_capturing(st);
   if (capturing) {
     if (!(flags & PIGO_FRAMES_DEVICE) || !(flags & PIGO_OUT_DEVICE)) return set_err(PIGO_E_INVALID, "stream capture needs device frames and device outputs");
-    if (w->p_rows != rows || w->p_cols != cols || w->p_min != min_size || w->p_max != max_size || w->p_shift != shift_factor ||
-        w->p_scale != scale_factor)
+    if (!plan_cached())
       return set_err(PIGO_E_INVALID, "stream capture: run the same call once outside the capture first (the plan upload synchronises)");
-    g.w = nullptr;
+    w.keep();
   }
 
   // plan (cached per workspace)
-  if (w->p_rows != rows || w->p_cols != cols || w->p_min != min_size || w->p_max != max_size || w->p_shift != shift_factor ||
-      w->p_scale != scale_factor) {
+  if (!plan_cached()) {
     rc = build_plan(rows, cols, min_size, max_size, shift_factor, scale_factor, w->plan_host, w->wins);
     if (rc) { w->p_rows = -1; return rc; }
     if ((rc = w->plan.reserve((w->plan_host.size() + 1) * sizeof(ScaleEntry)))) return rc;
@@ -380,11 +411,10 @@ static int scan_batch_on(pigo_cascade* c, int dev, const uint8_t* frames, int nf
   const int nscales = (int)w->plan_host.size();
   const int cap = cap_per_frame > 0 ? cap_per_frame : 1;
 
-  // device buffers.  A host frame is only guaranteed to hold (rows-1)*dim + cols bytes (what the reference indexes,
-  // core/pigo.go:126 with Dim >= Cols): never read more than that from the caller's buffer.
+  // device buffers.  A host frame is only guaranteed to hold its readable bytes.
   const uint8_t* d_frames = frames;
   const size_t frame_bytes = (size_t)rows * dim;
-  const size_t frame_min = rows > 0 ? (size_t)(rows - 1) * dim + cols : 0;
+  const size_t frame_min = readable_bytes(rows, cols, dim);
   size_t d_stride = frame_stride;
   uint8_t* d_frames_w = host_frames_dst;
   if (!frames_dev) {
@@ -409,11 +439,7 @@ static int scan_batch_on(pigo_cascade* c, int dev, const uint8_t* frames, int nf
   // Sub-batch pipeline: the batch is cut into groups of frames (group_schedule) that alternate between `lanes` internal
   // streams.  (1) The deferred queue (Q2) of a group is bounded and consumed soon after they are filled;
   // (2) with host frames, the H2D copy of group k+1 overlaps the scan of group k.
-  int rot_slot = -1;
-  if (angle > 0.0) {                      // core/pigo.go:232-236
-    const double a = angle > 1.0 ? 1.0 : angle;
-    rot_slot = (int)(32.0 * a);           // :159
-  }
+  const int rot_slot = rot_slot_of(angle);
   // Host frames, streamed: the copy stream moves the frames up chunk by chunk and bumps a ready counter after each chunk;
   // the fused kernel (whose tile / block order is frame-major) waits in-kernel for the frame it is about to touch, so the
   // scan runs right behind the copy at frame granularity instead of group granularity.  Only the fused kernel polls: the
@@ -525,6 +551,20 @@ static int check_batch_args(const pigo_cascade* c, const uint8_t* frames, int nf
 // (128 x 894,448), so that the deep queue of a group stays as bounded as the uniform path's.
 static constexpr uint64_t kImagesGroupWindows = 128ull * 894448ull;
 
+// Geometry of images[0..nimages): rows and cols at least min_edge (1 where images are refined on, which needs a pixel) and
+// dim >= cols; with `pixels` also at most 2^31 bytes and non-null pixels.
+static int check_image_geometry(const pigo_image* images, int nimages, int min_edge, bool pixels) {
+  for (int i = 0; i < nimages; ++i) {
+    const pigo_image& im = images[i];
+    if (im.rows < min_edge || im.cols < min_edge || im.dim < im.cols)
+      return set_err(PIGO_E_INVALID, "image %d: bad geometry rows=%d cols=%d dim=%d", i, im.rows, im.cols, im.dim);
+    if (!pixels) continue;
+    if ((uint64_t)im.rows * (uint64_t)im.dim > 0x7fffffffull) return set_err(PIGO_E_INVALID, "image %d: larger than 2^31 bytes", i);
+    if (!im.pixels) return set_err(PIGO_E_INVALID, "image %d: null pixels", i);
+  }
+  return PIGO_OK;
+}
+
 static int check_images_args(const pigo_cascade* c, const pigo_image* images, int nimages, const pigo_det* out, int cap_per_image,
                              const int* n_out) {
   if (nimages < 0 || nimages > 65535) return set_err(PIGO_E_INVALID, "nimages must be 0..65535");
@@ -532,26 +572,37 @@ static int check_images_args(const pigo_cascade* c, const pigo_image* images, in
   if (!n_out) return set_err(PIGO_E_INVALID, "null n_out");
   if (cap_per_image < 0) return set_err(PIGO_E_INVALID, "negative capacity");
   if (!out && cap_per_image > 0) return set_err(PIGO_E_INVALID, "null out");
-  for (int i = 0; i < nimages; ++i) {
-    const pigo_image& im = images[i];
-    if (im.rows < 0 || im.cols < 0 || im.dim < im.cols)
-      return set_err(PIGO_E_INVALID, "image %d: bad geometry rows=%d cols=%d dim=%d", i, im.rows, im.cols, im.dim);
-    if ((uint64_t)im.rows * (uint64_t)im.dim > 0x7fffffffull) return set_err(PIGO_E_INVALID, "image %d: larger than 2^31 bytes", i);
-    if (!im.pixels) return set_err(PIGO_E_INVALID, "image %d: null pixels", i);
-  }
+  const int rc = check_image_geometry(images, nimages, 0, true);
+  if (rc) return rc;
   if (!c) return set_err(PIGO_E_INVALID, "null cascade");
   return PIGO_OK;
 }
 
-// Per-image ladders (host only).  `longest` = the image with the longest ladder; every other ladder must be a prefix of it
-// (the rotated node table and the meaning of a ladder index are shared by the whole call).
-static int build_image_plans(const pigo_image* images, int nimages, int min_size, int max_size, double shift, double scale_factor,
-                             std::vector<std::vector<ScaleEntry>>& plans, std::vector<uint64_t>& wins, int& longest) {
+// The ladders of a mixed-size call's images (host only).  `longest` = the first image with the strictly longest ladder;
+// every other ladder is a prefix of it (the rotated node table and the meaning of a ladder index are shared by the whole call).
+struct ImagePlans {
+  std::vector<std::vector<ScaleEntry>> plans;
+  std::vector<uint64_t> wins;
+  int longest = 0;
+  // The ladders of entries [lo, lo+n), the shard of a sharded call that starts at entry lo.
+  ImagePlans slice(int lo, int n) const {
+    ImagePlans s;
+    s.plans.assign(plans.begin() + lo, plans.begin() + lo + n);
+    s.wins.assign(wins.begin() + lo, wins.begin() + lo + n);
+    for (int i = 0; i < n; ++i)
+      if (s.plans[i].size() > s.plans[s.longest].size()) s.longest = i;
+    return s;
+  }
+};
+
+static int build_image_plans(const pigo_image* images, int nimages, int min_size, int max_size, double shift, double scale_factor, ImagePlans& ip) {
+  auto& plans = ip.plans;
   plans.assign(nimages, {});
-  wins.assign(nimages, 0);
+  ip.wins.assign(nimages, 0);
+  int& longest = ip.longest;
   longest = 0;
   for (int i = 0; i < nimages; ++i) {
-    int rc = build_plan(images[i].rows, images[i].cols, min_size, max_size, shift, scale_factor, plans[i], wins[i]);
+    int rc = build_plan(images[i].rows, images[i].cols, min_size, max_size, shift, scale_factor, plans[i], ip.wins[i]);
     if (rc) return rc;
     if (plans[i].size() > plans[longest].size()) longest = i;
   }
@@ -563,10 +614,6 @@ static int build_image_plans(const pigo_image* images, int nimages, int min_size
     }
   return PIGO_OK;
 }
-
-// Table slot of a rotated scan, core/pigo.go:159,:232-236: angle > 0 rotates, angle > 1 is clamped to 1, and angle <= 0
-// or NaN scans unrotated (-1).
-static int rot_slot_of(double angle) { return angle > 0.0 ? (int)(32.0 * (angle > 1.0 ? 1.0 : angle)) : -1; }
 
 // Bound on the rotated node tables one pass of a mixed-size call keeps on the device (one table per distinct slot, each
 // over the call's longest ladder, at most 512 MB).  A call whose slots need more runs its rotated images in several passes.
@@ -595,6 +642,26 @@ static size_t arena_layout(const pigo_image* images, int n, std::vector<size_t>&
                       [](const pigo_image& im) { return (size_t)im.rows * im.dim; }, off, first);
 }
 
+// Host images into one arena in w->frames (arena_layout: each distinct image once), copying only their readable bytes;
+// pixels[i] = image i's device copy.  Given `wins`, images without windows are not copied: a scan never reads them.
+static int stage_pixels(Workspace* w, const pigo_image* images, int nimages, const std::vector<uint64_t>* wins, cudaStream_t st,
+                        std::vector<const uint8_t*>& pixels) {
+  std::vector<size_t> off;
+  std::vector<char> first;
+  const size_t total = arena_layout(images, nimages, off, first);
+  const int rc = w->frames.reserve(total + 256);
+  if (rc) return rc;
+  pixels.resize(nimages);
+  for (int i = 0; i < nimages; ++i) {
+    uint8_t* dst = (uint8_t*)w->frames.p + off[i];
+    pixels[i] = dst;
+    if (!first[i] || (wins && (*wins)[i] == 0)) continue;   // a repeat, or never read
+    const pigo_image& im = images[i];
+    CUDA_TRY(cudaMemcpyAsync(dst, im.pixels, readable_bytes(im.rows, im.cols, im.dim), cudaMemcpyHostToDevice, st));
+  }
+  return PIGO_OK;
+}
+
 // Decoded images of pigo_gray_images: byte-identical descriptors share a slot of width*height gray bytes.
 static size_t arena_layout(const pigo_decoded* src, int n, std::vector<size_t>& off, std::vector<char>& first) {
   return arena_layout(src, n,
@@ -609,9 +676,9 @@ static size_t arena_layout(const pigo_decoded* src, int n, std::vector<size_t>& 
 // in passes: the unrotated images in caller order, then the rotated ones ordered by (slot, caller index), cut into
 // passes of at most kImagesRotBytes of node tables.  That order does not depend on how the caller interleaves images and
 // angles.  Each pass is grouped and scheduled from its own windows; finalize writes every image to its caller index.
-static int scan_images_on(pigo_cascade* c, int dev, const pigo_image* images, int nimages, const std::vector<std::vector<ScaleEntry>>& plans,
-                          const std::vector<uint64_t>& wins, int longest, int min_size, int max_size, double shift_factor, double scale_factor,
-                          const double* angles, pigo_det* out, int cap_per_image, int* n_out, unsigned flags, void* stream_) {
+static int scan_images_on(pigo_cascade* c, int dev, const pigo_image* images, int nimages, const ImagePlans& ip, int min_size, int max_size,
+                          double shift_factor, double scale_factor, const double* angles, pigo_det* out, int cap_per_image, int* n_out,
+                          unsigned flags, void* stream_) {
   int rc = PIGO_OK;
   FaceReplica* R = face_replica(c, dev, &rc);
   if (!R) return rc;
@@ -620,13 +687,10 @@ static int scan_images_on(pigo_cascade* c, int dev, const pigo_image* images, in
   std::vector<int> slot(nimages);
   bool any_rot = false;
   for (int i = 0; i < nimages; ++i) { slot[i] = rot_slot_of(angles[i]); any_rot |= slot[i] >= 0; }
-  const int nlad = (int)plans[longest].size();
-  const int max_scale = nlad > 0 ? plans[longest].back().s : 0;
+  const int nlad = (int)ip.plans[ip.longest].size();
+  const int max_scale = nlad > 0 ? ip.plans[ip.longest].back().s : 0;
   const size_t rot_bytes = (size_t)nlad * (size_t)R->tab.ntrees * 64 * sizeof(RotNode);
-  const long long mode = g_opt.scan_mode.load();
-  const bool fast = R->tab.depth == 6 && R->tiled_tab.p != nullptr && mode != 1 &&
-                    (!any_rot || (g_opt.rot_mode.load() == 0 && max_scale <= 32000 && rot_bytes <= ((size_t)1 << 29)));
-  if (!fast) {
+  if (!block_path(R, any_rot, max_scale, rot_bytes)) {
     // cascades of depth != 6 and the universal-kernel options: the single-image path, image by image at its own angle
     int rc_cap = PIGO_OK;
     for (int i = 0; i < nimages; ++i) {
@@ -639,11 +703,9 @@ static int scan_images_on(pigo_cascade* c, int dev, const pigo_image* images, in
     return rc_cap == PIGO_OK ? PIGO_OK : set_err(PIGO_E_CAP, "output capacity %d per image too small", cap_per_image);
   }
 
-  WsGuard g(R->pool);
-  Workspace* w = g.w;
-  if (!w) return set_err(PIGO_E_CUDA, "could not create a CUDA stream");
-  cudaStream_t st = stream_ ? (cudaStream_t)stream_ : w->stream;
-  if ((rc = ws_enter(w, st))) return rc;
+  Borrow w(R->pool, stream_);
+  if (w.rc) return w.rc;
+  cudaStream_t st = w.st;
   const int cap = cap_per_image > 0 ? cap_per_image : 1;
 
   // order[j] = caller index of the image at position j of the call's image table; passes are ranges of positions
@@ -675,8 +737,10 @@ static int scan_images_on(pigo_cascade* c, int dev, const pigo_image* images, in
   for (size_t pi = 0; pi < passes.size(); ++pi) {
     const Pass& p = passes[pi];
     uint64_t pass_windows = 0;
-    for (int j = p.first; j < p.first + p.n; ++j) pass_windows += wins[order[j]];
-    sched[pi] = images_schedule(pass_windows, !p.slots.empty());
+    for (int j = p.first; j < p.first + p.n; ++j) pass_windows += ip.wins[order[j]];
+    // (gather-v2 is the whole scan here, as on the rotated path: large unrotated calls keep 24 trees, not run_scan's 16,
+    // since the hand-over point was not re-measured for it)
+    sched[pi] = images_schedule(pass_windows, !p.slots.empty(), 24);
     const int GB = 1 << sched[pi].gb_shift;
     // groups of about equal window counts (a uniform 1080p batch gets the uniform path's groups of 128)
     const uint64_t ngroups = std::max<uint64_t>(1, (pass_windows + kImagesGroupWindows - 1) / kImagesGroupWindows);
@@ -684,13 +748,13 @@ static int scan_images_on(pigo_cascade* c, int dev, const pigo_image* images, in
     const size_t first_group = groups.size();
     for (int j = p.first; j < p.first + p.n; ++j) {
       const int i = order[j];
-      if (groups.size() == first_group || (groups.back().windows > 0 && groups.back().windows + wins[i] > group_target) ||
+      if (groups.size() == first_group || (groups.back().windows > 0 && groups.back().windows + ip.wins[i] > group_target) ||
           (sub > 0 && groups.back().n >= sub))
         groups.push_back(Group{j, 0, 0, 0, (int)pi});
       Group& G = groups.back();
       ImageDesc& d = desc[j];
       d.rows = images[i].rows; d.cols = images[i].cols; d.dim = images[i].dim;
-      d.nscales = (int)plans[i].size();
+      d.nscales = (int)ip.plans[i].size();
       d.plan_off = (uint32_t)plan_all.size();
       d.block_base = G.blocks;
       d.rot_slot = slot[i];
@@ -699,31 +763,23 @@ static int scan_images_on(pigo_cascade* c, int dev, const pigo_image* images, in
         d.rot_off = (uint32_t)((std::find(p.slots.begin(), p.slots.end(), slot[i]) - p.slots.begin()) * (size_t)nlad * R->tab.ntrees);
       d.out_index = i;
       uint32_t nb = 0;
-      for (ScaleEntry e : plans[i]) {
+      for (ScaleEntry e : ip.plans[i]) {
         e.pad = nb;
         nb += (uint32_t)((e.ncols + GB - 1) / GB) * (uint32_t)((e.nrows + GB - 1) / GB);
         plan_all.push_back(e);
       }
       if ((uint64_t)G.blocks + nb > 0xffffffffull) return set_err(PIGO_E_INVALID, "image %d: too many windows", i);
-      G.blocks += nb; G.windows += wins[i]; G.n++;
+      G.blocks += nb; G.windows += ip.wins[i]; G.n++;
     }
   }
 
-  // pixels: device images in place; host images in one 256-byte-aligned arena (each distinct image once), reading only
-  // what the reference may index
+  // pixels: device images in place, host images staged
   if (frames_dev) {
     for (int j = 0; j < nimages; ++j) desc[j].base = images[order[j]].pixels;
   } else {
-    std::vector<size_t> off;
-    std::vector<char> first;
-    const size_t total = arena_layout(images, nimages, off, first);
-    if ((rc = w->frames.reserve(total + 256))) return rc;
-    for (int j = 0; j < nimages; ++j) desc[j].base = (const uint8_t*)w->frames.p + off[order[j]];
-    for (int i = 0; i < nimages; ++i) {
-      if (!first[i] || wins[i] == 0) continue;   // a repeat, or never read
-      const size_t frame_min = (size_t)(images[i].rows - 1) * images[i].dim + images[i].cols;
-      CUDA_TRY(cudaMemcpyAsync((uint8_t*)w->frames.p + off[i], images[i].pixels, frame_min, cudaMemcpyHostToDevice, st));
-    }
+    std::vector<const uint8_t*> pixels;
+    if ((rc = stage_pixels(w, images, nimages, &ip.wins, st, pixels))) return rc;
+    for (int j = 0; j < nimages; ++j) desc[j].base = pixels[order[j]];
   }
 
   // image table + concatenated plan (this call's own buffer: the workspace's cached uniform plan stays as it is)
@@ -736,7 +792,7 @@ static int scan_images_on(pigo_cascade* c, int dev, const pigo_image* images, in
   CUDA_TRY(cudaMemcpyAsync(w->img_tab.p, tab.data(), tab.size(), cudaMemcpyHostToDevice, st));
   const ImageDesc* d_desc = (const ImageDesc*)w->img_tab.p;
   const ScaleEntry* d_plan = (const ScaleEntry*)((const uint8_t*)w->img_tab.p + desc_bytes);
-  const int longest_pos = (int)(std::find(order.begin(), order.end(), longest) - order.begin());
+  const int longest_pos = (int)(std::find(order.begin(), order.end(), ip.longest) - order.begin());
   // the node tables of a pass over the longest ladder, one per slot, cached per workspace by (slots, ladder)
   if (max_tables > 0 && nlad > 0) {
     const size_t cap0 = w->img_rot.cap;
@@ -785,7 +841,7 @@ static int scan_images_on(pigo_cascade* c, int dev, const pigo_image* images, in
       tables_of = G.pass;
     }
     int first_live = G.first;
-    while (wins[order[first_live]] == 0) ++first_live;
+    while (ip.wins[order[first_live]] == 0) ++first_live;
     ScanArgs A{};
     A.tab = R->tab;
     A.frames = desc[first_live].base;   // a readable pixel for the idle lanes of the kernels
@@ -929,37 +985,17 @@ static int check_puploc_seeds(const pigo_point* seeds, int nseeds, const int32_t
   return PIGO_OK;
 }
 
-// Geometry of the images of a RunDetector or pipeline call: every image is refined on, so it needs at least one pixel.
-static int check_image_geometry(const pigo_image* images, int nimages) {
-  for (int i = 0; i < nimages; ++i) {
-    const pigo_image& im = images[i];
-    if (im.rows <= 0 || im.cols <= 0 || im.dim < im.cols)
-      return set_err(PIGO_E_INVALID, "image %d: bad geometry rows=%d cols=%d dim=%d", i, im.rows, im.cols, im.dim);
-    if ((uint64_t)im.rows * (uint64_t)im.dim > 0x7fffffffull) return set_err(PIGO_E_INVALID, "image %d: larger than 2^31 bytes", i);
-    if (!im.pixels) return set_err(PIGO_E_INVALID, "image %d: null pixels", i);
-  }
-  return PIGO_OK;
-}
-
-// Pixels of a mixed-size call on the device.  Device images stay where they are; host images go to one 256-byte-aligned
-// arena in w->frames (arena_layout: a round256(rows*dim) slot per distinct image), of which only the (rows-1)*dim + cols
-// bytes the reference may index are copied.  The call's ImageDesc table (pixels, rows, cols, pitch and, given `angles`,
+// Pixels of a mixed-size call on the device.  Device images stay where they are; host images are staged, every one of
+// them (the RunDetector stages read each image).  The call's ImageDesc table (pixels, rows, cols, pitch and, given `angles`,
 // each image's rotation slot) goes to w->img_tab; `staged` receives the device descriptors of the images.
 static int stage_images(Workspace* w, const pigo_image* images, int nimages, const double* angles, bool frames_dev, cudaStream_t st,
                         const ImageDesc** d_desc, std::vector<pigo_image>& staged) {
   int rc = PIGO_OK;
   staged.assign(images, images + nimages);
   if (!frames_dev) {
-    std::vector<size_t> off;
-    std::vector<char> first;
-    const size_t total = arena_layout(images, nimages, off, first);
-    if ((rc = w->frames.reserve(total + 256))) return rc;
-    for (int i = 0; i < nimages; ++i) {
-      uint8_t* dst = (uint8_t*)w->frames.p + off[i];
-      if (first[i])
-        CUDA_TRY(cudaMemcpyAsync(dst, images[i].pixels, (size_t)(images[i].rows - 1) * images[i].dim + images[i].cols, cudaMemcpyHostToDevice, st));
-      staged[i].pixels = dst;
-    }
+    std::vector<const uint8_t*> pixels;
+    if ((rc = stage_pixels(w, images, nimages, nullptr, st, pixels))) return rc;
+    for (int i = 0; i < nimages; ++i) staged[i].pixels = pixels[i];
   }
   std::vector<ImageDesc> desc(nimages);
   for (int i = 0; i < nimages; ++i) {
@@ -991,18 +1027,16 @@ static int puploc_run_on(pigo_puploc* p, const pigo_point* seeds, int nseeds, co
   PuplocReplica* R = puploc_replica(p, dev, &rc);
   if (!R) return rc;
   const bool frames_dev = flags & PIGO_FRAMES_DEVICE, out_dev = flags & PIGO_OUT_DEVICE;
-  WsGuard g(R->pool);
-  Workspace* w = g.w;
-  if (!w) return set_err(PIGO_E_CUDA, "could not create a CUDA stream");
-  cudaStream_t st = stream_ ? (cudaStream_t)stream_ : w->stream;
-  if ((rc = ws_enter(w, st))) return rc;
+  Borrow w(R->pool, stream_);
+  if (w.rc) return w.rc;
+  cudaStream_t st = w.st;
   const uint8_t* d_pix = px.frames;
   const ImageDesc* d_img = nullptr;
   if (px.images) {
     std::vector<pigo_image> staged;
     if ((rc = stage_images(w, px.images, px.nframes, nullptr, frames_dev, st, &d_img, staged))) return rc;
   } else if (!frames_dev) {
-    const size_t bytes = px.stride * (size_t)(px.nframes - 1) + (size_t)(px.rows - 1) * px.dim + px.cols;   // what the reference may index
+    const size_t bytes = px.stride * (size_t)(px.nframes - 1) + readable_bytes(px.rows, px.cols, px.dim);
     if ((rc = w->frames.reserve(px.stride * (size_t)(px.nframes - 1) + (size_t)px.rows * px.dim))) return rc;
     CUDA_TRY(cudaMemcpyAsync(w->frames.p, px.frames, bytes, cudaMemcpyHostToDevice, st));
     d_pix = (const uint8_t*)w->frames.p;
@@ -1266,29 +1300,48 @@ int pigo_run_cascade(const pigo_cascade* c, const uint8_t* pixels, int rows, int
 
 }  // extern "C"
 
-// pigo_run_cascade_images and pigo_run_cascade_images_angles: image i at angles[i].  `fn` names the entry point in messages.
-static int run_cascade_images(const char* fn, const pigo_cascade* cc, const pigo_image* images, int nimages, const double* angles, int min_size,
-                              int max_size, double shift_factor, double scale_factor, pigo_det* out, int cap_per_image, int* n_out,
+// The entry points whose host work synchronises refuse a caller's stream that is capturing a CUDA graph.
+static int refuse_capture(const char* fn, void* stream_) {
+  if (stream_ && stream_capturing((cudaStream_t)stream_)) return set_err(PIGO_E_INVALID, "%s does not support stream capture", fn);
+  return PIGO_OK;
+}
+
+// `angles`, or when it is nullptr n copies of `angle`, held in `store`.
+static const double* angles_or(const double* angles, double angle, int n, std::vector<double>& store) {
+  if (angles) return angles;
+  store.assign(n, angle);
+  return store.data();
+}
+
+// The start of a mixed-size call after its argument checks: the ladders of its n scan entries (a sweep's expanded list),
+// the default device and the refusal of stream capture (`fn` names the entry point).  With n == 0 nothing more is to do.
+static int images_prologue(const char* fn, const pigo_image* images, int n, int min_size, int max_size, double shift_factor, double scale_factor,
+                           void* stream_, ImagePlans& ip) {
+  int rc = build_image_plans(images, n, min_size, max_size, shift_factor, scale_factor, ip);
+  if (rc) return rc;
+  if ((rc = ensure_device())) return rc;
+  return refuse_capture(fn, stream_);
+}
+
+// pigo_run_cascade_images and pigo_run_cascade_images_angles: image i at angles[i] (nullptr: `angle` for every image).  `fn`
+// names the entry point in messages.
+static int run_cascade_images(const char* fn, const pigo_cascade* cc, const pigo_image* images, int nimages, const double* angles, double angle,
+                              int min_size, int max_size, double shift_factor, double scale_factor, pigo_det* out, int cap_per_image, int* n_out,
                               unsigned flags, void* stream_) {
   int rc = check_images_args(cc, images, nimages, out, cap_per_image, n_out);
   if (rc) return rc;
-  std::vector<std::vector<ScaleEntry>> plans;
-  std::vector<uint64_t> wins;
-  int longest = 0;
-  if ((rc = build_image_plans(images, nimages, min_size, max_size, shift_factor, scale_factor, plans, wins, longest))) return rc;
-  if ((rc = ensure_device())) return rc;
-  if (stream_ && stream_capturing((cudaStream_t)stream_)) return set_err(PIGO_E_INVALID, "%s does not support stream capture", fn);
-  if (nimages == 0) return PIGO_OK;
-  return scan_images_on(const_cast<pigo_cascade*>(cc), default_device(), images, nimages, plans, wins, longest, min_size, max_size,
-                        shift_factor, scale_factor, angles, out, cap_per_image, n_out, flags, stream_);
+  ImagePlans ip;
+  std::vector<double> uniform;
+  if ((rc = images_prologue(fn, images, nimages, min_size, max_size, shift_factor, scale_factor, stream_, ip)) || nimages == 0) return rc;
+  return scan_images_on(const_cast<pigo_cascade*>(cc), default_device(), images, nimages, ip, min_size, max_size, shift_factor, scale_factor,
+                        angles_or(angles, angle, nimages, uniform), out, cap_per_image, n_out, flags, stream_);
 }
 
 extern "C" {
 
 int pigo_run_cascade_images(const pigo_cascade* cc, const pigo_image* images, int nimages, int min_size, int max_size, double shift_factor,
                             double scale_factor, double angle, pigo_det* out, int cap_per_image, int* n_out, unsigned flags, void* stream_) {
-  const std::vector<double> angles(nimages > 0 && nimages <= 65535 ? nimages : 0, angle);   // (other counts are rejected)
-  return run_cascade_images("pigo_run_cascade_images", cc, images, nimages, angles.data(), min_size, max_size, shift_factor, scale_factor,
+  return run_cascade_images("pigo_run_cascade_images", cc, images, nimages, nullptr, angle, min_size, max_size, shift_factor, scale_factor,
                             out, cap_per_image, n_out, flags, stream_);
 }
 
@@ -1296,7 +1349,7 @@ int pigo_run_cascade_images_angles(const pigo_cascade* cc, const pigo_image* ima
                                    int max_size, double shift_factor, double scale_factor, pigo_det* out, int cap_per_image, int* n_out,
                                    unsigned flags, void* stream_) {
   if (nimages > 0 && !angles) return set_err(PIGO_E_INVALID, "null angles");
-  return run_cascade_images("pigo_run_cascade_images_angles", cc, images, nimages, angles, min_size, max_size, shift_factor, scale_factor,
+  return run_cascade_images("pigo_run_cascade_images_angles", cc, images, nimages, angles, 0.0, min_size, max_size, shift_factor, scale_factor,
                             out, cap_per_image, n_out, flags, stream_);
 }
 
@@ -1341,11 +1394,9 @@ static int cluster_batch_on(int dev, pigo_det* dets, const int* n, int nframes, 
   int rc = use_device(dev);
   if (rc) return rc;
   const bool on_dev = (flags & PIGO_OUT_DEVICE) != 0;  // dets, n, out, n_out all on the device
-  WsGuard g(g_misc_pool[dev]);
-  Workspace* w = g.w;
-  if (!w) return set_err(PIGO_E_CUDA, "could not create a CUDA stream");
-  cudaStream_t st = stream_ ? (cudaStream_t)stream_ : w->stream;
-  if ((rc = ws_enter(w, st))) return rc;
+  Borrow w(g_misc_pool[dev], stream_);
+  if (w.rc) return w.rc;
+  cudaStream_t st = w.st;
   const int cap = std::max(cap_per_frame, 1), ocap = std::max(out_cap_per_frame, 1);
   const size_t nd = (size_t)nframes * cap;
   if ((rc = w->scratch_a.reserve(nd * sizeof(pigo_det)))) return rc;
@@ -1470,7 +1521,7 @@ int pigo_puploc_run_images(const pigo_puploc* pc, const pigo_point* seeds, int n
   if (nimages < 1 || nimages > 65535) return set_err(PIGO_E_INVALID, "nimages must be 1..65535");
   if (!images) return set_err(PIGO_E_INVALID, "null images");
   if (nimages > 1 && !seed_image) return set_err(PIGO_E_INVALID, "seed_image is required when nimages > 1");
-  int rc = check_image_geometry(images, nimages);
+  int rc = check_image_geometry(images, nimages, 1, true);
   if (rc) return rc;
   bool wide = false;
   if (!(flags & PIGO_OUT_DEVICE) && (rc = check_puploc_seeds(seeds, nseeds, seed_image, nimages, "image", &wide))) return rc;
@@ -1552,11 +1603,9 @@ static int detect_on(int dev, pigo_cascade* face, pigo_puploc* puploc, pigo_pupl
   const bool out_dev = flags & PIGO_OUT_DEVICE;
   const int det_cap = P.det_cap > 0 ? P.det_cap : 2048;
 
-  WsGuard g(R->pool);
-  Workspace* w = g.w;
-  if (!w) return set_err(PIGO_E_CUDA, "could not create a CUDA stream");
-  cudaStream_t st = stream_ ? (cudaStream_t)stream_ : w->stream;
-  if ((rc = ws_enter(w, st))) return rc;
+  Borrow w(R->pool, stream_);
+  if (w.rc) return w.rc;
+  cudaStream_t st = w.st;
 
   const size_t nslots = (size_t)nframes * face_cap * stride, nscan = (size_t)nframes * nangles;
   // scratch: raw detections + counts, clusters + counts, seeds, points, faces, work counters
@@ -1646,37 +1695,37 @@ static int detect_batch_on(int dev, pigo_cascade* face, pigo_puploc* puploc, pig
     int rc = PIGO_OK;
     W.frames = frames; W.frame_stride = frame_stride; W.nrows = rows; W.ncols = cols; W.dim = dim;
     W.rot_slot = rot_slot_of(P.angle);
-    if (frames_dev)
-      return scan_batch_on(face, dev, frames, nframes, frame_stride, rows, cols, dim, P.min_size, P.max_size, P.shift_factor, P.scale_factor,
-                           P.angle, d_dets, det_cap, d_cnt, PIGO_FRAMES_DEVICE | PIGO_OUT_DEVICE, st);
-    // the scan call streams the host frames into THIS buffer (chunked copy overlapped with the scan kernels); the
-    // pupil / landmark stages gather from it afterwards
-    W.frame_stride = ((size_t)rows * dim + 255) & ~(size_t)255;
-    if ((rc = w->frames.reserve(W.frame_stride * nframes + 256))) return rc;
-    W.frames = (const uint8_t*)w->frames.p;
+    if (!frames_dev) {
+      // the scan call streams the host frames into THIS buffer (chunked copy overlapped with the scan kernels); the
+      // pupil / landmark stages gather from it afterwards
+      W.frame_stride = ((size_t)rows * dim + 255) & ~(size_t)255;
+      if ((rc = w->frames.reserve(W.frame_stride * nframes + 256))) return rc;
+      W.frames = (const uint8_t*)w->frames.p;
+    }
     return scan_batch_on(face, dev, frames, nframes, frame_stride, rows, cols, dim, P.min_size, P.max_size, P.shift_factor, P.scale_factor,
-                         P.angle, d_dets, det_cap, d_cnt, PIGO_OUT_DEVICE, st, (uint8_t*)w->frames.p);
+                         P.angle, d_dets, det_cap, d_cnt, (flags & PIGO_FRAMES_DEVICE) | PIGO_OUT_DEVICE, st,
+                         frames_dev ? nullptr : (uint8_t*)w->frames.p);
   };
   return detect_on(dev, face, puploc, flp, flp_flip, ncalls, nframes, 1, "frame", P, randoms, rng_seed, slot_base, faces, face_cap, n_faces, points,
                    nullptr, flags, stream_, scan, ClusterFrames{dev, nframes, P.iou_threshold, face_cap});
 }
 
 // Mixed-size form: the images' pixels are staged once (stage_images) and both the images scan and the RunDetector stages
-// read them; `plans` / `wins` / `longest` are the call's ladders (build_image_plans).  Image i is scanned and its eyes are
-// refined at angles[i] (P.angle is not used).  slot_base offsets the generator key as in detect_batch_on (a shard that
-// starts at image lo of a larger call passes lo*face_cap*(2+ncalls)).
+// read them; `ip` holds the call's ladders (build_image_plans).  Image i is scanned and its eyes are refined at angles[i]
+// (P.angle is not used).  slot_base offsets the generator key as in detect_batch_on (a shard that starts at image lo of a
+// larger call passes lo*face_cap*(2+ncalls)).
 static int detect_images_on(int dev, pigo_cascade* face, pigo_puploc* puploc, pigo_puploc* const* flp, const uint8_t* flp_flip, int ncalls,
-                            const pigo_image* images, int nimages, const double* angles, const std::vector<std::vector<ScaleEntry>>& plans,
-                            const std::vector<uint64_t>& wins, int longest, const pigo_pipeline_params& P, const float* randoms, uint64_t rng_seed,
-                            uint64_t slot_base, pigo_det* faces, int face_cap, int* n_faces, pigo_point* points, unsigned flags, void* stream_) {
+                            const pigo_image* images, int nimages, const double* angles, const ImagePlans& ip, const pigo_pipeline_params& P,
+                            const float* randoms, uint64_t rng_seed, uint64_t slot_base, pigo_det* faces, int face_cap, int* n_faces,
+                            pigo_point* points, unsigned flags, void* stream_) {
   const bool frames_dev = flags & PIGO_FRAMES_DEVICE;
   auto scan = [&](Workspace* w, cudaStream_t st, pigo_det* d_dets, int det_cap, int32_t* d_cnt, PupWork& W) {
     std::vector<pigo_image> staged;
     int rc = stage_images(w, images, nimages, angles, frames_dev, st, &W.images, staged);
     if (rc) return rc;
     W.rot_slot = kRotSlotPerImage;
-    return scan_images_on(face, dev, staged.data(), nimages, plans, wins, longest, P.min_size, P.max_size, P.shift_factor, P.scale_factor,
-                          angles, d_dets, det_cap, d_cnt, PIGO_FRAMES_DEVICE | PIGO_OUT_DEVICE, st);
+    return scan_images_on(face, dev, staged.data(), nimages, ip, P.min_size, P.max_size, P.shift_factor, P.scale_factor, angles, d_dets,
+                          det_cap, d_cnt, PIGO_FRAMES_DEVICE | PIGO_OUT_DEVICE, st);
   };
   return detect_on(dev, face, puploc, flp, flp_flip, ncalls, nimages, 1, "image", P, randoms, rng_seed, slot_base, faces, face_cap, n_faces, points,
                    nullptr, flags, stream_, scan, ClusterFrames{dev, nimages, P.iou_threshold, face_cap});
@@ -1735,29 +1784,24 @@ static int sweep_raw_cap(const int32_t* cnt, int nimages, int nangles, int det_c
   return PIGO_OK;
 }
 
-static int sweep_scan_on(pigo_cascade* c, int dev, const pigo_image* images, int nimages, const double* angles, int nangles,
-                         const std::vector<std::vector<ScaleEntry>>& plans, const std::vector<uint64_t>& wins, int longest, int min_size, int max_size,
-                         double shift_factor, double scale_factor, double iou, int det_cap, pigo_det* out, int32_t* angle_index, int cap_per_image,
-                         int* n_out, unsigned flags, void* stream_) {
+// ex / ex_angles: the expanded list (sweep_entries), ip: its ladders.
+static int sweep_scan_on(pigo_cascade* c, int dev, const pigo_image* ex, const double* ex_angles, int nimages, const double* angles, int nangles,
+                         const ImagePlans& ip, int min_size, int max_size, double shift_factor, double scale_factor, double iou, int det_cap,
+                         pigo_det* out, int32_t* angle_index, int cap_per_image, int* n_out, unsigned flags, void* stream_) {
   int rc = PIGO_OK;
   FaceReplica* R = face_replica(c, dev, &rc);
   if (!R) return rc;
   if ((rc = use_device(dev))) return rc;
   const bool out_dev = flags & PIGO_OUT_DEVICE;
-  WsGuard g(R->pool);
-  Workspace* w = g.w;
-  if (!w) return set_err(PIGO_E_CUDA, "could not create a CUDA stream");
-  cudaStream_t st = stream_ ? (cudaStream_t)stream_ : w->stream;
-  if ((rc = ws_enter(w, st))) return rc;
+  Borrow w(R->pool, stream_);
+  if (w.rc) return w.rc;
+  cudaStream_t st = w.st;
   const int E = nimages * nangles, ocap = std::max(cap_per_image, 1);
   if ((rc = w->raw.reserve((size_t)E * det_cap * sizeof(pigo_det))) || (rc = w->nout.reserve(((size_t)E + nimages) * 4))) return rc;
   pigo_det* d_raw = (pigo_det*)w->raw.p;
   int32_t* d_cnt = (int32_t*)w->nout.p;
-  std::vector<pigo_image> ex;
-  std::vector<double> ex_angles;
-  sweep_entries(images, nimages, angles, nangles, ex, ex_angles);
-  if ((rc = scan_images_on(c, dev, ex.data(), E, plans, wins, longest, min_size, max_size, shift_factor, scale_factor, ex_angles.data(), d_raw, det_cap,
-                           d_cnt, (flags & PIGO_FRAMES_DEVICE) | PIGO_OUT_DEVICE, st)))
+  if ((rc = scan_images_on(c, dev, ex, E, ip, min_size, max_size, shift_factor, scale_factor, ex_angles, d_raw, det_cap, d_cnt,
+                           (flags & PIGO_FRAMES_DEVICE) | PIGO_OUT_DEVICE, st)))
     return rc;
   pigo_det* d_out = out;
   int32_t* d_nout = n_out;
@@ -1772,21 +1816,11 @@ static int sweep_scan_on(pigo_cascade* c, int dev, const pigo_image* images, int
                         &d_rot)))
     return rc;
   if (out_dev) return ws_leave_async(w, st);
+  // d_cnt holds the E raw-list counts, then (d_nout = d_cnt + E) the clusters': one copy brings both back.  The raw-list
+  // error wins over the cluster-capacity error, whose message this function words itself.
   std::vector<int32_t> cnt((size_t)E + nimages);
-  CUDA_TRY(cudaMemcpyAsync(cnt.data(), d_cnt, cnt.size() * 4, cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaStreamSynchronize(st));
-  size_t max_n = 0;
-  for (int i = 0; i < nimages; ++i) {
-    n_out[i] = cnt[(size_t)E + i];
-    max_n = std::max(max_n, (size_t)std::min(n_out[i], cap_per_image));
-  }
-  if (max_n > 0) {
-    CUDA_TRY(cudaMemcpy2DAsync(out, (size_t)cap_per_image * sizeof(pigo_det), d_out, (size_t)ocap * sizeof(pigo_det), max_n * sizeof(pigo_det),
-                               nimages, cudaMemcpyDeviceToHost, st));
-    if (angle_index)
-      CUDA_TRY(cudaMemcpy2DAsync(angle_index, (size_t)cap_per_image * 4, d_tags, (size_t)ocap * 4, max_n * 4, nimages, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
-  }
+  rc = copy_results_to_host(d_out, d_cnt, ocap, nimages, out, cap_per_image, n_out, st, d_tags, angle_index, E, cnt.data());
+  if (rc != PIGO_OK && rc != PIGO_E_CAP) return rc;
   if ((rc = sweep_raw_cap(cnt.data(), nimages, nangles, det_cap, "det_cap"))) return rc;
   for (int i = 0; i < nimages; ++i)
     if (n_out[i] > cap_per_image) return set_err(PIGO_E_CAP, "image %d has %d clusters, cap_per_image is %d", i, n_out[i], cap_per_image);
@@ -1797,9 +1831,9 @@ static int sweep_scan_on(pigo_cascade* c, int dev, const pigo_image* images, int
 // landmark stages through the call's ImageDesc table.  The eyes of face k of image i are refined at angles[tag], tag being
 // the face's angle index (kRotSlotPerFace); the generator key and randoms layout are pigo_detect_images'.
 static int detect_sweep_on(int dev, pigo_cascade* face, pigo_puploc* puploc, pigo_puploc* const* flp, const uint8_t* flp_flip, int ncalls,
-                           const pigo_image* images, int nimages, const double* angles, int nangles, const std::vector<std::vector<ScaleEntry>>& plans,
-                           const std::vector<uint64_t>& wins, int longest, const pigo_pipeline_params& P, const float* randoms, uint64_t rng_seed,
-                           pigo_det* faces, int face_cap, int* n_faces, pigo_point* points, int32_t* face_angle, unsigned flags, void* stream_) {
+                           const pigo_image* images, int nimages, const double* angles, int nangles, const ImagePlans& ip,
+                           const pigo_pipeline_params& P, const float* randoms, uint64_t rng_seed, pigo_det* faces, int face_cap, int* n_faces,
+                           pigo_point* points, int32_t* face_angle, unsigned flags, void* stream_) {
   const bool frames_dev = flags & PIGO_FRAMES_DEVICE, out_dev = flags & PIGO_OUT_DEVICE;
   auto scan = [&](Workspace* w, cudaStream_t st, pigo_det* d_dets, int det_cap, int32_t* d_cnt, PupWork& W) {
     std::vector<pigo_image> staged, ex;
@@ -1808,8 +1842,8 @@ static int detect_sweep_on(int dev, pigo_cascade* face, pigo_puploc* puploc, pig
     if (rc) return rc;
     W.rot_slot = kRotSlotPerFace;
     sweep_entries(staged.data(), nimages, angles, nangles, ex, ex_angles);
-    return scan_images_on(face, dev, ex.data(), nimages * nangles, plans, wins, longest, P.min_size, P.max_size, P.shift_factor, P.scale_factor,
-                          ex_angles.data(), d_dets, det_cap, d_cnt, PIGO_FRAMES_DEVICE | PIGO_OUT_DEVICE, st);
+    return scan_images_on(face, dev, ex.data(), nimages * nangles, ip, P.min_size, P.max_size, P.shift_factor, P.scale_factor, ex_angles.data(),
+                          d_dets, det_cap, d_cnt, PIGO_FRAMES_DEVICE | PIGO_OUT_DEVICE, st);
   };
   auto cluster = [&](Workspace* w, cudaStream_t st, pigo_det* d_dets, int det_cap, int32_t* d_cnt, pigo_det* d_clusters, int32_t* d_ncl, PupWork& W,
                      int32_t** d_tags) {
@@ -1868,18 +1902,34 @@ static int check_decoded(const pigo_decoded* src, int n) {
   return PIGO_OK;
 }
 
+// The landmark cascade handles flp[0..ncalls) of a pipeline call.
+static int check_landmarks(const pigo_puploc* const* flp, int ncalls) {
+  for (int i = 0; i < ncalls; ++i)
+    if (!flp[i]) return set_err(PIGO_E_INVALID, "null landmark cascade %d", i);
+  return PIGO_OK;
+}
+
+// The pipeline parameters of the pigo_detect_* calls: ncalls, the flp array (and, with `handles`, its entries), face_cap and
+// the Perturbs of prm (not null).
+static int check_pipeline_params(int ncalls, const pigo_puploc* const* flp, bool handles, int face_cap, const pigo_pipeline_params& prm) {
+  if (ncalls < 0 || ncalls > 30) return set_err(PIGO_E_INVALID, "ncalls must be 0..30");
+  if (ncalls > 0 && !flp) return set_err(PIGO_E_INVALID, "null flp");
+  int rc = PIGO_OK;
+  if (handles && (rc = check_landmarks(flp, ncalls))) return rc;
+  if (face_cap < 1 || face_cap > 4096) return set_err(PIGO_E_INVALID, "face_cap must be 1..4096");
+  if (prm.eye_perturbs < 0 || prm.eye_perturbs > 63 || prm.flp_perturbs < 0 || prm.flp_perturbs > 63)
+    return set_err(PIGO_E_INVALID, "Perturbs outside 0..63 (the reference panics, core/puploc.go:261)");
+  return PIGO_OK;
+}
+
 extern "C" {
 
 static int check_detect_args(const pigo_cascade* face, const pigo_puploc* puploc, const pigo_puploc* const* flp, int ncalls, const uint8_t* frames,
                              int nframes, size_t frame_stride, int rows, int cols, int dim, const pigo_pipeline_params* prm,
                              const pigo_det* faces, int face_cap, const int* n_faces, const pigo_point* points) {
   if (!face || !puploc || !prm || !faces || !n_faces || !points || (ncalls > 0 && !flp)) return set_err(PIGO_E_INVALID, "null argument");
-  if (ncalls < 0 || ncalls > 30) return set_err(PIGO_E_INVALID, "ncalls must be 0..30");
-  for (int i = 0; i < ncalls; ++i)
-    if (!flp[i]) return set_err(PIGO_E_INVALID, "null landmark cascade %d", i);
-  if (face_cap < 1 || face_cap > 4096) return set_err(PIGO_E_INVALID, "face_cap must be 1..4096");
-  if (prm->eye_perturbs < 0 || prm->eye_perturbs > 63 || prm->flp_perturbs < 0 || prm->flp_perturbs > 63)
-    return set_err(PIGO_E_INVALID, "Perturbs outside 0..63 (the reference panics, core/puploc.go:261)");
+  const int rc = check_pipeline_params(ncalls, flp, true, face_cap, *prm);
+  if (rc) return rc;
   if (rows <= 0 || cols <= 0) return set_err(PIGO_E_INVALID, "bad geometry");
   return check_batch_args(face, frames, nframes, frame_stride, rows, cols, dim, faces, face_cap, n_faces);
 }
@@ -1922,20 +1972,14 @@ static int check_detect_images_args(const pigo_cascade* face, const pigo_puploc*
   if (!faces) return set_err(PIGO_E_INVALID, "null faces");
   if (!n_faces) return set_err(PIGO_E_INVALID, "null n_faces");
   if (!points) return set_err(PIGO_E_INVALID, "null points");
-  if (ncalls < 0 || ncalls > 30) return set_err(PIGO_E_INVALID, "ncalls must be 0..30");
-  if (ncalls > 0 && !flp) return set_err(PIGO_E_INVALID, "null flp");
-  if (face_cap < 1 || face_cap > 4096) return set_err(PIGO_E_INVALID, "face_cap must be 1..4096");
-  if (prm->eye_perturbs < 0 || prm->eye_perturbs > 63 || prm->flp_perturbs < 0 || prm->flp_perturbs > 63)
-    return set_err(PIGO_E_INVALID, "Perturbs outside 0..63 (the reference panics, core/puploc.go:261)");
+  int rc = check_pipeline_params(ncalls, flp, false, face_cap, *prm);
+  if (rc) return rc;
   if ((uint64_t)nimages * (uint64_t)face_cap * (uint64_t)(2 + ncalls) > 0x7fffffffull)
     return set_err(PIGO_E_INVALID, "nimages*face_cap*(2+ncalls) exceeds 2^31-1 pupil work items");
-  int rc = check_image_geometry(images, nimages);
-  if (rc) return rc;
+  if ((rc = check_image_geometry(images, nimages, 1, true))) return rc;
   if (!face) return set_err(PIGO_E_INVALID, "null cascade");
   if (!puploc) return set_err(PIGO_E_INVALID, "null pupil cascade");
-  for (int i = 0; i < ncalls; ++i)
-    if (!flp[i]) return set_err(PIGO_E_INVALID, "null landmark cascade %d", i);
-  return PIGO_OK;
+  return check_landmarks(flp, ncalls);
 }
 
 // pigo_detect_images and pigo_detect_images_angles: image i at angles[i] (nullptr: prm->angle for every image).  `fn`
@@ -1946,18 +1990,13 @@ static int detect_images(const char* fn, const pigo_cascade* face, const pigo_pu
                          void* stream) {
   int rc = check_detect_images_args(face, puploc, flp, ncalls, images, nimages, prm, faces, face_cap, n_faces, points);
   if (rc) return rc;
-  std::vector<std::vector<ScaleEntry>> plans;
-  std::vector<uint64_t> wins;
-  int longest = 0;
-  if ((rc = build_image_plans(images, nimages, prm->min_size, prm->max_size, prm->shift_factor, prm->scale_factor, plans, wins, longest))) return rc;
-  if ((rc = ensure_device())) return rc;
-  if (stream && stream_capturing((cudaStream_t)stream)) return set_err(PIGO_E_INVALID, "%s does not support stream capture", fn);
-  if (nimages == 0) return PIGO_OK;
+  ImagePlans ip;
   std::vector<double> uniform;
-  if (!angles) { uniform.assign(nimages, prm->angle); angles = uniform.data(); }
+  if ((rc = images_prologue(fn, images, nimages, prm->min_size, prm->max_size, prm->shift_factor, prm->scale_factor, stream, ip)) || nimages == 0)
+    return rc;
   return detect_images_on(default_device(), const_cast<pigo_cascade*>(face), const_cast<pigo_puploc*>(puploc), (pigo_puploc* const*)flp, flp_flip,
-                          ncalls, images, nimages, angles, plans, wins, longest, *prm, randoms, rng_seed, 0, faces, face_cap, n_faces, points, flags,
-                          stream);
+                          ncalls, images, nimages, angles_or(angles, prm->angle, nimages, uniform), ip, *prm, randoms, rng_seed, 0, faces, face_cap,
+                          n_faces, points, flags, stream);
 }
 
 int pigo_detect_images(const pigo_cascade* face, const pigo_puploc* puploc, const pigo_puploc* const* flp, const uint8_t* flp_flip, int ncalls,
@@ -2002,15 +2041,12 @@ int pigo_run_cascade_images_sweep(const pigo_cascade* cc, const pigo_image* imag
   std::vector<pigo_image> ex;
   std::vector<double> ex_angles;
   sweep_entries(images, nimages, angles, nangles, ex, ex_angles);
-  std::vector<std::vector<ScaleEntry>> plans;
-  std::vector<uint64_t> wins;
-  int longest = 0;
-  if ((rc = build_image_plans(ex.data(), (int)ex.size(), min_size, max_size, shift_factor, scale_factor, plans, wins, longest))) return rc;
-  if ((rc = ensure_device())) return rc;
-  if (stream_ && stream_capturing((cudaStream_t)stream_)) return set_err(PIGO_E_INVALID, "pigo_run_cascade_images_sweep does not support stream capture");
-  if (nimages == 0) return PIGO_OK;
-  return sweep_scan_on(const_cast<pigo_cascade*>(cc), default_device(), images, nimages, angles, nangles, plans, wins, longest, min_size, max_size,
-                       shift_factor, scale_factor, iou_threshold, dcap, out, angle_index, cap_per_image, n_out, flags, stream_);
+  ImagePlans ip;
+  if ((rc = images_prologue("pigo_run_cascade_images_sweep", ex.data(), (int)ex.size(), min_size, max_size, shift_factor, scale_factor, stream_,
+                            ip)) || nimages == 0)
+    return rc;
+  return sweep_scan_on(const_cast<pigo_cascade*>(cc), default_device(), ex.data(), ex_angles.data(), nimages, angles, nangles, ip, min_size,
+                       max_size, shift_factor, scale_factor, iou_threshold, dcap, out, angle_index, cap_per_image, n_out, flags, stream_);
 }
 
 int pigo_detect_images_sweep(const pigo_cascade* face, const pigo_puploc* puploc, const pigo_puploc* const* flp, const uint8_t* flp_flip, int ncalls,
@@ -2024,17 +2060,13 @@ int pigo_detect_images_sweep(const pigo_cascade* face, const pigo_puploc* puploc
   std::vector<pigo_image> ex;
   std::vector<double> ex_angles;
   sweep_entries(images, nimages, angles, nangles, ex, ex_angles);
-  std::vector<std::vector<ScaleEntry>> plans;
-  std::vector<uint64_t> wins;
-  int longest = 0;
-  if ((rc = build_image_plans(ex.data(), (int)ex.size(), prm->min_size, prm->max_size, prm->shift_factor, prm->scale_factor, plans, wins, longest)))
+  ImagePlans ip;
+  if ((rc = images_prologue("pigo_detect_images_sweep", ex.data(), (int)ex.size(), prm->min_size, prm->max_size, prm->shift_factor,
+                            prm->scale_factor, stream, ip)) || nimages == 0)
     return rc;
-  if ((rc = ensure_device())) return rc;
-  if (stream && stream_capturing((cudaStream_t)stream)) return set_err(PIGO_E_INVALID, "pigo_detect_images_sweep does not support stream capture");
-  if (nimages == 0) return PIGO_OK;
   return detect_sweep_on(default_device(), const_cast<pigo_cascade*>(face), const_cast<pigo_puploc*>(puploc), (pigo_puploc* const*)flp, flp_flip,
-                         ncalls, images, nimages, angles, nangles, plans, wins, longest, *prm, randoms, rng_seed, faces, face_cap, n_faces, points,
-                         face_angle, flags, stream);
+                         ncalls, images, nimages, angles, nangles, ip, *prm, randoms, rng_seed, faces, face_cap, n_faces, points, face_angle,
+                         flags, stream);
 }
 
 // ---- RgbToGrayscale, core/grayscale.go:8-23 ----------------------------------------------------------------
@@ -2044,11 +2076,9 @@ int pigo_rgba_to_gray(const uint8_t* rgba, size_t npixels, uint8_t* gray, unsign
   int rc = ensure_device();
   if (rc) return rc;
   const int dev = default_device();
-  WsGuard g(g_misc_pool[dev]);
-  Workspace* w = g.w;
-  if (!w) return set_err(PIGO_E_CUDA, "could not create a CUDA stream");
-  cudaStream_t st = stream_ ? (cudaStream_t)stream_ : w->stream;
-  if ((rc = ws_enter(w, st))) return rc;   // a device-output call returns while the kernel still reads the staging buffer
+  Borrow w(g_misc_pool[dev], stream_);   // a device-output call returns while the kernel still reads the staging buffer
+  if (w.rc) return w.rc;
+  cudaStream_t st = w.st;
   const bool in_dev = flags & PIGO_FRAMES_DEVICE, out_dev = flags & PIGO_OUT_DEVICE;
   const uint8_t* d_in = rgba;
   uint8_t* d_out = gray;
@@ -2087,11 +2117,9 @@ int pigo_ycbcr_to_nrgba(const uint8_t* y, const uint8_t* cb, const uint8_t* cr, 
   int rc = ensure_device();
   if (rc) return rc;
   const int dev = default_device();
-  WsGuard g(g_misc_pool[dev]);
-  Workspace* w = g.w;
-  if (!w) return set_err(PIGO_E_CUDA, "could not create a CUDA stream");
-  cudaStream_t st = stream_ ? (cudaStream_t)stream_ : w->stream;
-  if ((rc = ws_enter(w, st))) return rc;
+  Borrow w(g_misc_pool[dev], stream_);
+  if (w.rc) return w.rc;
+  cudaStream_t st = w.st;
   const bool in_dev = flags & PIGO_FRAMES_DEVICE, out_dev = flags & PIGO_OUT_DEVICE;
   const uint8_t *d_y = y, *d_cb = cb, *d_cr = cr;
   if (!in_dev) {
@@ -2133,11 +2161,9 @@ static int gray_images_on(int dev, const pigo_decoded* src, int n, const std::ve
                           unsigned flags, void* stream_) {
   int rc = use_device(dev);
   if (rc) return rc;
-  WsGuard g(g_misc_pool[dev]);
-  Workspace* w = g.w;
-  if (!w) return set_err(PIGO_E_CUDA, "could not create a CUDA stream");
-  cudaStream_t st = stream_ ? (cudaStream_t)stream_ : w->stream;
-  if ((rc = ws_enter(w, st))) return rc;
+  Borrow w(g_misc_pool[dev], stream_);
+  if (w.rc) return w.rc;
+  cudaStream_t st = w.st;
   const bool in_dev = flags & PIGO_FRAMES_DEVICE;
 
   // the distinct sources, the ones gray_images_kernel<false> converts first (nnarrow of them); host planes go to one
@@ -2227,7 +2253,7 @@ int pigo_gray_images(const pigo_decoded* src, int n, uint8_t* gray, size_t* gray
   }
   if (n == 0) return PIGO_OK;
   if ((rc = ensure_device())) return rc;
-  if (stream_ && stream_capturing((cudaStream_t)stream_)) return set_err(PIGO_E_INVALID, "pigo_gray_images does not support stream capture");
+  if ((rc = refuse_capture("pigo_gray_images", stream_))) return rc;
   for (int i = 0; i < n; ++i) images[i] = pigo_image{gray + off[i], src[i].height, src[i].width, src[i].width};
   return gray_images_on(default_device(), src, n, off, first, gray, flags, stream_);
 }
@@ -2244,108 +2270,75 @@ static std::vector<pigo_image> decoded_geometry(const pigo_decoded* src, int n) 
   return v;
 }
 
-// The ladders of entries [lo, lo+n) of a call (a shard plans and schedules its own entries).
-struct ShardPlans {
-  std::vector<std::vector<ScaleEntry>> plans;
-  std::vector<uint64_t> wins;
-  int longest = 0;
-};
-static int shard_plans(const pigo_image* images, int n, int min_size, int max_size, double shift, double scale_factor, ShardPlans& sp) {
-  return build_image_plans(images, n, min_size, max_size, shift, scale_factor, sp.plans, sp.wins, sp.longest);
-}
-
-// Converts a shard's decoded sources into the gray arena of workspace `wa` on device dev, on wa's stream, and fills
-// images[0..n) with the device images (the layout pigo_gray_images gives the same sources).
-static int gray_shard(int dev, Workspace* wa, const pigo_decoded* src, int n, std::vector<pigo_image>& images) {
-  std::vector<size_t> off;
-  std::vector<char> first;
-  const size_t total = arena_layout(src, n, off, first);
-  int rc = wa->gray_arena.reserve(total + 256);
-  if (rc) return rc;
-  uint8_t* gray = (uint8_t*)wa->gray_arena.p;
-  images.resize(n);
-  for (int i = 0; i < n; ++i) images[i] = pigo_image{gray + off[i], src[i].height, src[i].width, src[i].width};
-  return gray_images_on(dev, src, n, off, first, gray, PIGO_MEM_HOST, wa->stream);
-}
-
-// Runs fn(device, workspace holding the shard's gray arena, device images) for a decoded shard.  Everything of the shard
-// is ordered on the workspace's stream: the copies and conversion, then the scan or pipeline that reads the arena.
+// Runs fn(device images, stream) for a decoded shard on device dev.  The sources are converted into the gray arena of a
+// borrowed workspace (the layout pigo_gray_images gives them), and everything of the shard is ordered on the workspace's
+// own stream: the copies and conversion, then the scan or pipeline that reads the arena.
 template <typename F>
 static int with_gray_shard(int dev, const pigo_decoded* src, int n, F fn) {
   int rc = use_device(dev);
   if (rc) return rc;
-  WsGuard ga(g_misc_pool[dev]);
-  Workspace* wa = ga.w;
-  if (!wa) return set_err(PIGO_E_CUDA, "could not create a CUDA stream");
-  if ((rc = ws_enter(wa, wa->stream))) return rc;   // behind the last asynchronous user of this workspace
-  std::vector<pigo_image> images;
-  if ((rc = gray_shard(dev, wa, src, n, images))) return rc;
-  return fn(wa, images);
+  Borrow w(g_misc_pool[dev], nullptr);
+  if (w.rc) return w.rc;
+  std::vector<size_t> off;
+  std::vector<char> first;
+  const size_t total = arena_layout(src, n, off, first);
+  if ((rc = w->gray_arena.reserve(total + 256))) return rc;
+  uint8_t* gray = (uint8_t*)w->gray_arena.p;
+  std::vector<pigo_image> images(n);
+  for (int i = 0; i < n; ++i) images[i] = pigo_image{gray + off[i], src[i].height, src[i].width, src[i].width};
+  if ((rc = gray_images_on(dev, src, n, off, first, gray, PIGO_MEM_HOST, w.st))) return rc;
+  return fn(images.data(), (void*)w.st);
+}
+
+// A sharded mixed-size call over `images` (host pixels, or with src the geometry of the decoded sources) at angles[]
+// (nullptr: `angle` for every image): the call's ladders, its split over the devices, and for the shard of entries
+// [lo, lo+n) on device dev fn(dev, images, n, lo, angles, ladders, flags, stream) over the shard's host images, or over
+// the device images of its converted sources on the stream that converted them.
+template <typename F>
+static int run_sharded(const pigo_image* images, const pigo_decoded* src, int nimages, const double* angles, double angle, int min_size,
+                       int max_size, double shift_factor, double scale_factor, F fn) {
+  ImagePlans ip;
+  int rc = build_image_plans(images, nimages, min_size, max_size, shift_factor, scale_factor, ip);
+  if (rc) return rc;
+  if (nimages == 0) return ensure_device();
+  std::vector<double> uniform;
+  angles = angles_or(angles, angle, nimages, uniform);
+  const std::vector<int> devs = sharded_devices();
+  if (devs.empty()) return PIGO_E_NODEVICE;   // message set by pigo_init
+  const std::vector<int> first = plan_shards(ip.wins, angles, shard_count((int)devs.size()));
+  return for_each_shard(devs, first, [&](int, int dev, int lo, int n) {
+    const ImagePlans sp = ip.slice(lo, n);
+    if (!src) return fn(dev, images + lo, n, lo, angles + lo, sp, PIGO_MEM_HOST, nullptr);
+    return with_gray_shard(dev, src + lo, n, [&](const pigo_image* dimg, void* st) {
+      return fn(dev, dimg, n, lo, angles + lo, sp, PIGO_FRAMES_DEVICE, st);
+    });
+  });
 }
 
 static int run_cascade_sharded(const pigo_cascade* cc, const pigo_image* images, const pigo_decoded* src, int nimages, const double* angles,
                                int min_size, int max_size, double shift_factor, double scale_factor, pigo_det* out, int cap_per_image, int* n_out) {
-  // images: the call's images (host pixels), or (src != nullptr) the geometry of the decoded sources
-  std::vector<std::vector<ScaleEntry>> plans;
-  std::vector<uint64_t> wins;
-  int longest = 0;
-  int rc = build_image_plans(images, nimages, min_size, max_size, shift_factor, scale_factor, plans, wins, longest);
-  if (rc) return rc;
-  if (nimages == 0) return ensure_device();
-  const std::vector<double> zeros(angles ? 0 : nimages, 0.0);
-  if (!angles) angles = zeros.data();
-  const std::vector<int> devs = sharded_devices();
-  if (devs.empty()) return PIGO_E_NODEVICE;   // message set by pigo_init
-  const std::vector<int> first = plan_shards(wins, angles, shard_count((int)devs.size()));
   pigo_cascade* c = const_cast<pigo_cascade*>(cc);
-  return for_each_shard(devs, first, [&](int, int dev, int lo, int n) {
-    ShardPlans sp;
-    int rc = shard_plans(images + lo, n, min_size, max_size, shift_factor, scale_factor, sp);
-    if (rc) return rc;
-    pigo_det* o = out ? out + (size_t)lo * cap_per_image : nullptr;
-    if (!src)
-      return scan_images_on(c, dev, images + lo, n, sp.plans, sp.wins, sp.longest, min_size, max_size, shift_factor, scale_factor, angles + lo, o,
-                            cap_per_image, n_out + lo, PIGO_MEM_HOST, nullptr);
-    return with_gray_shard(dev, src + lo, n, [&](Workspace* wa, const std::vector<pigo_image>& dimg) {
-      return scan_images_on(c, dev, dimg.data(), n, sp.plans, sp.wins, sp.longest, min_size, max_size, shift_factor, scale_factor, angles + lo, o,
-                            cap_per_image, n_out + lo, PIGO_FRAMES_DEVICE, wa->stream);
-    });
-  });
+  return run_sharded(images, src, nimages, angles, 0.0, min_size, max_size, shift_factor, scale_factor,
+                     [&](int dev, const pigo_image* im, int n, int lo, const double* a, const ImagePlans& sp, unsigned flags, void* st) {
+                       return scan_images_on(c, dev, im, n, sp, min_size, max_size, shift_factor, scale_factor, a,
+                                             out ? out + (size_t)lo * cap_per_image : nullptr, cap_per_image, n_out + lo, flags, st);
+                     });
 }
 
 static int detect_sharded(const pigo_cascade* face, const pigo_puploc* puploc, const pigo_puploc* const* flp, const uint8_t* flp_flip, int ncalls,
                           const pigo_image* images, const pigo_decoded* src, int nimages, const double* angles, const pigo_pipeline_params* prm,
                           const float* randoms, uint64_t rng_seed, pigo_det* faces, int face_cap, int* n_faces, pigo_point* points) {
-  std::vector<std::vector<ScaleEntry>> plans;
-  std::vector<uint64_t> wins;
-  int longest = 0;
-  int rc = build_image_plans(images, nimages, prm->min_size, prm->max_size, prm->shift_factor, prm->scale_factor, plans, wins, longest);
-  if (rc) return rc;
-  if (nimages == 0) return ensure_device();
-  const std::vector<double> uniform(angles ? 0 : nimages, prm->angle);
-  if (!angles) angles = uniform.data();
-  const std::vector<int> devs = sharded_devices();
-  if (devs.empty()) return PIGO_E_NODEVICE;
-  const std::vector<int> first = plan_shards(wins, angles, shard_count((int)devs.size()));
   const size_t per_image = (size_t)face_cap * (2 + ncalls);
   pigo_cascade* fc = const_cast<pigo_cascade*>(face);
   pigo_puploc* pc = const_cast<pigo_puploc*>(puploc);
-  return for_each_shard(devs, first, [&](int, int dev, int lo, int n) {
-    ShardPlans sp;
-    int rc = shard_plans(images + lo, n, prm->min_size, prm->max_size, prm->shift_factor, prm->scale_factor, sp);
-    if (rc) return rc;
-    // the shard's generator keys and injected randoms are those of images lo.. in the whole call
-    const float* rnd = randoms ? randoms + (size_t)lo * per_image * 189 : nullptr;
-    pigo_det* f = faces + (size_t)lo * face_cap;
-    pigo_point* p = points + (size_t)lo * per_image;
-    if (!src)
-      return detect_images_on(dev, fc, pc, (pigo_puploc* const*)flp, flp_flip, ncalls, images + lo, n, angles + lo, sp.plans, sp.wins, sp.longest,
-                              *prm, rnd, rng_seed, (uint64_t)lo * per_image, f, face_cap, n_faces + lo, p, PIGO_MEM_HOST, nullptr);
-    return with_gray_shard(dev, src + lo, n, [&](Workspace* wa, const std::vector<pigo_image>& dimg) {
-      return detect_images_on(dev, fc, pc, (pigo_puploc* const*)flp, flp_flip, ncalls, dimg.data(), n, angles + lo, sp.plans, sp.wins, sp.longest,
-                              *prm, rnd, rng_seed, (uint64_t)lo * per_image, f, face_cap, n_faces + lo, p, PIGO_FRAMES_DEVICE, wa->stream);
-    });
-  });
+  return run_sharded(images, src, nimages, angles, prm->angle, prm->min_size, prm->max_size, prm->shift_factor, prm->scale_factor,
+                     [&](int dev, const pigo_image* im, int n, int lo, const double* a, const ImagePlans& sp, unsigned flags, void* st) {
+                       // the shard's generator keys and injected randoms are those of images lo.. in the whole call
+                       const float* rnd = randoms ? randoms + (size_t)lo * per_image * 189 : nullptr;
+                       return detect_images_on(dev, fc, pc, (pigo_puploc* const*)flp, flp_flip, ncalls, im, n, a, sp, *prm, rnd, rng_seed,
+                                               (uint64_t)lo * per_image, faces + (size_t)lo * face_cap, face_cap, n_faces + lo,
+                                               points + (size_t)lo * per_image, flags, st);
+                     });
 }
 
 // Arguments of the decoded forms: what pigo_gray_images checks, before the checks of the matching mixed-size call.
@@ -2398,18 +2391,12 @@ int pigo_shard_plan(const pigo_image* images, int nimages, const double* angles,
   if (nimages > 0 && !images) return set_err(PIGO_E_INVALID, "null images");
   if (!n_used) return set_err(PIGO_E_INVALID, "null n_used");
   if (nshards < 0) return set_err(PIGO_E_INVALID, "negative nshards");
-  for (int i = 0; i < nimages; ++i) {
-    const pigo_image& im = images[i];
-    if (im.rows < 0 || im.cols < 0 || im.dim < im.cols)
-      return set_err(PIGO_E_INVALID, "image %d: bad geometry rows=%d cols=%d dim=%d", i, im.rows, im.cols, im.dim);
-  }
-  std::vector<std::vector<ScaleEntry>> plans;
-  std::vector<uint64_t> wins;
-  int longest = 0;
-  int rc = build_image_plans(images, nimages, min_size, max_size, shift_factor, scale_factor, plans, wins, longest);
+  int rc = check_image_geometry(images, nimages, 0, false);
   if (rc) return rc;
+  ImagePlans ip;
+  if ((rc = build_image_plans(images, nimages, min_size, max_size, shift_factor, scale_factor, ip))) return rc;
   if (nshards == 0) nshards = shard_count(std::max(1, (int)shard_devices().size()));
-  const std::vector<int> cut = plan_shards(wins, angles, nshards);
+  const std::vector<int> cut = plan_shards(ip.wins, angles, nshards);
   *n_used = (int)cut.size() - 1;
   if (first) std::copy(cut.begin(), cut.end(), first);
   return PIGO_OK;

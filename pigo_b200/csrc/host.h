@@ -401,13 +401,15 @@ int build_block_tables(const FaceTables& tab, const std::vector<int8_t>& codes, 
                        const std::vector<float>& thr, DevBuf& out);
 int describe_plan(const std::vector<ScaleEntry>& plan, uint64_t wins, int ntrees, int batch_frames, char* buf, size_t cap);
 int run_scan(FaceReplica* c, Workspace* w, int lane, ScanArgs& A, unsigned long long* d_work, cudaStream_t st, int num_sms);
+// Whether a scan of cascade c runs on the block/deep kernels rather than the universal gather kernel (scan_driver.cu).
+bool block_path(const FaceReplica* c, bool rot, int max_scale, size_t rot_bytes);
 struct ImagesSchedule {
   int gb_shift;       // log2 of the gather block edge in windows
   int gather_limit;   // trees a window walks in the gather-v2 kernel before it goes to the deep kernel
   int deep_group;     // lanes per window in the deep kernel
   bool deep_ordered;  // the deep kernel takes its queue in image order (launch_deep_sort)
 };
-ImagesSchedule images_schedule(uint64_t call_windows, bool rot);
+ImagesSchedule images_schedule(uint64_t call_windows, bool rot, int large_limit);
 int run_scan_images(FaceReplica* c, Workspace* w, ScanArgs& A, const ImagesSchedule& P, uint32_t group_blocks, uint64_t group_windows,
                     int max_rows, int max_cols, unsigned long long* d_work, cudaStream_t st, int num_sms);
 FaceReplica* face_replica(pigo_cascade* c, int dev, int* rc);

@@ -363,6 +363,31 @@ static int sort_deep_queue(Workspace* w, int lane, ScanArgs& D, int rows, int co
   return PIGO_OK;
 }
 
+// The block/deep kernels need a depth-6 cascade with its tiled table and scan_mode != 1.  A rotated scan on them also needs
+// rot_mode 0, windows of at most 32000 pixels and a node table (one RotNode per ladder entry, tree and node) of at most 512 MB.
+bool block_path(const FaceReplica* c, bool rot, int max_scale, size_t rot_bytes) {
+  if (c->tab.depth != 6 || c->tiled_tab.p == nullptr || g_opt.scan_mode.load() == 1) return false;
+  return !rot || (g_opt.rot_mode.load() == 0 && max_scale <= 32000 && rot_bytes <= ((size_t)1 << 29));
+}
+
+// The choices a scan makes from the window count of its whole API call.  "Small call" = at most 4 M windows (a 1080p frame
+// has 0.9 M, a 4K frame 3.7 M): latency matters, not throughput.  Small calls cannot fill the GPU with 256-window gather
+// blocks (they use 64-window blocks) and give a window 32 deep lanes (the latency of a full survivor matters).  A gather
+// window hands over to the deep kernel after 8 trees in a small rotated call or an unrotated one of up to 40 M windows,
+// else after 24 trees (rotated) or `large_limit` (unrotated: run_scan and the mixed-size scan each give theirs).
+ImagesSchedule images_schedule(uint64_t call_windows, bool rot, int large_limit) {
+  ImagesSchedule P;
+  const bool small = call_windows <= 4000000ull;
+  long long glimit = g_opt.gather_limit.load();
+  if (glimit <= 0) glimit = rot ? (small ? 8 : 24) : (call_windows <= 40000000ull ? 8 : large_limit);
+  P.gather_limit = (int)std::min<long long>(glimit, 1 << 20);
+  P.gb_shift = (g_opt.gather_block.load() == 8 || (g_opt.gather_block.load() == 0 && small)) ? 3 : 4;
+  P.deep_group = (int)g_opt.deep_group.load();
+  if (P.deep_group != 8 && P.deep_group != 16 && P.deep_group != 32) P.deep_group = small ? 32 : 8;
+  P.deep_ordered = deep_ordered(call_windows);
+  return P;
+}
+
 int run_scan(FaceReplica* c, Workspace* w, int lane, ScanArgs& A, unsigned long long* d_work, cudaStream_t st, int num_sms) {
   int rc;
   const bool rot = A.rot_slot >= 0;
@@ -373,13 +398,10 @@ int run_scan(FaceReplica* c, Workspace* w, int lane, ScanArgs& A, unsigned long 
   A.chunk = (uint32_t)std::max<long long>(32, g_opt.chunk.load());
   A.chunk_counter = d_work + 4;
 
-  // Rotated scan on the block/deep structure: needs the per-call node table (one RotNode per ladder entry, tree, node).
+  // Rotated scan on the block/deep structure: needs the per-call node table.
   const size_t rot_bytes = (size_t)A.nscales * (size_t)A.tab.ntrees * 64 * sizeof(RotNode);
   const int max_scale = w->plan_host.empty() ? 0 : w->plan_host.back().s;
-  const bool rot_fast = rot && A.tab.depth == 6 && c->tiled_tab.p != nullptr && mode != 1 && g_opt.rot_mode.load() == 0 &&
-                        max_scale <= 32000 && rot_bytes <= ((size_t)1 << 29);
-  const bool fast = (!rot || rot_fast) && A.tab.depth == 6 && c->tiled_tab.p != nullptr && mode != 1;
-  if (!fast) {
+  if (!block_path(c, rot, max_scale, rot_bytes)) {
     // ---- universal path: standalone gather kernel over every scale (any tree depth, scan_mode=1, rot_mode=1)
     ScanArgs G = A;
     G.scale_lo = 0; G.scale_hi = A.nscales;
@@ -393,7 +415,7 @@ int run_scan(FaceReplica* c, Workspace* w, int lane, ScanArgs& A, unsigned long 
     g_launches++;
     return check_launch("gather scan");
   }
-  if (rot_fast) {
+  if (rot) {
     if (w->rot_slot != A.rot_slot || w->rot_tab.p == nullptr) {
       if ((rc = w->rot_tab.reserve(rot_bytes))) return rc;
       timing_begin(T_ROTTAB, st);
@@ -428,17 +450,13 @@ int run_scan(FaceReplica* c, Workspace* w, int lane, ScanArgs& A, unsigned long 
   // how long a gather-role window stays in the fused kernel before it leaves for the deep kernel (which walks a window with a
   // lane group and is the cheaper place for long walks): calls of up to 40 M windows hand over after 8 trees, larger ones after
   // 16.  (H100, 256 x 1080p: 8 and 16 trees took 0.7 and 0.6 ms off the 24 used before; but 8 made the 64-frame ShiftFactor 0.1
-  // batch 2 % slower than the previous build, and 16 did not.)
-  long long glimit = g_opt.gather_limit.load();
+  // batch 2 % slower than the previous build, and 16 did not.)  The rotated scan has no fused kernel: its block kernel keeps
+  // 24 trees unless the call is small.  All of it is decided from the frames of the whole API call, not of this pipeline
+  // group: the block prefix lives in the shared plan.
   const unsigned long long call_windows = (unsigned long long)A.wins_per_frame * (unsigned long long)std::max(1, A.batch_frames);
-  // "small call" = at most 4 M windows in the whole API call (a 1080p frame has 0.9 M, a 4K frame 3.7 M): latency matters, not throughput
-  const bool small_call = call_windows <= 4000000ull;
-  // (the rotated scan has no fused kernel: its block kernel keeps 24 trees unless the call is small)
-  if (glimit <= 0) glimit = rot ? (small_call ? 8 : 24) : (call_windows <= 40000000ull ? 8 : 16);
-  T.gather_limit = (int)std::min<long long>(glimit, 1 << 20);
-  // small batches (a frame or two) cannot fill the GPU with 256-window blocks: use 64-window blocks then
-  // (decided from the frames of the whole API call, not of this pipeline group: the block prefix lives in the shared plan)
-  T.gb_shift = (g_opt.gather_block.load() == 8 || (g_opt.gather_block.load() == 0 && small_call)) ? 3 : 4;
+  const ImagesSchedule S = images_schedule(call_windows, rot, 16);
+  T.gather_limit = S.gather_limit;
+  T.gb_shift = S.gb_shift;
 
   // ---- fused kernel: tile warps over the small scales (+ optional gather warps over the rest)
   auto round_ks = [&](long long v) {
@@ -556,11 +574,9 @@ int run_scan(FaceReplica* c, Workspace* w, int lane, ScanArgs& A, unsigned long 
       launch_deep_smem(A, d_work + 2, (const uint8_t*)c->tiled_tab.p, num_sms, threads, group, (int)std::min<long long>(std::max<long long>(0, g_opt.deep_smem_lo.load()), 1 << 20),
                        (int)std::min<long long>(std::max<long long>(2, g_opt.deep_smem_k.load()), 1 << 20), st);
     } else {
-      if (group != 8 && group != 16 && group != 32) group = small_call ? 32 : 8;   // small call: the latency of a full survivor matters
       ScanArgs D = A;
-      const bool ordered = deep_ordered(call_windows);
-      if (ordered && (rc = sort_deep_queue(w, lane, D, A.rows, A.cols, q2_cap, num_sms, st))) return rc;
-      launch_deep(D, d_work + 2, num_sms, group, ordered, st);
+      if (S.deep_ordered && (rc = sort_deep_queue(w, lane, D, A.rows, A.cols, q2_cap, num_sms, st))) return rc;
+      launch_deep(D, d_work + 2, num_sms, S.deep_group, S.deep_ordered, st);
     }
     timing_end(T_DEEP, st);
     g_launches++;
@@ -570,21 +586,6 @@ int run_scan(FaceReplica* c, Workspace* w, int lane, ScanArgs& A, unsigned long 
 }
 
 // ---- mixed-size calls (pigo_run_cascade_images) ------------------------------------------------------------------------
-// The per-call choices run_scan makes from the call's window count, made from the total over all images.
-ImagesSchedule images_schedule(uint64_t call_windows, bool rot) {
-  ImagesSchedule P;
-  const bool small_call = call_windows <= 4000000ull;
-  long long glimit = g_opt.gather_limit.load();
-  // (not run_scan's rule: here gather-v2 is the whole scan, as on the rotated path, and the hand-over point was not re-measured)
-  if (glimit <= 0) glimit = (rot ? small_call : call_windows <= 40000000ull) ? 8 : 24;
-  P.gather_limit = (int)std::min<long long>(glimit, 1 << 20);
-  P.gb_shift = (g_opt.gather_block.load() == 8 || (g_opt.gather_block.load() == 0 && small_call)) ? 3 : 4;
-  P.deep_group = (int)g_opt.deep_group.load();
-  if (P.deep_group != 8 && P.deep_group != 16 && P.deep_group != 32) P.deep_group = small_call ? 32 : 8;
-  P.deep_ordered = deep_ordered(call_windows);
-  return P;
-}
-
 // One group of images: the gather-v2 kernel over every ladder entry of every image (in blocks of 16x16 or 8x8 windows,
 // located through the image table), then the deep kernel over its survivors -- the kernel pair scan_mode=3 runs for a
 // uniform batch.  The caller has set A.images / A.plan (block prefixes built for P.gb_shift) and, rotated, A.rot_tab.

@@ -202,13 +202,11 @@ def detect_images_sweep_device(clf: Pigo, plc: PuplocCascade, flpcs: Dict[str, P
     randoms: optional [N][face_cap][17][63][3] float32.  Returns List[List[(Face, angle)]] with `angle` the listed value
     (raw=True: the (faces, n_faces, points, face_angle) arrays, face_angle indexing `angles`)."""
     import ctypes as C
-    from . import DET_DTYPE, POINT_DTYPE, FRAMES_DEVICE, MEM_HOST, PipelineParams, _check, _pixels, image_descs, lib
+    from . import DET_DTYPE, POINT_DTYPE, PipelineParams, _check, _image_table, lib
     hs, fl = landmark_call_arrays(flpcs)
     ncalls = len(fl)
     n = len(images)
-    on_dev = n > 0 and all(isinstance(im.Pixels, int) for im in images)
-    keep = [None if on_dev else _pixels(im) for im in images]   # host pixels stay alive for the call
-    desc = image_descs([(im.Pixels if on_dev else p.ctypes.data, im.Rows, im.Cols, im.Dim) for im, p in zip(images, keep)])
+    desc, flags, keep = _image_table(images)
     ang = np.ascontiguousarray(angles, dtype=np.float64)
     prm = PipelineParams(cp.MinSize, cp.MaxSize, cp.ShiftFactor, cp.ScaleFactor, 0.0, iou, min_face, eye_perturbs, flp_perturbs, det_cap)
     rnd = None
@@ -221,7 +219,7 @@ def detect_images_sweep_device(clf: Pigo, plc: PuplocCascade, flpcs: Dict[str, P
     face_angle = np.full((n, face_cap), -1, dtype=np.int32)
     _check(lib().pigo_detect_images_sweep(clf._h, plc._h, hs, fl.ctypes.data, ncalls, desc, n, ang.ctypes.data, len(ang), C.byref(prm),
                                           rnd.ctypes.data if rnd is not None else None, rng_seed, faces.ctypes.data, face_angle.ctypes.data,
-                                          face_cap, nfaces.ctypes.data, points.ctypes.data, FRAMES_DEVICE if on_dev else MEM_HOST, None))
+                                          face_cap, nfaces.ctypes.data, points.ctypes.data, flags, None))
     if raw:
         return faces, nfaces[:n], points, face_angle
     return [[(fc, float(ang[face_angle[i, k]])) for k, fc in enumerate(row)] for i, row in enumerate(_faces_of(faces, nfaces, points, min_face))]
@@ -256,19 +254,17 @@ def detect_images_sharded(clf: Pigo, plc: PuplocCascade, flpcs: Dict[str, Puploc
 def _detect_images(clf, plc, flpcs, images, cp, iou, min_face, eye_perturbs, flp_perturbs, face_cap, angle, angles, randoms, rng_seed, det_cap,
                    raw, sharded=False, sources=None):
     import ctypes as C
-    from . import DET_DTYPE, POINT_DTYPE, FRAMES_DEVICE, MEM_HOST, PipelineParams, _check, _pixels, image_descs, lib
+    from . import DET_DTYPE, POINT_DTYPE, FRAMES_DEVICE, MEM_HOST, PipelineParams, _check, _image_table, lib
     from . import decoded_descs
     hs, fl = landmark_call_arrays(flpcs)
     ncalls = len(fl)
     if sources is not None:   # decoded sources (host planes): converted on the devices by the call
         n = len(sources)
         desc = decoded_descs(sources)
-        on_dev = False
+        flags = MEM_HOST
     else:
         n = len(images)
-        on_dev = n > 0 and all(isinstance(im.Pixels, int) for im in images)
-        keep = [None if on_dev else _pixels(im) for im in images]   # host pixels stay alive for the call
-        desc = image_descs([(im.Pixels if on_dev else p.ctypes.data, im.Rows, im.Cols, im.Dim) for im, p in zip(images, keep)])
+        desc, flags, keep = _image_table(images)
     prm = PipelineParams(cp.MinSize, cp.MaxSize, cp.ShiftFactor, cp.ScaleFactor, angle, iou, min_face, eye_perturbs, flp_perturbs, det_cap)
     rnd = None
     if randoms is not None:
@@ -277,10 +273,9 @@ def _detect_images(clf, plc, flpcs, images, cp, iou, min_face, eye_perturbs, flp
     faces = np.zeros((n, face_cap), dtype=DET_DTYPE)
     nfaces = np.zeros(max(n, 1), dtype=np.int32)
     points = np.zeros((n, face_cap, 2 + ncalls), dtype=POINT_DTYPE)
-    flags = FRAMES_DEVICE if on_dev else MEM_HOST
     rptr = rnd.ctypes.data if rnd is not None else None
     if sharded:
-        if on_dev:
+        if flags == FRAMES_DEVICE:
             raise ValueError("the sharded calls take host images")
         ang = np.ascontiguousarray(angles, dtype=np.float64) if angles is not None else None
         fn = lib().pigo_detect_decoded_sharded if sources is not None else lib().pigo_detect_images_sharded
