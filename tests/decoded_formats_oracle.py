@@ -6,10 +6,6 @@ numpy here.  decoded_gray extends decoded_oracle.decoded_gray, which it calls fo
 from __future__ import annotations
 
 import ctypes as C
-import hashlib
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 
@@ -18,24 +14,13 @@ import oracle_lib as O
 
 GRAY16, RGBA64, NRGBA64, CMYK, PALETTED = 5, 6, 7, 8, 9
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SRC = os.path.join(_HERE, "decoded_formats_oracle.c")
 _LIB = None
 
 
 def lib() -> C.CDLL:
-    """Compiles decoded_formats_oracle.c like oracle/Makefile compiles the main oracle (-ffp-contract=off), outside the tree."""
     global _LIB
     if _LIB is None:
-        with open(_SRC, "rb") as f:
-            tag = hashlib.sha256(f.read()).hexdigest()[:16]
-        so = os.path.join(tempfile.gettempdir(), f"pigo_decoded_formats_oracle_{os.getuid()}_{tag}.so")
-        if not os.path.exists(so):
-            tmp = f"{so}.{os.getpid()}"
-            subprocess.check_call([os.environ.get("CC", "gcc"), "-O2", "-fPIC", "-std=c11", "-Wall", "-Wextra", "-ffp-contract=off", "-shared",
-                                   "-o", tmp, _SRC])
-            os.replace(tmp, so)
-        L = C.CDLL(so)
+        L = decoded_oracle.compile_c("decoded_formats_oracle")
         for name in ("oracle_gray16_to_nrgba", "oracle_cmyk_to_nrgba"):
             getattr(L, name).argtypes = [C.c_void_p, C.c_int64, C.c_void_p]
             getattr(L, name).restype = None

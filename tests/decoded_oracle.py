@@ -15,23 +15,28 @@ import numpy as np
 import oracle_lib as O
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-_SRC = os.path.join(_HERE, "decoded_oracle.c")
 _LIB = None
 
 
+def compile_c(name: str) -> C.CDLL:
+    """Compiles tests/<name>.c like oracle/Makefile compiles the main oracle (-ffp-contract=off), into the temporary directory,
+    once per version of the source, and loads it."""
+    src = os.path.join(_HERE, name + ".c")
+    with open(src, "rb") as f:
+        tag = hashlib.sha256(f.read()).hexdigest()[:16]
+    so = os.path.join(tempfile.gettempdir(), f"pigo_{name}_{os.getuid()}_{tag}.so")
+    if not os.path.exists(so):
+        tmp = f"{so}.{os.getpid()}"
+        subprocess.check_call([os.environ.get("CC", "gcc"), "-O2", "-fPIC", "-std=c11", "-Wall", "-Wextra", "-ffp-contract=off", "-shared",
+                               "-o", tmp, src])
+        os.replace(tmp, so)
+    return C.CDLL(so)
+
+
 def lib() -> C.CDLL:
-    """Compiles decoded_oracle.c like oracle/Makefile compiles the main oracle (-ffp-contract=off), outside the tree."""
     global _LIB
     if _LIB is None:
-        with open(_SRC, "rb") as f:
-            tag = hashlib.sha256(f.read()).hexdigest()[:16]
-        so = os.path.join(tempfile.gettempdir(), f"pigo_decoded_oracle_{os.getuid()}_{tag}.so")
-        if not os.path.exists(so):
-            tmp = f"{so}.{os.getpid()}"
-            subprocess.check_call([os.environ.get("CC", "gcc"), "-O2", "-fPIC", "-std=c11", "-Wall", "-Wextra", "-ffp-contract=off", "-shared",
-                                   "-o", tmp, _SRC])
-            os.replace(tmp, so)
-        L = C.CDLL(so)
+        L = compile_c("decoded_oracle")
         L.oracle_rgba_to_nrgba.argtypes = [C.c_void_p, C.c_int64, C.c_void_p]
         L.oracle_rgba_to_nrgba.restype = None
         _LIB = L

@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 
 import pigo_b200
+from abi_cases import calls, go_source, header_protos
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -87,53 +88,16 @@ def test_options_round_trip_and_unknown_names():
     assert pigo_b200.get_option("t_tiled_n") == 0
 
 
-def _split_top_level(argtext: str):
-    args, depth, cur = [], 0, ""
-    for ch in argtext:
-        if ch in "([{":
-            depth += 1
-        elif ch in ")]}":
-            depth -= 1
-        if ch == "," and depth == 0:
-            args.append(cur)
-            cur = ""
-        else:
-            cur += ch
-    if cur.strip():
-        args.append(cur)
-    return args
-
-
-def _calls(text: str, prefix: str):
-    """(name, number of top-level arguments) of every `<prefix>pigo_xxx(...)` call / prototype in text."""
-    out = []
-    for m in re.finditer(re.escape(prefix) + r"(pigo_[a-z_]+)\s*\(", text):
-        i, depth = m.end(), 1
-        while depth and i < len(text):
-            depth += text[i] == "("
-            depth -= text[i] == ")"
-            i += 1
-        body = text[m.end():i - 1].strip()
-        out.append((m.group(1), 0 if body in ("", "void") else len(_split_top_level(body))))
-    return out
-
-
 def test_go_shim_calls_match_the_header():
     """go/pigo/pigo.go cannot be compiled here (no Go toolchain): at least every C function it calls must be declared in
     include/pigo_b200.h with the same number of arguments, so the shim cannot silently drift from the ABI."""
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    header = open(os.path.join(root, "include", "pigo_b200.h")).read()
-    header = re.sub(r"/\*.*?\*/", "", header, flags=re.S)
-    protos = dict(_calls(header, ""))
-    import glob
-    go = "\n".join(open(f).read() for f in sorted(glob.glob(os.path.join(root, "go", "pigo", "*.go"))))
-    go = re.sub(r"//[^\n]*", "", go)
-    calls = _calls(go, "C.")
-    assert len(calls) >= 16
+    protos, go = header_protos(), go_source()
+    bound = calls(go, "C.")
+    assert len(bound) >= 16
     for needed in ("pigo_rgba_to_gray", "pigo_ycbcr_to_nrgba", "pigo_detect_batch", "pigo_detect_batch_sharded", "pigo_run_cascade_batch_sharded",
                    "pigo_init_devices"):
-        assert needed in dict(calls), f"the Go shim does not bind {needed}"
-    for name, nargs in calls:
+        assert needed in dict(bound), f"the Go shim does not bind {needed}"
+    for name, nargs in bound:
         assert name in protos, f"{name} is not declared in pigo_b200.h"
         assert nargs == protos[name], f"{name}: Go passes {nargs} arguments, the header declares {protos[name]}"
 

@@ -4,29 +4,24 @@ byte for byte, and the C oracle up to 1080p.  Rotated angles go only on images w
 rotated column clamp (Rows-1, core/pigo.go:168,:171) indexes past the image, where the reference itself would too."""
 import ctypes as C
 import math
-import os
-import subprocess
 import threading
 
 import numpy as np
 import pytest
 
-import oracle_lib as O
 import pigo_b200
-from pigo_b200 import CascadeParams, ImageParams, pipeline, synth
+import pipeline_oracle as P
+from mixed_images import (CLI_PARAMS, DOC_PARAMS, KNOBS, MIXED, NCALLS, TEST_PARAMS, assert_slices, canonical, cascades, cp_of, image_of,  # noqa: F401 (fixtures)
+                          images, lone_scan, make_image, randoms_for, run_cpp_mirror, same)
+from pigo_b200 import ImageParams, pipeline, synth
 from option_guard import options, options_at_defaults   # noqa: F401 (autouse: every test ends with the options at their defaults)
-from test_images_gpu import CLI_PARAMS, DOC_PARAMS, KNOBS, MIXED, TEST_PARAMS, assert_slices, cp_of, lone, make_image
+from synthetic import synthetic_cascade
 
 pytestmark = pytest.mark.gpu
 
 ANGLES = [0.0, -0.1, math.nan, 1 / 64, 1 / 32, 7 / 32, 0.25, 0.5, 31 / 32, 1.0, 1.3, math.inf]
 UNROTATED = [0.0, -0.1, math.nan]
 SWEEP = [0.0] + [k / 32 for k in range(1, 33)]
-
-
-def canonical(a):
-    """The angle the reference scans at (core/pigo.go:232-238): <= 0 and NaN unrotated, > 1 clamped to 1."""
-    return 0.0 if not a > 0 else min(a, 1.0)
 
 
 def draw_angles(images, seed):
@@ -61,7 +56,7 @@ def run(face, images, angles, params=TEST_PARAMS, cap=1024):
 @pytest.mark.parametrize("params", [TEST_PARAMS, CLI_PARAMS, DOC_PARAMS])
 def test_each_image_equals_a_lone_call_at_its_angle(gpu_face, oracle_face, mixed, mixed_angles, params):
     dets, cnt = run(gpu_face, mixed, mixed_angles, params)
-    expect = [lone(gpu_face, im, params, a) for im, a in zip(mixed, mixed_angles)]
+    expect = [lone_scan(gpu_face, im, params, a) for im, a in zip(mixed, mixed_angles)]
     assert_slices(dets, cnt, expect)
     assert sum(len(e) for e, a in zip(expect, mixed_angles) if a > 0) > 0
     for i, (im, a) in enumerate(zip(mixed, mixed_angles)):
@@ -73,7 +68,7 @@ def test_each_image_equals_a_lone_call_at_its_angle(gpu_face, oracle_face, mixed
 def test_sweep_equals_lone_calls_in_either_listing(gpu_face, sweep):
     base, ims, angles = sweep
     d0, c0 = run(gpu_face, ims, angles)
-    assert_slices(d0, c0, [lone(gpu_face, im, TEST_PARAMS, a) for im, a in zip(ims, angles)])
+    assert_slices(d0, c0, [lone_scan(gpu_face, im, TEST_PARAMS, a) for im, a in zip(ims, angles)])
     # angle-major: position p lists image p % 4 at angle p // 4, i.e. the image-major entry (p % 4) * 33 + p // 4
     nb, na = len(base), len(SWEEP)
     perm = [(p % nb) * na + p // nb for p in range(nb * na)]
@@ -99,7 +94,7 @@ def test_repeated_host_descriptors_device_and_stream_forms_agree(gpu_face, sweep
     ims = [im for im in base for _ in angles]
     ang = [a for _ in base for a in angles]
     hd, hc = run(gpu_face, ims, ang)
-    assert_slices(hd, hc, [lone(gpu_face, im, TEST_PARAMS, a) for im, a in zip(ims, ang)])
+    assert_slices(hd, hc, [lone_scan(gpu_face, im, TEST_PARAMS, a) for im, a in zip(ims, ang)])
     bufs = [torch.from_numpy(np.ascontiguousarray(im.Pixels).reshape(-1)[:im.Rows * im.Dim].copy()).cuda() for im in base]
     dev = [(b.data_ptr(), im.Rows, im.Cols, im.Dim) for b, im in zip(bufs, base) for _ in angles]
     dd, dc = run(gpu_face, [ImageParams(p, r, c, d) for p, r, c, d in dev], ang)
@@ -129,11 +124,10 @@ def test_options_leave_the_outputs_unchanged(gpu_face, mixed, mixed_angles, knob
 
 
 def test_cascade_of_another_depth_takes_the_single_image_path(mixed, mixed_angles):
-    from test_oracle_pins import _synthetic_cascade
-    face = pigo_b200.NewPigo().Unpack(_synthetic_cascade(4, 9, seed=409))
+    face = pigo_b200.NewPigo().Unpack(synthetic_cascade(4, 9, seed=409))
     some, angles = mixed[:12], mixed_angles[:12]
     dets, cnt = run(face, some, angles)
-    assert_slices(dets, cnt, [lone(face, im, TEST_PARAMS, a) for im, a in zip(some, angles)])
+    assert_slices(dets, cnt, [lone_scan(face, im, TEST_PARAMS, a) for im, a in zip(some, angles)])
     assert cnt.sum() > 0
 
 
@@ -149,7 +143,7 @@ def test_tables_past_the_bound_run_in_passes(gpu_face):
         d, c = run(gpu_face, lst, ang, params)
         builds = pigo_b200.get_option("t_rottab_n")
     assert builds == 2, builds
-    assert_slices(d, c, [lone(gpu_face, im, params, a) for im, a in zip(lst, ang)])
+    assert_slices(d, c, [lone_scan(gpu_face, im, params, a) for im, a in zip(lst, ang)])
     assert c.sum() > 0
 
 
@@ -194,9 +188,9 @@ def test_a_sweep_leaves_the_single_image_cache_alone(gpu_face, oracle_face, swee
     base, ims, angles = sweep
     found = 0
     for im, a in ((base[1], 0.6), (base[2], 0.05), (base[0], 1 / 32), (base[0], 2 / 32)):
-        before = lone(gpu_face, im, TEST_PARAMS, a)
+        before = lone_scan(gpu_face, im, TEST_PARAMS, a)
         run(gpu_face, ims, angles)
-        after = lone(gpu_face, im, TEST_PARAMS, a)
+        after = lone_scan(gpu_face, im, TEST_PARAMS, a)
         o = oracle_face.run_cascade(im.Pixels, im.Rows, im.Cols, im.Dim, *TEST_PARAMS, a)
         assert before.tobytes() == after.tobytes() == o.tobytes()
         found += len(o)
@@ -204,24 +198,6 @@ def test_a_sweep_leaves_the_single_image_cache_alone(gpu_face, oracle_face, swee
 
 
 # ---- pipeline ----------------------------------------------------------------------------------------------------------
-from test_detect_images_gpu import GEOMS, NCALLS, make_image as make_pipeline_image, randoms_for   # noqa: E402
-
-
-@pytest.fixture(scope="module")
-def cascades():
-    plc = pigo_b200.NewPuplocCascade().UnpackCascade(pigo_b200.load_cascade("puploc"))
-    names = sorted(set(pipeline.EYE_CASCADES + pipeline.MOUTH_CASCADES))
-    flp = {n: pigo_b200.NewPuplocCascade().UnpackCascade(pigo_b200.load_cascade("lps/" + n)) for n in names}
-    oplc = O.OraclePuploc(pigo_b200.load_cascade("puploc"))
-    oflp = {n: O.OraclePuploc(pigo_b200.load_cascade("lps/" + n)) for n in names}
-    return plc, flp, oplc, oflp
-
-
-@pytest.fixture(scope="module")
-def images():
-    return [make_pipeline_image(r, c, d, k, 21 + i) for i, (r, c, d, k) in enumerate(GEOMS)]
-
-
 @pytest.fixture(scope="module")
 def image_angles(images):
     """Small tilts as well as large ones, so that rotated eye refinement runs on faces the rotated scan still finds."""
@@ -234,10 +210,6 @@ def face_cap(gpu_face, cascades, images, image_angles):
     plc, flp, _, _ = cascades
     _, n, _ = pipeline.detect_images_angles_device(gpu_face, plc, flp, images, cp_of(TEST_PARAMS), image_angles, face_cap=256, raw=True)
     return int(max(n.max(), 1))
-
-
-def same(a, b):
-    return all(x.tobytes() == y.tobytes() for x, y in zip(a, b))
 
 
 @pytest.mark.parametrize("stage", [1, 2])
@@ -268,35 +240,16 @@ def test_pipeline_equal_angles_equal_detect_images_with_the_library_generator(gp
 
 def test_pipeline_replays_on_the_oracle(gpu_face, oracle_face, cascades):
     """Step by step on the C oracle, each image at its own angle: two rotated wide images and one unrotated image."""
-    plc, flp, oplc, oflp = cascades
-    ims = [make_pipeline_image(540, 960, 960, "F", 51), make_pipeline_image(300, 900, 912, "F", 52), ImageParams(synth.sample_gray(), 400, 320, 320)]
+    plc, flp, _, _ = cascades
+    ims = [make_image(540, 960, 960, "F", 51), make_image(300, 900, 912, "F", 52), ImageParams(synth.sample_gray(), 400, 320, 320)]
     angles = [0.03, 0.05, 0.0]
     eye = 50
     rnd = randoms_for(len(ims), 8, 43)
     faces, nfaces, points = pipeline.detect_images_angles_device(gpu_face, plc, flp, ims, cp_of(TEST_PARAMS), angles, face_cap=8, randoms=rnd,
                                                                  eye_perturbs=eye, raw=True)
-    calls = pipeline.landmark_calls()
-    refined = 0
-    for i, (im, a) in enumerate(zip(ims, angles)):
-        px, r, c, d = im.Pixels, im.Rows, im.Cols, im.Dim
-        _, cl = O.cluster(oracle_face.run_cascade(px, r, c, d, *TEST_PARAMS, a), 0.1)
-        assert int(nfaces[i]) == len(cl) and faces[i, :len(cl)].tobytes() == cl.tobytes(), i
-        for k, f in enumerate(cl):
-            pts = points[i, k]
-            if f["scale"] <= 50:
-                continue
-            refined += a > 0
-            ls, rs = pipeline.eye_seeds(int(f["row"]), int(f["col"]), int(f["scale"]), eye)
-            le = oplc.run_detector(ls.Row, ls.Col, ls.Scale, eye, rnd[i, k, 0], px, r, c, d, a)
-            re_ = oplc.run_detector(rs.Row, rs.Col, rs.Scale, eye, rnd[i, k, 1], px, r, c, d, a)
-            for p, e in ((pts[0], le), (pts[1], re_)):
-                assert (int(p["row"]), int(p["col"]), np.float32(p["scale"])) == (e[0], e[1], np.float32(e[2])), (i, k)
-            r0, c0, s0 = O.landmark_seed(le[0], le[1], re_[0], re_[1])
-            for ci, (name, flip) in enumerate(calls):
-                e = oflp[name].run_detector(r0, c0, float(s0), 63, rnd[i, k, 2 + ci], px, r, c, d, 0.0, flip)
-                p = pts[2 + ci]
-                assert (int(p["row"]), int(p["col"]), np.float32(p["scale"])) == (e[0], e[1], np.float32(e[2])), (i, k, ci)
-    assert refined >= 1
+    cases = [(i, image_of(im), P.oracle_clusters(oracle_face, image_of(im), TEST_PARAMS, a), a) for i, (im, a) in enumerate(zip(ims, angles))]
+    _, rotated = P.replay(cascades[2:], cases, lambda i, k, slot: rnd[i, k, slot], eye, (faces, nfaces, points))
+    assert rotated >= 1
 
 
 def test_pipeline_capacity_errors_report_the_required_counts(gpu_face, cascades, images, image_angles, face_cap):
@@ -325,8 +278,4 @@ def test_pipeline_capacity_errors_report_the_required_counts(gpu_face, cascades,
 def test_cpp_mirror_sample_in_a_sweep():
     """tests/cpp/test_detect_images_angles.cpp (built by build()): the sample at angles 0, 0.1 and 0.5 through
     DetectImagesAngles; its angle-0 entry passes the reference's landmark assertions."""
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    exe = os.path.join(root, "tests", "cpp", "test_detect_images_angles")
-    assert os.path.exists(exe), "run __graft_entry__.build() first"
-    p = subprocess.run([exe, root], capture_output=True, text=True, timeout=300)
-    assert p.returncode == 0, p.stdout + p.stderr
+    run_cpp_mirror("test_detect_images_angles")

@@ -2,8 +2,6 @@
 pigo_puploc_run_images.  Bar: every image's slices equal a lone pigo_detect_batch(nframes=1) on that image byte for byte
 with the same randoms, and up to 1080p the C oracle replays the sequence step by step."""
 import ctypes as C
-import os
-import subprocess
 import threading
 
 import numpy as np
@@ -11,51 +9,13 @@ import pytest
 
 import oracle_lib as O
 import pigo_b200
+import pipeline_oracle as P
+from mixed_images import (CLI_PARAMS, EYE, GEOMS, NCALLS, TEST_PARAMS, assert_same_outputs, cascades, cp_of, image_of, images,  # noqa: F401 (fixtures)
+                          lone_detect_batch, make_image, randoms_for, run_cpp_mirror)
 from pigo_b200 import CascadeParams, ImageParams, Puploc, pipeline, synth
 from option_guard import options, options_at_defaults   # noqa: F401 (autouse: every test ends with the options at their defaults)
 
 pytestmark = pytest.mark.gpu
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-TEST_PARAMS = (20, 1000, 0.2, 1.1)   # core/pigo_test.go:44-50 (eye Perturbs 50, core/flploc_test.go:107)
-CLI_PARAMS = (20, 1000, 0.15, 1.15)  # cmd/pigo/main.go:110-111 (eye Perturbs 63)
-EYE = {TEST_PARAMS: 50, CLI_PARAMS: 63}
-NCALLS = 15
-
-# (rows, cols, dim, content class): no windows (10x10, 21 rows), the sample, face frames of several sizes with dim > cols,
-# 1080p, one 4K frame, tall and wide shapes, noise and smooth content
-GEOMS = [(10, 10, 10, "U"), (21, 300, 300, "U"), (400, 320, 320, "sample"), (540, 960, 960, "F"), (480, 640, 656, "F"),
-         (333, 517, 531, "F"), (1080, 1920, 1920, "F"), (2160, 3840, 3840, "F"), (700, 260, 272, "F"), (300, 900, 912, "F"),
-         (600, 800, 800, "F"), (45, 1200, 1216, "U"), (360, 640, 640, "S"), (272, 480, 496, "F"), (1000, 700, 701, "F"),
-         (200, 200, 200, "F"), (900, 41, 48, "U"), (50, 60, 64, "S"), (768, 1024, 1024, "U"), (301, 299, 301, "F")]
-
-
-def make_image(rows, cols, dim, cls, seed) -> ImageParams:
-    if cls == "sample":
-        return ImageParams(synth.sample_gray(), rows, cols, dim)
-    buf = np.full((rows, dim), 0xA5, dtype=np.uint8)   # the bytes past Cols are never read
-    if cls == "U":
-        buf[:, :cols] = synth.frame_noise(rows, cols, seed)
-    elif cls == "S":
-        buf[:, :cols] = synth.frame_smooth(rows, cols, seed)
-    else:
-        buf[:, :cols] = synth.frame_faces(None, rows, cols, shift=((37 * seed) % 400, (53 * seed) % 320), noise_seed=seed)
-    return ImageParams(buf, rows, cols, dim)
-
-
-@pytest.fixture(scope="module")
-def images():
-    return [make_image(r, c, d, k, 21 + i) for i, (r, c, d, k) in enumerate(GEOMS)]
-
-
-@pytest.fixture(scope="module")
-def cascades():
-    plc = pigo_b200.NewPuplocCascade().UnpackCascade(pigo_b200.load_cascade("puploc"))
-    names = sorted(set(pipeline.EYE_CASCADES + pipeline.MOUTH_CASCADES))
-    flp = {n: pigo_b200.NewPuplocCascade().UnpackCascade(pigo_b200.load_cascade("lps/" + n)) for n in names}
-    oplc = O.OraclePuploc(pigo_b200.load_cascade("puploc"))
-    oflp = {n: O.OraclePuploc(pigo_b200.load_cascade("lps/" + n)) for n in names}
-    return plc, flp, oplc, oflp
 
 
 @pytest.fixture(scope="module")
@@ -65,62 +25,6 @@ def face_cap(gpu_face, cascades, images):
     _, n, _ = pipeline.detect_images_device(gpu_face, plc, flp, images, cp_of(CLI_PARAMS), face_cap=256, raw=True)
     _, n2, _ = pipeline.detect_images_device(gpu_face, plc, flp, images, cp_of(TEST_PARAMS), face_cap=256, raw=True)
     return int(max(n.max(), n2.max(), 1))
-
-
-def cp_of(params):
-    return CascadeParams(ImageParams(), *params)
-
-
-def randoms_for(n, face_cap, seed):
-    return np.random.default_rng(seed).random((n, face_cap, 2 + NCALLS, 63, 3), dtype=np.float32)
-
-
-def lone(gpu_face, cascades, im, params, face_cap, randoms, angle, eye):
-    plc, flp, _, _ = cascades
-    frame = np.ascontiguousarray(im.Pixels).reshape(1, im.Rows, im.Dim)
-    cp = CascadeParams(ImageParams(None, im.Rows, im.Cols, im.Dim), *params)
-    return pipeline.detect_batch_device(gpu_face, plc, flp, frame, cp, face_cap=face_cap, randoms=randoms, angle=angle, eye_perturbs=eye, raw=True)
-
-
-def assert_same_outputs(a, b, idx_a=None, idx_b=None):
-    fa, na, pa = a
-    fb, nb, pb = b
-    ia = range(len(na)) if idx_a is None else idx_a
-    ib = range(len(nb)) if idx_b is None else idx_b
-    for i, j in zip(ia, ib):
-        assert int(na[i]) == int(nb[j]), (i, j)
-        assert fa[i].tobytes() == fb[j].tobytes(), f"faces of image {i} differ"
-        assert pa[i].tobytes() == pb[j].tobytes(), f"points of image {i} differ"
-
-
-def replay_on_oracle(got, images, params, angle, randoms, eye, oracle_face, cascades):
-    """Step by step on the C oracle: RunCascade -> ClusterDetections -> eye seeds -> RunDetector x2 -> landmark seeds ->
-    15 x RunDetector, each image with its own rows, cols and dim (images up to 1080p)."""
-    _, _, oplc, oflp = cascades
-    faces, nfaces, points = got
-    calls = pipeline.landmark_calls()
-    for i, im in enumerate(images):
-        if im.Rows * im.Cols > 1080 * 1920:
-            continue
-        px, r, c, d = im.Pixels, im.Rows, im.Cols, im.Dim
-        _, cl = O.cluster(oracle_face.run_cascade(px, r, c, d, *params, angle), 0.1)
-        assert int(nfaces[i]) == len(cl), i
-        assert faces[i, :len(cl)].tobytes() == cl.tobytes(), i
-        for k, f in enumerate(cl):
-            pts = points[i, k]
-            if f["scale"] <= 50:
-                assert not pts.tobytes().strip(b"\0"), (i, k)
-                continue
-            ls, rs = pipeline.eye_seeds(int(f["row"]), int(f["col"]), int(f["scale"]), eye)
-            le = oplc.run_detector(ls.Row, ls.Col, ls.Scale, eye, randoms[i, k, 0], px, r, c, d, angle)
-            re_ = oplc.run_detector(rs.Row, rs.Col, rs.Scale, eye, randoms[i, k, 1], px, r, c, d, angle)
-            for p, e in ((pts[0], le), (pts[1], re_)):
-                assert (int(p["row"]), int(p["col"]), np.float32(p["scale"])) == (e[0], e[1], np.float32(e[2])), (i, k)
-            r0, c0, s0 = O.landmark_seed(le[0], le[1], re_[0], re_[1])
-            for ci, (name, flip) in enumerate(calls):
-                e = oflp[name].run_detector(r0, c0, float(s0), 63, randoms[i, k, 2 + ci], px, r, c, d, 0.0, flip)
-                p = pts[2 + ci]
-                assert (int(p["row"]), int(p["col"]), np.float32(p["scale"])) == (e[0], e[1], np.float32(e[2])), (i, k, ci)
 
 
 @pytest.mark.parametrize("stage", [1, 2])
@@ -134,12 +38,15 @@ def test_each_image_equals_a_lone_detect_batch(gpu_face, oracle_face, cascades, 
         got = pipeline.detect_images_device(gpu_face, plc, flp, images, cp_of(params), face_cap=face_cap, randoms=rnd, angle=angle,
                                             eye_perturbs=eye, raw=True)
         for i, im in enumerate(images):
-            assert_same_outputs(got, lone(gpu_face, cascades, im, params, face_cap, rnd[i:i + 1], angle, eye), [i], [0])
+            assert_same_outputs(got, lone_detect_batch(gpu_face, cascades, im, params, face_cap, rnd[i:i + 1], angle, eye), [i], [0])
     faces, nfaces, _ = got
     refined = {GEOMS[i][:3] for i in range(len(images)) if (faces[i, :nfaces[i]]["scale"] > 50).any()}
     assert len(refined) >= 3, refined
     if stage == 2 and params == TEST_PARAMS:
-        replay_on_oracle(got, images, params, angle, rnd, eye, oracle_face, cascades)
+        # step by step on the C oracle, each image with its own rows, cols and dim (images up to 1080p)
+        cases = [(i, image_of(im), P.oracle_clusters(oracle_face, image_of(im), params, angle), angle)
+                 for i, im in enumerate(images) if im.Rows * im.Cols <= 1080 * 1920]
+        P.replay(cascades[2:], cases, lambda i, k, slot: rnd[i, k, slot], eye, got)
 
 
 def test_one_geometry_with_the_library_generator_equals_detect_batch(gpu_face, cascades):
@@ -293,7 +200,4 @@ def _puploc_run_images_matches_the_oracle():
 def test_cpp_mirror_detect_images():
     """tests/cpp/test_detect_images.cpp (built by build()): the reference's landmark assertions on the sample placed among
     other images, through DetectImages of include/pigo_b200.hpp, and its PIGO_E_CAP retry."""
-    exe = os.path.join(ROOT, "tests", "cpp", "test_detect_images")
-    assert os.path.exists(exe), "run __graft_entry__.build() first"
-    p = subprocess.run([exe, ROOT], capture_output=True, text=True, timeout=300)
-    assert p.returncode == 0, p.stdout + p.stderr
+    run_cpp_mirror("test_detect_images")

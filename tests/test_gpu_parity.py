@@ -7,7 +7,10 @@ import pytest
 import oracle_lib as O
 import pigo_b200
 from pigo_b200 import CascadeParams, ImageParams, Puploc, synth
+import pipeline_oracle as P
+from mixed_images import cascades, run_cpp_mirror   # noqa: F401 (fixture)
 from option_guard import options, options_at_defaults   # noqa: F401 (autouse: every test ends with the options at their defaults)
+from synthetic import synthetic_cascade
 
 pytestmark = pytest.mark.gpu
 
@@ -236,8 +239,7 @@ def test_get_landmark_point_vs_oracle(sample_gray):
     le, re_ = Puploc(186, 118, 0, 0), Puploc(188, 205, 0, 0)
     for fl in (False, True):
         p = flp.GetLandmarkPoint(le, re_, img, 63, fl, randoms=rnd)
-        r0, c0, s0 = O.landmark_seed(le.Row, le.Col, re_.Row, re_.Col)
-        e = ora.run_detector(r0, c0, float(s0), 63, rnd, sample_gray, 400, 320, 320, 0.0, fl)
+        e = P.oracle_landmark(ora, (le.Row, le.Col), (re_.Row, re_.Col), rnd, (sample_gray, 400, 320, 320), fl)
         assert (p.Row, p.Col) == (e[0], e[1]) and np.float32(p.Scale) == e[2]
 
 
@@ -335,56 +337,28 @@ def test_scan_variants_agree_with_oracle(gpu_face, oracle_face, sample_gray, var
 
 def test_cpp_mirror_replays_reference_test():
     """include/pigo_b200.hpp (C++ mirror of the Go API) -> C-ABI -> GPU: core/pigo_test.go:68-84 on the sample image."""
-    import os
-    import subprocess
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    exe = os.path.join(root, "tests", "cpp", "test_mirror")
-    if not os.path.exists(exe):
-        import __graft_entry__
-        __graft_entry__.build()
-    r = subprocess.run([exe, root], capture_output=True, text=True, timeout=120)
-    assert r.returncode == 0, r.stdout + r.stderr
-    assert "dets=4 clusters=1" in r.stdout
+    assert "dets=4 clusters=1" in run_cpp_mirror("test_mirror", timeout=120)
 
 
-def test_full_pipeline_batch_vs_oracle(gpu_face, oracle_face, sample_gray):
+def test_full_pipeline_batch_vs_oracle(gpu_face, oracle_face, sample_gray, cascades):
     """BASELINE.json configs[4] shape: face -> cluster -> 2 pupils -> 15 landmarks per face, per frame of a batch,
     replayed on the CPU oracle with the same injected randoms (sequencing of core/flploc_test.go:75-154)."""
     from pigo_b200 import pipeline
     frames = np.stack([synth.frame_faces(sample_gray, 540, 960, shift=(40 * i, 25 * i), noise_seed=30 + i) for i in range(3)])
     cp = cp_of(None, 540, 960, 960, TEST_PARAMS)
-    plc = pigo_b200.NewPuplocCascade().UnpackCascade(pigo_b200.load_cascade("puploc"))
-    names = sorted(set(pipeline.EYE_CASCADES + pipeline.MOUTH_CASCADES))
-    flp = {n: pigo_b200.NewPuplocCascade().UnpackCascade(pigo_b200.load_cascade("lps/" + n)) for n in names}
-    oplc = O.OraclePuploc(pigo_b200.load_cascade("puploc"))
-    oflp = {n: O.OraclePuploc(pigo_b200.load_cascade("lps/" + n)) for n in names}
+    plc, flp, _, _ = cascades
 
     def randoms_for(f, call):
         return np.random.default_rng(10_000 * f + call).random((63, 3), dtype=np.float32)
 
     got = pipeline.detect_batch(gpu_face, plc, flp, frames, cp, iou=0.1, randoms_for=randoms_for)
-    nfaces = 0
-    for f in range(3):
-        d = oracle_face.run_cascade(frames[f], 540, 960, 960, *TEST_PARAMS, 0.0)
-        _, cl = O.cluster(d, 0.1)
-        assert [(int(x["row"]), int(x["col"]), int(x["scale"])) for x in cl] == [fc.det[:3] for fc in got[f]]
-        call = 0
-        for c, fc in zip(cl, got[f]):
-            assert np.float32(c["q"]) == np.float32(fc.det[3])
-            if c["scale"] <= 50:
-                continue
-            nfaces += 1
-            ls, rs = pipeline.eye_seeds(int(c["row"]), int(c["col"]), int(c["scale"]), 50)
-            le = oplc.run_detector(ls.Row, ls.Col, ls.Scale, 50, randoms_for(f, call), frames[f], 540, 960, 960)
-            re_ = oplc.run_detector(rs.Row, rs.Col, rs.Scale, 50, randoms_for(f, call + 1), frames[f], 540, 960, 960)
-            call += 2
-            assert (fc.left_eye.Row, fc.left_eye.Col, np.float32(fc.left_eye.Scale)) == (le[0], le[1], le[2])
-            assert (fc.right_eye.Row, fc.right_eye.Col, np.float32(fc.right_eye.Scale)) == (re_[0], re_[1], re_[2])
-            for (name, flip), lm in zip(pipeline.landmark_calls(), fc.landmarks):
-                r0, c0, s0 = O.landmark_seed(le[0], le[1], re_[0], re_[1])
-                e = oflp[name].run_detector(r0, c0, float(s0), 63, randoms_for(f, call), frames[f], 540, 960, 960, 0.0, flip)
-                call += 1
-                assert (lm.Row, lm.Col, np.float32(lm.Scale)) == (e[0], e[1], e[2])
+    images = [(frames[f], 540, 960, 960) for f in range(3)]
+    cls = [P.oracle_clusters(oracle_face, im, TEST_PARAMS, 0.0) for im in images]
+
+    def randoms(f, k, slot):   # calls are numbered in sequence within a frame, 2 + 15 per refined face
+        return randoms_for(f, int((cls[f]["scale"][:k] > 50).sum()) * (2 + len(pipeline.landmark_calls())) + slot)
+
+    nfaces, _ = P.replay(cascades[2:], [(f, images[f], cls[f], 0.0) for f in range(3)], randoms, 50, P.face_arrays(got))
     assert nfaces >= 3
 
 
@@ -448,24 +422,11 @@ def test_device_resident_async_api_matches_host_api(gpu_face, oracle_face):
         assert o[f, :len(e)].tobytes() == e.tobytes()
 
 
-def _synthetic_cascade(depth: int, ntrees: int, seed: int) -> bytes:
-    """A random cascade in the facefinder binary layout (core/pigo.go:51-110) with thresholds loose enough to let windows through."""
-    rng = np.random.default_rng(seed)
-    L = 1 << depth
-    out = bytearray(b"\x03\x00\x00\x00\x81\x7f\x81\x7f")
-    out += np.uint32(depth).tobytes() + np.uint32(ntrees).tobytes()
-    for t in range(ntrees):
-        out += rng.integers(-128, 128, size=4 * L - 4, dtype=np.int8).tobytes()
-        out += rng.uniform(-1.0, 1.0, size=L).astype("<f4").tobytes()
-        out += np.float32(-0.6 - 0.25 * t).tobytes()
-    return bytes(out)
-
-
 @pytest.mark.parametrize("depth,ntrees", [(6, 3), (6, 70), (4, 9), (1, 2), (8, 5), (6, 1)])
 def test_synthetic_cascades_other_depths_and_sizes(depth, ntrees):
     """Generic tree depth (universal gather kernel) and tiny / odd-sized depth-6 cascades (resident prefix larger than the
     cascade, Q2 never used, ...), unrotated and rotated."""
-    pk = _synthetic_cascade(depth, ntrees, seed=depth * 100 + ntrees)
+    pk = synthetic_cascade(depth, ntrees, seed=depth * 100 + ntrees)
     clf = pigo_b200.NewPigo().Unpack(pk)
     ora = O.OracleFace(pk)
     assert (clf.treeDepth, clf.treeNum) == (depth, ntrees) == (ora.depth, ora.ntrees)
@@ -632,50 +593,13 @@ def _puploc_kernels_agree_with_oracle(sample_gray):
                 assert (o.Row, o.Col) == (e[0], e[1]) and np.float32(o.Scale) == e[2]
 
 
-def _pipeline_cascades():
-    from pigo_b200 import pipeline
-    plc = pigo_b200.NewPuplocCascade().UnpackCascade(pigo_b200.load_cascade("puploc"))
-    names = sorted(set(pipeline.EYE_CASCADES + pipeline.MOUTH_CASCADES))
-    flp = {n: pigo_b200.NewPuplocCascade().UnpackCascade(pigo_b200.load_cascade("lps/" + n)) for n in names}
-    oplc = O.OraclePuploc(pigo_b200.load_cascade("puploc"))
-    oflp = {n: O.OraclePuploc(pigo_b200.load_cascade("lps/" + n)) for n in names}
-    return plc, flp, oplc, oflp
-
-
-def _check_pipeline_against_oracle(got, frames, rows, cols, oracle_face, oplc, oflp, randoms, face_cap, eye_perturbs=50, angle=0.0):
-    from pigo_b200 import pipeline
-    calls = pipeline.landmark_calls()
-    nrefined = 0
-    for f in range(len(frames)):
-        d = oracle_face.run_cascade(frames[f], rows, cols, cols, *TEST_PARAMS, angle)
-        _, cl = O.cluster(d, 0.1)
-        assert len(cl) <= face_cap
-        assert [(int(x["row"]), int(x["col"]), int(x["scale"])) for x in cl] == [fc.det[:3] for fc in got[f]]
-        for k, (c, fc) in enumerate(zip(cl, got[f])):
-            assert np.float32(c["q"]) == np.float32(fc.det[3])
-            if c["scale"] <= 50:
-                assert fc.left_eye is None
-                continue
-            nrefined += 1
-            ls, rs = pipeline.eye_seeds(int(c["row"]), int(c["col"]), int(c["scale"]), eye_perturbs)
-            le = oplc.run_detector(ls.Row, ls.Col, ls.Scale, eye_perturbs, randoms[f, k, 0], frames[f], rows, cols, cols, angle)
-            re_ = oplc.run_detector(rs.Row, rs.Col, rs.Scale, eye_perturbs, randoms[f, k, 1], frames[f], rows, cols, cols, angle)
-            assert (fc.left_eye.Row, fc.left_eye.Col, np.float32(fc.left_eye.Scale)) == (le[0], le[1], le[2])
-            assert (fc.right_eye.Row, fc.right_eye.Col, np.float32(fc.right_eye.Scale)) == (re_[0], re_[1], re_[2])
-            r0, c0, s0 = O.landmark_seed(le[0], le[1], re_[0], re_[1])
-            for ci, ((name, flip), lm) in enumerate(zip(calls, fc.landmarks)):
-                e = oflp[name].run_detector(r0, c0, float(s0), 63, randoms[f, k, 2 + ci], frames[f], rows, cols, cols, 0.0, flip)
-                assert (lm.Row, lm.Col, np.float32(lm.Scale)) == (e[0], e[1], e[2])
-    return nrefined
-
-
 @pytest.mark.parametrize("angle,stage", [(0.0, 1), (0.03, 1), (0.0, 2), (0.03, 2)])
-def test_device_pipeline_vs_oracle(gpu_face, oracle_face, sample_gray, angle, stage):
+def test_device_pipeline_vs_oracle(gpu_face, oracle_face, sample_gray, cascades, angle, stage):
     """pigo_detect_batch (SURVEY.md 8f N1): the whole face -> cluster -> eye seeds -> RunDetector x2 -> landmark seeds ->
     15 x RunDetector sequence on the device in one call, replayed step by step on the CPU oracle with the same injected
     randoms (core/flploc_test.go:75-154; angle > 0 like cmd/pigo/main.go:422 passes det.angle to the eye RunDetector)."""
     from pigo_b200 import pipeline
-    plc, flp, oplc, oflp = _pipeline_cascades()
+    plc, flp, _, _ = cascades
     frames = np.stack([synth.frame_faces(sample_gray, 540, 960, shift=(40 * i, 25 * i), noise_seed=30 + i) for i in range(3)] +
                       [synth.frame_noise(540, 960, 5)])
     cp = cp_of(None, 540, 960, 960, TEST_PARAMS)
@@ -689,17 +613,20 @@ def test_device_pipeline_vs_oracle(gpu_face, oracle_face, sample_gray, angle, st
             got2 = pipeline.detect_batch_device(gpu_face, plc, flp, df, cp, iou=0.1, face_cap=face_cap, randoms=randoms, angle=angle)
         finally:
             df.free()
-    n = _check_pipeline_against_oracle(got, frames, 540, 960, oracle_face, oplc, oflp, randoms, face_cap, angle=angle)
+    images = [(frames[f], 540, 960, 960) for f in range(4)]
+    cls = [P.oracle_clusters(oracle_face, im, TEST_PARAMS, angle) for im in images]
+    assert all(len(cl) <= face_cap for cl in cls)
+    n, _ = P.replay(cascades[2:], [(f, images[f], cls[f], angle) for f in range(4)], lambda f, k, slot: randoms[f, k, slot], 50, P.face_arrays(got))
     assert n >= 3 or angle > 0
     assert got[3] == [] or all(fc.left_eye is None or fc.det[2] > 50 for fc in got[3])
     assert got2 == got
 
 
-def test_device_pipeline_capacity_and_rng_mode(gpu_face, sample_gray):
+def test_device_pipeline_capacity_and_rng_mode(gpu_face, sample_gray, cascades):
     """face_cap / det_cap too small -> PIGO_E_CAP (with the required count); library generator: deterministic, and
     independent of how the batch is split (keys are (seed, frame, cluster, call))."""
     from pigo_b200 import pipeline
-    plc, flp, _, _ = _pipeline_cascades()
+    plc, flp, _, _ = cascades
     frames = np.stack([synth.frame_faces(sample_gray, 540, 960, shift=(11 * i, 7 * i), noise_seed=90 + i) for i in range(4)])
     cp = cp_of(None, 540, 960, 960, TEST_PARAMS)
     with pytest.raises(pigo_b200.PigoError) as e:
@@ -753,17 +680,10 @@ def test_cpp_sharded_over_every_visible_device():
     pigo_run_cascade_batch_sharded, pigo_detect_batch_sharded) and requires byte-identical results to the 1-GPU calls.
     With one GPU this exercises the same code with a single shard; on a machine with two GPUs it is the 2-device test."""
     import os
-    import subprocess
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    exe = os.path.join(root, "tests", "cpp", "test_sharded")
-    if not os.path.exists(exe):
-        import __graft_entry__
-        __graft_entry__.build()
-    r = subprocess.run([exe, root], capture_output=True, text=True, timeout=300)
-    assert r.returncode == 0, r.stdout + r.stderr
-    assert "== single device" in r.stdout
+    out = run_cpp_mirror("test_sharded")
+    assert "== single device" in out
     need = int(os.environ.get("PIGO_REQUIRE_DEVICES", "1"))
-    assert int(r.stdout.split("devices=")[1].split()[0]) >= need
+    assert int(out.split("devices=")[1].split()[0]) >= need
 
 
 # ---------------------------------------------------------------------------------------------------------------

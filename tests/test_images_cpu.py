@@ -1,55 +1,23 @@
 """CPU-side checks of pigo_run_cascade_images (mixed-size RunCascade): every invalid argument is rejected with
 PIGO_E_INVALID before any device work, and the Go shim binds the entry point."""
-import glob
-import os
 import re
 
-import numpy as np
 import pytest
 
 import pigo_b200
-from test_abi import _calls
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from abi_cases import IMAGE_CASES, descs, go_binds, go_source, header_protos, scan
 
 
-def _run(images, nimages, cap=4, with_n_out=True):
-    """Calls the entry point with a NULL cascade: the cascade is validated last, so the message names the first bad argument."""
-    L = pigo_b200.lib()
-    out = np.zeros((2, max(cap, 1)), dtype=pigo_b200.DET_DTYPE)
-    cnt = np.zeros(2, dtype=np.int32)
-    rc = L.pigo_run_cascade_images(None, images, nimages, 20, 1000, 0.2, 1.1, 0.0, out.ctypes.data, cap,
-                                   cnt.ctypes.data if with_n_out else None, pigo_b200.MEM_HOST, None)
-    return rc, L.pigo_last_error().decode()
-
-
-PIX = np.zeros(64 * 64, dtype=np.uint8)
-
-
-def _descs(*geoms, pixels=PIX.ctypes.data):
-    return pigo_b200.image_descs([(pixels, r, c, d) for r, c, d in geoms])
-
-
-@pytest.mark.parametrize("case,images,nimages,kw,msg", [
-    ("null images", None, 2, {}, "null images"),
-    ("too many images", _descs((8, 8, 8)), 65536, {}, "nimages"),
-    ("negative count", _descs((8, 8, 8)), -1, {}, "nimages"),
-    ("negative rows", _descs((8, 8, 8), (-1, 8, 8)), 2, {}, "image 1: bad geometry"),
-    ("dim < cols", _descs((8, 9, 8)), 1, {}, "image 0: bad geometry"),
-    ("rows*dim >= 2^31", _descs((65536, 32768, 32768)), 1, {}, "image 0: larger than 2^31"),
-    ("negative capacity", _descs((8, 8, 8)), 1, {"cap": -1}, "negative capacity"),
-    ("null n_out", _descs((8, 8, 8)), 1, {"with_n_out": False}, "null n_out"),
-    ("null pixels", _descs((8, 8, 8), pixels=None), 1, {}, "image 0: null pixels"),
-])
+@pytest.mark.parametrize("case,images,nimages,kw,msg", IMAGE_CASES)
 def test_invalid_arguments_are_rejected_before_the_device(case, images, nimages, kw, msg):
-    rc, err = _run(images, nimages, **kw)
+    rc, err = scan("pigo_run_cascade_images", images, nimages, **kw)
     assert rc == pigo_b200.PIGO_E_INVALID, case
     assert msg in err, (case, err)
 
 
 def test_valid_arguments_reach_the_cascade_check():
     """Control for the cases above: the same call with valid images fails only on the NULL cascade."""
-    rc, err = _run(_descs((64, 64, 64), (1, 1, 1), (0, 0, 0)), 3)
+    rc, err = scan("pigo_run_cascade_images", descs((64, 64, 64), (1, 1, 1), (0, 0, 0)), 3)
     assert rc == pigo_b200.PIGO_E_INVALID and "null cascade" in err
 
 
@@ -61,13 +29,8 @@ def test_descriptor_layout_matches_the_header():
 
 
 def test_go_shim_binds_run_cascade_images():
-    header = open(os.path.join(ROOT, "include", "pigo_b200.h")).read()
-    header = re.sub(r"/\*.*?\*/", "", header, flags=re.S)
-    protos = dict(_calls(header, ""))
-    go = "\n".join(open(f).read() for f in sorted(glob.glob(os.path.join(ROOT, "go", "pigo", "*.go"))))
-    go = re.sub(r"//[^\n]*", "", go)
-    calls = [n for name, n in _calls(go, "C.") if name == "pigo_run_cascade_images"]
-    assert calls and all(n == protos["pigo_run_cascade_images"] == 13 for n in calls)
+    protos, go = header_protos(), go_source()
+    assert protos["pigo_run_cascade_images"] == 13 and go_binds(go, "pigo_run_cascade_images", protos)
     assert re.search(r"^func \(pg \*Pigo\) RunCascadeImages\(images \[\]ImageParams, cp CascadeParams, angle float64\) \[\]\[\]Detection \{",
                      go, flags=re.M)
     assert "C.pigo_alloc_pinned" in go and "C.malloc" in go   # pixels and descriptors in C memory (cgo pointer rules)

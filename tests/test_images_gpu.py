@@ -1,44 +1,17 @@
 """pigo_run_cascade_images: RunCascade over images of different sizes in one call.  Bar: every image's slice equals a
 lone pigo_run_cascade on that image byte for byte (emission order, bit-equal Q) and, up to 1080p, the C oracle."""
-import os
-import subprocess
 import threading
 
 import numpy as np
 import pytest
 
 import pigo_b200
+from mixed_images import CLI_PARAMS, DOC_PARAMS, KNOBS, MIXED, TEST_PARAMS, assert_slices, cp_of, lone_scan, make_image, run_cpp_mirror
 from pigo_b200 import CascadeParams, ImageParams, synth
 from option_guard import options, options_at_defaults   # noqa: F401 (autouse: every test ends with the options at their defaults)
+from synthetic import synthetic_cascade
 
 pytestmark = pytest.mark.gpu
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-TEST_PARAMS = (20, 1000, 0.2, 1.1)   # core/pigo_test.go:44-50
-DOC_PARAMS = (20, 1000, 0.1, 1.1)    # README
-CLI_PARAMS = (20, 1000, 0.15, 1.15)  # cmd/pigo/main.go:110-111
-
-# (rows, cols, dim, content class): no windows (1x1, 10x10, 21 rows), exactly one window (22x22), the sample, common sizes
-# up to 4K, odd sizes and strides (dim > cols), wide and tall shapes
-MIXED = [(1, 1, 1, "U"), (10, 10, 10, "U"), (22, 22, 22, "U"), (400, 320, 320, "sample"), (480, 640, 640, "F"),
-         (720, 1280, 1280, "S"), (1080, 1920, 1920, "F"), (2160, 3840, 3840, "F"), (97, 131, 160, "U"), (333, 517, 531, "F"),
-         (240, 320, 320, "S"), (600, 800, 800, "F"), (123, 777, 800, "U"), (50, 60, 64, "S"), (768, 1024, 1024, "U"),
-         (301, 299, 301, "F"), (1080, 1920, 1920, "S"), (45, 1200, 1216, "F"), (900, 41, 48, "U"), (360, 640, 640, "F"),
-         (511, 383, 400, "S"), (200, 200, 200, "F"), (64, 64, 80, "U"), (1000, 700, 701, "F"), (150, 1500, 1500, "S"),
-         (480, 640, 700, "U"), (21, 300, 300, "F"), (272, 480, 496, "F"), (540, 960, 960, "U"), (333, 250, 256, "S")]
-
-
-def make_image(rows, cols, dim, cls, seed) -> ImageParams:
-    if cls == "sample":
-        return ImageParams(synth.sample_gray(), rows, cols, dim)
-    buf = np.full((rows, dim), 0xA5, dtype=np.uint8)   # the bytes past Cols are never read
-    if cls == "U":
-        buf[:, :cols] = synth.frame_noise(rows, cols, seed)
-    elif cls == "S":
-        buf[:, :cols] = synth.frame_smooth(rows, cols, seed)
-    else:
-        buf[:, :cols] = synth.frame_faces(None, rows, cols, shift=((37 * seed) % 400, (53 * seed) % 320), noise_seed=seed)
-    return ImageParams(buf, rows, cols, dim)
 
 
 @pytest.fixture(scope="module")
@@ -53,25 +26,10 @@ def wide(mixed):
     return [im for im in mixed if im.Cols >= im.Rows] + [make_image(300, 900, 900, "F", 5), make_image(200, 1200, 1216, "S", 6)]
 
 
-def cp_of(params):
-    return CascadeParams(ImageParams(), *params)
-
-
-def lone(face, im, params, angle=0.0):
-    return face.run_cascade_array(CascadeParams(im, *params), angle)
-
-
-def assert_slices(dets, cnt, expect):
-    assert len(cnt) == len(expect)
-    for i, e in enumerate(expect):
-        assert int(cnt[i]) == len(e), f"image {i}: {int(cnt[i])} detections vs {len(e)}"
-        assert dets[i, :len(e)].tobytes() == e.tobytes(), f"image {i} differs"
-
-
 @pytest.mark.parametrize("params", [TEST_PARAMS, CLI_PARAMS, DOC_PARAMS])
 def test_each_image_equals_a_lone_call_and_the_oracle(gpu_face, oracle_face, mixed, params):
     dets, cnt = gpu_face.RunCascadeImages(mixed, cp_of(params))
-    expect = [lone(gpu_face, im, params) for im in mixed]
+    expect = [lone_scan(gpu_face, im, params) for im in mixed]
     assert_slices(dets, cnt, expect)
     assert sum(len(e) for e in expect) > 0
     for i, im in enumerate(mixed):
@@ -83,7 +41,7 @@ def test_each_image_equals_a_lone_call_and_the_oracle(gpu_face, oracle_face, mix
 @pytest.mark.parametrize("angle", [1 / 32, 7 / 32, 16 / 32, 31 / 32, 1.0, 1.3])
 def test_rotated_each_image_equals_a_lone_call(gpu_face, wide, angle):
     dets, cnt = gpu_face.RunCascadeImages(wide, cp_of(TEST_PARAMS), angle)
-    assert_slices(dets, cnt, [lone(gpu_face, im, TEST_PARAMS, angle) for im in wide])
+    assert_slices(dets, cnt, [lone_scan(gpu_face, im, TEST_PARAMS, angle) for im in wide])
 
 
 @pytest.mark.parametrize("angle", [0.0, 0.25])
@@ -128,12 +86,6 @@ def test_host_device_and_stream_forms_agree(gpu_face, mixed):
         assert o[i, :hc[i]].tobytes() == hd[i, :hc[i]].tobytes()
 
 
-KNOBS = [{"queue_cap": 1}, {"queue_cap": 16, "gather_ks": 2}, {"gather_ks": 8}, {"gather_block": 8}, {"gather_block": 16},
-         {"deep_group": 8}, {"deep_group": 32}, {"gather_ctas_per_sm": 1}, {"gather_ni": 2}, {"gather_ni": 3}, {"gather_limit": 3},
-         {"sub_batch": 4},                     # several groups of images per call
-         {"scan_mode": 1}, {"rot_mode": 1}]    # universal kernel: the single-image path, image by image
-
-
 @pytest.mark.parametrize("knobs", KNOBS)
 def test_options_leave_the_outputs_unchanged(gpu_face, wide, knobs):
     expect = {a: gpu_face.RunCascadeImages(wide, cp_of(TEST_PARAMS), a) for a in (0.0, 0.5)}
@@ -146,11 +98,10 @@ def test_options_leave_the_outputs_unchanged(gpu_face, wide, knobs):
 
 
 def test_cascade_of_another_depth_takes_the_single_image_path(mixed):
-    from test_oracle_pins import _synthetic_cascade
-    face = pigo_b200.NewPigo().Unpack(_synthetic_cascade(4, 9, seed=409))
+    face = pigo_b200.NewPigo().Unpack(synthetic_cascade(4, 9, seed=409))
     some = mixed[:12]
     dets, cnt = face.RunCascadeImages(some, cp_of(TEST_PARAMS), 0.0)
-    assert_slices(dets, cnt, [lone(face, im, TEST_PARAMS) for im in some])
+    assert_slices(dets, cnt, [lone_scan(face, im, TEST_PARAMS) for im in some])
     assert cnt.sum() > 0
 
 
@@ -178,7 +129,7 @@ def test_mixed_calls_leave_the_uniform_plan_cache_alone(gpu_face, wide, angle):
     m1, k1 = gpu_face.RunCascadeImages(wide, cp_of(TEST_PARAMS), angle)
     assert np.array_equal(c0, c1) and d0.tobytes() == d1.tobytes()
     assert np.array_equal(k0, k1) and m0.tobytes() == m1.tobytes()
-    assert_slices(m0, k0, [lone(gpu_face, im, TEST_PARAMS, angle) for im in wide])
+    assert_slices(m0, k0, [lone_scan(gpu_face, im, TEST_PARAMS, angle) for im in wide])
 
 
 def test_concurrent_mixed_calls_on_one_classifier(gpu_face, mixed):
@@ -215,7 +166,4 @@ def test_cluster_batch_on_the_output_equals_per_image_clustering(gpu_face, mixed
 def test_cpp_mirror_sample_inside_a_mixed_batch():
     """tests/cpp/test_images.cpp (built by build()): the reference's >= 1 face assertion on the sample image placed inside a
     mixed-size batch, through include/pigo_b200.hpp."""
-    exe = os.path.join(ROOT, "tests", "cpp", "test_images")
-    assert os.path.exists(exe), "run __graft_entry__.build() first"
-    p = subprocess.run([exe, ROOT], capture_output=True, text=True, timeout=300)
-    assert p.returncode == 0, p.stdout + p.stderr
+    run_cpp_mirror("test_images")

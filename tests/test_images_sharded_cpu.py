@@ -9,7 +9,8 @@ import numpy as np
 import pytest
 
 import pigo_b200
-from pigo_b200 import CascadeParams, ImageParams, PipelineParams
+from abi_cases import IMAGE_CASES, PIPELINE_CASES, descs, detect, scan
+from pigo_b200 import CascadeParams, ImageParams
 
 TEST_PARAMS = (20, 1000, 0.2, 1.1)   # core/pigo_test.go:44-50
 ROT, UNROT, IMG = 14, 10, 4096 * 10   # the cost model in tenths of a window (pigo_b200/csrc/api.cu)
@@ -145,80 +146,43 @@ def test_plan_argument_errors():
 
 
 # ---- argument errors of the four calls: all reached before any device work ---------------------------------------------
-def _images(items):
-    keep = [np.zeros(max(r * d, 1), dtype=np.uint8) for r, c, d in items]
-    return keep, pigo_b200.image_descs([(k.ctypes.data, r, c, d) for k, (r, c, d) in zip(keep, items)])
-
-
 def test_run_cascade_images_sharded_argument_errors():
-    L = pigo_b200.lib()
-    keep, d = _images([(40, 40, 40), (30, 50, 50)])
-    out = np.zeros((2, 8), dtype=pigo_b200.DET_DTYPE)
-    cnt = np.zeros(2, dtype=np.int32)
-    args = lambda **kw: {"c": None, "im": d, "n": 2, "ang": None, "out": out.ctypes.data, "cap": 8, "cnt": cnt.ctypes.data, **kw}
-    call = lambda a: L.pigo_run_cascade_images_sharded(a["c"], a["im"], a["n"], a["ang"], *TEST_PARAMS, a["out"], a["cap"], a["cnt"])
-    for bad in ({"n": -1}, {"n": 70000}, {"im": None}, {"cnt": None}, {"cap": -1}, {"out": None}, {}):   # {}: null cascade, checked last
-        assert call(args(**bad)) == pigo_b200.PIGO_E_INVALID, bad
-    _, tall = _images([(40, 40, 39)])
-    assert call(args(im=tall, n=1)) == pigo_b200.PIGO_E_INVALID
-
-
-def _params(**kw):
-    p = PipelineParams(20, 1000, 0.2, 1.1, 0.0, 0.1, 50, 50, 63, 0)
-    for k, v in kw.items():
-        setattr(p, k, v)
-    return p
+    for case, images, nimages, kw, msg in IMAGE_CASES + [("valid images", descs((40, 40, 40), (30, 50, 50)), 2, {}, "null cascade")]:
+        rc, err = scan("pigo_run_cascade_images_sharded", images, nimages, angles=False, **kw)
+        assert rc == pigo_b200.PIGO_E_INVALID, case
+        assert msg in err, (case, err)
 
 
 def test_detect_images_sharded_argument_errors():
-    L = pigo_b200.lib()
-    keep, d = _images([(40, 40, 40), (30, 50, 50)])
-    faces = np.zeros((2, 4), dtype=pigo_b200.DET_DTYPE)
-    nf = np.zeros(2, dtype=np.int32)
-    pts = np.zeros((2, 4, 2), dtype=pigo_b200.POINT_DTYPE)
-    base = {"im": d, "n": 2, "prm": _params(), "faces": faces.ctypes.data, "cap": 4, "nf": nf.ctypes.data, "pts": pts.ctypes.data, "ncalls": 0}
-
-    def call(**kw):
-        a = {**base, **kw}
-        prm = C.byref(a["prm"]) if a["prm"] is not None else None
-        return L.pigo_detect_images_sharded(None, None, None, None, a["ncalls"], a["im"], a["n"], None, prm, None, 0, a["faces"], a["cap"], a["nf"],
-                                            a["pts"])
-    _, zero = _images([(0, 10, 10)])
-    for bad in ({"n": -1}, {"im": None}, {"prm": None}, {"faces": None}, {"nf": None}, {"pts": None}, {"ncalls": 31}, {"ncalls": 1},
-                {"cap": 0}, {"cap": 5000}, {"prm": _params(eye_perturbs=64)}, {"im": zero, "n": 1}, {}):
-        assert call(**bad) == pigo_b200.PIGO_E_INVALID, bad
-
-
-def _decoded(w=40, h=30, fmt=pigo_b200.DECODED_GRAY):
-    pix = np.zeros(w * h * 8, dtype=np.uint8)
-    return pix, pigo_b200.DecodedImage(fmt, w, h, (pix,), (w * (8 if fmt in (6, 7) else 1), 0))
+    for case, images, nimages, kw, msg in PIPELINE_CASES + [("valid images", descs((40, 40, 40), (30, 50, 50)), 2, {}, "null cascade")]:
+        rc, err = detect("pigo_detect_images_sharded", images, nimages, angles=False, **kw)
+        assert rc == pigo_b200.PIGO_E_INVALID, case
+        assert msg in err, (case, err)
 
 
 def test_decoded_sharded_argument_errors():
-    L = pigo_b200.lib()
-    pix, good = _decoded()
-    out = np.zeros((2, 8), dtype=pigo_b200.DET_DTYPE)
-    cnt = np.zeros(2, dtype=np.int32)
-    faces = np.zeros((2, 4), dtype=pigo_b200.DET_DTYPE)
-    pts = np.zeros((2, 4, 2), dtype=pigo_b200.POINT_DTYPE)
+    pix = np.zeros(40 * 30 * 8, dtype=np.uint8)
+    good = pigo_b200.DecodedImage(pigo_b200.DECODED_GRAY, 40, 30, (pix,), (40, 0))
     bad_fmt = pigo_b200.DecodedImage(4, 40, 30, (pix,), (40, 0))
     short = pigo_b200.DecodedImage(pigo_b200.DECODED_RGBA64, 40, 30, (pix,), (100, 0))
     no_plane = pigo_b200.DecodedImage(pigo_b200.DECODED_GRAY, 40, 30, (None,), (40, 0))
     empty = pigo_b200.DecodedImage(pigo_b200.DECODED_GRAY, 0, 30, (pix,), (40, 0))
-    prm = _params()
-    for srcs, n in (([good, bad_fmt], 2), ([good, short], 2), ([no_plane, good], 2), ([empty], 1), ([good], -1), ([good], 70000), (None, 1),
-                    ([good, good], 2)):   # the last: valid sources, null cascade
+    one = pigo_b200.decoded_descs([good])
+    cases = [([good, bad_fmt], 2, "source 1: unknown format 4"), ([good, short], 2, "source 1: stride 100 below the row"),
+             ([no_plane, good], 2, "source 0: null plane"), ([empty], 1, "source 0: bad size 0x30"),
+             ([good], -1, "-1 sources: outside 0..65535"), ([good], 70000, "70000 sources: outside 0..65535"), (None, 1, "null src"),
+             ([good, good], 2, "null cascade")]   # the last: valid sources, null cascade
+    for srcs, n, msg in cases:
         desc = pigo_b200.decoded_descs(srcs) if srcs is not None else None
-        assert L.pigo_run_cascade_decoded_sharded(None, desc, n, None, *TEST_PARAMS, out.ctypes.data, 8, cnt.ctypes.data) == pigo_b200.PIGO_E_INVALID
-        assert L.pigo_detect_decoded_sharded(None, None, None, None, 0, desc, n, None, C.byref(prm), None, 0, faces.ctypes.data, 4, cnt.ctypes.data,
-                                             pts.ctypes.data) == pigo_b200.PIGO_E_INVALID
-    desc = pigo_b200.decoded_descs([good])
-    assert L.pigo_run_cascade_decoded_sharded(None, desc, 1, None, *TEST_PARAMS, None, 8, cnt.ctypes.data) == pigo_b200.PIGO_E_INVALID
-    assert L.pigo_run_cascade_decoded_sharded(None, desc, 1, None, *TEST_PARAMS, out.ctypes.data, 8, None) == pigo_b200.PIGO_E_INVALID
-    assert L.pigo_detect_decoded_sharded(None, None, None, None, 0, desc, 1, None, None, None, 0, faces.ctypes.data, 4, cnt.ctypes.data,
-                                         pts.ctypes.data) == pigo_b200.PIGO_E_INVALID
-    assert L.pigo_detect_decoded_sharded(None, None, None, None, 0, desc, 1, None, C.byref(prm), None, 0, faces.ctypes.data, 0, cnt.ctypes.data,
-                                         pts.ctypes.data) == pigo_b200.PIGO_E_INVALID
+        for entry, call in (("pigo_run_cascade_decoded_sharded", scan), ("pigo_detect_decoded_sharded", detect)):
+            rc, err = call(entry, desc, n, angles=False)
+            assert rc == pigo_b200.PIGO_E_INVALID and msg in err, (entry, msg, err)
+    for entry, call, kw, msg in (("pigo_run_cascade_decoded_sharded", scan, {"with_out": False}, "null out"),
+                                 ("pigo_run_cascade_decoded_sharded", scan, {"with_n_out": False}, "null n_out"),
+                                 ("pigo_detect_decoded_sharded", detect, {"params": False}, "null params"),
+                                 ("pigo_detect_decoded_sharded", detect, {"face_cap": 0}, "face_cap")):
+        rc, err = call(entry, one, 1, angles=False, **kw)
+        assert rc == pigo_b200.PIGO_E_INVALID and msg in err, (entry, msg, err)
 
 
 def test_mirrors_check_the_angle_count():

@@ -4,34 +4,23 @@ for byte: pigo_run_cascade_images_angles for the scan, pigo_detect_images_angles
 and with the library generator, whose keys must not depend on the split), pigo_gray_images + the matching call for the
 decoded forms.  A too-small capacity reports every shard's counts; a sampled image is checked against the C oracle."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
-import oracle_lib as O
 import pigo_b200
-from pigo_b200 import CascadeParams, ImageParams, pipeline, synth
+from decoded_sources import face_sources, host_images, narrow_sources, wide_sources, ycbcr_src  # noqa: F401 (fixtures)
+from mixed_images import MIXED, NCALLS, TEST_PARAMS, canonical, cascades, cp_of, make_image, run_cpp_mirror  # noqa: F401 (fixture)
+from pigo_b200 import pipeline, synth
 from option_guard import options, options_at_defaults   # noqa: F401 (autouse: every test ends with the options at their defaults)
-from test_decoded_formats_gpu import PALETTED, face_sources, narrow_sources, sources, wide_src  # noqa: F401 (fixtures)
-from test_decoded_gpu import host_images, ycbcr_src
-from test_images_gpu import MIXED, make_image
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-TEST_PARAMS = (20, 1000, 0.2, 1.1)   # core/pigo_test.go:44-50
-NCALLS = 15
 SWEEP = [0.0] + [k / 32 for k in range(1, 33)]
 
 
 def splits(n):
     return [0, 2, 3, 7, n + 2]
-
-
-def cp_of(params=TEST_PARAMS):
-    return CascadeParams(ImageParams(), *params)
 
 
 @pytest.fixture(autouse=True)
@@ -43,7 +32,7 @@ def shard_split():
 
 @pytest.fixture(scope="module")
 def mixed():
-    """The mixed geometries of test_images_gpu (odd sizes, dim > cols, no-window images, 1080p, one 4K frame), seeded."""
+    """The MIXED geometries (odd sizes, dim > cols, no-window images, 1080p, one 4K frame), seeded."""
     return [make_image(r, c, d, k, 31 + i) for i, (r, c, d, k) in enumerate(MIXED)]
 
 
@@ -52,18 +41,6 @@ def mixed_angles(mixed):
     rng = np.random.default_rng(17)
     # rotated angles only where Cols >= Rows (see test_angles_gpu)
     return [float(rng.choice([0.0, 0.1, 0.25, 0.5, 1.0, -0.2])) if im.Cols >= im.Rows else 0.0 for im in mixed]
-
-
-@pytest.fixture(scope="module")
-def cascades():
-    plc = pigo_b200.NewPuplocCascade().UnpackCascade(pigo_b200.load_cascade("puploc"))
-    names = sorted(set(pipeline.EYE_CASCADES + pipeline.MOUTH_CASCADES))
-    flp = {n: pigo_b200.NewPuplocCascade().UnpackCascade(pigo_b200.load_cascade("lps/" + n)) for n in names}
-    return plc, flp
-
-
-def canonical(a):
-    return 0.0 if not a > 0 else min(a, 1.0)
 
 
 def check_oracle(oracle_face, images, angles, dets, cnt, seed):
@@ -136,14 +113,14 @@ def pipe_angles(pipe_images):
 
 @pytest.fixture(scope="module")
 def face_cap(gpu_face, cascades, pipe_images, pipe_angles):
-    plc, flp = cascades
+    plc, flp, _, _ = cascades
     _, n, _ = pipeline.detect_images_angles_device(gpu_face, plc, flp, pipe_images, cp_of(), pipe_angles, face_cap=256, raw=True)
     return int(max(n.max(), 1))
 
 
 @pytest.mark.parametrize("injected", [True, False])
 def test_pipeline_equals_the_single_device_call_for_every_split(gpu_face, cascades, pipe_images, pipe_angles, face_cap, injected, shard_split):
-    plc, flp = cascades
+    plc, flp, _, _ = cascades
     n = len(pipe_images)
     rnd = np.random.default_rng(5).random((n, face_cap, 2 + NCALLS, 63, 3), dtype=np.float32) if injected else None
     want = pipeline.detect_images_angles_device(gpu_face, plc, flp, pipe_images, cp_of(), pipe_angles, face_cap=face_cap, randoms=rnd,
@@ -158,7 +135,7 @@ def test_pipeline_equals_the_single_device_call_for_every_split(gpu_face, cascad
 
 
 def test_pipeline_angle_none_uses_the_params_angle(gpu_face, cascades, pipe_images, face_cap, shard_split):
-    plc, flp = cascades
+    plc, flp, _, _ = cascades
     ims = [im for im in pipe_images if im.Cols >= im.Rows]
     want = pipeline.detect_images_device(gpu_face, plc, flp, ims, cp_of(), face_cap=face_cap, angle=0.1, rng_seed=3, raw=True)
     shard_split(3)
@@ -167,7 +144,7 @@ def test_pipeline_angle_none_uses_the_params_angle(gpu_face, cascades, pipe_imag
 
 
 def test_pipeline_capacity_reports_every_shard_and_the_retry_matches(gpu_face, cascades, pipe_images, pipe_angles, face_cap, shard_split):
-    plc, flp = cascades
+    plc, flp, _, _ = cascades
     want = pipeline.detect_images_angles_device(gpu_face, plc, flp, pipe_images, cp_of(), pipe_angles, face_cap=face_cap, rng_seed=9, raw=True)
     assert face_cap > 1
     hs, fl = pipeline.landmark_call_arrays(flp)
@@ -193,7 +170,7 @@ def test_the_reference_landmark_assertions_hold_on_the_sample_among_other_images
                                                                                   shard_split):
     """core/flploc_test.go:75-154 on the sample (entries 1 and 8 of the call, both at angle 0): at least one face, and the
     refined face's 15 landmark points inside the image."""
-    plc, flp = cascades
+    plc, flp, _, _ = cascades
     for k in (0, 3):
         shard_split(k)
         res = pipeline.detect_images_sharded(gpu_face, plc, flp, pipe_images, cp_of(), pipe_angles, face_cap=face_cap, rng_seed=1)
@@ -206,9 +183,9 @@ def test_the_reference_landmark_assertions_hold_on_the_sample_among_other_images
 
 # ---- decoded sources ---------------------------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
-def decoded_mix(sources, face_sources):
+def decoded_mix(wide_sources, face_sources):
     """All nine formats, face content in five of them, with repeats, as host sources."""
-    nine = narrow_sources() + [sources[k] for k in (4, 12, 20, 28, 36)]
+    nine = narrow_sources() + [wide_sources[k] for k in (4, 12, 20, 28, 36)]
     faces = face_sources + [ycbcr_src(2, 320, 400, 1, 1, 24, luma=synth.sample_gray())]
     picks = [faces[5], nine[0], faces[0], nine[8], faces[1], nine[4], faces[2], faces[5], nine[1], faces[3], nine[5], nine[2], faces[4],
              nine[6], nine[7], nine[3], faces[0]]
@@ -234,7 +211,7 @@ def test_decoded_scan_equals_gray_images_and_the_single_device_call(gpu_face, de
 
 @pytest.mark.parametrize("injected", [True, False])
 def test_decoded_pipeline_equals_detect_decoded_for_every_split(gpu_face, cascades, decoded_mix, injected, shard_split):
-    plc, flp = cascades
+    plc, flp, _, _ = cascades
     srcs = [s.decoded() for s in decoded_mix]
     n = len(srcs)
     rnd = np.random.default_rng(8).random((n, 8, 2 + NCALLS, 63, 3), dtype=np.float32) if injected else None
@@ -261,9 +238,4 @@ def test_decoded_capacity_reports_every_shard(gpu_face, decoded_mix, shard_split
 # ---- the C++ mirror -----------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("split", [0, 3, 9])
 def test_cpp_mirror(split):
-    exe = os.path.join(ROOT, "tests", "cpp", "test_images_sharded")
-    if not os.path.exists(exe):
-        import __graft_entry__
-        __graft_entry__.build()
-    r = subprocess.run([exe, ROOT, str(split)], capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0, r.stdout + r.stderr
+    run_cpp_mirror("test_images_sharded", split, timeout=600)

@@ -10,6 +10,7 @@ import oracle_lib as O
 import pigo_b200
 from oracle import np_oracle as NP
 from pigo_b200 import synth
+from synthetic import synthetic_cascade
 
 TEST_PARAMS = (20, 1000, 0.2, 1.1)  # core/pigo_test.go:44-50
 
@@ -144,25 +145,12 @@ def test_grayscale_restatements_agree():
     assert np.array_equal(O.rgba_to_gray(rgba), NP.rgb_to_grayscale(rgba[..., :3]))
 
 
-def _synthetic_cascade(depth: int, ntrees: int, seed: int) -> bytes:
-    """A random cascade in the facefinder binary layout (core/pigo.go:51-110), thresholds loose enough to let windows through."""
-    rng = np.random.default_rng(seed)
-    L = 1 << depth
-    out = bytearray(b"\x03\x00\x00\x00\x81\x7f\x81\x7f")
-    out += np.uint32(depth).tobytes() + np.uint32(ntrees).tobytes()
-    for t in range(ntrees):
-        out += rng.integers(-128, 128, size=4 * L - 4, dtype=np.int8).tobytes()
-        out += rng.uniform(-1.0, 1.0, size=L).astype("<f4").tobytes()
-        out += np.float32(-0.6 - 0.25 * t).tobytes()
-    return bytes(out)
-
-
 @pytest.mark.parametrize("depth,ntrees", [(6, 3), (6, 40), (4, 9), (1, 2), (8, 5), (6, 1)])
 def test_c_and_numpy_agree_on_random_cascades_of_any_depth(depth, ntrees):
     """Both restatements are generic in tree depth and count (core/pigo.go:113-147 reads them from the packet): random
     cascades, extreme codes (-128 / 127) included, unrotated and rotated, same detections and bit-equal scores."""
     from pigo_b200 import synth
-    pk = _synthetic_cascade(depth, ntrees, seed=depth * 100 + ntrees)
+    pk = synthetic_cascade(depth, ntrees, seed=depth * 100 + ntrees)
     c_or, np_or = O.OracleFace(pk), NP.FaceCascade(pk)
     assert (c_or.depth, c_or.ntrees) == (depth, ntrees) == (np_or.depth, np_or.ntrees)
     img = synth.frame_smooth(150, 210, seed=depth + ntrees, sigma=3.0)

@@ -3,20 +3,19 @@ image i's clusters are pigo_cluster of the concatenation of its RunCascadeImages
 indices of the largest-Q rule; on rotated samples and a 1080p frame they equal the oracle restatement (tests/sweep_oracle.py)
 byte for byte and recover the tilt within one slot; the pipeline replays on the C oracle with eyes at each face's angle."""
 import ctypes as C
-import os
-import subprocess
 import threading
 
 import numpy as np
 import pytest
 
-import oracle_lib as O
 import pigo_b200
+import pipeline_oracle as P
 import sweep_oracle as S
+from mixed_images import (CLI_PARAMS, DOC_PARAMS, MIXED, NCALLS, TEST_PARAMS, cascades, cp_of, image_of, images, make_image,  # noqa: F401 (fixtures)
+                          randoms_for, run_cpp_mirror, same)
 from pigo_b200 import ImageParams, pipeline
 from option_guard import options, options_at_defaults   # noqa: F401 (autouse: every test ends with the options at their defaults)
-from test_images_gpu import CLI_PARAMS, DOC_PARAMS, MIXED, TEST_PARAMS, cp_of, make_image
-from test_detect_images_gpu import GEOMS, NCALLS, make_image as make_pipeline_image, randoms_for
+from synthetic import synthetic_cascade
 
 pytestmark = pytest.mark.gpu
 
@@ -83,60 +82,23 @@ def test_rotated_samples_and_a_1080p_frame_equal_the_oracle(gpu_face, oracle_fac
 
 
 # ---- pipeline ----------------------------------------------------------------------------------------------------------
-@pytest.fixture(scope="module")
-def cascades():
-    plc = pigo_b200.NewPuplocCascade().UnpackCascade(pigo_b200.load_cascade("puploc"))
-    names = sorted(set(pipeline.EYE_CASCADES + pipeline.MOUTH_CASCADES))
-    flp = {n: pigo_b200.NewPuplocCascade().UnpackCascade(pigo_b200.load_cascade("lps/" + n)) for n in names}
-    oplc = O.OraclePuploc(pigo_b200.load_cascade("puploc"))
-    oflp = {n: O.OraclePuploc(pigo_b200.load_cascade("lps/" + n)) for n in names}
-    return plc, flp, oplc, oflp
-
-
-@pytest.fixture(scope="module")
-def images():
-    return [make_pipeline_image(r, c, d, k, 21 + i) for i, (r, c, d, k) in enumerate(GEOMS)]
-
-
 def sweep(gpu_face, cascades, ims, angles, **kw):
     plc, flp, _, _ = cascades
     return pipeline.detect_images_sweep_device(gpu_face, plc, flp, ims, cp_of(TEST_PARAMS), angles, raw=True, **kw)
 
 
-def same(a, b):
-    return all(x.tobytes() == y.tobytes() for x, y in zip(a, b))
-
-
 def test_pipeline_replays_on_the_oracle(gpu_face, oracle_face, cascades, tilted, frame1080):
     """Faces and angle indices equal the oracle sweep; eyes replay on the C oracle at angles[face_angle], landmarks at 0."""
-    _, _, oplc, oflp = cascades
     ims = tilted + [frame1080]
     fcap, eye = 32, 50
     rnd = randoms_for(len(ims), fcap, 47)
     faces, nfaces, points, fangle = sweep(gpu_face, cascades, ims, ANGLES, face_cap=fcap, randoms=rnd, eye_perturbs=eye)
-    calls = pipeline.landmark_calls()
-    rotated = 0
+    cases = []
     for i, im in enumerate(ims):
-        px, r, c, d = im.Pixels, im.Rows, im.Cols, im.Dim
-        cl, ix = S.sweep_oracle(oracle_face, (px, r, c, d), ANGLES, TEST_PARAMS, 0.1)
-        assert int(nfaces[i]) == len(cl) and faces[i, :len(cl)].tobytes() == cl.tobytes(), i
+        cl, ix = S.sweep_oracle(oracle_face, image_of(im), ANGLES, TEST_PARAMS, 0.1)
         assert np.array_equal(fangle[i, :len(cl)], ix), i
-        for k, f in enumerate(cl):
-            if f["scale"] <= 50:
-                continue
-            a = ANGLES[ix[k]]
-            rotated += a > 0
-            pts = points[i, k]
-            ls, rs = pipeline.eye_seeds(int(f["row"]), int(f["col"]), int(f["scale"]), eye)
-            le = oplc.run_detector(ls.Row, ls.Col, ls.Scale, eye, rnd[i, k, 0], px, r, c, d, a)
-            re_ = oplc.run_detector(rs.Row, rs.Col, rs.Scale, eye, rnd[i, k, 1], px, r, c, d, a)
-            for p, e in ((pts[0], le), (pts[1], re_)):
-                assert (int(p["row"]), int(p["col"]), np.float32(p["scale"])) == (e[0], e[1], np.float32(e[2])), (i, k)
-            r0, c0, s0 = O.landmark_seed(le[0], le[1], re_[0], re_[1])
-            for ci, (name, flip) in enumerate(calls):
-                e = oflp[name].run_detector(r0, c0, float(s0), 63, rnd[i, k, 2 + ci], px, r, c, d, 0.0, flip)
-                p = pts[2 + ci]
-                assert (int(p["row"]), int(p["col"]), np.float32(p["scale"])) == (e[0], e[1], np.float32(e[2])), (i, k, ci)
+        cases.append((i, image_of(im), cl, [ANGLES[j] for j in ix]))
+    _, rotated = P.replay(cascades[2:], cases, lambda i, k, slot: rnd[i, k, slot], eye, (faces, nfaces, points))
     assert rotated >= 2, rotated
 
 
@@ -258,8 +220,7 @@ def test_fallback_scans_give_the_same_outputs(gpu_face, cascades, tilted, knobs)
 
 
 def test_cascade_of_another_depth(tilted):
-    from test_oracle_pins import _synthetic_cascade
-    face = pigo_b200.NewPigo().Unpack(_synthetic_cascade(4, 9, seed=409))
+    face = pigo_b200.NewPigo().Unpack(synthetic_cascade(4, 9, seed=409))
     angles, params = ANGLES[::8], (60, 1000, 0.3, 1.2)   # a cascade that fires often: few windows keep the merged lists short
     got = face.RunCascadeImagesSweep(tilted[:2], cp_of(params), angles, 0.1)
     assert_sweep(got, reference_sweep(face, tilted[:2], angles, params, 0.1))
@@ -292,8 +253,4 @@ def test_concurrent_calls_on_one_classifier(gpu_face, tilted, frame1080):
 def test_cpp_mirror_sweep():
     """tests/cpp/test_sweep.cpp (built by build()): the sample swept through DetectImagesSweep passes the reference's
     landmark assertions, and RunCascadeImagesSweep agrees with it and, at one angle, with ClusterDetections of RunCascade."""
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    exe = os.path.join(root, "tests", "cpp", "test_sweep")
-    assert os.path.exists(exe), "run __graft_entry__.build() first"
-    p = subprocess.run([exe, root], capture_output=True, text=True, timeout=300)
-    assert p.returncode == 0, p.stdout + p.stderr
+    run_cpp_mirror("test_sweep")
