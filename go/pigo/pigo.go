@@ -371,6 +371,40 @@ func (pg *Pigo) RunCascadeImagesSharded(images []ImageParams, cp CascadeParams, 
 	})
 }
 
+// RunCascadeImagesParams runs the list of reference calls RunCascade(cps[i], angles[i]) as one call
+// (pigo_run_cascade_images_params): each CascadeParams carries its own ImageParams, MinSize, MaxSize, ShiftFactor and
+// ScaleFactor, and result[i] is what RunCascade(cps[i], angles[i]) returns.  angles is nil (every image unrotated) or has
+// one entry per image; any other length panics.  A pixel slice listed several times is copied once.
+func (pg *Pigo) RunCascadeImagesParams(cps []CascadeParams, angles []float64) [][]Detection {
+	n := len(cps)
+	if angles != nil && len(angles) != n {
+		panic("pigo: RunCascadeImagesParams needs nil angles or one angle per image")
+	}
+	if n == 0 {
+		return nil
+	}
+	images, prm, freePrm := cascadeParams(cps)
+	defer freePrm()
+	desc, free := packImages(images)
+	defer free()
+	return runCapped(n, func(buf *C.pigo_det, capacity C.int, cnt *C.int) C.int {
+		return C.pigo_run_cascade_images_params(pg.h, &desc[0], C.int(n), &prm[0], anglesPtr(angles), buf, capacity, cnt, C.PIGO_MEM_HOST, nil)
+	})
+}
+
+// cascadeParams splits cps into their images and their pigo_cascade_params (in C memory); free releases the latter.
+func cascadeParams(cps []CascadeParams) (images []ImageParams, prm []C.pigo_cascade_params, free func()) {
+	n := len(cps)
+	images = make([]ImageParams, n)
+	prm = unsafe.Slice((*C.pigo_cascade_params)(C.malloc(C.size_t(n)*C.size_t(unsafe.Sizeof(C.pigo_cascade_params{})))), n)
+	for i, cp := range cps {
+		images[i] = cp.ImageParams
+		prm[i] = C.pigo_cascade_params{min_size: C.int32_t(cp.MinSize), max_size: C.int32_t(cp.MaxSize), shift_factor: C.double(cp.ShiftFactor),
+			scale_factor: C.double(cp.ScaleFactor)}
+	}
+	return images, prm, func() { C.free(unsafe.Pointer(&prm[0])) }
+}
+
 // anglesPtr is the C view of angles (nil stays NULL).
 func anglesPtr(angles []float64) *C.double {
 	if len(angles) == 0 {

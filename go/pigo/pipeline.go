@@ -265,6 +265,57 @@ func (pg *Pigo) DetectImagesAngles(plc *PuplocCascade, calls []LandmarkCall, ima
 	}
 }
 
+// DetectImagesParams is DetectImagesAngles with every image's own CascadeParams (pigo_detect_images_params): image i is
+// cps[i].ImageParams, scanned with cps[i]'s MinSize, MaxSize, ShiftFactor and ScaleFactor, and its eyes are refined at
+// angles[i] (nil: every image unrotated; any other length than one per image panics).  pp.IoU, pp.MinFaceScale and both
+// perturbs are shared by every image; pp.Angle and pp.Sharded are not used.  A pixel slice listed several times is copied
+// once.
+func (pg *Pigo) DetectImagesParams(plc *PuplocCascade, calls []LandmarkCall, cps []CascadeParams, pp PipelineParams, angles []float64) [][]FaceResult {
+	n := len(cps)
+	if angles != nil && len(angles) != n {
+		panic("pigo: DetectImagesParams needs nil angles or one angle per image")
+	}
+	if n == 0 {
+		return nil
+	}
+	images, cprm, freePrm := cascadeParams(cps)
+	defer freePrm()
+	desc, free := packImages(images)
+	defer free()
+	ncalls := len(calls)
+	hs, fl := callArrays(calls)
+	defer C.free(unsafe.Pointer(hs))
+	prm := C.pigo_pipeline_params{iou_threshold: C.double(pp.IoU), min_face_scale: C.int32_t(pp.MinFaceScale), eye_perturbs: C.int32_t(pp.EyePerturbs),
+		flp_perturbs: C.int32_t(pp.FlpPerturbs)}
+	key := atomic.AddUint64(&plc.seed, 1)
+	faceCap := 32
+	for {
+		faces := make([]C.pigo_det, n*faceCap)
+		nfaces := make([]C.int, n)
+		points := make([]C.pigo_point, n*faceCap*(2+ncalls))
+		rc, err := call(func() C.int {
+			return C.pigo_detect_images_params(pg.h, plc.h, hs, &fl[0], C.int(ncalls), &desc[0], C.int(n), &cprm[0], anglesPtr(angles), &prm, nil,
+				C.uint64_t(key), &faces[0], C.int(faceCap), &nfaces[0], &points[0], C.PIGO_MEM_HOST, nil)
+		})
+		if rc == C.PIGO_E_CAP {
+			grown := false
+			for _, c := range nfaces {
+				if int(c) > faceCap {
+					faceCap, grown = int(c), true
+				}
+			}
+			if !grown {
+				prm.det_cap = 4 * (prm.det_cap + 512) // raw detections per image exceeded det_cap
+			}
+			continue
+		}
+		if err != nil {
+			panic(err)
+		}
+		return faceResults(faces, nfaces, points, faceCap, ncalls, pp.MinFaceScale)
+	}
+}
+
 // SweepFace is one merged face of DetectImagesSweep and the angle it was found at (the value the caller listed); its eyes
 // were refined at that angle.
 type SweepFace struct {

@@ -163,6 +163,26 @@ int pigo_run_cascade_images_angles(const pigo_cascade *c, const pigo_image *imag
                                    int min_size, int max_size, double shift_factor, double scale_factor, pigo_det *out,
                                    int cap_per_image, int *n_out, unsigned flags, void *stream);
 
+/* pigo.CascadeParams without its ImageParams (core/pigo.go:16-27). */
+typedef struct {
+  int32_t min_size, max_size;
+  double shift_factor, scale_factor;
+} pigo_cascade_params;
+
+/* Per-image CascadeParams: a list of RunCascade(cp, angle) calls is one call.  Image i is scanned with params[i] (a host
+ * array of nimages entries, required when nimages > 0) at angles[i] (a host array of nimages doubles, rules as
+ * pigo_run_cascade_images_angles; NULL = every image unrotated).  out[i][0..n_out[i]) is byte for byte what
+ * pigo_run_cascade returns for image i alone with params[i] and angles[i]; with every params[i] equal, the call is
+ * pigo_run_cascade_images_angles with those values, byte for byte.  The rotated images keep one node table per distinct
+ * (int(32*a), min_size, scale_factor) on the device, each over the longest ladder of that key (MaxSize, ShiftFactor and
+ * geometry only shorten a ladder); past 1 GiB of tables they run in several passes.  Each image's parameters go through
+ * the checks pigo_run_cascade applies, before any device work: a failure is PIGO_E_INVALID with a message that names the
+ * image.  Everything else, including the other errors, as pigo_run_cascade_images; a null `params` with nimages > 0
+ * fails with PIGO_E_INVALID. */
+int pigo_run_cascade_images_params(const pigo_cascade *c, const pigo_image *images, int nimages,
+                                   const pigo_cascade_params *params, const double *angles, pigo_det *out,
+                                   int cap_per_image, int *n_out, unsigned flags, void *stream);
+
 /* Multi-GPU form of the batch call: HOST frames (pinned memory from pigo_alloc_pinned recommended), sharded over
  * the devices of pigo_init_devices, one host thread and one stream per device, no data-path collective; every
  * device writes its frames' slices of `out` / `n_out`, so the result is identical to the single-GPU call.
@@ -280,6 +300,20 @@ int pigo_detect_images_angles(const pigo_cascade *face, const pigo_puploc *puplo
                               const uint8_t *flp_flip, int ncalls, const pigo_image *images, int nimages,
                               const double *angles, const pigo_pipeline_params *params, const float *randoms,
                               uint64_t rng_seed, pigo_det *faces, int face_cap, int *n_faces, pigo_point *points,
+                              unsigned flags, void *stream);
+
+/* Per-image CascadeParams: pigo_detect_images with cparams[i] and angles[i] in place of the scan fields of `params`
+ * (min_size, max_size, shift_factor, scale_factor) and params->angle for image i.  Those fields of `params` are ignored
+ * and not checked; iou_threshold, min_face_scale, both perturbs and det_cap stay shared.  `cparams` is a host array of
+ * nimages entries (required when nimages > 0); `angles` (may be NULL: every image unrotated) follows the rules of
+ * pigo_run_cascade_images_params.  Outputs, randoms layout, generator key, PIGO_E_CAP, flags and stream as
+ * pigo_detect_images, so with every cparams[i] equal the call is pigo_detect_images_angles byte for byte.  Invalid
+ * arguments as pigo_detect_images and pigo_run_cascade_images_params. */
+int pigo_detect_images_params(const pigo_cascade *face, const pigo_puploc *puploc, const pigo_puploc *const *flp,
+                              const uint8_t *flp_flip, int ncalls, const pigo_image *images, int nimages,
+                              const pigo_cascade_params *cparams, const double *angles,
+                              const pigo_pipeline_params *params, const float *randoms, uint64_t rng_seed,
+                              pigo_det *faces, int face_cap, int *n_faces, pigo_point *points,
                               unsigned flags, void *stream);
 
 /* ---- Angle sweep merged per image (additive).  A caller who does not know a photo's tilt scans it at several angles and

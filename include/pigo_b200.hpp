@@ -44,6 +44,15 @@ struct Puploc {                 // core/puploc.go:14-19
   int Perturbs = 0;
 };
 
+namespace detail {
+// the pigo_cascade_params of cps
+inline std::vector<pigo_cascade_params> params_of(const std::vector<CascadeParams>& cps) {
+  std::vector<pigo_cascade_params> prm;
+  for (const CascadeParams& cp : cps) prm.push_back(pigo_cascade_params{cp.MinSize, cp.MaxSize, cp.ShiftFactor, cp.ScaleFactor});
+  return prm;
+}
+}  // namespace detail
+
 inline void check(int rc) {
   if (rc != PIGO_OK) throw std::runtime_error(std::string("libpigo_b200: ") + pigo_last_error());
 }
@@ -155,22 +164,35 @@ class Pigo {                    // core/pigo.go:37-43
       return out;
     }
   }
+  // additive: the list of calls RunCascade(cps[i], angles[i]) as one call (pigo_run_cascade_images_params): each
+  // CascadeParams carries its own Image, MinSize, MaxSize, ShiftFactor and ScaleFactor; result i is what that RunCascade
+  // returns.  angles is empty (every image unrotated) or has one entry per image.
+  std::vector<std::vector<Detection>> RunCascadeImagesParams(const std::vector<CascadeParams>& cps, const std::vector<double>& angles = {}) const {
+    if (!angles.empty() && angles.size() != cps.size()) throw std::invalid_argument("RunCascadeImagesParams needs no angles or one angle per image");
+    std::vector<ImageParams> images;
+    for (const CascadeParams& cp : cps) images.push_back(cp.Image);
+    const std::vector<pigo_cascade_params> prm = detail::params_of(cps);
+    return runImages(images, CascadeParams{}, angles, false, prm.data());
+  }
   const pigo_cascade* handle() const { return h_.get(); }
 
  private:
+  // images with cp's parameters, or (params not null) image i with params[i]; angles empty = NULL
   std::vector<std::vector<Detection>> runImages(const std::vector<ImageParams>& images, const CascadeParams& cp, const std::vector<double>& angles,
-                                                bool sharded) const {
+                                                bool sharded, const pigo_cascade_params* params = nullptr) const {
     const int n = (int)images.size();
     std::vector<pigo_image> desc((size_t)n);
     for (int i = 0; i < n; ++i) desc[i] = pigo_image{images[i].Pixels, images[i].Rows, images[i].Cols, images[i].Dim};
+    const double* ang = angles.empty() ? nullptr : angles.data();
     int cap = 256;
     for (;;) {
       std::vector<pigo_det> buf((size_t)cap * (n > 0 ? n : 1));
       std::vector<int> cnt((size_t)(n > 0 ? n : 1));
-      const int rc = sharded ? pigo_run_cascade_images_sharded(h_.get(), desc.data(), n, angles.data(), cp.MinSize, cp.MaxSize, cp.ShiftFactor,
-                                                               cp.ScaleFactor, buf.data(), cap, cnt.data())
-                             : pigo_run_cascade_images_angles(h_.get(), desc.data(), n, angles.data(), cp.MinSize, cp.MaxSize, cp.ShiftFactor,
-                                                              cp.ScaleFactor, buf.data(), cap, cnt.data(), PIGO_MEM_HOST, nullptr);
+      const int rc = params ? pigo_run_cascade_images_params(h_.get(), desc.data(), n, params, ang, buf.data(), cap, cnt.data(), PIGO_MEM_HOST, nullptr)
+                     : sharded ? pigo_run_cascade_images_sharded(h_.get(), desc.data(), n, ang, cp.MinSize, cp.MaxSize, cp.ShiftFactor,
+                                                                 cp.ScaleFactor, buf.data(), cap, cnt.data())
+                               : pigo_run_cascade_images_angles(h_.get(), desc.data(), n, ang, cp.MinSize, cp.MaxSize, cp.ShiftFactor,
+                                                                cp.ScaleFactor, buf.data(), cap, cnt.data(), PIGO_MEM_HOST, nullptr);
       if (rc == PIGO_E_CAP) { for (int c : cnt) cap = c > cap ? c : cap; continue; }
       check(rc);
       std::vector<std::vector<Detection>> out((size_t)n);
@@ -270,7 +292,8 @@ inline std::vector<std::vector<FaceResult>> detectImages(const Pigo& face, const
                                                          const std::vector<std::pair<const PuplocCascade*, bool>>& calls,
                                                          const std::vector<ImageParams>& images, const CascadeParams& cp, double iou,
                                                          int min_face_scale, int eye_perturbs, int flp_perturbs, uint64_t rng_seed,
-                                                         const std::vector<double>& angles, int face_cap, bool sharded) {
+                                                         const std::vector<double>& angles, int face_cap, bool sharded,
+                                                         const pigo_cascade_params* cparams = nullptr) {
   const int ncalls = (int)calls.size(), n = (int)images.size();
   std::vector<const pigo_puploc*> hs;
   std::vector<uint8_t> fl;
@@ -284,9 +307,12 @@ inline std::vector<std::vector<FaceResult>> detectImages(const Pigo& face, const
     std::vector<pigo_det> faces((size_t)(n > 0 ? n : 1) * face_cap);
     std::vector<int> nfaces((size_t)(n > 0 ? n : 1));
     std::vector<pigo_point> pts((size_t)(n > 0 ? n : 1) * face_cap * (2 + ncalls));
-    const int rc = sharded ? pigo_detect_images_sharded(face.handle(), plc.handle(), hs.data(), fl.data(), ncalls, desc.data(), n, angles.data(), &prm,
-                                                        nullptr, rng_seed, faces.data(), face_cap, nfaces.data(), pts.data())
-                           : pigo_detect_images_angles(face.handle(), plc.handle(), hs.data(), fl.data(), ncalls, desc.data(), n, angles.data(), &prm,
+    const double* ang = angles.empty() ? nullptr : angles.data();
+    const int rc = cparams ? pigo_detect_images_params(face.handle(), plc.handle(), hs.data(), fl.data(), ncalls, desc.data(), n, cparams, ang, &prm,
+                                                       nullptr, rng_seed, faces.data(), face_cap, nfaces.data(), pts.data(), PIGO_MEM_HOST, nullptr)
+                   : sharded ? pigo_detect_images_sharded(face.handle(), plc.handle(), hs.data(), fl.data(), ncalls, desc.data(), n, angles.data(), &prm,
+                                                          nullptr, rng_seed, faces.data(), face_cap, nfaces.data(), pts.data())
+                             : pigo_detect_images_angles(face.handle(), plc.handle(), hs.data(), fl.data(), ncalls, desc.data(), n, angles.data(), &prm,
                                                        nullptr, rng_seed, faces.data(), face_cap, nfaces.data(), pts.data(), PIGO_MEM_HOST, nullptr);
     if (rc == PIGO_E_CAP) {
       bool grown = false;
@@ -325,6 +351,21 @@ inline std::vector<std::vector<FaceResult>> DetectImagesAngles(const Pigo& face,
                                                                const std::vector<double>& angles, int face_cap = 32) {
   if (angles.size() != images.size()) throw std::invalid_argument("DetectImagesAngles needs one angle per image");
   return detail::detectImages(face, plc, calls, images, cp, iou, min_face_scale, eye_perturbs, flp_perturbs, rng_seed, angles, face_cap, false);
+}
+// additive: DetectImagesAngles with every image's own CascadeParams (pigo_detect_images_params): image i is cps[i].Image, scanned
+// with cps[i]'s MinSize, MaxSize, ShiftFactor and ScaleFactor and refined at angles[i] (empty: every image unrotated); iou, the
+// face scale and the perturbs stay shared.  PIGO_E_CAP is retried as in DetectImagesAngles.
+inline std::vector<std::vector<FaceResult>> DetectImagesParams(const Pigo& face, const PuplocCascade& plc,
+                                                               const std::vector<std::pair<const PuplocCascade*, bool>>& calls,
+                                                               const std::vector<CascadeParams>& cps, double iou, int min_face_scale, int eye_perturbs,
+                                                               int flp_perturbs, uint64_t rng_seed, const std::vector<double>& angles = {},
+                                                               int face_cap = 32) {
+  if (!angles.empty() && angles.size() != cps.size()) throw std::invalid_argument("DetectImagesParams needs no angles or one angle per image");
+  std::vector<ImageParams> images;
+  for (const CascadeParams& cp : cps) images.push_back(cp.Image);
+  const std::vector<pigo_cascade_params> prm = detail::params_of(cps);
+  return detail::detectImages(face, plc, calls, images, CascadeParams{}, iou, min_face_scale, eye_perturbs, flp_perturbs, rng_seed, angles, face_cap,
+                              false, prm.data());
 }
 // additive: DetectImagesAngles over the GPUs of InitDevices (host pixels, contiguous shards of about equal modelled cost); the
 // result, generator keys included, equals the single-GPU call's

@@ -49,6 +49,7 @@ ABI_SYMBOLS = [
     "pigo_run_cascade_images_angles", "pigo_detect_images_angles", "pigo_gray_images", "pigo_cascade_block_table",
     "pigo_run_cascade_images_sharded", "pigo_detect_images_sharded", "pigo_run_cascade_decoded_sharded", "pigo_detect_decoded_sharded",
     "pigo_shard_plan", "pigo_describe_plan_frames", "pigo_run_cascade_images_sweep", "pigo_detect_images_sweep",
+    "pigo_run_cascade_images_params", "pigo_detect_images_params",
 ]
 
 
@@ -128,6 +129,8 @@ def lib() -> C.CDLL:
         L.pigo_shard_plan.argtypes = [vp, i, vp, i, i, d, d, i, vp, C.POINTER(i)]
         L.pigo_run_cascade_images_sweep.argtypes = [vp, vp, i, vp, i, i, i, d, d, d, i, vp, vp, i, vp, C.c_uint, vp]
         L.pigo_detect_images_sweep.argtypes = [vp, vp, vp, vp, i, vp, i, vp, i, vp, vp, u64, vp, vp, i, vp, vp, C.c_uint, vp]
+        L.pigo_run_cascade_images_params.argtypes = [vp, vp, i, vp, vp, vp, i, vp, C.c_uint, vp]
+        L.pigo_detect_images_params.argtypes = [vp, vp, vp, vp, i, vp, i, vp, vp, vp, vp, u64, vp, i, vp, vp, C.c_uint, vp]
         _lib = L
     return _lib
 
@@ -243,6 +246,20 @@ def image_descs(items) -> C.Array:
     arr = (PigoImage * max(len(items), 1))()
     for k, (p, r, c, d) in enumerate(items):
         arr[k] = PigoImage(p, r, c, d)
+    return arr
+
+
+class PigoCascadeParams(C.Structure):
+    """pigo_cascade_params (include/pigo_b200.h): pigo.CascadeParams without its ImageParams."""
+    _fields_ = [("min_size", C.c_int32), ("max_size", C.c_int32), ("shift_factor", C.c_double), ("scale_factor", C.c_double)]
+
+
+def cascade_params_array(items) -> C.Array:
+    """[CascadeParams or (MinSize, MaxSize, ShiftFactor, ScaleFactor)] -> the pigo_cascade_params array of a per-image-parameter
+    call (the CascadeParams' ImageParams are not read here)."""
+    arr = (PigoCascadeParams * max(len(items), 1))()
+    for k, cp in enumerate(items):
+        arr[k] = PigoCascadeParams(cp.MinSize, cp.MaxSize, cp.ShiftFactor, cp.ScaleFactor) if isinstance(cp, CascadeParams) else PigoCascadeParams(*cp)
     return arr
 
 
@@ -427,6 +444,31 @@ class Pigo:
         ang = np.ascontiguousarray(angles, dtype=np.float64)
         _check(lib().pigo_run_cascade_images_angles(self._h, image_descs(images), len(images), ang.ctypes.data, min_size, max_size, shift, scale,
                                                     out_ptr, cap_per_image, counts_ptr, FRAMES_DEVICE | OUT_DEVICE, stream or None))
+
+    def RunCascadeImagesParams(self, cps: Sequence[CascadeParams], angles: Optional[Sequence[float]] = None, cap_per_image: int = 1024):
+        """A list of RunCascade(cps[i], angles[i]) calls as one call (pigo_run_cascade_images_params): every CascadeParams carries
+        its own ImageParams, MinSize, MaxSize, ShiftFactor and ScaleFactor; angles None = every image unrotated.  Pixels as
+        RunCascadeImages.  Returns (dets[N, cap] DET_DTYPE, counts[N])."""
+        self._need()
+        n = len(cps)
+        desc, flags, keep = _image_table([cp.ImageParams for cp in cps])
+        prm = cascade_params_array(cps)
+        ang = _angles_array(angles, n)
+        return self._retry_cap(n, cap_per_image, lambda out, cap, cnt: lib().pigo_run_cascade_images_params(
+            self._h, desc, n, prm, ang.ctypes.data if ang is not None else None, out, cap, cnt, flags, None))
+
+    def run_cascade_images_params_device(self, images, params, angles: Optional[Sequence[float]], out_ptr: int, cap_per_image: int,
+                                         counts_ptr: int, stream: int = 0):
+        """Device-resident, asynchronous form of RunCascadeImagesParams: images = [(device pointer, rows, cols, dim)], params one
+        (MinSize, MaxSize, ShiftFactor, ScaleFactor) or CascadeParams per image, angles a host sequence or None, out [N][cap] and
+        counts [N] device pointers; no host sync."""
+        self._need()
+        if len(params) != len(images):
+            raise ValueError("params must have one entry per image")
+        ang = _angles_array(angles, len(images))
+        _check(lib().pigo_run_cascade_images_params(self._h, image_descs(images), len(images), cascade_params_array(params),
+                                                    ang.ctypes.data if ang is not None else None, out_ptr, cap_per_image, counts_ptr,
+                                                    FRAMES_DEVICE | OUT_DEVICE, stream or None))
 
     def RunCascadeImagesSweep(self, images: Sequence[ImageParams], cp: CascadeParams, angles: Sequence[float], iou: float, det_cap: int = 0,
                               cap_per_image: int = 256):

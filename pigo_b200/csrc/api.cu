@@ -578,45 +578,46 @@ static int check_images_args(const pigo_cascade* c, const pigo_image* images, in
   return PIGO_OK;
 }
 
-// The ladders of a mixed-size call's images (host only).  `longest` = the first image with the strictly longest ladder;
-// every other ladder is a prefix of it (the rotated node table and the meaning of a ladder index are shared by the whole call).
+// The CascadeParams and ladders of a mixed-size call's entries (host only).  Each entry has its own parameters; the
+// calls that share one set fill every entry with it.
 struct ImagePlans {
+  std::vector<pigo_cascade_params> params;
   std::vector<std::vector<ScaleEntry>> plans;
   std::vector<uint64_t> wins;
-  int longest = 0;
-  // The ladders of entries [lo, lo+n), the shard of a sharded call that starts at entry lo.
+  // The entries [lo, lo+n), the shard of a sharded call that starts at entry lo.
   ImagePlans slice(int lo, int n) const {
     ImagePlans s;
+    s.params.assign(params.begin() + lo, params.begin() + lo + n);
     s.plans.assign(plans.begin() + lo, plans.begin() + lo + n);
     s.wins.assign(wins.begin() + lo, wins.begin() + lo + n);
-    for (int i = 0; i < n; ++i)
-      if (s.plans[i].size() > s.plans[s.longest].size()) s.longest = i;
     return s;
   }
 };
 
-static int build_image_plans(const pigo_image* images, int nimages, int min_size, int max_size, double shift, double scale_factor, ImagePlans& ip) {
-  auto& plans = ip.plans;
-  plans.assign(nimages, {});
+// n copies of the CascadeParams (min_size, max_size, shift_factor, scale_factor), held in `store`.  An n outside 0..65535
+// is refused by the argument checks before any entry is read: no more than 65535 copies are made.
+static const pigo_cascade_params* uniform_params(int min_size, int max_size, double shift_factor, double scale_factor, int n,
+                                                 std::vector<pigo_cascade_params>& store) {
+  store.assign(std::min(std::max(n, 0), 65535), pigo_cascade_params{min_size, max_size, shift_factor, scale_factor});
+  return store.data();
+}
+
+// Entry i's ladder from params[i]; a ladder pigo_run_cascade rejects fails with a message naming image i / per_image (an
+// angle sweep lists each image per_image = nangles times).
+static int build_image_plans(const pigo_image* images, int nimages, const pigo_cascade_params* params, ImagePlans& ip, int per_image = 1) {
+  ip.params.assign(params, params + nimages);
+  ip.plans.assign(nimages, {});
   ip.wins.assign(nimages, 0);
-  int& longest = ip.longest;
-  longest = 0;
   for (int i = 0; i < nimages; ++i) {
-    int rc = build_plan(images[i].rows, images[i].cols, min_size, max_size, shift, scale_factor, plans[i], ip.wins[i]);
-    if (rc) return rc;
-    if (plans[i].size() > plans[longest].size()) longest = i;
+    const pigo_cascade_params& p = params[i];
+    const int rc = build_plan(images[i].rows, images[i].cols, p.min_size, p.max_size, p.shift_factor, p.scale_factor, ip.plans[i], ip.wins[i]);
+    if (rc) return set_err(rc, "image %d: %s", i / per_image, g_err.c_str());
   }
-  for (int i = 0; i < nimages; ++i)
-    for (size_t k = 0; k < plans[i].size(); ++k) {
-      const ScaleEntry &a = plans[i][k], &b = plans[longest][k];
-      if (a.s != b.s || a.step != b.step || a.off != b.off)
-        return set_err(PIGO_E_INVALID, "image %d: ladder entry %zu is not shared with the longest ladder", i, k);
-    }
   return PIGO_OK;
 }
 
-// Bound on the rotated node tables one pass of a mixed-size call keeps on the device (one table per distinct slot, each
-// over the call's longest ladder, at most 512 MB).  A call whose slots need more runs its rotated images in several passes.
+// Bound on the rotated node tables one pass of a mixed-size call keeps on the device (one table per distinct slot and
+// ladder key, each at most 512 MB).  A call whose tables need more runs its rotated images in several passes.
 static constexpr size_t kImagesRotBytes = (size_t)1 << 30;
 
 // The items of a call in one arena of 256-byte-aligned slots of bytes(item) bytes.  Items whose key(item) repeats an earlier
@@ -672,31 +673,56 @@ static size_t arena_layout(const pigo_decoded* src, int n, std::vector<size_t>& 
                       [](const pigo_decoded& d) { return (size_t)d.width * d.height; }, off, first);
 }
 
-// Image i is scanned at angles[i].  The rotated and the unrotated scan are different kernel variants, so the images run
-// in passes: the unrotated images in caller order, then the rotated ones ordered by (slot, caller index), cut into
-// passes of at most kImagesRotBytes of node tables.  That order does not depend on how the caller interleaves images and
-// angles.  Each pass is grouped and scheduled from its own windows; finalize writes every image to its caller index.
-static int scan_images_on(pigo_cascade* c, int dev, const pigo_image* images, int nimages, const ImagePlans& ip, int min_size, int max_size,
-                          double shift_factor, double scale_factor, const double* angles, pigo_det* out, int cap_per_image, int* n_out,
-                          unsigned flags, void* stream_) {
+// Image i is scanned with ip.params[i] at angles[i].  The rotated and the unrotated scan are different kernel variants, so
+// the images run in passes: the unrotated images in caller order, then the rotated ones ordered by (slot, ladder key, caller
+// index), cut into passes of at most kImagesRotBytes of node tables.  That order does not depend on how the caller
+// interleaves images, parameters and angles.  A node table row depends only on the window size and the slot, and the
+// window sizes of a ladder only on (MinSize, ScaleFactor): the ladders of one key are prefixes of one another, so the
+// rotated images of one (slot, key) share one table over the longest ladder of that key in the call.  Each pass is
+// grouped and scheduled from its own windows; finalize writes every image to its caller index.
+static int scan_images_on(pigo_cascade* c, int dev, const pigo_image* images, int nimages, const ImagePlans& ip, const double* angles,
+                          pigo_det* out, int cap_per_image, int* n_out, unsigned flags, void* stream_) {
   int rc = PIGO_OK;
   FaceReplica* R = face_replica(c, dev, &rc);
   if (!R) return rc;
   if ((rc = use_device(dev))) return rc;
   const bool frames_dev = flags & PIGO_FRAMES_DEVICE, out_dev = flags & PIGO_OUT_DEVICE;
+  const size_t ntrees = (size_t)R->tab.ntrees;
+  // per image: rotation slot and ladder key; per key: the first image with its strictly longest ladder
+  using LadderKey = std::pair<int, uint64_t>;
   std::vector<int> slot(nimages);
+  std::vector<LadderKey> key(nimages);
+  std::map<LadderKey, int> longest;
   bool any_rot = false;
-  for (int i = 0; i < nimages; ++i) { slot[i] = rot_slot_of(angles[i]); any_rot |= slot[i] >= 0; }
-  const int nlad = (int)ip.plans[ip.longest].size();
-  const int max_scale = nlad > 0 ? ip.plans[ip.longest].back().s : 0;
-  const size_t rot_bytes = (size_t)nlad * (size_t)R->tab.ntrees * 64 * sizeof(RotNode);
-  if (!block_path(R, any_rot, max_scale, rot_bytes)) {
-    // cascades of depth != 6 and the universal-kernel options: the single-image path, image by image at its own angle
+  int max_scale = 0;
+  for (int i = 0; i < nimages; ++i) {
+    slot[i] = rot_slot_of(angles[i]);
+    any_rot |= slot[i] >= 0;
+    uint64_t bits;
+    memcpy(&bits, &ip.params[i].scale_factor, sizeof(bits));
+    key[i] = LadderKey{ip.params[i].min_size, bits};
+    const auto ins = longest.emplace(key[i], i);
+    if (ip.plans[i].size() > ip.plans[ins.first->second].size()) ins.first->second = i;
+    if (!ip.plans[i].empty()) max_scale = std::max(max_scale, ip.plans[i].back().s);
+  }
+  std::vector<int> src(nimages);   // the image whose ladder image i's node table is built over
+  for (int i = 0; i < nimages; ++i) src[i] = longest.at(key[i]);
+  auto table_of = [&](int i) {   // image i's node table (slot, key, length)
+    return RotTableKey{slot[i], key[i].first, (int)ip.plans[src[i]].size(), key[i].second};
+  };
+  auto table_bytes = [&](const RotTableKey& t) { return (size_t)t.len * ntrees * 64 * sizeof(RotNode); };
+  size_t max_table = 0;
+  for (int i = 0; i < nimages; ++i)
+    if (slot[i] >= 0) max_table = std::max(max_table, table_bytes(table_of(i)));
+  if (!block_path(R, any_rot, max_scale, max_table)) {
+    // cascades of depth != 6 and the universal-kernel options: the single-image path, image by image with its own
+    // parameters at its own angle
     int rc_cap = PIGO_OK;
     for (int i = 0; i < nimages; ++i) {
       const pigo_image& im = images[i];
-      rc = scan_batch_on(c, dev, im.pixels, 1, (size_t)im.rows * im.dim, im.rows, im.cols, im.dim, min_size, max_size, shift_factor,
-                         scale_factor, angles[i], out ? out + (size_t)i * cap_per_image : nullptr, cap_per_image, n_out + i, flags, stream_);
+      const pigo_cascade_params& p = ip.params[i];
+      rc = scan_batch_on(c, dev, im.pixels, 1, (size_t)im.rows * im.dim, im.rows, im.cols, im.dim, p.min_size, p.max_size, p.shift_factor,
+                         p.scale_factor, angles[i], out ? out + (size_t)i * cap_per_image : nullptr, cap_per_image, n_out + i, flags, stream_);
       if (rc == PIGO_E_CAP) rc_cap = rc;
       else if (rc) return rc;
     }
@@ -711,21 +737,35 @@ static int scan_images_on(pigo_cascade* c, int dev, const pigo_image* images, in
   // order[j] = caller index of the image at position j of the call's image table; passes are ranges of positions
   std::vector<int> order(nimages);
   std::iota(order.begin(), order.end(), 0);
-  std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return slot[a] < slot[b]; });
-  struct Pass { int first, n; std::vector<int> slots; };   // slots: the pass's node tables in order (empty = unrotated)
+  std::stable_sort(order.begin(), order.end(), [&](int a, int b) {
+    if (slot[a] != slot[b]) return slot[a] < slot[b];
+    return slot[a] >= 0 && key[a] < key[b];
+  });
+  // tables: the pass's node tables in order (empty = unrotated); src: the image whose ladder each table is built over;
+  // off: where each table starts in img_rot, in units of 64 RotNode records.  rot_off[i]: image i's table (ImageDesc.rot_off),
+  // the pass's last table when the image is reached, since a (slot, key) run is contiguous in `order`
+  struct Pass { int first, n; std::vector<RotTableKey> tables; std::vector<int> src; std::vector<uint32_t> off; size_t bytes; };
   std::vector<Pass> passes;
-  const size_t slots_per_pass = std::max<size_t>(1, kImagesRotBytes / std::max<size_t>(rot_bytes, 1));
+  std::vector<uint32_t> rot_off(nimages, 0);
   for (int j = 0; j < nimages; ++j) {
-    const int s = slot[order[j]];
-    const bool new_slot = j == 0 || s != slot[order[j - 1]];
-    if (j == 0 || (s >= 0 && slot[order[j - 1]] < 0) || (new_slot && s >= 0 && passes.back().slots.size() == slots_per_pass))
-      passes.push_back(Pass{j, 0, {}});
+    const int i = order[j], prev = j > 0 ? order[j - 1] : -1;
+    const bool new_table = slot[i] >= 0 && (j == 0 || slot[prev] != slot[i] || key[prev] != key[i]);
+    const RotTableKey t = new_table ? table_of(i) : RotTableKey{};
+    if (j == 0 || (slot[i] >= 0 && slot[prev] < 0) ||
+        (new_table && !passes.back().tables.empty() && passes.back().bytes + table_bytes(t) > kImagesRotBytes))
+      passes.push_back(Pass{j, 0, {}, {}, {}, 0});
     Pass& p = passes.back();
-    if (new_slot && s >= 0) p.slots.push_back(s);
+    if (new_table) {
+      p.off.push_back((uint32_t)(p.bytes / (64 * sizeof(RotNode))));
+      p.tables.push_back(t);
+      p.src.push_back(src[i]);
+      p.bytes += table_bytes(t);
+    }
+    if (slot[i] >= 0) rot_off[i] = p.off.back();
     p.n++;
   }
-  size_t max_tables = 0;
-  for (const Pass& p : passes) max_tables = std::max(max_tables, p.slots.size());
+  size_t max_pass_bytes = 0;
+  for (const Pass& p : passes) max_pass_bytes = std::max(max_pass_bytes, p.bytes);
 
   // per pass: schedule from the pass's windows; block prefixes per image, groups of consecutive images
   std::vector<ImageDesc> desc(nimages);
@@ -740,7 +780,7 @@ static int scan_images_on(pigo_cascade* c, int dev, const pigo_image* images, in
     for (int j = p.first; j < p.first + p.n; ++j) pass_windows += ip.wins[order[j]];
     // (gather-v2 is the whole scan here, as on the rotated path: large unrotated calls keep 24 trees, not run_scan's 16,
     // since the hand-over point was not re-measured for it)
-    sched[pi] = images_schedule(pass_windows, !p.slots.empty(), 24);
+    sched[pi] = images_schedule(pass_windows, !p.tables.empty(), 24);
     const int GB = 1 << sched[pi].gb_shift;
     // groups of about equal window counts (a uniform 1080p batch gets the uniform path's groups of 128)
     const uint64_t ngroups = std::max<uint64_t>(1, (pass_windows + kImagesGroupWindows - 1) / kImagesGroupWindows);
@@ -758,9 +798,7 @@ static int scan_images_on(pigo_cascade* c, int dev, const pigo_image* images, in
       d.plan_off = (uint32_t)plan_all.size();
       d.block_base = G.blocks;
       d.rot_slot = slot[i];
-      d.rot_off = 0;
-      if (slot[i] >= 0)
-        d.rot_off = (uint32_t)((std::find(p.slots.begin(), p.slots.end(), slot[i]) - p.slots.begin()) * (size_t)nlad * R->tab.ntrees);
+      d.rot_off = rot_off[i];
       d.out_index = i;
       uint32_t nb = 0;
       for (ScaleEntry e : ip.plans[i]) {
@@ -792,25 +830,26 @@ static int scan_images_on(pigo_cascade* c, int dev, const pigo_image* images, in
   CUDA_TRY(cudaMemcpyAsync(w->img_tab.p, tab.data(), tab.size(), cudaMemcpyHostToDevice, st));
   const ImageDesc* d_desc = (const ImageDesc*)w->img_tab.p;
   const ScaleEntry* d_plan = (const ScaleEntry*)((const uint8_t*)w->img_tab.p + desc_bytes);
-  const int longest_pos = (int)(std::find(order.begin(), order.end(), ip.longest) - order.begin());
-  // the node tables of a pass over the longest ladder, one per slot, cached per workspace by (slots, ladder)
-  if (max_tables > 0 && nlad > 0) {
+  std::vector<int> pos(nimages);   // position of each caller index in the image table
+  for (int j = 0; j < nimages; ++j) pos[order[j]] = j;
+  // the node tables of a pass, cached per workspace by the pass's list of (slot, key, length)
+  if (max_pass_bytes > 0) {
     const size_t cap0 = w->img_rot.cap;
-    if ((rc = w->img_rot.reserve(max_tables * rot_bytes))) { w->img_rot_slots.clear(); return rc; }
-    if (w->img_rot.cap != cap0) w->img_rot_slots.clear();   // a new buffer holds no tables
+    if ((rc = w->img_rot.reserve(max_pass_bytes))) { w->img_rot_tables.clear(); return rc; }
+    if (w->img_rot.cap != cap0) w->img_rot_tables.clear();   // a new buffer holds no tables
   }
-  auto build_tables = [&](const std::vector<int>& slots) -> int {
-    if (w->img_rot_slots == slots && w->img_rot_len == nlad && w->img_rot_min == min_size && w->img_rot_scale == scale_factor) return PIGO_OK;
-    w->img_rot_slots.clear();
+  auto build_tables = [&](const Pass& p) -> int {
+    if (w->img_rot_tables == p.tables) return PIGO_OK;
+    w->img_rot_tables.clear();
     timing_begin(T_ROTTAB, st);
-    for (size_t k = 0; k < slots.size(); ++k) {
-      launch_rot_table(R->tab, d_plan + desc[longest_pos].plan_off, nlad, slots[k], (RotNode*)w->img_rot.p + k * (size_t)nlad * R->tab.ntrees * 64,
+    for (size_t k = 0; k < p.tables.size(); ++k) {
+      launch_rot_table(R->tab, d_plan + desc[pos[p.src[k]]].plan_off, p.tables[k].len, p.tables[k].slot, (RotNode*)w->img_rot.p + (size_t)p.off[k] * 64,
                        R->num_sms * 8, st);
       g_launches++;
     }
     timing_end(T_ROTTAB, st);
     CUDA_TRY(cudaGetLastError());
-    w->img_rot_slots = slots; w->img_rot_len = nlad; w->img_rot_min = min_size; w->img_rot_scale = scale_factor;
+    w->img_rot_tables = p.tables;
     return PIGO_OK;
   };
 
@@ -836,8 +875,8 @@ static int scan_images_on(pigo_cascade* c, int dev, const pigo_image* images, in
     const Group& G = groups[k];
     if (G.windows == 0 || R->tab.ntrees == 0) continue;
     const Pass& p = passes[G.pass];
-    if (!p.slots.empty() && tables_of != G.pass) {
-      if ((rc = build_tables(p.slots))) return rc;
+    if (!p.tables.empty() && tables_of != G.pass) {
+      if ((rc = build_tables(p))) return rc;
       tables_of = G.pass;
     }
     int first_live = G.first;
@@ -848,8 +887,8 @@ static int scan_images_on(pigo_cascade* c, int dev, const pigo_image* images, in
     A.nframes = G.n;
     A.plan = d_plan;
     // the images kernels read only whether the pass is rotated; each image's node table comes from its ImageDesc
-    A.rot_slot = p.slots.empty() ? -1 : p.slots[0];
-    A.rot_tab = p.slots.empty() ? nullptr : (const RotNode*)w->img_rot.p;
+    A.rot_slot = p.tables.empty() ? -1 : p.tables[0].slot;
+    A.rot_tab = p.tables.empty() ? nullptr : (const RotNode*)w->img_rot.p;
     A.batch_frames = nimages;
     A.raw = (RawDet*)w->raw.p + (size_t)G.first * cap; A.raw_count = d_rawcount + G.first; A.cap = cap;
     A.images = d_desc + G.first; A.nimages = G.n;
@@ -1313,44 +1352,55 @@ static const double* angles_or(const double* angles, double angle, int n, std::v
   return store.data();
 }
 
-// The start of a mixed-size call after its argument checks: the ladders of its n scan entries (a sweep's expanded list),
-// the default device and the refusal of stream capture (`fn` names the entry point).  With n == 0 nothing more is to do.
-static int images_prologue(const char* fn, const pigo_image* images, int n, int min_size, int max_size, double shift_factor, double scale_factor,
-                           void* stream_, ImagePlans& ip) {
-  int rc = build_image_plans(images, n, min_size, max_size, shift_factor, scale_factor, ip);
+// The start of a mixed-size call after its argument checks: the ladders of its n scan entries (a sweep's expanded list,
+// per_image entries per image) from their parameters, the default device and the refusal of stream capture (`fn` names
+// the entry point).  With n == 0 nothing more is to do.
+static int images_prologue(const char* fn, const pigo_image* images, int n, const pigo_cascade_params* params, void* stream_, ImagePlans& ip,
+                           int per_image = 1) {
+  int rc = build_image_plans(images, n, params, ip, per_image);
   if (rc) return rc;
   if ((rc = ensure_device())) return rc;
   return refuse_capture(fn, stream_);
 }
 
-// pigo_run_cascade_images and pigo_run_cascade_images_angles: image i at angles[i] (nullptr: `angle` for every image).  `fn`
-// names the entry point in messages.
+// pigo_run_cascade_images, pigo_run_cascade_images_angles and pigo_run_cascade_images_params: image i with params[i] at
+// angles[i] (nullptr: `angle` for every image).  `fn` names the entry point in messages.
 static int run_cascade_images(const char* fn, const pigo_cascade* cc, const pigo_image* images, int nimages, const double* angles, double angle,
-                              int min_size, int max_size, double shift_factor, double scale_factor, pigo_det* out, int cap_per_image, int* n_out,
-                              unsigned flags, void* stream_) {
+                              const pigo_cascade_params* params, pigo_det* out, int cap_per_image, int* n_out, unsigned flags, void* stream_) {
   int rc = check_images_args(cc, images, nimages, out, cap_per_image, n_out);
   if (rc) return rc;
   ImagePlans ip;
   std::vector<double> uniform;
-  if ((rc = images_prologue(fn, images, nimages, min_size, max_size, shift_factor, scale_factor, stream_, ip)) || nimages == 0) return rc;
-  return scan_images_on(const_cast<pigo_cascade*>(cc), default_device(), images, nimages, ip, min_size, max_size, shift_factor, scale_factor,
-                        angles_or(angles, angle, nimages, uniform), out, cap_per_image, n_out, flags, stream_);
+  if ((rc = images_prologue(fn, images, nimages, params, stream_, ip)) || nimages == 0) return rc;
+  return scan_images_on(const_cast<pigo_cascade*>(cc), default_device(), images, nimages, ip, angles_or(angles, angle, nimages, uniform), out,
+                        cap_per_image, n_out, flags, stream_);
 }
 
 extern "C" {
 
 int pigo_run_cascade_images(const pigo_cascade* cc, const pigo_image* images, int nimages, int min_size, int max_size, double shift_factor,
                             double scale_factor, double angle, pigo_det* out, int cap_per_image, int* n_out, unsigned flags, void* stream_) {
-  return run_cascade_images("pigo_run_cascade_images", cc, images, nimages, nullptr, angle, min_size, max_size, shift_factor, scale_factor,
-                            out, cap_per_image, n_out, flags, stream_);
+  std::vector<pigo_cascade_params> prm;
+  return run_cascade_images("pigo_run_cascade_images", cc, images, nimages, nullptr, angle,
+                            uniform_params(min_size, max_size, shift_factor, scale_factor, nimages, prm), out, cap_per_image, n_out,
+                            flags, stream_);
 }
 
 int pigo_run_cascade_images_angles(const pigo_cascade* cc, const pigo_image* images, int nimages, const double* angles, int min_size,
                                    int max_size, double shift_factor, double scale_factor, pigo_det* out, int cap_per_image, int* n_out,
                                    unsigned flags, void* stream_) {
   if (nimages > 0 && !angles) return set_err(PIGO_E_INVALID, "null angles");
-  return run_cascade_images("pigo_run_cascade_images_angles", cc, images, nimages, angles, 0.0, min_size, max_size, shift_factor, scale_factor,
-                            out, cap_per_image, n_out, flags, stream_);
+  std::vector<pigo_cascade_params> prm;
+  return run_cascade_images("pigo_run_cascade_images_angles", cc, images, nimages, angles, 0.0,
+                            uniform_params(min_size, max_size, shift_factor, scale_factor, nimages, prm), out, cap_per_image, n_out,
+                            flags, stream_);
+}
+
+int pigo_run_cascade_images_params(const pigo_cascade* cc, const pigo_image* images, int nimages, const pigo_cascade_params* params,
+                                   const double* angles, pigo_det* out, int cap_per_image, int* n_out, unsigned flags, void* stream_) {
+  if (nimages > 0 && !params) return set_err(PIGO_E_INVALID, "null params");
+  return run_cascade_images("pigo_run_cascade_images_params", cc, images, nimages, angles, 0.0, params, out, cap_per_image, n_out, flags,
+                            stream_);
 }
 
 // Multi-GPU form (SURVEY.md section 8e): HOST frames are sharded over the devices of pigo_init_devices; every device
@@ -1711,8 +1761,8 @@ static int detect_batch_on(int dev, pigo_cascade* face, pigo_puploc* puploc, pig
 }
 
 // Mixed-size form: the images' pixels are staged once (stage_images) and both the images scan and the RunDetector stages
-// read them; `ip` holds the call's ladders (build_image_plans).  Image i is scanned and its eyes are refined at angles[i]
-// (P.angle is not used).  slot_base offsets the generator key as in detect_batch_on (a shard that starts at image lo of a
+// read them; `ip` holds the call's parameters and ladders (build_image_plans).  Image i is scanned with ip.params[i] and
+// its eyes are refined at angles[i] (the scan fields of P and P.angle are not used).  slot_base offsets the generator key as in detect_batch_on (a shard that starts at image lo of a
 // larger call passes lo*face_cap*(2+ncalls)).
 static int detect_images_on(int dev, pigo_cascade* face, pigo_puploc* puploc, pigo_puploc* const* flp, const uint8_t* flp_flip, int ncalls,
                             const pigo_image* images, int nimages, const double* angles, const ImagePlans& ip, const pigo_pipeline_params& P,
@@ -1724,8 +1774,7 @@ static int detect_images_on(int dev, pigo_cascade* face, pigo_puploc* puploc, pi
     int rc = stage_images(w, images, nimages, angles, frames_dev, st, &W.images, staged);
     if (rc) return rc;
     W.rot_slot = kRotSlotPerImage;
-    return scan_images_on(face, dev, staged.data(), nimages, ip, P.min_size, P.max_size, P.shift_factor, P.scale_factor, angles, d_dets,
-                          det_cap, d_cnt, PIGO_FRAMES_DEVICE | PIGO_OUT_DEVICE, st);
+    return scan_images_on(face, dev, staged.data(), nimages, ip, angles, d_dets, det_cap, d_cnt, PIGO_FRAMES_DEVICE | PIGO_OUT_DEVICE, st);
   };
   return detect_on(dev, face, puploc, flp, flp_flip, ncalls, nimages, 1, "image", P, randoms, rng_seed, slot_base, faces, face_cap, n_faces, points,
                    nullptr, flags, stream_, scan, ClusterFrames{dev, nimages, P.iou_threshold, face_cap});
@@ -1786,8 +1835,8 @@ static int sweep_raw_cap(const int32_t* cnt, int nimages, int nangles, int det_c
 
 // ex / ex_angles: the expanded list (sweep_entries), ip: its ladders.
 static int sweep_scan_on(pigo_cascade* c, int dev, const pigo_image* ex, const double* ex_angles, int nimages, const double* angles, int nangles,
-                         const ImagePlans& ip, int min_size, int max_size, double shift_factor, double scale_factor, double iou, int det_cap,
-                         pigo_det* out, int32_t* angle_index, int cap_per_image, int* n_out, unsigned flags, void* stream_) {
+                         const ImagePlans& ip, double iou, int det_cap, pigo_det* out, int32_t* angle_index, int cap_per_image, int* n_out,
+                         unsigned flags, void* stream_) {
   int rc = PIGO_OK;
   FaceReplica* R = face_replica(c, dev, &rc);
   if (!R) return rc;
@@ -1800,8 +1849,7 @@ static int sweep_scan_on(pigo_cascade* c, int dev, const pigo_image* ex, const d
   if ((rc = w->raw.reserve((size_t)E * det_cap * sizeof(pigo_det))) || (rc = w->nout.reserve(((size_t)E + nimages) * 4))) return rc;
   pigo_det* d_raw = (pigo_det*)w->raw.p;
   int32_t* d_cnt = (int32_t*)w->nout.p;
-  if ((rc = scan_images_on(c, dev, ex, E, ip, min_size, max_size, shift_factor, scale_factor, ex_angles, d_raw, det_cap, d_cnt,
-                           (flags & PIGO_FRAMES_DEVICE) | PIGO_OUT_DEVICE, st)))
+  if ((rc = scan_images_on(c, dev, ex, E, ip, ex_angles, d_raw, det_cap, d_cnt, (flags & PIGO_FRAMES_DEVICE) | PIGO_OUT_DEVICE, st)))
     return rc;
   pigo_det* d_out = out;
   int32_t* d_nout = n_out;
@@ -1842,8 +1890,8 @@ static int detect_sweep_on(int dev, pigo_cascade* face, pigo_puploc* puploc, pig
     if (rc) return rc;
     W.rot_slot = kRotSlotPerFace;
     sweep_entries(staged.data(), nimages, angles, nangles, ex, ex_angles);
-    return scan_images_on(face, dev, ex.data(), nimages * nangles, ip, P.min_size, P.max_size, P.shift_factor, P.scale_factor, ex_angles.data(),
-                          d_dets, det_cap, d_cnt, PIGO_FRAMES_DEVICE | PIGO_OUT_DEVICE, st);
+    return scan_images_on(face, dev, ex.data(), nimages * nangles, ip, ex_angles.data(), d_dets, det_cap, d_cnt, PIGO_FRAMES_DEVICE | PIGO_OUT_DEVICE,
+                          st);
   };
   auto cluster = [&](Workspace* w, cudaStream_t st, pigo_det* d_dets, int det_cap, int32_t* d_cnt, pigo_det* d_clusters, int32_t* d_ncl, PupWork& W,
                      int32_t** d_tags) {
@@ -1982,28 +2030,29 @@ static int check_detect_images_args(const pigo_cascade* face, const pigo_puploc*
   return check_landmarks(flp, ncalls);
 }
 
-// pigo_detect_images and pigo_detect_images_angles: image i at angles[i] (nullptr: prm->angle for every image).  `fn`
-// names the entry point in messages.
+// pigo_detect_images, pigo_detect_images_angles and pigo_detect_images_params: image i with cparams[i] (nullptr: the scan
+// fields of prm for every image) at angles[i] (nullptr: `angle` for every image).  `fn` names the entry point in messages.
 static int detect_images(const char* fn, const pigo_cascade* face, const pigo_puploc* puploc, const pigo_puploc* const* flp, const uint8_t* flp_flip,
-                         int ncalls, const pigo_image* images, int nimages, const double* angles, const pigo_pipeline_params* prm,
-                         const float* randoms, uint64_t rng_seed, pigo_det* faces, int face_cap, int* n_faces, pigo_point* points, unsigned flags,
-                         void* stream) {
+                         int ncalls, const pigo_image* images, int nimages, const pigo_cascade_params* cparams, const double* angles, double angle,
+                         const pigo_pipeline_params* prm, const float* randoms, uint64_t rng_seed, pigo_det* faces, int face_cap, int* n_faces,
+                         pigo_point* points, unsigned flags, void* stream) {
   int rc = check_detect_images_args(face, puploc, flp, ncalls, images, nimages, prm, faces, face_cap, n_faces, points);
   if (rc) return rc;
   ImagePlans ip;
+  std::vector<pigo_cascade_params> uniform_prm;
   std::vector<double> uniform;
-  if ((rc = images_prologue(fn, images, nimages, prm->min_size, prm->max_size, prm->shift_factor, prm->scale_factor, stream, ip)) || nimages == 0)
-    return rc;
+  if (!cparams) cparams = uniform_params(prm->min_size, prm->max_size, prm->shift_factor, prm->scale_factor, nimages, uniform_prm);
+  if ((rc = images_prologue(fn, images, nimages, cparams, stream, ip)) || nimages == 0) return rc;
   return detect_images_on(default_device(), const_cast<pigo_cascade*>(face), const_cast<pigo_puploc*>(puploc), (pigo_puploc* const*)flp, flp_flip,
-                          ncalls, images, nimages, angles_or(angles, prm->angle, nimages, uniform), ip, *prm, randoms, rng_seed, 0, faces, face_cap,
+                          ncalls, images, nimages, angles_or(angles, angle, nimages, uniform), ip, *prm, randoms, rng_seed, 0, faces, face_cap,
                           n_faces, points, flags, stream);
 }
 
 int pigo_detect_images(const pigo_cascade* face, const pigo_puploc* puploc, const pigo_puploc* const* flp, const uint8_t* flp_flip, int ncalls,
                        const pigo_image* images, int nimages, const pigo_pipeline_params* prm, const float* randoms, uint64_t rng_seed,
                        pigo_det* faces, int face_cap, int* n_faces, pigo_point* points, unsigned flags, void* stream) {
-  return detect_images("pigo_detect_images", face, puploc, flp, flp_flip, ncalls, images, nimages, nullptr, prm, randoms, rng_seed, faces, face_cap,
-                       n_faces, points, flags, stream);
+  return detect_images("pigo_detect_images", face, puploc, flp, flp_flip, ncalls, images, nimages, nullptr, nullptr, prm ? prm->angle : 0.0, prm,
+                       randoms, rng_seed, faces, face_cap, n_faces, points, flags, stream);
 }
 
 int pigo_detect_images_angles(const pigo_cascade* face, const pigo_puploc* puploc, const pigo_puploc* const* flp, const uint8_t* flp_flip,
@@ -2011,8 +2060,17 @@ int pigo_detect_images_angles(const pigo_cascade* face, const pigo_puploc* puplo
                               const float* randoms, uint64_t rng_seed, pigo_det* faces, int face_cap, int* n_faces, pigo_point* points,
                               unsigned flags, void* stream) {
   if (nimages > 0 && !angles) return set_err(PIGO_E_INVALID, "null angles");
-  return detect_images("pigo_detect_images_angles", face, puploc, flp, flp_flip, ncalls, images, nimages, angles, prm, randoms, rng_seed, faces,
-                       face_cap, n_faces, points, flags, stream);
+  return detect_images("pigo_detect_images_angles", face, puploc, flp, flp_flip, ncalls, images, nimages, nullptr, angles, 0.0, prm, randoms,
+                       rng_seed, faces, face_cap, n_faces, points, flags, stream);
+}
+
+int pigo_detect_images_params(const pigo_cascade* face, const pigo_puploc* puploc, const pigo_puploc* const* flp, const uint8_t* flp_flip,
+                              int ncalls, const pigo_image* images, int nimages, const pigo_cascade_params* cparams, const double* angles,
+                              const pigo_pipeline_params* prm, const float* randoms, uint64_t rng_seed, pigo_det* faces, int face_cap,
+                              int* n_faces, pigo_point* points, unsigned flags, void* stream) {
+  if (nimages > 0 && !cparams) return set_err(PIGO_E_INVALID, "null cparams");
+  return detect_images("pigo_detect_images_params", face, puploc, flp, flp_flip, ncalls, images, nimages, cparams, angles, 0.0, prm, randoms,
+                       rng_seed, faces, face_cap, n_faces, points, flags, stream);
 }
 
 // Sweep arguments checked before the per-image ones: the angle list and the size of the expanded list (det_cap > 0).
@@ -2042,11 +2100,13 @@ int pigo_run_cascade_images_sweep(const pigo_cascade* cc, const pigo_image* imag
   std::vector<double> ex_angles;
   sweep_entries(images, nimages, angles, nangles, ex, ex_angles);
   ImagePlans ip;
-  if ((rc = images_prologue("pigo_run_cascade_images_sweep", ex.data(), (int)ex.size(), min_size, max_size, shift_factor, scale_factor, stream_,
-                            ip)) || nimages == 0)
+  std::vector<pigo_cascade_params> prm;
+  if ((rc = images_prologue("pigo_run_cascade_images_sweep", ex.data(), (int)ex.size(),
+                            uniform_params(min_size, max_size, shift_factor, scale_factor, (int)ex.size(), prm), stream_, ip, nangles)) ||
+      nimages == 0)
     return rc;
-  return sweep_scan_on(const_cast<pigo_cascade*>(cc), default_device(), ex.data(), ex_angles.data(), nimages, angles, nangles, ip, min_size,
-                       max_size, shift_factor, scale_factor, iou_threshold, dcap, out, angle_index, cap_per_image, n_out, flags, stream_);
+  return sweep_scan_on(const_cast<pigo_cascade*>(cc), default_device(), ex.data(), ex_angles.data(), nimages, angles, nangles, ip, iou_threshold,
+                       dcap, out, angle_index, cap_per_image, n_out, flags, stream_);
 }
 
 int pigo_detect_images_sweep(const pigo_cascade* face, const pigo_puploc* puploc, const pigo_puploc* const* flp, const uint8_t* flp_flip, int ncalls,
@@ -2061,8 +2121,10 @@ int pigo_detect_images_sweep(const pigo_cascade* face, const pigo_puploc* puploc
   std::vector<double> ex_angles;
   sweep_entries(images, nimages, angles, nangles, ex, ex_angles);
   ImagePlans ip;
-  if ((rc = images_prologue("pigo_detect_images_sweep", ex.data(), (int)ex.size(), prm->min_size, prm->max_size, prm->shift_factor,
-                            prm->scale_factor, stream, ip)) || nimages == 0)
+  std::vector<pigo_cascade_params> cparams;
+  if ((rc = images_prologue("pigo_detect_images_sweep", ex.data(), (int)ex.size(),
+                            uniform_params(prm->min_size, prm->max_size, prm->shift_factor, prm->scale_factor, (int)ex.size(), cparams), stream, ip,
+                            nangles)) || nimages == 0)
     return rc;
   return detect_sweep_on(default_device(), const_cast<pigo_cascade*>(face), const_cast<pigo_puploc*>(puploc), (pigo_puploc* const*)flp, flp_flip,
                          ncalls, images, nimages, angles, nangles, ip, *prm, randoms, rng_seed, faces, face_cap, n_faces, points, face_angle,
@@ -2298,7 +2360,8 @@ template <typename F>
 static int run_sharded(const pigo_image* images, const pigo_decoded* src, int nimages, const double* angles, double angle, int min_size,
                        int max_size, double shift_factor, double scale_factor, F fn) {
   ImagePlans ip;
-  int rc = build_image_plans(images, nimages, min_size, max_size, shift_factor, scale_factor, ip);
+  std::vector<pigo_cascade_params> prm;
+  int rc = build_image_plans(images, nimages, uniform_params(min_size, max_size, shift_factor, scale_factor, nimages, prm), ip);
   if (rc) return rc;
   if (nimages == 0) return ensure_device();
   std::vector<double> uniform;
@@ -2320,8 +2383,8 @@ static int run_cascade_sharded(const pigo_cascade* cc, const pigo_image* images,
   pigo_cascade* c = const_cast<pigo_cascade*>(cc);
   return run_sharded(images, src, nimages, angles, 0.0, min_size, max_size, shift_factor, scale_factor,
                      [&](int dev, const pigo_image* im, int n, int lo, const double* a, const ImagePlans& sp, unsigned flags, void* st) {
-                       return scan_images_on(c, dev, im, n, sp, min_size, max_size, shift_factor, scale_factor, a,
-                                             out ? out + (size_t)lo * cap_per_image : nullptr, cap_per_image, n_out + lo, flags, st);
+                       return scan_images_on(c, dev, im, n, sp, a, out ? out + (size_t)lo * cap_per_image : nullptr, cap_per_image, n_out + lo,
+                                             flags, st);
                      });
 }
 
@@ -2394,7 +2457,8 @@ int pigo_shard_plan(const pigo_image* images, int nimages, const double* angles,
   int rc = check_image_geometry(images, nimages, 0, false);
   if (rc) return rc;
   ImagePlans ip;
-  if ((rc = build_image_plans(images, nimages, min_size, max_size, shift_factor, scale_factor, ip))) return rc;
+  std::vector<pigo_cascade_params> prm;
+  if ((rc = build_image_plans(images, nimages, uniform_params(min_size, max_size, shift_factor, scale_factor, nimages, prm), ip))) return rc;
   if (nshards == 0) nshards = shard_count(std::max(1, (int)shard_devices().size()));
   const std::vector<int> cut = plan_shards(ip.wins, angles, nshards);
   *n_used = (int)cut.size() - 1;

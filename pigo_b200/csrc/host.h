@@ -209,6 +209,14 @@ struct DevBuf {
 
 constexpr int kMaxLanes = 4;
 
+// One rotated node table of a mixed-size call: rotation slot, then the ladder key (MinSize and the bits of ScaleFactor, which
+// alone fix a ladder's window sizes) and the number of ladder entries it covers.
+struct RotTableKey {
+  int slot, min_size, len;
+  uint64_t scale_bits;
+  bool operator==(const RotTableKey& o) const { return slot == o.slot && min_size == o.min_size && len == o.len && scale_bits == o.scale_bits; }
+};
+
 struct Workspace {
   cudaStream_t stream = nullptr;
   DevBuf frames, raw, counters, out, nout, plan, tiles, scratch_a, scratch_b, scratch_c, rot_tab, ptab;
@@ -255,9 +263,7 @@ struct Workspace {
   DevBuf img_tab, img_rot;
   DevBuf gray_arena;                           // a sharded decoded call's converted images on this device (pigo_*_decoded_sharded)
   DevBuf sweep;                                // an angle sweep's merge scratch and per-face outputs (pigo_*_images_sweep)
-  std::vector<int> img_rot_slots;                           // what img_rot was built for: one table per slot, in order (empty = nothing)
-  int img_rot_len = 0, img_rot_min = 0;
-  double img_rot_scale = 0;
+  std::vector<RotTableKey> img_rot_tables;     // what img_rot was built for: its tables, in order (empty = nothing)
   void* pinned = nullptr;
   size_t pinned_cap = 0;
   unsigned int* seq = nullptr;                 // pinned 1, 2, 3, ...: source of the ready-counter updates (host_stream)

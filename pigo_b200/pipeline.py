@@ -8,7 +8,7 @@ CPU oracle can replay the exact same pipeline; without it the library's counter-
 from __future__ import annotations
 
 from dataclasses import dataclass, field
-from typing import Callable, Dict, List, Optional
+from typing import Callable, Dict, List, Optional, Sequence
 
 import numpy as np
 
@@ -194,6 +194,18 @@ def detect_images_angles_device(clf: Pigo, plc: PuplocCascade, flpcs: Dict[str, 
                           det_cap, raw)
 
 
+def detect_images_params(clf: Pigo, plc: PuplocCascade, flpcs: Dict[str, PuplocCascade], cps: Sequence[CascadeParams], angles=None,
+                         iou: float = 0.1, min_face: int = 50, eye_perturbs: int = 50, flp_perturbs: int = 63, face_cap: int = 32,
+                         randoms: Optional[np.ndarray] = None, rng_seed: int = 0, det_cap: int = 0, raw: bool = False):
+    """detect_images_angles_device with every image's own CascadeParams (pigo_detect_images_params): image i is cps[i].ImageParams,
+    scanned with cps[i]'s MinSize / MaxSize / ShiftFactor / ScaleFactor and refined at angles[i] (None = every image unrotated).
+    iou, min_face, the perturbs and det_cap stay shared.  Pixels as detect_images_device."""
+    if angles is not None and len(angles) != len(cps):
+        raise ValueError("angles must have one entry per image")
+    return _detect_images(clf, plc, flpcs, [cp.ImageParams for cp in cps], CascadeParams(), iou, min_face, eye_perturbs, flp_perturbs, face_cap,
+                          0.0, angles, randoms, rng_seed, det_cap, raw, cparams=cps)
+
+
 def detect_images_sweep_device(clf: Pigo, plc: PuplocCascade, flpcs: Dict[str, PuplocCascade], images, cp: CascadeParams, angles,
                                iou: float = 0.1, min_face: int = 50, eye_perturbs: int = 50, flp_perturbs: int = 63, face_cap: int = 32,
                                randoms: Optional[np.ndarray] = None, rng_seed: int = 0, det_cap: int = 0, raw: bool = False):
@@ -252,10 +264,10 @@ def detect_images_sharded(clf: Pigo, plc: PuplocCascade, flpcs: Dict[str, Puploc
 
 
 def _detect_images(clf, plc, flpcs, images, cp, iou, min_face, eye_perturbs, flp_perturbs, face_cap, angle, angles, randoms, rng_seed, det_cap,
-                   raw, sharded=False, sources=None):
+                   raw, sharded=False, sources=None, cparams=None):
     import ctypes as C
     from . import DET_DTYPE, POINT_DTYPE, FRAMES_DEVICE, MEM_HOST, PipelineParams, _check, _image_table, lib
-    from . import decoded_descs
+    from . import cascade_params_array, decoded_descs
     hs, fl = landmark_call_arrays(flpcs)
     ncalls = len(fl)
     if sources is not None:   # decoded sources (host planes): converted on the devices by the call
@@ -281,6 +293,11 @@ def _detect_images(clf, plc, flpcs, images, cp, iou, min_face, eye_perturbs, flp
         fn = lib().pigo_detect_decoded_sharded if sources is not None else lib().pigo_detect_images_sharded
         _check(fn(clf._h, plc._h, hs, fl.ctypes.data, ncalls, desc, n, ang.ctypes.data if ang is not None else None, C.byref(prm), rptr, rng_seed,
                   faces.ctypes.data, face_cap, nfaces.ctypes.data, points.ctypes.data))
+    elif cparams is not None:
+        ang = np.ascontiguousarray(angles, dtype=np.float64) if angles is not None else None
+        _check(lib().pigo_detect_images_params(clf._h, plc._h, hs, fl.ctypes.data, ncalls, desc, n, cascade_params_array(cparams),
+                                               ang.ctypes.data if ang is not None else None, C.byref(prm), rptr, rng_seed, faces.ctypes.data,
+                                               face_cap, nfaces.ctypes.data, points.ctypes.data, flags, None))
     elif angles is None:
         _check(lib().pigo_detect_images(clf._h, plc._h, hs, fl.ctypes.data, ncalls, desc, n, C.byref(prm), rptr, rng_seed, faces.ctypes.data,
                                         face_cap, nfaces.ctypes.data, points.ctypes.data, flags, None))

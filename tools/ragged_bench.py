@@ -30,6 +30,10 @@ Usage: `python tools/ragged_bench.py [--frames 256]` on one GPU prints one JSON 
   sweep   : one 1080p frame and 16 wide images of the mix, each x 32 angles: one pigo_detect_images_sweep against
               pigo_detect_images_angles over the expanded list plus a merge through host memory; the merge kernels' own time
               (sweep_bench)
+  params  : the scan section's 256 images, each with one of the reference callers' 8 CascadeParams settings: one
+              pigo_run_cascade_images_params call against one pigo_run_cascade_images call per setting and one scan per image,
+              the same for the pipeline, and rotated: the wide images only, since a rotated scan of a tall image reads past
+              it in the reference (params_bench)
 `--sections scan,pipeline` (the default) selects the sections; `--sections angles` runs the sweeps alone.  Writes nothing
 to the tree.
 """
@@ -942,11 +946,179 @@ def sharded_bench(clf, dev: int) -> dict:
     return res
 
 
+# MinSize, MaxSize, ShiftFactor, ScaleFactor of the reference's callers: cmd/pigo, the test suite, puploc / facial_landmark,
+# facedet, talk_detector, masquerade, the wasm detector, blinkdet
+REFERENCE_SETTINGS = [(20, 1000, 0.15, 1.15), (20, 1000, 0.2, 1.1), (60, 600, 0.1, 1.1), (100, 600, 0.15, 1.1), (100, 600, 0.1, 1.1),
+                      (200, 600, 0.1, 1.1), (200, 480, 0.1, 1.1), (260, 640, 0.1, 1.1)]
+
+
+def params_bench(clf, dev: int, stream) -> dict:
+    """Per-image CascadeParams: the 256 images of the scan section, each with one of the reference's eight settings (seeded), three
+    ways, alternated in rounds (median of 5 after 2, CUDA events, device resident, outputs asserted identical): (a) one
+    pigo_run_cascade_images_params call, (b) one pigo_run_cascade_images call per distinct setting, (c) one scan per image
+    (pigo_run_cascade_batch, nframes = 1); the same three ways through the pipeline (pigo_detect_images_params / one
+    pigo_detect_images per setting / one pigo_detect_batch per image, injected randoms); (a) and (b) with every wide image
+    (Cols >= Rows) rotated at a seeded k/32, (b) then one pigo_run_cascade_images_angles call per setting."""
+    import ctypes as C
+    import torch
+    import pigo_b200
+    from pigo_b200 import pipeline
+    L = pigo_b200.lib()
+    st = stream.cuda_stream
+    cuda = f"cuda:{dev}"
+    imgs = ragged_images()
+    n = len(imgs)
+    rng = np.random.default_rng(5)
+    setting = [int(rng.integers(8)) for _ in range(n)]
+    prm = [REFERENCE_SETTINGS[s] for s in setting]
+    rot = [float(rng.integers(1, 33)) / 32 if c >= r else 0.0 for _, r, c, _ in imgs]
+    by_setting = {}
+    for i, s in enumerate(setting):
+        by_setting.setdefault(s, []).append(i)
+    W = int(sum(pigo_b200.count_windows(r, c, *p) for (_, r, c, _), p in zip(imgs, prm)))
+    offs, total = [], 0
+    for b, r, c, d in imgs:
+        offs.append(total)
+        total += (r * d + 255) & ~255
+    host = np.zeros(total, dtype=np.uint8)
+    for (b, r, c, d), o in zip(imgs, offs):
+        host[o:o + r * d] = b.reshape(-1)
+    dev_all = torch.from_numpy(host).to(cuda)
+    descs = [(dev_all.data_ptr() + o, r, c, d) for (b, r, c, d), o in zip(imgs, offs)]
+    cap = 4096
+
+    def check(rc):
+        if rc != 0:
+            raise RuntimeError(L.pigo_last_error().decode())
+
+    def rounds(ways, reps=5, warm=2):
+        """{way: median ms} of the callables in `ways`, run in alternated rounds."""
+        ts = {k: [] for k in ways}
+        for r in range(warm + reps):
+            for k, fn in ways.items():
+                a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                a.record(stream)
+                fn()
+                b.record(stream)
+                torch.cuda.synchronize()
+                if r >= warm:
+                    ts[k].append(a.elapsed_time(b))
+        return {k: float(np.median(v)) for k, v in ts.items()}
+
+    # ---- scan
+    out = {k: torch.zeros((n, cap, 4), dtype=torch.int32, device=cuda) for k in "abc"}
+    cnt = {k: torch.zeros(n, dtype=torch.int32, device=cuda) for k in "abc"}
+    sub = {s: (torch.zeros((len(idx), cap, 4), dtype=torch.int32, device=cuda), torch.zeros(len(idx), dtype=torch.int32, device=cuda))
+           for s, idx in by_setting.items()}
+
+    def scan_a(angles=None):
+        clf.run_cascade_images_params_device(descs, prm, angles, out["a"].data_ptr(), cap, cnt["a"].data_ptr(), st)
+
+    def scan_b(angles=None):
+        for s, idx in by_setting.items():
+            o, k = sub[s]
+            ims = [descs[i] for i in idx]
+            if angles is None:
+                clf.run_cascade_images_device(ims, *REFERENCE_SETTINGS[s], 0.0, o.data_ptr(), cap, k.data_ptr(), st)
+            else:
+                clf.run_cascade_images_angles_device(ims, [angles[i] for i in idx], *REFERENCE_SETTINGS[s], o.data_ptr(), cap, k.data_ptr(), st)
+
+    def scan_c():
+        for i, (p, r, c, d) in enumerate(descs):
+            clf.run_cascade_batch_device(p, 1, r * d, r, c, d, *prm[i], 0.0, out["c"][i].data_ptr(), cap, cnt["c"].data_ptr() + 4 * i, st)
+
+    def gather(dst_out, dst_cnt, parts):
+        for s, idx in by_setting.items():
+            dst_out[idx] = parts[s][0]
+            dst_cnt[idx] = parts[s][1]
+
+    def assert_same(what, ks):
+        c = {k: cnt[k].cpu().numpy() for k in ks}
+        o = {k: out[k].cpu().numpy() for k in ks}
+        assert int(c["a"].max()) <= cap, "raise cap: an image has more detections than the bench buffer"
+        for k in ks[1:]:
+            assert np.array_equal(c["a"], c[k]), f"{what}: counts of ({k}) differ"
+            for i in range(n):
+                assert o["a"][i, :c["a"][i]].tobytes() == o[k][i, :c["a"][i]].tobytes(), f"{what}: image {i} of ({k}) differs"
+        return int(c["a"].sum())
+
+    ms = rounds({"a": scan_a, "b": scan_b, "c": scan_c})
+    gather(out["b"], cnt["b"], sub)
+    dets = assert_same("params scan", "abc")
+    ms_rot = rounds({"a": lambda: scan_a(rot), "b": lambda: scan_b(rot)})
+    gather(out["b"], cnt["b"], sub)
+    dets_rot = assert_same("params scan, rotated", "ab")
+    del out, cnt, sub
+
+    # ---- pipeline: injected randoms, so that every way's points are comparable
+    plc = pigo_b200.NewPuplocCascade().UnpackCascade(pigo_b200.load_cascade("puploc"))
+    names = sorted(set(pipeline.EYE_CASCADES + pipeline.MOUTH_CASCADES))
+    flp = {nm: pigo_b200.NewPuplocCascade().UnpackCascade(pigo_b200.load_cascade("lps/" + nm)) for nm in names}
+    hs, fl = pipeline.landmark_call_arrays(flp)
+    ncalls = len(fl)
+    face_cap, det_cap = 512, 16384   # the MinSize 20 settings find several hundred faces on the largest images
+    flags = pigo_b200.FRAMES_DEVICE | pigo_b200.OUT_DEVICE
+    sptr = C.c_void_p(st)
+    pp = {s: pigo_b200.PipelineParams(*REFERENCE_SETTINGS[s], 0.0, 0.1, 50, 50, 63, det_cap) for s in range(8)}
+    cdesc = pigo_b200.image_descs(descs)
+    cprm = pigo_b200.cascade_params_array(prm)
+    rnd = torch.from_numpy(np.random.default_rng(11).random((n, face_cap, 2 + ncalls, 63, 3), dtype=np.float32)).to(cuda)
+    rnd_sub = {s: rnd[idx].contiguous() for s, idx in by_setting.items()}
+    desc_sub = {s: pigo_b200.image_descs([descs[i] for i in idx]) for s, idx in by_setting.items()}
+
+    def outputs(m):
+        return (torch.zeros((m, face_cap, 4), dtype=torch.int32, device=cuda), torch.zeros(m, dtype=torch.int32, device=cuda),
+                torch.zeros((m, face_cap, 2 + ncalls, 4), dtype=torch.int32, device=cuda))
+    po = {k: outputs(n) for k in "abc"}
+    psub = {s: outputs(len(idx)) for s, idx in by_setting.items()}
+
+    def det_a():
+        check(L.pigo_detect_images_params(clf._h, plc._h, hs, fl.ctypes.data, ncalls, cdesc, n, cprm, None, C.byref(pp[0]), rnd.data_ptr(), 7,
+                                          po["a"][0].data_ptr(), face_cap, po["a"][1].data_ptr(), po["a"][2].data_ptr(), flags, sptr))
+
+    def det_b():
+        for s, idx in by_setting.items():
+            o = psub[s]
+            check(L.pigo_detect_images(clf._h, plc._h, hs, fl.ctypes.data, ncalls, desc_sub[s], len(idx), C.byref(pp[s]), rnd_sub[s].data_ptr(), 7,
+                                       o[0].data_ptr(), face_cap, o[1].data_ptr(), o[2].data_ptr(), flags, sptr))
+
+    def det_c():
+        for i, (p, r, c, d) in enumerate(descs):
+            o = po["c"]
+            check(L.pigo_detect_batch(clf._h, plc._h, hs, fl.ctypes.data, ncalls, p, 1, r * d, r, c, d, C.byref(pp[setting[i]]), rnd[i].data_ptr(), 7,
+                                      o[0][i].data_ptr(), face_cap, o[1].data_ptr() + 4 * i, o[2][i].data_ptr(), flags, sptr))
+
+    pms = rounds({"a": det_a, "b": det_b, "c": det_c})
+    for s, idx in by_setting.items():
+        for t, u in zip(po["b"], psub[s]):
+            t[idx] = u
+    res = {k: [t.cpu().numpy() for t in po[k]] for k in "abc"}
+    assert int(res["a"][1].max()) <= face_cap, "raise face_cap: an image has more faces than the bench buffer"
+    for k in "bc":
+        assert all(x.tobytes() == y.tobytes() for x, y in zip(res["a"], res[k])), f"params pipeline: outputs of ({k}) differ"
+    faces = int(res["a"][1].sum())
+    refined = int((res["a"][0][..., 2] > 50).sum())
+
+    def way(t, calls):
+        return {"ms": t, "windows_per_s": W / (t * 1e-3), "calls": calls}
+    return {"workload": f"{n} images of the scan section, each with one of the reference's 8 settings (seed 5: "
+                        f"{ {str(REFERENCE_SETTINGS[s]): len(v) for s, v in sorted(by_setting.items())} }), device resident, "
+                        "CUDA events, ways alternated in rounds, median of 5 after 2",
+            "windows": W, "settings": len(by_setting),
+            "scan": {"a_one_params_call": way(ms["a"], 1), "b_images_call_per_setting": way(ms["b"], len(by_setting)),
+                     "c_call_per_image": way(ms["c"], n), "detections": dets, "outputs_identical": True},
+            "scan_rotated": {"rotated_images": int(sum(a > 0 for a in rot)), "a_one_params_call_ms": ms_rot["a"],
+                             "b_angles_call_per_setting_ms": ms_rot["b"], "detections": dets_rot, "outputs_identical": True},
+            "pipeline": {"a_one_detect_images_params_call_ms": pms["a"], "b_detect_images_per_setting_ms": pms["b"],
+                         "c_detect_batch_per_image_ms": pms["c"], "faces": faces, "refined_faces": refined,
+                         "outputs_identical_with_injected_randoms": True}}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--frames", type=int, default=256, help="frames of the uniform 1080p comparison")
     ap.add_argument("--pipeline-frames", type=int, default=64, help="frames of the uniform 1080p pipeline comparison")
-    ap.add_argument("--sections", default="scan,pipeline", help="comma-separated: scan, pipeline, angles, decoded, formats, sharded, sweep")
+    ap.add_argument("--sections", default="scan,pipeline", help="comma-separated: scan, pipeline, angles, decoded, formats, sharded, sweep, params")
     args = ap.parse_args()
     sections = set(args.sections.split(","))
     import torch
@@ -969,6 +1141,8 @@ def main():
         res["sharded"] = sharded_bench(clf, 0)
     if "sweep" in sections:
         res["sweep"] = sweep_bench(clf, 0, stream)
+    if "params" in sections:
+        res["params"] = params_bench(clf, 0, stream)
     res["gpu"] = torch.cuda.get_device_name(0)
     try:   # read-only query: the power limit belongs beside the numbers
         import subprocess
