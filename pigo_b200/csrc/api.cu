@@ -1313,7 +1313,8 @@ int pigo_describe_plan_frames(int rows, int cols, int min_size, int max_size, do
   uint64_t total = 0;
   int rc = build_plan(rows, cols, min_size, max_size, shift_factor, scale_factor, plan, total);
   if (rc) return rc;
-  return describe_plan(plan, total, 468, nframes, json, cap);   // geometry of the stock 468-tree facefinder cascade
+  // geometry of the stock 468-tree facefinder cascade, frames of Dim = cols (16-byte aligned when cols is)
+  return describe_plan(plan, total, 468, nframes, cols % 16 == 0 && g_opt.tile_tmap.load() != 0, (uint64_t)rows * (uint64_t)cols, json, cap);
 }
 int pigo_describe_plan(int rows, int cols, int min_size, int max_size, double shift_factor, double scale_factor, char* json, size_t cap) {
   return pigo_describe_plan_frames(rows, cols, min_size, max_size, shift_factor, scale_factor, 1 << 20, json, cap);

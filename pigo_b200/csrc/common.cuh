@@ -162,8 +162,33 @@ struct TileBand {
   int32_t tiles_x, ntiles;     // tiles per row / per frame
   int32_t pitch;               // shared-memory row pitch in bytes (multiple of 16)
   int32_t rows_t;              // tile rows: halo_lo + core + halo_hi
-  int32_t pad;
+  // region role (a CTA-wide region of core x core_y window centres per band): core_y, and the rows of one TMA box of the
+  // region's fill (a region is rows_t <= 2 * box_rows rows, filled by ceil(rows_t / box_rows) boxes of pitch x box_rows)
+  int32_t core_y, box_rows;
 };
+
+// Region role of the fused kernel: every region buffer has this row pitch (= the widest TMA box).  A multiple of 128, it also
+// keeps both buffers and every box of a region at the 128-byte alignment TMA tensor copies need.
+constexpr int kRegionPitch = 256;
+constexpr int kRegionMaxScales = 32;
+// One ladder entry's window sub-grid inside a region: windows [start, next start) of the region's scale-major list.
+struct RegionSub {
+  int32_t start, s, step, nj;
+  uint32_t magic;              // ceil(2^32 / nj): k / nj by __umulhi
+  uint32_t base;               // shared-memory offset of the sub-grid's first window centre
+  uint32_t wid0;               // its in-frame window index
+  int32_t ncols;
+};
+// Control block of one region buffer, written by the warp that fills the buffer before the fill's mbarrier arrive.
+struct RegionCtl {
+  int32_t n;                   // windows of the region
+  int32_t frame;               // -1: no region left for this CTA
+  int32_t pad[2];
+  RegionSub sub[kRegionMaxScales + 1];   // sub[nscales].start == n
+};
+// Region control in shared memory: RegionCtl[2], then full[2] and empty[2] mbarriers, the two buffers' dealing cursors and
+// the sequence number each buffer is claimed for next (TiledArgs.region_ctl, 8-byte aligned).
+constexpr uint32_t kRegionCtlBytes = 2 * sizeof(RegionCtl) + 48;
 
 struct TiledArgs {
   ScanArgs scan;
@@ -202,6 +227,10 @@ struct TiledArgs {
   uint32_t rounds_per_frame;
   uint32_t band_rounds[kMaxBands];
   int32_t head_back;                      // generic phase: with an empty ring and fewer live lanes than this, park them in the ring and go back to the head
+  // region role (scan_tiled_kernel<1, 1024, true>): band[] / tiles_per_frame / total_tiles describe regions; two buffers of
+  // region_bytes at region_off and region_off + region_bytes, their RegionCtl blocks and barriers at region_ctl
+  int32_t region;
+  uint32_t region_ctl, region_off, region_bytes;
 };
 
 // TMA descriptors of the frame batch, one per tile band (the box = the band's tile: pitch x rows_t x 1 frame), passed to the

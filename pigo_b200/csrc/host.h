@@ -71,6 +71,7 @@ struct Options {
   std::atomic<long long> puploc_mode{0};    // RunDetector kernel: 0 = (perturbation, tree)-pair kernel, 1 = warp-per-perturbation kernel
   std::atomic<long long> lanes{1};          // internal streams the groups alternate between
   std::atomic<long long> tile_tail_min{6};  // tail policy threshold
+  std::atomic<long long> tile_region{0};    // fused kernel, tile role: 0 = auto (regions for calls of > 2 M windows at <= 1 window per pixel), 1 = CTA-wide double-buffered regions, 2 = per-warp tiles
   std::atomic<long long> tile_band_ratio{0};    // a band spans scales up to ratio/100 x its first scale; 0 = auto (200, or 140 for calls of <= 2 M windows)
   std::atomic<long long> timing{0};         // 1 = bracket every kernel with CUDA events (bench.py roofline pass)
   std::atomic<long long> shard_split{0};    // sharded mixed-size / decoded calls: 0 = one shard per selected device, k > 0 = k shards,
@@ -86,7 +87,7 @@ struct Options {
          {"gather_block", &Options::gather_block}, {"deep_group", &Options::deep_group},
         {"sub_batch", &Options::sub_batch}, {"lanes", &Options::lanes}, {"tile_tail_min", &Options::tile_tail_min},
         {"tile_band_ratio", &Options::tile_band_ratio}, {"timing", &Options::timing}, {"host_stream", &Options::host_stream}, {"copy_chunk", &Options::copy_chunk}, {"stream_taper", &Options::stream_taper},
-        {"deep_flat", &Options::deep_flat}, {"tile_head", &Options::tile_head}, {"tile_ptab", &Options::tile_ptab}, {"queue_cap", &Options::queue_cap}, {"ptab_kt", &Options::ptab_kt}, {"ptab_ks", &Options::ptab_ks}, {"tile_core_cap", &Options::tile_core_cap}, {"walk_stats", &Options::walk_stats}, {"tile_tmap", &Options::tile_tmap}, {"gather_limit", &Options::gather_limit}, {"deep_smem", &Options::deep_smem}, {"deep_smem_threads", &Options::deep_smem_threads}, {"deep_smem_lo", &Options::deep_smem_lo}, {"deep_smem_k", &Options::deep_smem_k}, {"head_back", &Options::head_back}, {"rot_mode", &Options::rot_mode}, {"puploc_mode", &Options::puploc_mode}, {"puploc_stage", &Options::puploc_stage}, {"shard_split", &Options::shard_split}};
+        {"deep_flat", &Options::deep_flat}, {"tile_head", &Options::tile_head}, {"tile_ptab", &Options::tile_ptab}, {"queue_cap", &Options::queue_cap}, {"ptab_kt", &Options::ptab_kt}, {"ptab_ks", &Options::ptab_ks}, {"tile_core_cap", &Options::tile_core_cap}, {"walk_stats", &Options::walk_stats}, {"tile_tmap", &Options::tile_tmap}, {"gather_limit", &Options::gather_limit}, {"deep_smem", &Options::deep_smem}, {"deep_smem_threads", &Options::deep_smem_threads}, {"deep_smem_lo", &Options::deep_smem_lo}, {"deep_smem_k", &Options::deep_smem_k}, {"head_back", &Options::head_back}, {"rot_mode", &Options::rot_mode}, {"puploc_mode", &Options::puploc_mode}, {"puploc_stage", &Options::puploc_stage}, {"shard_split", &Options::shard_split}, {"tile_region", &Options::tile_region}};
     for (const Entry& e : table)
       if (k == e.name) return &(this->*e.field);
     return nullptr;
@@ -405,7 +406,8 @@ int build_tiled_tables(const FaceTables& tab, const std::vector<int8_t>& codes, 
                        const std::vector<float>& thr, DevBuf& out);
 int build_block_tables(const FaceTables& tab, const std::vector<int8_t>& codes, const std::vector<float>& preds,
                        const std::vector<float>& thr, DevBuf& out);
-int describe_plan(const std::vector<ScaleEntry>& plan, uint64_t wins, int ntrees, int batch_frames, char* buf, size_t cap);
+int describe_plan(const std::vector<ScaleEntry>& plan, uint64_t wins, int ntrees, int batch_frames, bool tmap_ok, uint64_t frame_pixels,
+                  char* buf, size_t cap);
 int run_scan(FaceReplica* c, Workspace* w, int lane, ScanArgs& A, unsigned long long* d_work, cudaStream_t st, int num_sms);
 // Whether a scan of cascade c runs on the block/deep kernels rather than the universal gather kernel (scan_driver.cu).
 bool block_path(const FaceReplica* c, bool rot, int max_scale, size_t rot_bytes);

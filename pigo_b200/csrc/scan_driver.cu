@@ -123,6 +123,64 @@ static TilePlan plan_bands(const std::vector<ScaleEntry>& plan, uint32_t tile_by
   return tp;
 }
 
+// A region band is tiled only while its buffer holds at most this many times the pixels its core's windows are centred on;
+// above that the gather role is the cheaper place for the band's few windows.  On 1080p this keeps bands 20-39 and 40-79 in
+// regions (1.4x and 1.8x).  With a bound of 4, the band 86-136 moved in as well, and the H100 ran a 256 x 1080p step in
+// 11.16 ms instead of 10.12 ms, because the deep kernel grew from 4.07 to 4.66 ms per step.
+constexpr int kRegionMaxHalo = 2;
+
+// Bands of the region role: each band's regions are core x core_y window centres plus the halo every sample of those
+// windows reaches, kRegionPitch bytes per row and at most two TMA boxes of at most 256 rows, in a buffer of region_bytes.
+static TilePlan plan_regions(const std::vector<ScaleEntry>& plan, uint32_t region_bytes, int max_scale, int ratio_pct, int min_core,
+                             int min_core_steps) {
+  TilePlan tp;
+  const int n = (int)plan.size();
+  const int rows_buf = (int)(region_bytes / kRegionPitch);
+  const int rows_max = rows_buf <= 256 ? rows_buf : 2 * std::min(256, rows_buf / 2);
+  int a = 0;
+  while (a < n && tp.nbands < kMaxBands) {
+    const int s0 = plan[a].s;
+    if (s0 > max_scale) break;
+    int best_b = -1, best_cx = 0, best_cy = 0;
+    for (int b = a + 1; b <= n && b - a <= kRegionMaxScales; ++b) {
+      const int smax = plan[b - 1].s;
+      if (smax > max_scale || (long long)smax * 100 > (long long)s0 * ratio_pct) break;
+      const int halo = (smax + 1) / 2 + ((127 * smax) >> 8);
+      const int cx = ((kRegionPitch - halo) / 16) * 16, cy = rows_max - halo;
+      const int step_max = plan[b - 1].step;
+      if (std::min(cx, cy) >= std::max(min_core, min_core_steps * step_max) &&
+          (long long)kRegionPitch * rows_max <= (long long)kRegionMaxHalo * cx * cy) {
+        best_b = b; best_cx = cx; best_cy = cy;
+      }
+    }
+    if (best_b < 0) break;
+    TileBand B{};
+    const int smax = plan[best_b - 1].s;
+    B.scale_lo = a; B.nscales = best_b - a;
+    B.halo_lo = (smax + 1) / 2;
+    B.core = best_cx; B.core_y = best_cy;
+    B.rows_t = B.halo_lo + best_cy + ((127 * smax) >> 8);
+    const int nbox = (B.rows_t + 255) / 256;
+    B.box_rows = (B.rows_t + nbox - 1) / nbox;
+    B.pitch = kRegionPitch;
+    int org = B.halo_lo % 16;
+    if (org > plan[a].off) org -= 16;
+    B.org_x = org;
+    int max_c = 0, max_r = 0;
+    for (int i = a; i < best_b; ++i) {
+      max_c = std::max(max_c, plan[i].off + (plan[i].ncols - 1) * plan[i].step);
+      max_r = std::max(max_r, plan[i].off + (plan[i].nrows - 1) * plan[i].step);
+    }
+    B.tiles_x = (max_c - B.org_x) / B.core + 1;
+    B.ntiles = B.tiles_x * (max_r / B.core_y + 1);
+    tp.band[tp.nbands++] = B;
+    tp.tiles_per_frame += (uint32_t)B.ntiles;
+    a = best_b;
+  }
+  tp.first_untiled = a;
+  return tp;
+}
+
 // Shared-memory layout of the fused kernel: mbarriers (384 B) | cascade prefix | per-warp tiles (128-byte aligned).
 struct FusedLayout {
   bool ok = false;
@@ -158,8 +216,15 @@ struct FusedPlan {
   int head = 0;   // trees of the dense head (0 = classic tile role)
   int kt = 0;     // trees of the per-scale offset tables (0 = classic tile role)
   int band_ratio = 0;   // a band spans scales up to band_ratio/100 x its first scale
+  // region role (the fused kernel runs it instead of the per-warp tiles above when `region`): bands of regions, shared-memory
+  // offsets of the control block and of the two buffers
+  bool region = false;
+  TilePlan rp;
+  uint32_t region_ctl = 0, region_off = 0, region_bytes = 0;
 };
-static FusedPlan plan_fused(const std::vector<ScaleEntry>& plan, int ntrees, int batch_frames = 1 << 20) {
+// tmap_ok: the frames can be filled by TMA tensor copies (16-byte aligned base, stride and Dim, option tile_tmap), which the
+// region role needs; frame_pixels: rows * cols of one frame.
+static FusedPlan plan_fused(const std::vector<ScaleEntry>& plan, int ntrees, int batch_frames, bool tmap_ok, uint64_t frame_pixels) {
   FusedPlan P;
   P.ni = (int)std::min<long long>(std::max<long long>(1, g_opt.tile_ni.load()), 4);
   const int max_warps = tiled_max_threads(P.ni) / 32;
@@ -222,6 +287,25 @@ static FusedPlan plan_fused(const std::vector<ScaleEntry>& plan, int ntrees, int
       plan_with(0);
     }
   }
+  // Region role (auto): calls of more than 2 M windows with at most one window per frame pixel.  On the H100 it took a
+  // 256 x 1080p step at ShiftFactor 0.2 (0.43 windows per pixel) from 11.1 to 10.1 ms, but made 64 frames at ShiftFactor 0.1
+  // (2 windows per pixel) 10 % slower; single frames keep the per-warp tiles, whose shorter tiles finish a partial wave earlier
+  // (DESIGN.md section 3.1).  The options that name another tile role, or cap the shared memory, keep that role.
+  const long long region_opt = g_opt.tile_region.load();
+  const unsigned long long frame_windows = call_windows / (unsigned long long)std::max(1, batch_frames);
+  const bool region_auto = call_windows > 2000000ull && frame_windows <= frame_pixels;
+  if ((region_opt == 1 || (region_opt == 0 && region_auto)) && tmap_ok && P.W > 0 && P.ni == 1 && P.head == 0 &&
+      P.kt == 0 && g_opt.tile_prefetch.load() == 0 && g_opt.fused_smem_kb.load() <= 0) {
+    const size_t casc_bytes = ((size_t)P.ks * kTreeRec + 15) & ~(size_t)15;
+    P.region_ctl = (uint32_t)((384 + casc_bytes + 127) & ~(size_t)127);
+    P.region_off = (uint32_t)((P.region_ctl + kRegionCtlBytes + 127) & ~(size_t)127);
+    if (P.region_off + 2 * 16 * (size_t)kRegionPitch <= kSmemPerCta) {
+      P.region_bytes = (uint32_t)((kSmemPerCta - P.region_off) / 2 / kRegionPitch * kRegionPitch);
+      P.rp = plan_regions(plan, P.region_bytes, max_scale, band_ratio,
+                          (int)std::max<long long>(16, g_opt.tile_min_core.load()), (int)std::max<long long>(1, g_opt.tile_min_core_steps.load()));
+      P.region = P.rp.nbands > 0;
+    }
+  }
   return P;
 }
 
@@ -250,8 +334,11 @@ static int upload_block_prefix(Workspace* w, int lo, int hi, int gb_shift, cudaS
 // per-scale offset tables, both 0: classic), for a call of `batch_frames` frames of this geometry (the frame count decides
 // the band ratio, as in run_scan).  JSON text; used by tests/test_plan_cpu.py to check on the CPU that the tiles partition
 // the windows of their scales exactly and that every sample stays inside its tile.
-int describe_plan(const std::vector<ScaleEntry>& plan, uint64_t wins, int ntrees, int batch_frames, char* buf, size_t cap) {
-  const FusedPlan P = plan_fused(plan, ntrees, batch_frames);
+// "region" says whether the fused kernel runs the region role for that call (frames whose Dim is a multiple of 16: tmap_ok);
+// "regions" and "region_bytes" describe the region plan whenever one fits, "region_first_untiled" its first gather-role entry.
+int describe_plan(const std::vector<ScaleEntry>& plan, uint64_t wins, int ntrees, int batch_frames, bool tmap_ok, uint64_t frame_pixels,
+                  char* buf, size_t cap) {
+  const FusedPlan P = plan_fused(plan, ntrees, batch_frames, tmap_ok, frame_pixels);
   const TilePlan& tp = P.tp;
   const uint32_t tile_bytes = P.L.ok ? P.L.tile_bytes : 0;
   std::string s = "{";
@@ -266,6 +353,16 @@ int describe_plan(const std::vector<ScaleEntry>& plan, uint64_t wins, int ntrees
     const TileBand& B = tp.band[b];
     snprintf(tmp, sizeof(tmp), "%s{\"scale_lo\": %d, \"nscales\": %d, \"halo_lo\": %d, \"core\": %d, \"org_x\": %d, \"tiles_x\": %d, \"ntiles\": %d, "
              "\"pitch\": %d, \"rows_t\": %d}", b ? ", " : "", B.scale_lo, B.nscales, B.halo_lo, B.core, B.org_x, B.tiles_x, B.ntiles, B.pitch, B.rows_t);
+    s += tmp;
+  }
+  snprintf(tmp, sizeof(tmp), "], \"region\": %d, \"region_bytes\": %u, \"region_first_untiled\": %d, \"regions\": [", P.region ? 1 : 0,
+           P.region_bytes, P.rp.first_untiled);
+  s += tmp;
+  for (int b = 0; b < P.rp.nbands; ++b) {
+    const TileBand& B = P.rp.band[b];
+    snprintf(tmp, sizeof(tmp), "%s{\"scale_lo\": %d, \"nscales\": %d, \"halo_lo\": %d, \"core_x\": %d, \"core_y\": %d, \"org_x\": %d, "
+             "\"regions_x\": %d, \"nregions\": %d, \"pitch\": %d, \"rows_r\": %d, \"box_rows\": %d}", b ? ", " : "", B.scale_lo, B.nscales,
+             B.halo_lo, B.core, B.core_y, B.org_x, B.tiles_x, B.ntiles, B.pitch, B.rows_t, B.box_rows);
     s += tmp;
   }
   s += "], \"scales\": [";
@@ -329,13 +426,15 @@ static EncodeTiledFn encode_tiled_fn() {
   }();
   return fn;
 }
-// frames [nframes][rows][dim] u8 (frames `frame_stride` bytes apart) as a 3-D tensor; box = one tile of band B
+// frames [nframes][rows][dim] u8 (frames `frame_stride` bytes apart) as a 3-D tensor; box = one tile of band B (a region
+// band: one of the region's boxes of box_rows rows)
 static bool encode_tile_map(CUtensorMap* m, const ScanArgs& A, const TileBand& B) {
   EncodeTiledFn fn = encode_tiled_fn();
-  if (!fn || B.pitch > 256 || B.rows_t > 256 || (A.dim % 16) || (A.frame_stride % 16) || ((uintptr_t)A.frames % 16)) return false;
+  const int box_rows = B.box_rows > 0 ? B.box_rows : B.rows_t;
+  if (!fn || B.pitch > 256 || box_rows > 256 || (A.dim % 16) || (A.frame_stride % 16) || ((uintptr_t)A.frames % 16)) return false;
   const cuuint64_t gdim[3] = {(cuuint64_t)A.dim, (cuuint64_t)A.rows, (cuuint64_t)A.nframes};
   const cuuint64_t gstride[2] = {(cuuint64_t)A.dim, (cuuint64_t)A.frame_stride};
-  const cuuint32_t box[3] = {(cuuint32_t)B.pitch, (cuuint32_t)B.rows_t, 1};
+  const cuuint32_t box[3] = {(cuuint32_t)B.pitch, (cuuint32_t)box_rows, 1};
   const cuuint32_t estr[3] = {1, 1, 1};
   return fn(m, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, (void*)A.frames, gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
             CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
@@ -466,11 +565,18 @@ int run_scan(FaceReplica* c, Workspace* w, int lane, ScanArgs& A, unsigned long 
   int first_untiled = 0;
   bool blocks_done = false;
   if (mode != 3 && !rot) {
-    FusedPlan P = plan_fused(w->plan_host, A.tab.ntrees, A.batch_frames);
-    const TilePlan& tp = P.tp;
+    const bool aligned = (A.dim % 16 == 0) && (A.frame_stride % 16 == 0) && (((uintptr_t)A.frames) % 16 == 0);
+    FusedPlan P = plan_fused(w->plan_host, A.tab.ntrees, A.batch_frames, aligned && g_opt.tile_tmap.load() != 0,
+                             (uint64_t)A.rows * (uint64_t)A.cols);
+    TileMaps TM{};
+    if (P.region) {   // the region role needs a tensor map per band; without one the per-warp tiles run
+      for (int b = 0; b < P.rp.nbands && P.region; ++b)
+        if (!encode_tile_map(&TM.m[b], A, P.rp.band[b])) P.region = false;
+    }
+    const TilePlan& tp = P.region ? P.rp : P.tp;
     const int W = P.W;
     int Wg = (int)std::min<long long>(std::max<long long>(0, g_opt.gather_warps.load()), tiled_max_threads(P.ni) / 32 - W);
-    if (P.L.ok && tp.nbands > 0) {
+    if ((P.L.ok || P.region) && tp.nbands > 0) {
       TiledArgs F = T;
       F.ks = P.ks; F.tile_bytes = P.L.tile_bytes; F.nbands = tp.nbands;
       F.tail_min = (int)g_opt.tile_tail_min.load();
@@ -490,9 +596,17 @@ int run_scan(FaceReplica* c, Workspace* w, int lane, ScanArgs& A, unsigned long 
       } else {
         Wg = 0;
       }
-      F.aligned = ((A.dim % 16 == 0) && (A.frame_stride % 16 == 0) && (((uintptr_t)A.frames) % 16 == 0)) ? 1 : 0;
+      F.aligned = aligned ? 1 : 0;
       long long grid = num_sms;
       if (Wg == 0) grid = std::max<long long>(1, std::min<long long>(num_sms, (long long)((F.total_tiles + W - 1) / W)));
+      size_t smem = P.L.tiles_off + (size_t)P.L.tile_bytes * W;
+      if (P.region) {
+        F.region = 1;
+        F.region_ctl = P.region_ctl; F.region_off = P.region_off; F.region_bytes = P.region_bytes;
+        F.use_tmap = 1;
+        smem = P.region_off + 2 * (size_t)P.region_bytes;
+        if (Wg == 0) grid = std::max<long long>(1, std::min<long long>(num_sms, (long long)F.total_tiles));
+      }
       if (P.kt > 0) {
         // per-scale offset tables: rounds of W tiles of one band; tables cached per workspace for this geometry
         F.kt = P.kt;
@@ -515,11 +629,11 @@ int run_scan(FaceReplica* c, Workspace* w, int lane, ScanArgs& A, unsigned long 
         F.ptab = (const uint8_t*)w->ptab.p;
         if (Wg == 0) grid = std::max<long long>(1, std::min<long long>(num_sms, (long long)F.rounds_per_frame * A.nframes));
       }
-      const size_t smem = P.L.tiles_off + (size_t)P.L.tile_bytes * W;
-      TileMaps TM{};
-      F.use_tmap = (F.aligned && g_opt.tile_tmap.load() != 0) ? 1 : 0;
-      for (int b = 0; b < tp.nbands && F.use_tmap; ++b)
-        if (!encode_tile_map(&TM.m[b], A, tp.band[b])) F.use_tmap = 0;
+      if (!P.region) {
+        F.use_tmap = (F.aligned && g_opt.tile_tmap.load() != 0) ? 1 : 0;
+        for (int b = 0; b < tp.nbands && F.use_tmap; ++b)
+          if (!encode_tile_map(&TM.m[b], A, tp.band[b])) F.use_tmap = 0;
+      }
       timing_begin(T_TILED, st);
       launch_scan_tiled(F, TM, (int)grid, (W + Wg) * 32, smem, P.ni, st);
       timing_end(T_TILED, st);

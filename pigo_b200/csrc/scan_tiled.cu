@@ -323,7 +323,278 @@ __global__ void __launch_bounds__(256, MINB) scan_gather2_kernel(const TiledArgs
   gather_role<NG, ROT, IMG>(A, smem, casc, casc + casc_bytes);
 }
 
-template <int NI, int MAXT>
+// ---- region role ---------------------------------------------------------------------------------------------
+// The tile warps of a CTA share two region buffers of ~100 KB instead of owning one small tile each.  A region is a
+// core x core_y rectangle of window centres of one band plus its halo (kRegionPitch bytes per row); the CTA takes regions
+// frame-major from the global cursor, one per buffer, and region k + 2 reuses region k's buffer.  The tile warps deal the
+// windows of the newer region from a shared-memory cursor (one atomic per warp refill) while the older region's last
+// windows finish; a warp that runs out of the newer region's windows first hands the older region's windows it still holds
+// to the deep queue, then releases that buffer (empty barrier).  The warp whose release completes the barrier claims the
+// next region and issues its TMA copies (full barrier), so the next fill is in flight while the current region is walked.
+// Walk, hand-over at tree KS, overflow path and detection append are the classic role's.
+
+// Claims this CTA's next region into buffer `b` (sequence number q) and issues its fill.  Executed by one whole tile warp.
+__device__ __forceinline__ void region_fill(const TiledArgs& A, const TileMaps& TM, uint8_t* smem, uint32_t smem_base, uint32_t q) {
+  const unsigned FULL = 0xffffffffu;
+  const int lane = threadIdx.x & 31;
+  const ScanArgs& S = A.scan;
+  const uint32_t b = q & 1u;
+  RegionCtl* ctl = reinterpret_cast<RegionCtl*>(smem + A.region_ctl) + b;
+  const uint32_t fullbar = smem_base + A.region_ctl + 2 * (uint32_t)sizeof(RegionCtl) + 8 * b;
+  unsigned* cursor = reinterpret_cast<unsigned*>(smem + A.region_ctl + 2 * sizeof(RegionCtl) + 32);
+  unsigned long long g = 0;
+  if (lane == 0) g = atomicAdd(S.chunk_counter, 1ull);
+  g = __shfl_sync(FULL, g, 0);
+  if (g >= A.total_tiles) {
+    if (lane == 0) { ctl->n = 0; ctl->frame = -1; cursor[b] = 0; }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(fullbar);
+    return;
+  }
+  const int frame = (int)(g / A.tiles_per_frame);
+  int tf = (int)(g % A.tiles_per_frame);
+  int bi = 0;
+  while (bi + 1 < A.nbands && tf >= A.band[bi].ntiles) { tf -= A.band[bi].ntiles; ++bi; }
+  const TileBand& B = A.band[bi];
+  const int ry = tf / B.tiles_x, rx = tf - ry * B.tiles_x;
+  const int cx0 = B.org_x + rx * B.core, cy0 = ry * B.core_y;      // core origin (window centres)
+  const int gx0 = cx0 - B.halo_lo, gy0 = cy0 - B.halo_lo;          // region origin in the frame (gx0 % 16 == 0)
+  const uint32_t buf = A.region_off + b * A.region_bytes;
+  // lane l: ladder entry scale_lo + l, its sub-grid of window centres in the core
+  int n = 0;
+  RegionSub sub{};
+  if (lane < B.nscales) {
+    const ScaleEntry e = S.plan[B.scale_lo + lane];
+    const int i0 = ceil_div_pos(cy0 - e.off, e.step), i1 = min(e.nrows, ceil_div_pos(cy0 + B.core_y - e.off, e.step));
+    const int j0 = ceil_div_pos(cx0 - e.off, e.step), j1 = min(e.ncols, ceil_div_pos(cx0 + B.core - e.off, e.step));
+    sub.nj = max(0, j1 - j0);
+    n = max(0, i1 - i0) * sub.nj;
+    sub.s = e.s; sub.step = e.step; sub.ncols = e.ncols;
+    sub.magic = sub.nj > 1 ? (uint32_t)((0x100000000ull + (unsigned)sub.nj - 1) / (unsigned)sub.nj) : 0u;
+    sub.base = buf + (uint32_t)((e.off + i0 * e.step - gy0) * kRegionPitch + (e.off + j0 * e.step - gx0));
+    sub.wid0 = e.wbase + (uint32_t)i0 * (uint32_t)e.ncols + (uint32_t)j0;
+  }
+  int incl = n;   // inclusive prefix over the lanes
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const int v = __shfl_up_sync(FULL, incl, d);
+    if (lane >= d) incl += v;
+  }
+  const int total = __shfl_sync(FULL, incl, 31);
+  sub.start = incl - n;
+  if (lane < B.nscales) ctl->sub[lane] = sub;
+  if (lane == 0) { ctl->sub[B.nscales].start = total; ctl->n = total; ctl->frame = frame; cursor[b] = 0; }
+  if (total > 0) wait_frames(S.ready, S.frame_base + (unsigned)frame + 1u);
+  __threadfence_block();
+  __syncwarp();
+  if (lane == 0) {
+    if (total > 0) {
+      const int nbox = (B.rows_t + B.box_rows - 1) / B.box_rows;
+      mbar_expect_tx(fullbar, (uint32_t)(nbox * B.box_rows * kRegionPitch));
+      for (int k = 0; k < nbox; ++k)
+        tma_tile_g2s(smem_base + buf + (uint32_t)(k * B.box_rows * kRegionPitch), &TM.m[bi], gx0, gy0 + k * B.box_rows, frame, fullbar);
+    } else {
+      mbar_arrive(fullbar);
+    }
+  }
+}
+
+__device__ __forceinline__ void region_role(const TiledArgs& A, const TileMaps& TM, uint8_t* smem, uint32_t smem_base, uint32_t casc,
+                                            uint32_t casc_end) {
+  const unsigned FULL = 0xffffffffu;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const ScanArgs& S = A.scan;
+  const RegionCtl* ctl = reinterpret_cast<const RegionCtl*>(smem + A.region_ctl);
+  const uint32_t fullbar = smem_base + A.region_ctl + 2 * (uint32_t)sizeof(RegionCtl);
+  const uint32_t emptybar = fullbar + 16;
+  unsigned* cursor = reinterpret_cast<unsigned*>(smem + A.region_ctl + 2 * sizeof(RegionCtl) + 32);
+  unsigned* issued = cursor + 2;
+  const bool all_resident = A.ks >= S.tab.ntrees;
+  bool overflow_mode = false;
+
+  if (warp == 0) { region_fill(A, TM, smem, smem_base, 0); region_fill(A, TM, smem, smem_base, 1); }
+
+  // Leaves region q (its buffer q & 1): one arrive per warp; the warp that completes the phase and wins the claim fills the
+  // buffer with the CTA's region q + 2.
+  auto leave = [&](uint32_t q) {
+    const uint32_t b = q & 1u;
+    __syncwarp();
+    if (lane == 0) mbar_arrive(emptybar + 8 * b);
+    bool fill = false;
+    if (lane == 0) fill = mbar_test(emptybar + 8 * b, (q >> 1) & 1u) && atomicCAS(&issued[b], q, q + 2u) == q;
+    if (__shfl_sync(FULL, fill, 0)) region_fill(A, TM, smem, smem_base, q + 2);
+  };
+
+  uint32_t kc = 0, kb = 0;      // sequence number and buffer of the region this warp deals from
+  mbar_wait(fullbar, 0);
+  bool done = ctl[0].frame < 0;
+  bool held_prev = false;       // region kc - 1 is not released yet by this warp
+  int u_sc = 0;                 // sub-grid of the warp's last dealt window (the cursor only grows)
+
+  bool alive = false;
+  uint32_t pb = casc, tbo = casc, wid = 0, wb = 0;   // wb: buffer of the lane's window
+  int sv = 0;
+  float acc = 0.f;
+
+  for (;;) {
+    // ================= refill dead lanes from the region cursor =====================================================
+    unsigned need = __ballot_sync(FULL, !alive);
+    while (need != 0u && !done) {
+      const int cnt = __popc(need);
+      unsigned base = 0;
+      if (lane == 0) base = atomicAdd(&cursor[kb], (unsigned)cnt);
+      base = __shfl_sync(FULL, base, 0);
+      const unsigned n = (unsigned)ctl[kb].n;
+      const unsigned rank = __popc(need & lanemask_lt());
+      int sc = u_sc;
+      if (!alive && base + rank < n) {
+        const unsigned k = base + rank;
+        const RegionSub* sb = ctl[kb].sub;
+        while ((unsigned)sb[sc + 1].start <= k) ++sc;
+        const RegionSub e = sb[sc];
+        const uint32_t kk = k - (uint32_t)e.start;
+        const uint32_t i = e.nj > 1 ? __umulhi(kk, e.magic) : kk;   // kk / nj, exact for kk * nj < 2^32
+        const uint32_t j = kk - i * (uint32_t)e.nj;
+        pb = e.base + i * (uint32_t)(e.step * kRegionPitch) + j * (uint32_t)e.step;
+        wid = e.wid0 + i * (uint32_t)e.ncols + j;
+        sv = e.s; tbo = casc; acc = 0.f; wb = kb;
+        alive = true;
+      }
+      u_sc = (int)__reduce_max_sync(FULL, (unsigned)sc);
+      if (base + (unsigned)cnt < n) break;
+      // region kc is dealt out: the warp moves on to kc + 1, whose buffer still holds region kc - 1
+      if (held_prev) {
+        unsigned prev = __ballot_sync(FULL, alive && wb != kb);
+        if (prev != 0u && !overflow_mode) {
+          unsigned qbase = 0;
+          if (lane == 0) qbase = atomicAdd(S.long_count, (unsigned)__popc(prev));
+          qbase = __shfl_sync(FULL, qbase, 0);
+          const unsigned pos = qbase + __popc(prev & lanemask_lt());
+          if (alive && wb != kb && pos < S.long_cap) {
+            S.longq[pos] = DeepItem{wid, pack_frame_si(ctl[wb].frame, scale_index_of(smem, sv)), (int)((tbo - casc) / kTreeRec), acc};
+            alive = false; tbo = casc; sv = 0; pb = casc;
+          }
+          prev = __ballot_sync(FULL, alive && wb != kb);
+          if (prev) overflow_mode = true;   // queue full: finish these windows here first
+        }
+        if (prev != 0u) break;              // they keep their buffer pinned until they are done
+        leave(kc - 1);
+        held_prev = false;
+      }
+      ++kc; kb ^= 1u;
+      mbar_wait(fullbar + 8 * kb, (kc >> 1) & 1u);
+      held_prev = true;
+      u_sc = 0;
+      done = ctl[kb].frame < 0;
+      need = __ballot_sync(FULL, !alive);
+    }
+    // an older region no lane of this warp holds any more is released at once
+    if (held_prev && __ballot_sync(FULL, alive && wb != kb) == 0u) { leave(kc - 1); held_prev = false; }
+    unsigned live = __ballot_sync(FULL, alive);
+    if (done) {
+      // ---- no region left: a thin warp hands its last windows to the deep queue (the classic tail policy)
+      if (live != 0u && __popc(live) < A.tail_min && !overflow_mode) {
+        unsigned qbase = 0;
+        if (lane == 0) qbase = atomicAdd(S.long_count, (unsigned)__popc(live));
+        qbase = __shfl_sync(FULL, qbase, 0);
+        const unsigned pos = qbase + __popc(live & lanemask_lt());
+        if (alive && pos < S.long_cap) {
+          S.longq[pos] = DeepItem{wid, pack_frame_si(ctl[wb].frame, scale_index_of(smem, sv)), (int)((tbo - casc) / kTreeRec), acc};
+          alive = false; tbo = casc; sv = 0; pb = casc;
+        }
+        live = __ballot_sync(FULL, alive);
+        if (live) overflow_mode = true;
+      }
+      if (live == 0u) break;
+    }
+
+    if (A.stats != nullptr) {   // developer counter: useful (live) lanes per walk iteration of the tile role
+      if (lane == 0) { atomicAdd(A.stats, (unsigned long long)__popc(live)); atomicAdd(A.stats + 1, 1ull); }
+    }
+    // ================= one tree per live window (dead lanes: tree 0 with s = 0 at a cascade byte) ==================
+    if (!overflow_mode) {
+      int idx = 1, cw;
+#pragma unroll
+      for (int j = 0; j < 6; ++j) {
+        cw = *reinterpret_cast<const int*>(smem + tbo + 4 * idx);
+        // ((r*256 + code*s) >> 8) == r + ((code*s) >> 8)  (core/pigo.go:126-127)
+        const int o1 = ((sx0(cw) * sv) >> 8) * kRegionPitch + ((sx1(cw) * sv) >> 8);
+        const int o2 = ((sx2(cw) * sv) >> 8) * kRegionPitch + ((sx3(cw) * sv) >> 8);
+        const uint32_t p1 = smem[pb + o1], p2 = smem[pb + o2];
+        idx = 2 * idx + (p1 <= p2 ? 1 : 0);                                   // core/pigo.go:129-135
+      }
+      cw = *reinterpret_cast<const int*>(smem + tbo + 4 * idx);              // leaf (words 64..127)
+      const float thr = *reinterpret_cast<const float*>(smem + tbo + 512);
+      acc += __int_as_float(cw);                                             // core/pigo.go:137 (float32, tree order)
+      alive = alive && !(acc <= thr);                                        // :139-141
+      tbo += kTreeRec;
+      const bool at_end = alive && tbo == casc_end;
+      if (__any_sync(FULL, at_end)) {                                        // passed the last resident tree (rare)
+        if (all_resident) {
+          if (at_end) {
+            const float q = acc - thr;                                       // :144
+            if (q > 0.0f) {                                                  // :246
+              const int fr = ctl[wb].frame;
+              const int pos = atomicAdd(S.raw_count + fr, 1);
+              if (pos < S.cap) S.raw[(size_t)fr * S.cap + pos] = RawDet{wid, q};
+            }
+            alive = false;
+          }
+        } else {
+          const unsigned mb = __ballot_sync(FULL, at_end);
+          unsigned qbase = 0;
+          if (lane == 0) qbase = atomicAdd(S.long_count, (unsigned)__popc(mb));
+          qbase = __shfl_sync(FULL, qbase, 0);
+          const unsigned pos = qbase + __popc(mb & lanemask_lt());
+          bool failed = false;
+          if (at_end) {
+            if (pos < S.long_cap) {
+              S.longq[pos] = DeepItem{wid, pack_frame_si(ctl[wb].frame, scale_index_of(smem, sv)), A.ks, acc};
+              alive = false;
+            } else {
+              failed = true;
+            }
+          }
+          if (__any_sync(FULL, failed)) overflow_mode = true;
+        }
+      }
+      if (!alive) { tbo = casc; sv = 0; pb = casc; }
+    } else {
+      // ---- overflow mode (deep queue full, pathological): correct but slow; cascade rows beyond KS from global memory
+      const int tv = (int)((tbo - casc) / kTreeRec);
+      const bool res = tbo < casc_end;
+      int idx = 1;
+      for (int j = 0; j < 6; ++j) {
+        const int cw = res ? *reinterpret_cast<const int*>(smem + tbo + 4 * idx)
+                           : __ldg(reinterpret_cast<const int*>(S.tab.codes + (size_t)tv * 256) + idx);
+        const int o1 = ((sx0(cw) * sv) >> 8) * kRegionPitch + ((sx1(cw) * sv) >> 8);
+        const int o2 = ((sx2(cw) * sv) >> 8) * kRegionPitch + ((sx3(cw) * sv) >> 8);
+        const uint32_t p1 = smem[pb + o1], p2 = smem[pb + o2];
+        idx = 2 * idx + (p1 <= p2 ? 1 : 0);
+      }
+      const float pred = res ? *reinterpret_cast<const float*>(smem + tbo + 4 * idx) : __ldg(S.tab.preds + (size_t)tv * 64 + idx - 64);
+      const float thr = res ? *reinterpret_cast<const float*>(smem + tbo + 512) : __ldg(S.tab.thresh + tv);
+      if (alive) {
+        acc += pred;
+        tbo += kTreeRec;
+        if (acc <= thr) {
+          alive = false;
+        } else if (tv + 1 == S.tab.ntrees) {
+          const float q = acc - thr;
+          if (q > 0.0f) {
+            const int fr = ctl[wb].frame;
+            const int pos = atomicAdd(S.raw_count + fr, 1);
+            if (pos < S.cap) S.raw[(size_t)fr * S.cap + pos] = RawDet{wid, q};
+          }
+          alive = false;
+        }
+        if (!alive) { tbo = casc; sv = 0; pb = casc; }
+      }
+    }
+  }
+}
+
+template <int NI, int MAXT, bool REGION = false>
 __global__ void __launch_bounds__(MAXT, 1) scan_tiled_kernel(const TiledArgs A, const __grid_constant__ TileMaps TM) {
   extern __shared__ __align__(128) uint8_t smem[];
   const unsigned FULL = 0xffffffffu;
@@ -338,8 +609,15 @@ __global__ void __launch_bounds__(MAXT, 1) scan_tiled_kernel(const TiledArgs A, 
 
   // ---- stage the cascade prefix with the TMA bulk engine (one elected thread issues, all threads wait)
   if (lane == 0 && warp < A.tile_warps) mbar_init(wbar, 1);
+  if (REGION && threadIdx.x == 0) {   // full[2] (the filling warp's expect_tx), empty[2] (one arrive per tile warp)
+    const uint32_t bars = smem_base + A.region_ctl + 2 * (uint32_t)sizeof(RegionCtl);
+    mbar_init(bars, 1); mbar_init(bars + 8, 1);
+    mbar_init(bars + 16, (uint32_t)A.tile_warps); mbar_init(bars + 24, (uint32_t)A.tile_warps);
+    unsigned* issued = reinterpret_cast<unsigned*>(smem + A.region_ctl + 2 * sizeof(RegionCtl) + 40);
+    issued[0] = 0; issued[1] = 1;
+  }
   if (threadIdx.x < kLutSizes) smem[kLutOff + threadIdx.x] = 0xff;
-  stage_cascade(A, smem_base, casc, (casc_bytes + 15u) & ~15u);
+  stage_cascade(A, smem_base, casc, (casc_bytes + 15u) & ~15u);   // (its fence + barrier also publish the barriers above)
   if ((int)threadIdx.x < A.scan.nscales && threadIdx.x < 255) {
     const int sz = A.scan.plan[threadIdx.x].s;
     if (sz >= 0 && sz < kLutSizes) smem[kLutOff + sz] = (uint8_t)threadIdx.x;     // sizes are distinct along the ladder
@@ -353,6 +631,10 @@ __global__ void __launch_bounds__(MAXT, 1) scan_tiled_kernel(const TiledArgs A, 
     const uint32_t g_end = casc + (uint32_t)min(A.ks, max(1, A.gather_limit)) * kTreeRec;
     if (A.gather_ni >= 2) gather_role<2, 0>(A, smem, casc, g_end);
     else gather_role<1, 0>(A, smem, casc, g_end);
+    return;
+  }
+  if constexpr (REGION) {
+    region_role(A, TM, smem, smem_base, casc, casc_end);
     return;
   }
   uint32_t tile_phase = 0;
@@ -1435,6 +1717,11 @@ void launch_scan_tiled(const TiledArgs& A, const TileMaps& TM, int grid, int thr
   if (A.head_trees > 0) {
     raise_dyn_smem((const void*)scan_head_kernel<1024>, (int)smem);
     scan_head_kernel<1024><<<grid, threads, smem, st>>>(A, TM);
+    return;
+  }
+  if (A.region) {
+    raise_dyn_smem((const void*)scan_tiled_kernel<1, 1024, true>, (int)smem);
+    scan_tiled_kernel<1, 1024, true><<<grid, threads, smem, st>>>(A, TM);
     return;
   }
   switch (ni) {
