@@ -34,7 +34,7 @@ struct TimingSlot {
 };
 static TimingSlot g_tslot[T_NSLOTS];
 static std::mutex g_tmu;
-static const char* kSlotNames[T_NSLOTS] = {"tiled", "gather", "deep", "finalize", "cluster", "puploc", "gray", "seeds", "rottab", "ycbcr", "gray_images", "merge"};
+static const char* kSlotNames[T_NSLOTS] = {"tiled", "gather", "deep", "finalize", "cluster", "puploc", "gray", "seeds", "rottab", "ycbcr", "gray_images", "merge", "region"};
 
 void timing_reset() {
   std::lock_guard<std::mutex> g(g_tmu);

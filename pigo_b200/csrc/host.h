@@ -19,8 +19,10 @@ extern std::atomic<long long> g_launches;
 void raise_dyn_smem(const void* fn, int bytes);
 
 // Per-kernel CUDA-event timing (enabled by option "timing"): every launch of kernel class `slot` is bracketed by an
-// event pair on its stream; "t_<name>_ns" / "t_<name>_n" return the summed device time and the launch count.
-enum TimeSlot { T_TILED = 0, T_GATHER, T_DEEP, T_FINALIZE, T_CLUSTER, T_PUPLOC, T_GRAY, T_SEEDS, T_ROTTAB, T_YCBCR, T_GRAY_IMAGES, T_MERGE, T_NSLOTS };
+// event pair on its stream; "t_<name>_ns" / "t_<name>_n" return the summed device time and the launch count.  T_REGION
+// brackets, inside T_TILED, only the fused launches that run the region role (after their tensor maps were encoded).
+enum TimeSlot { T_TILED = 0, T_GATHER, T_DEEP, T_FINALIZE, T_CLUSTER, T_PUPLOC, T_GRAY, T_SEEDS, T_ROTTAB, T_YCBCR, T_GRAY_IMAGES, T_MERGE, T_REGION,
+                T_NSLOTS };
 void timing_reset();
 void walk_stats_reset();
 long long walk_stats_query(int which);

@@ -427,12 +427,14 @@ static EncodeTiledFn encode_tiled_fn() {
   return fn;
 }
 // frames [nframes][rows][dim] u8 (frames `frame_stride` bytes apart) as a 3-D tensor; box = one tile of band B (a region
-// band: one of the region's boxes of box_rows rows)
+// band: one of the region's boxes of box_rows rows).  The column extent is Cols, not Dim: device frames may be packed
+// (rows-1)*Dim + Cols bytes apart, so columns [Cols, Dim) of the last frame's last row need not be readable.  No unrotated
+// window samples a column >= Cols (its centre is at most Cols - (s/2+1)), so the zero fill there changes no result.
 static bool encode_tile_map(CUtensorMap* m, const ScanArgs& A, const TileBand& B) {
   EncodeTiledFn fn = encode_tiled_fn();
   const int box_rows = B.box_rows > 0 ? B.box_rows : B.rows_t;
   if (!fn || B.pitch > 256 || box_rows > 256 || (A.dim % 16) || (A.frame_stride % 16) || ((uintptr_t)A.frames % 16)) return false;
-  const cuuint64_t gdim[3] = {(cuuint64_t)A.dim, (cuuint64_t)A.rows, (cuuint64_t)A.nframes};
+  const cuuint64_t gdim[3] = {(cuuint64_t)A.cols, (cuuint64_t)A.rows, (cuuint64_t)A.nframes};
   const cuuint64_t gstride[2] = {(cuuint64_t)A.dim, (cuuint64_t)A.frame_stride};
   const cuuint32_t box[3] = {(cuuint32_t)B.pitch, (cuuint32_t)box_rows, 1};
   const cuuint32_t estr[3] = {1, 1, 1};
@@ -635,7 +637,9 @@ int run_scan(FaceReplica* c, Workspace* w, int lane, ScanArgs& A, unsigned long 
           if (!encode_tile_map(&TM.m[b], A, tp.band[b])) F.use_tmap = 0;
       }
       timing_begin(T_TILED, st);
+      if (P.region) timing_begin(T_REGION, st);   // "t_region_n": the fused launches that really ran the region role
       launch_scan_tiled(F, TM, (int)grid, (W + Wg) * 32, smem, P.ni, st);
+      if (P.region) timing_end(T_REGION, st);
       timing_end(T_TILED, st);
       g_launches++;
       if ((rc = check_launch("fused scan"))) return rc;

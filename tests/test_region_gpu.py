@@ -15,12 +15,14 @@ pytestmark = pytest.mark.gpu
 def run_timed(fn):
     with options(timing=1):
         out = fn()
-        launches = {k: pigo_b200.get_option(k) for k in ("t_tiled_n", "t_gather_n", "t_deep_n")}
+        launches = {k: pigo_b200.get_option(k) for k in ("t_tiled_n", "t_gather_n", "t_deep_n", "t_region_n")}
     return out, launches
 
 
 def assert_region_ran(launches, rows, cols, prm, nframes, groups=1, gather=False):
-    assert launches == {"t_tiled_n": groups, "t_gather_n": groups * gather, "t_deep_n": groups}, launches
+    """Every fused launch of the call ran the region role (t_region_n counts those, after their tensor maps were encoded:
+    a fallback to the per-warp tiles shows as 0), and the planner says so too."""
+    assert launches == {"t_tiled_n": groups, "t_gather_n": groups * gather, "t_deep_n": groups, "t_region_n": groups}, launches
     assert pigo_b200.describe_plan(rows, cols, *prm, nframes=nframes)["region"] == 1
 
 
@@ -89,7 +91,7 @@ def test_full_size_batch_region_role_equals_per_warp_tiles(gpu_face, oracle_face
     with options(tile_region=2):
         (cnt2, dets2), launches2 = run_timed(run)
         assert pigo_b200.describe_plan(R, C, *TEST_PARAMS, nframes=nf)["region"] == 0
-    assert launches2 == launches
+    assert launches2 == dict(launches, t_region_n=0)
     assert int(cnt.max()) <= cap
     assert cnt.tobytes() == cnt2.tobytes() and dets.tobytes() == dets2.tobytes()
     for f in (0, 5, 255):

@@ -20,7 +20,7 @@ def _check_regions(rows, cols, prm, nframes=None):
         assert p["region"] == 0
         return p
     assert p["region_bytes"] % 256 == 0
-    assert p["tiles_off"] <= SMEM_PER_CTA and 2 * p["region_bytes"] + 384 + 48 * 520 <= SMEM_PER_CTA
+    assert p["tiles_off"] <= SMEM_PER_CTA and 2 * p["region_bytes"] + 384 + p["ks"] * 520 <= SMEM_PER_CTA
     covered = 0
     for b in p["regions"]:
         assert 1 <= b["nscales"] <= 32
@@ -95,3 +95,108 @@ def test_region_plan_for_the_call_s_frame_count(frames):
         for geom in GEOMS:
             for prm in PARAMS:
                 _check_regions(geom[0], geom[1], prm, nframes=frames)
+
+
+def _ceil_div_pos(num, den):
+    return np.where(num <= 0, 0, (num + den - 1) // den)
+
+
+def _row_of(kk, nj, magic):
+    """region_role's kk / nj: __umulhi(kk, magic) for nj > 1, kk itself for nj <= 1."""
+    kk = np.asarray(kk, dtype=np.uint64)
+    return np.where(nj > 1, (kk * np.asarray(magic, dtype=np.uint64)) >> np.uint64(32), kk).astype(np.int64)
+
+
+def _partitions(lo, hi, n):
+    """The non-empty intervals [lo, hi) cover 0..n-1 exactly once (and nothing outside)."""
+    keep = hi > lo
+    assert (lo[keep] >= 0).all() and (hi[keep] <= n).all()
+    cover = np.zeros(n + 1, dtype=np.int64)
+    np.add.at(cover, lo[keep], 1)
+    np.add.at(cover, hi[keep], -1)
+    assert (np.cumsum(cover)[:n] == 1).all()
+
+
+def _deal_regions(p, checked_nj):
+    """region_fill's sub-grid arithmetic (scan_tiled.cu) restated in numpy for every band, region and scale of the plan, and
+    the dealing of region_role: window k of a sub-grid is row i = kk / nj (by __umulhi(kk, magic)), column kk - i * nj, id
+    wid0 + i * ncols + j, buffer offset base + i * step * pitch + j * step.  Region (ry, rx) deals the windows of rows
+    [i0, i1) x columns [j0, j1) of each scale, so every window of a band's scales is dealt exactly once iff the row intervals
+    of the ry and the column intervals of the rx each partition the scale's rows and columns, and the division is exact for
+    every kk < n (checked for each distinct nj over all kk below the largest n it occurs with; checked_nj caches those).
+    The id and buffer offset are checked against the window's centre at the four corners of every sub-grid.  Returns the
+    windows dealt."""
+    scales = p["scales"]
+    dealt = 0
+    for b in p["regions"]:
+        regions_y = b["nregions"] // b["regions_x"]
+        for s, step, off, nrows, ncols, wbase in scales[b["scale_lo"]:b["scale_lo"] + b["nscales"]]:
+            cy0 = np.arange(regions_y, dtype=np.int64) * b["core_y"]
+            cx0 = b["org_x"] + np.arange(b["regions_x"], dtype=np.int64) * b["core_x"]
+            i0 = _ceil_div_pos(cy0 - off, step)
+            i1 = np.minimum(nrows, _ceil_div_pos(cy0 + b["core_y"] - off, step))
+            j0 = _ceil_div_pos(cx0 - off, step)
+            j1 = np.minimum(ncols, _ceil_div_pos(cx0 + b["core_x"] - off, step))
+            _partitions(i0, i1, nrows)
+            _partitions(j0, j1, ncols)
+            # per region (ry, rx): lane l's RegionSub of region_fill
+            I0, J0 = np.meshgrid(i0, j0, indexing="ij")
+            NI, NJ = np.meshgrid(np.maximum(0, i1 - i0), np.maximum(0, j1 - j0), indexing="ij")
+            gy0 = (cy0 - b["halo_lo"])[:, None]
+            gx0 = (cx0 - b["halo_lo"])[None, :]
+            n = NI * NJ
+            magic = np.where(NJ > 1, ((1 << 32) + NJ - 1) // np.maximum(NJ, 1), 0)
+            assert magic.max() < (1 << 32)
+            base = (off + I0 * step - gy0) * 256 + (off + J0 * step - gx0)
+            wid0 = wbase + I0 * ncols + J0
+            for nj_ in np.unique(NJ[n > 0]):
+                top = int(n[NJ == nj_].max())
+                if checked_nj.get(int(nj_), 0) < top:
+                    kk = np.arange(top, dtype=np.int64)
+                    m = ((1 << 32) + int(nj_) - 1) // int(nj_) if nj_ > 1 else 0
+                    np.testing.assert_array_equal(_row_of(kk, nj_, m), kk // nj_)   # __umulhi(kk, magic) == kk / nj
+                    checked_nj[int(nj_)] = top
+            live = n > 0
+            for kk in (np.zeros_like(n), NJ - 1, n - NJ, n - 1):   # the corners of each sub-grid
+                kk, nj_, m = kk[live], NJ[live], magic[live]
+                i = _row_of(kk, nj_, m)
+                j = kk - i * nj_
+                wid = wid0[live] + i * ncols + j
+                r, c = off + step * ((wid - wbase) // ncols), off + step * ((wid - wbase) % ncols)
+                assert ((wid >= wbase) & (wid < wbase + nrows * ncols)).all()
+                np.testing.assert_array_equal(base[live] + i * step * 256 + j * step,
+                                              (r - np.broadcast_to(gy0, n.shape)[live]) * 256 + (c - np.broadcast_to(gx0, n.shape)[live]))
+            dealt += int(n.sum())
+    return dealt
+
+
+# option settings that change the region plan: the resident prefix (and with it the buffer size: at 400 trees the buffers
+# are about 11 KB and may hold no band), the band width, the largest tiled scale, and the core limits at their extremes
+PLAN_OPTIONS = ([{"tile_ks": k} for k in (1, 6, 120, 250, 400)] + [{"tile_band_ratio": r} for r in (100, 110, 400)] +
+                [{"tile_max_scale": m} for m in (24, 40, 80)] +
+                [{"tile_min_core": 16, "tile_min_core_steps": 1}, {"tile_min_core": 240}, {"tile_min_core": 4000},
+                 {"tile_min_core_steps": 40}, {"tile_min_core": 16, "tile_min_core_steps": 1, "tile_ks": 250}])
+# settings under which no geometry of the grid gets a region band: 11 KB buffers, a core limit above every region's core
+NO_BANDS = [{"tile_ks": 400}, {"tile_min_core": 4000}]
+
+
+@pytest.mark.parametrize("opt", PLAN_OPTIONS, ids=["-".join(f"{k}{v}" for k, v in o.items()) for o in PLAN_OPTIONS])
+def test_region_plan_under_options(opt):
+    """_check_regions over the geometry / parameter grid under options that change the region plan, and the sub-grid
+    arithmetic of region_fill over every band, region and scale of those plans."""
+    planned = 0
+    checked_nj = {}
+    with options(tile_region=1, **opt):
+        for geom in GEOMS:
+            for prm in PARAMS:
+                p = _check_regions(geom[0], geom[1], prm, nframes=3)
+                if "tile_ks" in opt:
+                    assert p["ks"] == min(opt["tile_ks"], 468)
+                if p["regions"]:
+                    planned += 1
+                    last = p["regions"][-1]
+                    covered = sum(e[3] * e[4] for e in p["scales"][:last["scale_lo"] + last["nscales"]])
+                    assert _deal_regions(p, checked_nj) == covered
+                    assert p["scales"][last["scale_lo"] + last["nscales"] - 1][0] <= opt.get("tile_max_scale", 1 << 30)
+                    assert min(min(b["core_x"], b["core_y"]) for b in p["regions"]) >= opt.get("tile_min_core", 32)
+    assert (planned == 0) == (opt in NO_BANDS)
