@@ -214,7 +214,11 @@ int pigo_puploc_info(const pigo_puploc *p, uint32_t *stages, float *scale_mul, u
  * (`randoms` = [nseeds][63][3] float32 in [0,1), row/col/scale order) or passes NULL and the
  * library draws them from a counter-based generator keyed by (`rng_seed`, seed index).
  * Slots >= perturbs of the 63-entry pool are zero (fresh sync.Pool object, :228-236).
- * flipv: per-seed array (0/1) or NULL for all-false.  out[i].perturbs is 0 like the reference's. */
+ * flipv: per-seed array (0/1) or NULL for all-false.  out[i].perturbs is 0 like the reference's.
+ * With PIGO_OUT_DEVICE (seeds, randoms, flipv, out on the device) the seeds are not checked on the host, so the caller
+ * keeps them to: perturbs 0..63 (above 63 runs as 63; a negative perturbs leaves out[i] untouched), and
+ * |scale| * max(1, |scales|)^(stages-1) <= 16384 (the 32-bit kernel's exact range; host seeds outside it run on the
+ * 64-bit kernel).  Pool entries are ordered with every NaN above every number, ties by slot. */
 int pigo_puploc_run(const pigo_puploc *p, const pigo_point *seeds, int nseeds, const float *randoms,
                     uint64_t rng_seed, const uint8_t *pixels, int rows, int cols, int dim, double angle,
                     const uint8_t *flipv, pigo_point *out, unsigned flags, void *stream);

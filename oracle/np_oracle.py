@@ -213,7 +213,7 @@ class PuplocCascade:
                     if flipv:   # int8 negation wraps: -(-128) == -128
                         cd[1] = int(np.int8(np.uint8((-cd[1]) & 0xFF)))
                         cd[3] = int(np.int8(np.uint8((-cd[3]) & 0xFF)))
-                    ir, ic = int(r), int(c)   # truncation toward zero
+                    ir, ic = _go_int(r), _go_int(c)
                     if not rotated:
                         rs = int(_go_round(float(s)))
                         r1 = min(rows - 1, max(0, (256 * ir + cd[0] * rs) >> 8))
@@ -247,9 +247,28 @@ class PuplocCascade:
             colf = f32(f32(col) + f32(t1 * f32(f32(0.5) - rnd[i, 1])))
             sc = f32(f32(scale) * f32(f32(0.925) + f32(f32(0.15) * rnd[i, 2])))
             pr[i], pc[i], ps[i] = self.classify(rowf, colf, sc, pixels, rows, cols, dim, angle, flipv)
-        pr.sort(); pc.sort(); ps.sort()
         mid = int(_go_round(perturbs / 2))
-        return int(pr[mid]), int(pc[mid]), ps[mid]
+        return _to_i32(_pool_median(pr, mid)), _to_i32(_pool_median(pc, mid)), _pool_median(ps, mid)
+
+
+def _go_int(v) -> int:
+    """int(r) as the sample arithmetic sees it: truncation toward zero; Go on amd64 gives the int64 minimum for NaN and
+    out-of-range values, and 256 * (or 65536 *) that minimum wraps to 0."""
+    return int(v) if abs(float(v)) < 2.0 ** 63 else 0
+
+
+def _pool_median(pool, mid):
+    """Entry `mid` of the 63-slot pool in RunDetector's order (core/puploc.go:267-269): numbers ascending (-0 == +0), every
+    NaN above every number, ties by slot -- the total order the library picks where Go's order with NaNs is an accident."""
+    order = sorted(range(63), key=lambda k: (bool(np.isnan(pool[k])), 0.0 if np.isnan(pool[k]) else float(pool[k]), k))
+    return pool[order[mid]]
+
+
+def _to_i32(v) -> int:
+    """int() into the 32-bit Row / Col field: truncation, saturated at the int32 range, NaN -> 0."""
+    if np.isnan(v):
+        return 0
+    return int(min(max(float(v), -2.0 ** 31), 2.0 ** 31 - 1))
 
 
 def _go_round(x: float) -> float:

@@ -433,6 +433,14 @@ void oracle_puploc_info(const oracle_puploc *p, uint32_t *stages, float *scales,
 /* int8 negation wraps (-(-128) == -128 in Go's int8): puploc.go:124-125 */
 static inline int64_t neg_i8(int8_t v) { return (int64_t)(int8_t)(uint8_t)(0u - (uint8_t)v); }
 
+/* Go's int(r) on amd64 (CVTTSS2SQ): truncation, and the int64 minimum for NaN and out-of-range values.  The products
+ * 256*int(r) and 65536*int(r) below wrap like Go's int64 arithmetic, so that minimum samples like int(r) == 0. */
+static inline int64_t go_int_f32(float v) {
+  if (!(v > -9223372036854775808.0f && v < 9223372036854775808.0f)) return INT64_MIN;
+  return (int64_t)v;
+}
+static inline int64_t go_mul_add(int64_t k, int64_t a, int64_t b) { return (int64_t)((uint64_t)k * (uint64_t)a + (uint64_t)b); }
+
 /* ---- core/puploc.go:106-154 classifyRegion ------------------------------ */
 static void puploc_classify(const oracle_puploc *plc, float r, float c, float s, int64_t nrows, int64_t ncols,
                             const uint8_t *pixels, int64_t dim, int flipV, float res[3]) {
@@ -445,15 +453,15 @@ static void puploc_classify(const oracle_puploc *plc, float r, float c, float s,
       for (uint32_t k = 0; k < plc->depth; k++) {
         const int8_t *cd = plc->codes + root + 4 * idx;
         int64_t rs = (int64_t)go_math_round((double)s);
-        int64_t r1 = go_min(nrows - 1, go_max(0, (256 * (int64_t)r + (int64_t)cd[0] * rs) >> 8));  /* :118 */
-        int64_t r2 = go_min(nrows - 1, go_max(0, (256 * (int64_t)r + (int64_t)cd[2] * rs) >> 8));  /* :119 */
+        int64_t r1 = go_min(nrows - 1, go_max(0, go_mul_add(256, go_int_f32(r), (int64_t)cd[0] * rs) >> 8));  /* :118 */
+        int64_t r2 = go_min(nrows - 1, go_max(0, go_mul_add(256, go_int_f32(r), (int64_t)cd[2] * rs) >> 8));  /* :119 */
         int64_t c1, c2;
         if (flipV) {                                                                                 /* :123-129 */
-          c1 = go_min(ncols - 1, go_max(0, (256 * (int64_t)c + neg_i8(cd[1]) * rs) >> 8));
-          c2 = go_min(ncols - 1, go_max(0, (256 * (int64_t)c + neg_i8(cd[3]) * rs) >> 8));
+          c1 = go_min(ncols - 1, go_max(0, go_mul_add(256, go_int_f32(c), neg_i8(cd[1]) * rs) >> 8));
+          c2 = go_min(ncols - 1, go_max(0, go_mul_add(256, go_int_f32(c), neg_i8(cd[3]) * rs) >> 8));
         } else {
-          c1 = go_min(ncols - 1, go_max(0, (256 * (int64_t)c + (int64_t)cd[1] * rs) >> 8));
-          c2 = go_min(ncols - 1, go_max(0, (256 * (int64_t)c + (int64_t)cd[3] * rs) >> 8));
+          c1 = go_min(ncols - 1, go_max(0, go_mul_add(256, go_int_f32(c), (int64_t)cd[1] * rs) >> 8));
+          c2 = go_min(ncols - 1, go_max(0, go_mul_add(256, go_int_f32(c), (int64_t)cd[3] * rs) >> 8));
         }
         idx = 2 * idx + 1 + (pixels[r1 * dim + c1] > pixels[r2 * dim + c2] ? 1 : 0);                /* :130-136 */
       }
@@ -493,10 +501,10 @@ static void puploc_classify_rotated(const oracle_puploc *plc, float r, float c, 
         if (flipV) { col1 = neg_i8(cd[1]); col2 = neg_i8(cd[3]); }
         else { col1 = (int64_t)cd[1]; col2 = (int64_t)cd[3]; }
         int64_t iqc = (int64_t)qcos, iqs = (int64_t)qsin;
-        int64_t r1 = go_min(nrows - 1, go_max(0, 65536 * (int64_t)r + iqc * row1 - iqs * col1) >> 16);  /* :188 */
-        int64_t c1 = go_min(ncols - 1, go_max(0, 65536 * (int64_t)c + iqs * row1 + iqc * col1) >> 16);  /* :189 */
-        int64_t r2 = go_min(nrows - 1, go_max(0, 65536 * (int64_t)r + iqc * row2 - iqs * col2) >> 16);  /* :190 */
-        int64_t c2 = go_min(ncols - 1, go_max(0, 65536 * (int64_t)c + iqs * row2 + iqc * col2) >> 16);  /* :191 */
+        int64_t r1 = go_min(nrows - 1, go_max(0, go_mul_add(65536, go_int_f32(r), iqc * row1 - iqs * col1)) >> 16);  /* :188 */
+        int64_t c1 = go_min(ncols - 1, go_max(0, go_mul_add(65536, go_int_f32(c), iqs * row1 + iqc * col1)) >> 16);  /* :189 */
+        int64_t r2 = go_min(nrows - 1, go_max(0, go_mul_add(65536, go_int_f32(r), iqc * row2 - iqs * col2)) >> 16);  /* :190 */
+        int64_t c2 = go_min(ncols - 1, go_max(0, go_mul_add(65536, go_int_f32(c), iqs * row2 + iqc * col2)) >> 16);  /* :191 */
         idx = 2 * idx + 1 + (pixels[r1 * dim + c1] <= pixels[r2 * dim + c2] ? 1 : 0);                   /* :193-199 */
       }
       int64_t lutIdx = 2 * ((int64_t)plc->trees * treeDepth * i + treeDepth * j + idx - (treeDepth - 1));
@@ -523,9 +531,30 @@ void oracle_puploc_classify(const oracle_puploc *plc, float r, float c, float s,
   }
 }
 
+/* Pool order of RunDetector's three sorts (:267-269), on (value, slot) pairs: numbers ascending (-0 == +0), every NaN
+ * above every number, ties (NaNs among themselves too) by slot.  A total order, the same as the kernels' rank sorts:
+ * with NaNs in the pool the order Go's sort.Sort leaves is an accident of its algorithm (DESIGN.md section 3.3). */
+typedef struct { float v; int slot; } pool_entry;
 static int cmp_f32(const void *a, const void *b) {
-  float x = *(const float *)a, y = *(const float *)b;
-  return (x > y) - (x < y);
+  const pool_entry *x = (const pool_entry *)a, *y = (const pool_entry *)b;
+  const int nx = x->v != x->v, ny = y->v != y->v;
+  if (nx != ny) return nx - ny;
+  if (!nx && x->v != y->v) return (x->v > y->v) - (x->v < y->v);
+  return (x->slot > y->slot) - (x->slot < y->slot);
+}
+static float pool_median(const float *pool, int mid) {
+  pool_entry e[63];
+  for (int i = 0; i < 63; i++) { e[i].v = pool[i]; e[i].slot = i; }
+  qsort(e, 63, sizeof(pool_entry), cmp_f32);
+  return e[mid].v;
+}
+/* int() of the picked row / col into the 32-bit field: truncation, saturated at the int32 range, NaN -> 0 (the CUDA
+ * conversion; the reference's int is 64-bit and has no such bound) */
+static int f32_to_i32(float v) {
+  if (v != v) return 0;
+  if (v >= 2147483648.0f) return INT32_MAX;
+  if (v <= -2147483648.0f) return INT32_MIN;
+  return (int)v;
 }
 
 /* ---- core/puploc.go:239-277 RunDetector --------------------------------- */
@@ -547,13 +576,10 @@ int oracle_puploc_run_detector(const oracle_puploc *plc, int row, int col, float
     oracle_puploc_classify(plc, rowf, colf, sc, angle, rows, cols, pixels, dim, flipV, res);
     prow[i] = res[0]; pcol[i] = res[1]; pscale[i] = res[2];          /* :261-263 */
   }
-  qsort(prow, 63, sizeof(float), cmp_f32);     /* :267-269 sorts ALL 63 pooled slots */
-  qsort(pcol, 63, sizeof(float), cmp_f32);
-  qsort(pscale, 63, sizeof(float), cmp_f32);
-  int mid = (int)go_math_round((double)perturbs / 2);   /* :273 */
-  *out_row = (int)prow[mid];
-  *out_col = (int)pcol[mid];
-  *out_scale = pscale[mid];
+  int mid = (int)go_math_round((double)perturbs / 2);   /* :273; :267-269 sort ALL 63 pooled slots */
+  *out_row = f32_to_i32(pool_median(prow, mid));
+  *out_col = f32_to_i32(pool_median(pcol, mid));
+  *out_scale = pool_median(pscale, mid);
   return 0;
 }
 

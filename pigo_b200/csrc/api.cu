@@ -34,7 +34,8 @@ struct TimingSlot {
 };
 static TimingSlot g_tslot[T_NSLOTS];
 static std::mutex g_tmu;
-static const char* kSlotNames[T_NSLOTS] = {"tiled", "gather", "deep", "finalize", "cluster", "puploc", "gray", "seeds", "rottab", "ycbcr", "gray_images", "merge", "region"};
+static const char* kSlotNames[T_NSLOTS] = {"tiled", "gather", "deep", "finalize", "cluster", "puploc", "gray", "seeds", "rottab", "ycbcr", "gray_images", "merge", "region",
+                                             "puploc_warp"};
 
 void timing_reset() {
   std::lock_guard<std::mutex> g(g_tmu);
@@ -1012,14 +1013,25 @@ static std::vector<int> plan_shards(const std::vector<uint64_t>& wins, const dou
 }
 
 // ---- RunDetector over uniform frames or over an image table (pigo_puploc_run_frames / pigo_puploc_run_images) -----------
+// How much a perturbation's scale can grow over the stages of cascade p: it is multiplied by `scales` after every stage
+// (core/puploc.go:151), so the last stage samples with up to max(1, |scales|)^(stages-1) times the initial scale.
+static double puploc_growth(const pigo_puploc* p) {
+  const double m = std::max(1.0, std::fabs((double)p->scales));
+  return p->stages > 1 ? std::pow(m, (double)(p->stages - 1)) : 1.0;
+}
+// The pair kernel's unrotated offsets (code * int(Round(s))) >> 8 are 32-bit, exact while |s| < 2^24 at every stage.  It is
+// given the seeds with |Scale| * growth <= 16384 (the initial scale is at most 1.075 |Scale|), far inside that bound.
+static bool puploc_in_envelope(float scale, double growth) { return std::fabs((double)scale) * growth <= 16384.0; }
+
 // Host seeds of a standalone RunDetector call: Perturbs range and frame / image index.  *wide = some seed lies outside the
-// 32-bit envelope of the pair kernel (it then runs on the warp-per-perturbation kernel).
-static int check_puploc_seeds(const pigo_point* seeds, int nseeds, const int32_t* seed_frame, int nframes, const char* unit, bool* wide) {
+// 32-bit envelope of the pair kernel for a cascade of this growth (the call then runs on the warp-per-perturbation kernel).
+static int check_puploc_seeds(double growth, const pigo_point* seeds, int nseeds, const int32_t* seed_frame, int nframes, const char* unit,
+                              bool* wide) {
   for (int i = 0; i < nseeds; ++i) {
     if (seeds[i].perturbs < 0 || seeds[i].perturbs > 63)
       return set_err(PIGO_E_INVALID, "seed %d: Perturbs=%d outside 0..63 (the reference panics, core/puploc.go:261)", i, seeds[i].perturbs);
     if (seed_frame && (seed_frame[i] < 0 || seed_frame[i] >= nframes)) return set_err(PIGO_E_INVALID, "seed %d: %s index out of range", i, unit);
-    if (!(std::fabs(seeds[i].scale) <= 16384.0f)) *wide = true;
+    if (!puploc_in_envelope(seeds[i].scale, growth)) *wide = true;
   }
   return PIGO_OK;
 }
@@ -1117,10 +1129,14 @@ static int puploc_run_on(pigo_puploc* p, const pigo_point* seeds, int nseeds, co
     W.seeds = d_seeds; W.out = d_out; W.randoms = d_rnd; W.rng_seed = rng_seed; W.frames = d_pix; W.frame_stride = px.stride;
     W.slot_frame = d_sf; W.flipv = d_flip; W.slots_per_frame = 0; W.nrows = px.rows; W.ncols = px.cols; W.dim = px.dim; W.rot_slot = rot_slot;
     W.first = 0; W.span = 1; W.stride = 1; W.nwork = nseeds; W.ntabs = 1; W.tab[0] = R->tab; W.images = d_img;
+    W.stats = walk_stats_buffer(dev);
     done = launch_puploc_pairs(W, (unsigned int*)w->counters.p, R->num_sms, st) == 0;
   }
-  if (!done)
+  if (!done) {
+    timing_begin(T_PUPLOC_WARP, st);   // "t_puploc_warp_n": the calls that ran the 64-bit kernel
     launch_puploc(R->tab, d_seeds, nseeds, d_rnd, rng_seed, d_pix, d_sf, px.stride, px.rows, px.cols, px.dim, rot_slot, d_flip, d_out, d_img, st);
+    timing_end(T_PUPLOC_WARP, st);
+  }
   timing_end(T_PUPLOC, st);
   g_launches++;
   CUDA_TRY(cudaGetLastError());
@@ -1558,7 +1574,7 @@ int pigo_puploc_run_frames(const pigo_puploc* pc, const pigo_point* seeds, int n
   if (rc) return rc;
   if (nseeds == 0) return PIGO_OK;
   bool wide = false;
-  if (!(flags & PIGO_OUT_DEVICE) && (rc = check_puploc_seeds(seeds, nseeds, seed_frame, nframes, "frame", &wide))) return rc;
+  if (!(flags & PIGO_OUT_DEVICE) && (rc = check_puploc_seeds(puploc_growth(p), seeds, nseeds, seed_frame, nframes, "frame", &wide))) return rc;
   const PuplocPixels px{pixels, nframes, frame_stride, rows, cols, dim, nullptr};
   return puploc_run_on(p, seeds, nseeds, seed_frame, randoms, rng_seed, px, angle, flipv, out, wide, flags, stream_);
 }
@@ -1575,7 +1591,8 @@ int pigo_puploc_run_images(const pigo_puploc* pc, const pigo_point* seeds, int n
   int rc = check_image_geometry(images, nimages, 1, true);
   if (rc) return rc;
   bool wide = false;
-  if (!(flags & PIGO_OUT_DEVICE) && (rc = check_puploc_seeds(seeds, nseeds, seed_image, nimages, "image", &wide))) return rc;
+  if (!(flags & PIGO_OUT_DEVICE) && (rc = check_puploc_seeds(pc ? puploc_growth(pc) : 1.0, seeds, nseeds, seed_image, nimages, "image", &wide)))
+    return rc;
   if (!pc) return set_err(PIGO_E_INVALID, "null cascade");
   if ((rc = ensure_device())) return rc;
   if (nseeds == 0) return PIGO_OK;
@@ -1634,6 +1651,11 @@ static int detect_on(int dev, pigo_cascade* face, pigo_puploc* puploc, pigo_pupl
   if (!R) return rc;
   PuplocReplica* PR = puploc_replica(puploc, dev, &rc);
   if (!PR) return rc;
+  // Every RunDetector call of the pipeline runs on the pair kernel, whose unrotated offsets are exact while |s| < 2^24 at
+  // every stage: a cascade whose scale grows by more than 512 over its stages could leave that range from a seed of 16384.
+  for (int cidx = -1; cidx < ncalls; ++cidx)
+    if (puploc_growth(cidx < 0 ? puploc : flp[cidx]) > 512.0)
+      return set_err(PIGO_E_INVALID, "%s cascade: |scales|^(stages-1) exceeds 512, beyond the pipeline kernel's 32-bit range", cidx < 0 ? "pupil" : "landmark");
   const int stride = 2 + ncalls;
   PupWork W{};
   W.ntabs = 1; W.tab[0] = PR->tab;
@@ -1651,6 +1673,7 @@ static int detect_on(int dev, pigo_cascade* face, pigo_puploc* puploc, pigo_pupl
     W.tab_of[cidx] = (uint8_t)k; W.flip_of[cidx] = flp_flip && flp_flip[cidx] ? 1 : 0;
   }
   if ((rc = use_device(dev))) return rc;
+  W.stats = walk_stats_buffer(dev);
   const bool out_dev = flags & PIGO_OUT_DEVICE;
   const int det_cap = P.det_cap > 0 ? P.det_cap : 2048;
 

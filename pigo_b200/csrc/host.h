@@ -20,13 +20,16 @@ void raise_dyn_smem(const void* fn, int bytes);
 
 // Per-kernel CUDA-event timing (enabled by option "timing"): every launch of kernel class `slot` is bracketed by an
 // event pair on its stream; "t_<name>_ns" / "t_<name>_n" return the summed device time and the launch count.  T_REGION
-// brackets, inside T_TILED, only the fused launches that run the region role (after their tensor maps were encoded).
+// brackets, inside T_TILED, only the fused launches that run the region role (after their tensor maps were encoded);
+// T_PUPLOC_WARP brackets, inside T_PUPLOC, only the launches of the 64-bit warp-per-perturbation kernel (puploc_kernel).
 enum TimeSlot { T_TILED = 0, T_GATHER, T_DEEP, T_FINALIZE, T_CLUSTER, T_PUPLOC, T_GRAY, T_SEEDS, T_ROTTAB, T_YCBCR, T_GRAY_IMAGES, T_MERGE, T_REGION,
-                T_NSLOTS };
+                T_PUPLOC_WARP, T_NSLOTS };
 void timing_reset();
 void walk_stats_reset();
 long long walk_stats_query(int which);
-unsigned long long* walk_stats_buffer(int dev);   // nullptr unless option walk_stats is on
+// nullptr unless option walk_stats is on; [0], [1]: the tile role's live lanes and walk iterations, [2], [3]: stages of the
+// RunDetector pair kernel served from its shared pixel patch / gathered from global memory
+unsigned long long* walk_stats_buffer(int dev);
 long long timing_query(const std::string& key);
 void timing_begin(int slot, cudaStream_t st);
 void timing_end(int slot, cudaStream_t st);
@@ -55,6 +58,7 @@ struct Options {
   std::atomic<long long> copy_chunk{8};     // host_stream: frames per H2D copy chunk
   std::atomic<long long> tile_tmap{1};      // tile fill: 1 = one TMA tensor copy per tile (cuTensorMapEncodeTiled descriptors), 0 = one bulk copy per tile row
   std::atomic<long long> walk_stats{0};     // 1 = count live lanes per walk iteration of the tile role ("walk_useful" / "walk_iters" read them back)
+                                            // and the pair kernel's patch / global stages ("pup_patch_stages" / "pup_global_stages")
   std::atomic<long long> tile_core_cap{0};  // largest tile core edge in pixels; 0 = unlimited
   std::atomic<long long> deep_smem{0};      // deep kernel with the tree records in shared memory: 0 = auto, 1 = on, 2 = off; deep_smem_threads = CTA size
   std::atomic<long long> deep_smem_threads{256};
@@ -106,6 +110,8 @@ struct Options {
     if (k.rfind("t_", 0) == 0) return timing_query(k);
     if (k == "walk_useful") return walk_stats_query(0);
     if (k == "walk_iters") return walk_stats_query(1);
+    if (k == "pup_patch_stages") return walk_stats_query(2);
+    if (k == "pup_global_stages") return walk_stats_query(3);
     std::atomic<long long>* f = find(k);
     return f ? f->load() : -1;
   }
@@ -141,6 +147,7 @@ struct PupWork {
   uint8_t tab_of[32], flip_of[32];
   const ImageDesc* images;     // mixed-size call: the image table the frame indices refer to (frames .. dim unused); nullptr = uniform frames
   const int32_t* face_rot;     // angle sweep (rot_slot == kRotSlotPerFace, with images): rotation slot of face slot `slot / stride`
+  unsigned long long* stats;   // option walk_stats (else nullptr): [2] += 1 per stage served from the pixel patch, [3] += 1 per other stage
 };
 
 // Angle sweep merge (cluster.cu).  cluster_kernel<true> reads the sorted keys (position in D_i in the low 32 bits) and the

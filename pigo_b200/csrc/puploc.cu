@@ -29,6 +29,17 @@ __device__ __forceinline__ uint32_t mix64(uint64_t x) {
   return (uint32_t)(x >> 40);  // 24 random bits
 }
 
+// Rank order of the 63-slot pool sorts, a total order so that exactly
+// one slot has each rank: numbers ascending (-0 == +0), every NaN above every number, ties (NaNs among themselves too)
+// by slot index.  The reference's sort.Sort order is an accident of its algorithm once NaNs take part (DESIGN.md §3.3).
+// rank_key maps a value to an unsigned key in that order; value j comes before value i when key j < key i, or when the keys
+// are equal and j < i.
+__device__ __forceinline__ unsigned rank_key(float v) {
+  if (v != v) return 0xFFFFFFFFu;
+  const unsigned b = __float_as_uint(v == 0.f ? 0.f : v);
+  return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+}
+
 // One CTA (32 warps) per seed; one WARP per perturbation (two rounds cover the 63 slots) and one LANE per tree of the
 // current stage: the trees of a stage are independent of each other (they all start from the stage's (r, c, s)), only
 // the float32 sums dr, dc are order-sensitive -- lanes walk the trees in parallel, then the sums are formed in tree order
@@ -52,8 +63,10 @@ __global__ void __launch_bounds__(1024, 1) puploc_kernel(PuplocTables T, const p
   if (IMG && rot_slot == kRotSlotPerImage) rot_slot = im.rot_slot;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   __shared__ float rows_[64], cols_[64], scal_[64];
+  __shared__ unsigned krow_[64], kcol_[64], kscal_[64];   // their rank_key
   const pigo_point seed = seeds[sidx];
-  const int P = seed.perturbs;
+  if (seed.perturbs < 0) return;               // inactive seed (CTA-uniform): out[sidx] is left as it is, like the pair kernel's
+  const int P = min(seed.perturbs, 63);        // device seeds are not checked on the host: Perturbs above 63 run as 63
   const bool flip = flipv_arr ? (flipv_arr[sidx] != 0) : false;
   const int L = T.leaves;
   const int tree_codes = 4 * L;   // device layout: one pad word, then the 4L-4 code bytes (node i at word i+1), see PuplocTables
@@ -130,23 +143,23 @@ __global__ void __launch_bounds__(1024, 1) puploc_kernel(PuplocTables T, const p
       }
     }
     // pool slots >= Perturbs stay 0 (fresh pool object, :228-236); all 63 slots are sorted (:267-269)
-    if (lane == 0) { rows_[i] = r; cols_[i] = c; scal_[i] = s; }
+    if (lane == 0) { rows_[i] = r; cols_[i] = c; scal_[i] = s; krow_[i] = rank_key(r); kcol_[i] = rank_key(c); kscal_[i] = rank_key(s); }
   }
   __syncthreads();
   const int i = threadIdx.x;
   const int mid = (int)llround((double)P / 2);  // int(math.Round(float64(Perturbs)/2)), :273
   if (i < 63) {
-    // rank sort of 63 values (ties: index order); the thread whose rank == mid publishes it
-    const float vr = rows_[i], vc = cols_[i], vs = scal_[i];
+    // rank sort of 63 values (rank_key, ties: index order); the thread whose rank == mid publishes it
+    const unsigned vr = krow_[i], vc = kcol_[i], vs = kscal_[i];
     int kr = 0, kc = 0, ks = 0;
     for (int j = 0; j < 63; ++j) {
-      kr += (rows_[j] < vr || (rows_[j] == vr && j < i)) ? 1 : 0;
-      kc += (cols_[j] < vc || (cols_[j] == vc && j < i)) ? 1 : 0;
-      ks += (scal_[j] < vs || (scal_[j] == vs && j < i)) ? 1 : 0;
+      kr += (krow_[j] < vr || (krow_[j] == vr && j < i)) ? 1 : 0;
+      kc += (kcol_[j] < vc || (kcol_[j] == vc && j < i)) ? 1 : 0;
+      ks += (kscal_[j] < vs || (kscal_[j] == vs && j < i)) ? 1 : 0;
     }
-    if (kr == mid) out[sidx].row = (int)vr;      // int() truncation, :273
-    if (kc == mid) out[sidx].col = (int)vc;
-    if (ks == mid) out[sidx].scale = vs;
+    if (kr == mid) out[sidx].row = (int)rows_[i];      // int() truncation, :273
+    if (kc == mid) out[sidx].col = (int)cols_[i];
+    if (ks == mid) out[sidx].scale = scal_[i];
     if (i == 0) out[sidx].perturbs = 0;          // the returned Puploc leaves Perturbs unset (:272-276)
   }
 }
@@ -163,7 +176,8 @@ __global__ void __launch_bounds__(1024, 1) puploc_kernel(PuplocTables T, const p
 // Inactive slots (seed.perturbs < 0) are skipped.  32-bit coordinate arithmetic, exact because
 //   (256*int(r) + code*rs) >> 8  ==  int(r) + ((code*rs) >> 8)        (256*int(r) is a multiple of 256), and
 //   max(0, 65536*int(r) + x) >> 16  ==  max(0, int(r) + (x >> 16))    (rotated variant, see RotNode in common.cuh);
-// seeds with |Scale| > 16384 (products would leave 32 bits) are left to the 64-bit kernel above by the host.
+// exact while |int(Round(s))| < 2^24 at every stage; the host leaves seeds with |Scale| * max(1, |scales|)^(stages-1) > 16384
+// to the 64-bit kernel above (standalone calls) or refuses cascades whose scale grows by more than 512 (pipeline).
 constexpr int kPairThreads = 512;
 // Sample area of one perturbation in the coming stage: centre +- (|rs|/2 + 1) unrotated ((code*rs) >> 8 with |code| <= 128);
 // rotated: the offsets are (iqc*k0 -+ iqs*k1) >> 16 with iqc, iqs fixed from the INITIAL scale of the perturbation (core/puploc.go:166),
@@ -214,8 +228,8 @@ __global__ void __launch_bounds__(kPairThreads, PATCH ? 2 : 3) puploc_pair_kerne
     const int j = (int)(w % (unsigned)W.span);
     const int slot = (int)(w / (unsigned)W.span) * W.stride + W.first + j;
     const pigo_point seed = W.seeds[slot];
-    const int P = seed.perturbs;
-    if (P < 0) continue;                                   // inactive slot (CTA-uniform)
+    if (seed.perturbs < 0) continue;                       // inactive slot (CTA-uniform)
+    const int P = min(seed.perturbs, 63);                  // device seeds are not checked on the host: Perturbs above 63 run as 63
     const PuplocTables T = W.tab[W.tab_of[j]];
     const bool flip = W.flipv ? (W.flipv[slot] != 0) : (W.flip_of[j] != 0);
     const int frame = W.slots_per_frame > 0 ? slot / W.slots_per_frame : (W.slot_frame ? W.slot_frame[slot] : 0);
@@ -291,6 +305,7 @@ __global__ void __launch_bounds__(kPairThreads, PATCH ? 2 : 3) puploc_pair_kerne
 
     const int npairs = P * T.trees;
     for (int st = 0; st < T.stages; ++st) {
+      if (W.stats && tid == 0) atomicAdd(W.stats + ((PATCH && p_use) ? 2 : 3), 1ull);   // option walk_stats: patch / global stages
       for (int p = tid; p < npairs; p += nt) {
         const int i = p / T.trees, t = p - i * T.trees;
         const int ir = s_ir[i], ic = s_ic[i], rs = s_rs[i];
@@ -362,19 +377,25 @@ __global__ void __launch_bounds__(kPairThreads, PATCH ? 2 : 3) puploc_pair_kerne
         if (tid == 0) { s_box[0] = INT_MAX; s_box[1] = INT_MIN; s_box[2] = INT_MAX; s_box[3] = INT_MIN; }
       }
     }
-    // pool slots >= Perturbs stay 0 (fresh pool object, :228-236); all 63 slots are sorted (:267-269)
+    // pool slots >= Perturbs stay 0 (fresh pool object, :228-236); all 63 slots are sorted (:267-269) by their rank_key,
+    // which take the place of the integer coordinates (no longer read)
+    unsigned* k_r = reinterpret_cast<unsigned*>(s_ir);
+    unsigned* k_c = reinterpret_cast<unsigned*>(s_ic);
+    unsigned* k_s = reinterpret_cast<unsigned*>(s_rs);
+    if (tid < 63) { k_r[tid] = rank_key(s_r[tid]); k_c[tid] = rank_key(s_c[tid]); k_s[tid] = rank_key(s_s[tid]); }
+    __syncthreads();
     if (tid < 63) {
       const int mid = (int)llround((double)P / 2);   // int(math.Round(float64(Perturbs)/2)), :273
-      const float vr = s_r[tid], vc = s_c[tid], vs = s_s[tid];
+      const unsigned vr = k_r[tid], vc = k_c[tid], vs = k_s[tid];
       int kr = 0, kc = 0, ks = 0;
       for (int q = 0; q < 63; ++q) {
-        kr += (s_r[q] < vr || (s_r[q] == vr && q < tid)) ? 1 : 0;
-        kc += (s_c[q] < vc || (s_c[q] == vc && q < tid)) ? 1 : 0;
-        ks += (s_s[q] < vs || (s_s[q] == vs && q < tid)) ? 1 : 0;
+        kr += (k_r[q] < vr || (k_r[q] == vr && q < tid)) ? 1 : 0;
+        kc += (k_c[q] < vc || (k_c[q] == vc && q < tid)) ? 1 : 0;
+        ks += (k_s[q] < vs || (k_s[q] == vs && q < tid)) ? 1 : 0;
       }
-      if (kr == mid) W.out[slot].row = (int)vr;      // int() truncation, :273
-      if (kc == mid) W.out[slot].col = (int)vc;
-      if (ks == mid) W.out[slot].scale = vs;
+      if (kr == mid) W.out[slot].row = (int)s_r[tid];      // int() truncation, :273
+      if (kc == mid) W.out[slot].col = (int)s_c[tid];
+      if (ks == mid) W.out[slot].scale = s_s[tid];
       if (tid == 0) W.out[slot].perturbs = 0;        // the returned Puploc leaves Perturbs unset (:272-276)
     }
   }

@@ -377,13 +377,13 @@ int describe_plan(const std::vector<ScaleEntry>& plan, uint64_t wins, int ntrees
   return PIGO_OK;
 }
 
-// ---- developer counter: live lanes per walk iteration of the tile role (option walk_stats) ----------------------------------
+// ---- developer counters (option walk_stats): live lanes per walk iteration of the tile role, the pair kernel's patch stages --------
 static unsigned long long* g_walk_stats[kMaxDevices] = {};
 unsigned long long* walk_stats_buffer(int dev) {
   if (!g_opt.walk_stats.load() || dev < 0 || dev >= kMaxDevices) return nullptr;
   if (!g_walk_stats[dev]) {
-    if (cudaMalloc((void**)&g_walk_stats[dev], 16) != cudaSuccess) { cudaGetLastError(); return nullptr; }
-    cudaMemset(g_walk_stats[dev], 0, 16);
+    if (cudaMalloc((void**)&g_walk_stats[dev], 32) != cudaSuccess) { cudaGetLastError(); return nullptr; }
+    cudaMemset(g_walk_stats[dev], 0, 32);
   }
   return g_walk_stats[dev];
 }
@@ -391,7 +391,7 @@ void walk_stats_reset() {
   int cur = 0;
   cudaGetDevice(&cur);
   for (int d = 0; d < kMaxDevices; ++d)
-    if (g_walk_stats[d]) { cudaSetDevice(d); cudaMemset(g_walk_stats[d], 0, 16); }
+    if (g_walk_stats[d]) { cudaSetDevice(d); cudaMemset(g_walk_stats[d], 0, 32); }
   cudaSetDevice(cur);
 }
 long long walk_stats_query(int which) {
@@ -400,11 +400,11 @@ long long walk_stats_query(int which) {
   cudaGetDevice(&cur);
   for (int d = 0; d < kMaxDevices; ++d)
     if (g_walk_stats[d]) {
-      unsigned long long v[2] = {0, 0};
+      unsigned long long v[4] = {0, 0, 0, 0};
       cudaSetDevice(d);
       cudaDeviceSynchronize();
-      cudaMemcpy(v, g_walk_stats[d], 16, cudaMemcpyDeviceToHost);
-      total += (long long)v[which & 1];
+      cudaMemcpy(v, g_walk_stats[d], 32, cudaMemcpyDeviceToHost);
+      total += (long long)v[which & 3];
     }
   cudaSetDevice(cur);
   return total;
