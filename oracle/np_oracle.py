@@ -106,7 +106,7 @@ class FaceCascade:
                 idx = 2 * idx + (flat[x1] <= flat[x2])
             out[alive] = out[alive] + self.preds[t][idx - self.leaves]   # float32 add, tree order
             ntre[alive] += 1
-            keep = out[alive] > self.thresh[t]
+            keep = ~(out[alive] <= self.thresh[t])   # core/pigo.go:139-141: a NaN sum or threshold does not reject
             alive = alive[keep]
         if self.ntrees > 0:
             result[alive] = out[alive] - self.thresh[self.ntrees - 1]

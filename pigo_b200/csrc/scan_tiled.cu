@@ -115,6 +115,7 @@ __device__ __forceinline__ void gather_role(const TiledArgs& A, const uint8_t* s
   const uint8_t* b_base = S.frames;
   uint32_t b_wid0 = 0;
   bool more = true;
+  bool queue_full = false;   // the deep queue refused one of this lane's windows: its later windows finish here too
 
   for (;;) {
     unsigned live_any = 0;
@@ -268,7 +269,7 @@ __device__ __forceinline__ void gather_role(const TiledArgs& A, const uint8_t* s
 #pragma unroll
     for (int u = 0; u < NG; ++u) {
       if (alive[u]) {
-        acc[u] += pred[u];                               // core/pigo.go:137
+        acc[u] += pred[u];                              // core/pigo.go:137
         tbo[u] += kTreeRec;
         if (ROT) sv[u] += 1;                             // next tree's node table
         if (acc[u] <= thr[u]) {                          // :139-141
@@ -280,13 +281,18 @@ __device__ __forceinline__ void gather_role(const TiledArgs& A, const uint8_t* s
             if (pos < S.cap) S.raw[(size_t)fr[u] * S.cap + pos] = RawDet{wid[u], q};
           }
           alive[u] = false;
-        } else if (tbo[u] >= casc_end && S.longq != nullptr) {
+        } else if (tbo[u] >= casc_end && S.longq != nullptr && !queue_full) {
           // survived the resident trees: hand over to the deep (GROUP-trees-per-step) kernel; if its queue is full
           // the window simply continues here on the global tables
           const unsigned pos = atomicAdd(S.long_count, 1u);
           if (pos < S.long_cap) {
             S.longq[pos] = DeepItem{wid[u], pack_frame_si(fr[u], wsi[u]), (int)((tbo[u] - casc) / kTreeRec), acc[u]};
             alive[u] = false;
+          } else {
+            // After its first refusal a lane asks no more (at most one refusal per lane): a window that kept asking
+            // after every later tree would add one to the u32 count per tree, and enough asks wrap it back into
+            // [0, long_cap), where new items would overwrite queued ones.
+            queue_full = true;
           }
         }
       }
