@@ -314,3 +314,120 @@ func (pg *Pigo) DetectDecoded(plc *PuplocCascade, calls []LandmarkCall, imgs []i
 		return faceResults(faces, nfaces, points, faceCap, ncalls, pp.MinFaceScale)
 	}
 }
+
+// BlurParams selects and sizes the face blur of BlurFaces and BlurDecoded (pigo_blur_params): every face with Q >= MinQ is
+// blurred over a disc of radius int(Scale*DiscRatio) with a box of radius min(1023, max(Radius, int(Scale*RadiusRatio))),
+// a pixel covered by several discs taking the largest box.  examples/facedet/faceblur.py's values are
+// BlurParams{MinQ: 5, DiscRatio: 0.5, Radius: 15}.
+type BlurParams struct {
+	MinQ, DiscRatio, RadiusRatio float64
+	Radius                       int
+}
+
+func (bp BlurParams) c() C.pigo_blur_params {
+	return C.pigo_blur_params{min_q: C.double(bp.MinQ), disc_ratio: C.double(bp.DiscRatio), radius_ratio: C.double(bp.RadiusRatio),
+		radius: C.int32_t(bp.Radius)}
+}
+
+// blurPack packs imgs to pinned memory as packDecoded does; unpack copies the blurred planes back into the images' Pix (Y, Cb
+// and Cr).  The blur writes *image.YCbCr (Rect.Min >= 0), *image.NRGBA, *image.RGBA, *image.Gray and *image.CMYK values in
+// place; any other type panics, and so does an image listed twice (its planes would be blurred twice).
+func blurPack(fn string, imgs []image.Image) (desc []C.pigo_decoded, unpack, free func()) {
+	for _, img := range imgs {
+		switch src := img.(type) {
+		case *image.YCbCr:
+			if b := src.Bounds(); b.Min.X < 0 || b.Min.Y < 0 {
+				panic("pigo: " + fn + " needs a YCbCr rectangle origin >= 0")
+			}
+		case *image.NRGBA, *image.RGBA, *image.Gray, *image.CMYK:
+		default:
+			panic("pigo: " + fn + " blurs *image.YCbCr, *image.NRGBA, *image.RGBA, *image.Gray and *image.CMYK images")
+		}
+	}
+	desc, free = packDecoded(imgs)
+	unpack = func() {
+		for i, img := range imgs {
+			for j, pl := range partOf(img).planes {
+				if len(pl) > 0 {
+					copy(pl, unsafe.Slice((*uint8)(unsafe.Pointer(desc[i].plane[j])), len(pl)))
+				}
+			}
+		}
+	}
+	return desc, unpack, free
+}
+
+// BlurFaces blurs faces[i] of imgs[i] in place (pigo_blur_faces), with the coordinates RunCascadeDecoded and DetectDecoded
+// return.  The planes cross PCIe once in each direction.
+func BlurFaces(imgs []image.Image, faces [][]Detection, bp BlurParams) {
+	n := len(imgs)
+	if len(faces) != n {
+		panic("pigo: BlurFaces needs one face list per image")
+	}
+	if n == 0 {
+		return
+	}
+	desc, unpack, free := blurPack("BlurFaces", imgs)
+	defer free()
+	capacity := 1
+	for _, f := range faces {
+		capacity = max(capacity, len(f))
+	}
+	buf := make([]C.pigo_det, n*capacity)
+	cnt := make([]C.int, n)
+	for i, f := range faces {
+		cnt[i] = C.int(len(f))
+		for k, d := range f {
+			buf[i*capacity+k] = C.pigo_det{row: C.int32_t(d.Row), col: C.int32_t(d.Col), scale: C.int32_t(d.Scale), q: C.float(d.Q)}
+		}
+	}
+	prm := bp.c()
+	if _, err := call(func() C.int {
+		return C.pigo_blur_faces(&desc[0], C.int(n), &buf[0], C.int(capacity), &cnt[0], &prm, C.PIGO_MEM_HOST, nil)
+	}); err != nil {
+		panic(err)
+	}
+	unpack()
+}
+
+// BlurDecoded detects and blurs the faces of decoded images in one call (pigo_blur_decoded): RunCascade on
+// RgbToGrayscale(ImgToNRGBA(imgs[i])) with cps[i]'s MinSize, MaxSize, ShiftFactor and ScaleFactor (its ImageParams is not
+// used) at angles[i] (nil: every image at 0), ClusterDetections(iou), then BlurFaces on every cluster, all on the GPU.
+// Returns the face lists, list i as ClusterDetections returns it for image i.  Image types as BlurFaces.
+func (pg *Pigo) BlurDecoded(imgs []image.Image, cps []CascadeParams, angles []float64, iou float64, bp BlurParams) [][]Detection {
+	n := len(imgs)
+	if len(cps) != n {
+		panic("pigo: BlurDecoded needs one CascadeParams per image")
+	}
+	angles = decodedAngles("BlurDecoded", angles, n)
+	if n == 0 {
+		return nil
+	}
+	desc, unpack, free := blurPack("BlurDecoded", imgs)
+	defer free()
+	_, prm, freePrm := cascadeParams(cps)
+	defer freePrm()
+	bpc := bp.c()
+	detCap := 2048 // face_cap = det_cap: an image never has more clusters than raw detections
+	for {
+		faces := make([]C.pigo_det, n*detCap)
+		nfaces := make([]C.int, n)
+		rc, err := call(func() C.int {
+			return C.pigo_blur_decoded(pg.h, &desc[0], C.int(n), &prm[0], anglesPtr(angles), C.double(iou), C.int(detCap), &bpc, &faces[0],
+				C.int(detCap), &nfaces[0], C.PIGO_MEM_HOST, nil)
+		})
+		if rc == C.PIGO_E_CAP {
+			detCap *= 4 // an image has more raw detections than det_cap: no plane was written
+			continue
+		}
+		if err != nil {
+			panic(err)
+		}
+		unpack()
+		out := make([][]Detection, n)
+		for i := range out {
+			out[i] = toGo(faces[i*detCap:(i+1)*detCap], int(nfaces[i]))
+		}
+		return out
+	}
+}

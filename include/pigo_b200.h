@@ -425,6 +425,47 @@ typedef struct {
 int pigo_gray_images(const pigo_decoded *src, int n, uint8_t *gray, size_t *gray_bytes, pigo_image *images, unsigned flags,
                      void *stream);
 
+/* ---- Face blur of decoded images, in place (additive; what examples/facedet/faceblur.py does with the faces of
+ * examples/facedet/pigo.go).  Per entry i, in the rectangle-relative coordinates of the gray image pigo_gray_images makes:
+ *   blurred faces: f with (double)f.q >= min_q (a NaN q never), skipping scale < 0, |row| > 2^24, |col| > 2^24, scale > 2^24;
+ *   disc:          d = (int64)(scale * disc_ratio) in float64; luma pixel (y, x) is covered iff (y-row)^2 + (x-col)^2 <= d^2;
+ *   box radius:    R_f = min(1023, max(radius, (int64)(scale * radius_ratio))); a covered pixel uses Rmax(y, x), the largest
+ *                  R_f of the faces covering it (the result does not depend on face order);
+ *   value:         the box mean over [j-ry, j+ry] x [i-rx, i+rx] of the plane's samples, indices clamped to the plane,
+ *                  (sum + n/2) / n in integers with n = (2ry+1)(2rx+1), every mean over the input as it was before the call;
+ *   Gray, NRGBA, RGBA, CMYK: ry = rx = Rmax, every byte channel alone, alpha included.  YCbCr: the Y plane as Gray; a Cb / Cr
+ *   sample (j, i) is blurred iff its anchor luma ((min_y>>ys)+j << ys, (min_x>>xs)+i << xs), clamped into the rectangle and
+ *   made relative, is covered, with ry = Rmax >> ys, rx = Rmax >> xs over the chroma extent of the rectangle.
+ * Other samples keep their bytes; bytes past a row's end are never written.  faceblur.py's values are min_q 5, disc_ratio
+ * 0.5, radius 15, radius_ratio 0 (a 31x31 box where its cv2.blur uses 30x30). */
+typedef struct {
+  double min_q, disc_ratio, radius_ratio;
+  int32_t radius;
+} pigo_blur_params;
+
+#define PIGO_FACES_DEVICE 4u   /* pigo_blur_faces: `faces` and `n_faces` are device pointers */
+
+/* Blurs the planes of src[0..n) in place around faces[i][0..n_faces[i]) ([n][face_cap] as pigo_cluster_batch and
+ * pigo_detect_images write them; n_faces[i] is clamped to 0..face_cap).  flags: PIGO_FRAMES_DEVICE = the planes are device
+ * pointers (on a caller's stream the call then returns without synchronising), PIGO_FACES_DEVICE = faces and n_faces are.
+ * Host planes are copied to the device and written back before return (only the bytes of each row's samples).
+ * PIGO_E_INVALID before any device work and without a device: what pigo_gray_images rejects, a format other than YCbCr, NRGBA,
+ * RGBA, Gray and CMYK, two byte-identical descriptors, a null bp, radius outside 0..1023, a ratio that is NaN, negative or above
+ * 16, a NaN min_q, a negative face_cap, null faces (face_cap > 0) or n_faces; and a stream that is being captured. */
+int pigo_blur_faces(const pigo_decoded *src, int n, const pigo_det *faces, int face_cap, const int *n_faces,
+                    const pigo_blur_params *bp, unsigned flags, void *stream);
+
+/* The whole job in one call: pigo_gray_images of src, pigo_run_cascade_images_params of its images with cparams and angles
+ * (det_cap raw detections per entry, 0 = 2048), pigo_cluster_batch(iou_threshold), then pigo_blur_faces of the clusters; host
+ * planes cross PCIe once in each direction.  faces[n][face_cap] / n_faces[n] are byte for byte what that composition
+ * returns (faces may be NULL when face_cap == 0).  Every cluster is blurred; if an entry has more than face_cap the call
+ * returns PIGO_E_CAP with the required counts in n_faces.  An entry with more than det_cap raw detections fails with
+ * PIGO_E_CAP naming it, before any plane is written.  Invalid arguments as pigo_blur_faces and pigo_run_cascade_images_params
+ * on the decoded geometry (a null face cascade, cparams or n_faces, a negative det_cap). */
+int pigo_blur_decoded(const pigo_cascade *face, const pigo_decoded *src, int n, const pigo_cascade_params *cparams,
+                      const double *angles, double iou_threshold, int det_cap, const pigo_blur_params *bp,
+                      pigo_det *faces, int face_cap, int *n_faces, unsigned flags, void *stream);
+
 /* ---- Multi-GPU forms of the mixed-size and decoded calls: HOST inputs and HOST outputs, over the devices of
  * pigo_init_devices (the default device if none were selected), one host thread per shard, no data-path collective.
  * The entries are cut into contiguous ranges of the caller's order (an entry is never split) that balance a modelled

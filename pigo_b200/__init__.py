@@ -29,7 +29,7 @@ DATA_DIR = os.path.join(_HERE, "data")
 CASCADE_DIR = os.path.join(DATA_DIR, "cascade")
 
 PIGO_OK, PIGO_E_INVALID, PIGO_E_CUDA, PIGO_E_CAP, PIGO_E_NOMEM, PIGO_E_NODEVICE = 0, -1, -2, -3, -4, -5
-MEM_HOST, FRAMES_DEVICE, OUT_DEVICE = 0, 1, 2
+MEM_HOST, FRAMES_DEVICE, OUT_DEVICE, FACES_DEVICE = 0, 1, 2, 4
 DECODED_YCBCR, DECODED_NRGBA, DECODED_RGBA, DECODED_GRAY = 0, 1, 2, 3
 DECODED_GRAY16, DECODED_RGBA64, DECODED_NRGBA64, DECODED_CMYK, DECODED_PALETTED = 5, 6, 7, 8, 9
 
@@ -49,7 +49,7 @@ ABI_SYMBOLS = [
     "pigo_run_cascade_images_angles", "pigo_detect_images_angles", "pigo_gray_images", "pigo_cascade_block_table",
     "pigo_run_cascade_images_sharded", "pigo_detect_images_sharded", "pigo_run_cascade_decoded_sharded", "pigo_detect_decoded_sharded",
     "pigo_shard_plan", "pigo_describe_plan_frames", "pigo_run_cascade_images_sweep", "pigo_detect_images_sweep",
-    "pigo_run_cascade_images_params", "pigo_detect_images_params",
+    "pigo_run_cascade_images_params", "pigo_detect_images_params", "pigo_blur_faces", "pigo_blur_decoded",
 ]
 
 
@@ -131,6 +131,8 @@ def lib() -> C.CDLL:
         L.pigo_detect_images_sweep.argtypes = [vp, vp, vp, vp, i, vp, i, vp, i, vp, vp, u64, vp, vp, i, vp, vp, C.c_uint, vp]
         L.pigo_run_cascade_images_params.argtypes = [vp, vp, i, vp, vp, vp, i, vp, C.c_uint, vp]
         L.pigo_detect_images_params.argtypes = [vp, vp, vp, vp, i, vp, i, vp, vp, vp, vp, u64, vp, i, vp, vp, C.c_uint, vp]
+        L.pigo_blur_faces.argtypes = [vp, i, vp, i, vp, vp, C.c_uint, vp]
+        L.pigo_blur_decoded.argtypes = [vp, vp, i, vp, vp, d, i, vp, vp, i, vp, C.c_uint, vp]
         _lib = L
     return _lib
 
@@ -531,6 +533,34 @@ class Pigo:
         return self._retry_cap(n, cap_per_image, lambda out, cap, cnt: lib().pigo_run_cascade_decoded_sharded(
             self._h, desc, n, ang.ctypes.data if ang is not None else None, cp.MinSize, cp.MaxSize, cp.ShiftFactor, cp.ScaleFactor, out, cap, cnt))
 
+    def BlurDecoded(self, sources: Sequence["DecodedImage"], cps: Sequence[CascadeParams], angles: Optional[Sequence[float]], iou: float,
+                    params: "BlurParams", det_cap: int = 0, face_cap: Optional[int] = None, device_sources: bool = False, stream=None):
+        """Blurs the faces of decoded images in place, in one call (pigo_blur_decoded): gray_images of `sources`, RunCascade of
+        image i with cps[i]'s MinSize / MaxSize / ShiftFactor / ScaleFactor at angles[i] (None = unrotated), ClusterDetections(iou),
+        then blur_faces on every cluster.  Returns the face lists, list i as ClusterDetections returns it for image i.  An entry
+        past det_cap raw detections (0 = 2048) leaves the planes alone and is retried with a larger det_cap; face_cap None
+        returns every cluster, a smaller face_cap that an image exceeds raises PIGO_E_CAP after the blur."""
+        self._need()
+        n = len(sources)
+        desc = decoded_descs(sources)
+        prm = cascade_params_array(cps)
+        if len(cps) != n:
+            raise ValueError("cps must have one entry per source")
+        ang = _angles_array(angles, n)
+        flags = FRAMES_DEVICE if device_sources else MEM_HOST
+        sptr = (stream.cuda_stream if hasattr(stream, "cuda_stream") else int(stream)) if stream is not None else None
+        while True:
+            cap = face_cap if face_cap is not None else (det_cap or 2048)
+            faces = np.zeros((n, max(cap, 1)), dtype=DET_DTYPE)
+            cnt = np.zeros(max(n, 1), dtype=np.int32)
+            rc = lib().pigo_blur_decoded(self._h, desc, n, prm, ang.ctypes.data if ang is not None else None, iou, det_cap, C.byref(params),
+                                         faces.ctypes.data, cap, cnt.ctypes.data, flags, sptr)
+            if rc == PIGO_E_CAP and "raw detections" in lib().pigo_last_error().decode():
+                det_cap = 4 * (det_cap or 2048)
+                continue
+            _check(rc)
+            return [_array_to_dets(faces[i, :cnt[i]]) for i in range(n)]
+
     @staticmethod
     def _retry_cap(n: int, cap: int, fn):
         """Calls fn(out, cap, counts) until the output capacity is enough (PIGO_E_CAP retries with the reported count)."""
@@ -930,6 +960,37 @@ def gray_images(sources: Sequence[DecodedImage], stream=None, device_sources: bo
     size = C.c_size_t(arena.numel())
     _check(lib().pigo_gray_images(desc, n, arena.data_ptr() if arena.numel() else None, C.byref(size), imgs, flags, sptr))
     return arena, [DeviceImage(imgs[k].pixels, imgs[k].rows, imgs[k].cols, imgs[k].dim) for k in range(n)]
+
+
+class BlurParams(C.Structure):
+    """pigo_blur_params (include/pigo_b200.h): faces with Q >= min_q are blurred over a disc of radius int(Scale*disc_ratio)
+    with a box of radius min(1023, max(radius, int(Scale*radius_ratio))).  examples/facedet/faceblur.py's values are
+    BlurParams(5.0, 0.5, 0.0, 15)."""
+    _fields_ = [("min_q", C.c_double), ("disc_ratio", C.c_double), ("radius_ratio", C.c_double), ("radius", C.c_int32)]
+
+
+def blur_faces(sources: Sequence[DecodedImage], faces, counts, params: BlurParams, stream=None, device_sources: bool = False,
+               device_faces: bool = False):
+    """Blurs the faces of every source in place (pigo_blur_faces).  faces is [N][face_cap] DET_DTYPE and counts [N] (what
+    cluster_batch_array and the pipeline calls return), or with device_faces device pointers / CUDA tensors of that layout
+    (faces then a tensor of shape [N, face_cap, 4] int32, or (pointer, face_cap)).  Planes are host numpy arrays, written
+    back before return, or (device_sources) device pointers / CUDA tensors; `stream` (a torch.cuda.Stream or a cudaStream_t as
+    int) orders the call on the caller's stream, and with device planes the call then returns without synchronising."""
+    n = len(sources)
+    desc = decoded_descs(sources)
+    if device_faces:
+        fptr, face_cap = (int(faces.data_ptr()), int(faces.shape[1])) if hasattr(faces, "data_ptr") else (int(faces[0]), int(faces[1]))
+        cptr = int(counts.data_ptr()) if hasattr(counts, "data_ptr") else int(counts)
+    else:
+        f = np.ascontiguousarray(faces, dtype=DET_DTYPE).reshape(n, -1) if n else np.zeros((0, 0), dtype=DET_DTYPE)
+        face_cap = f.shape[1] if n else 0
+        c = np.ascontiguousarray(counts, dtype=np.int32).reshape(-1)
+        if len(c) != n:
+            raise ValueError("counts must have one entry per source")
+        fptr, cptr = (f.ctypes.data if f.size else None), (c.ctypes.data if n else None)
+    flags = (FRAMES_DEVICE if device_sources else MEM_HOST) | (FACES_DEVICE if device_faces else 0)
+    sptr = (stream.cuda_stream if hasattr(stream, "cuda_stream") else int(stream)) if stream is not None else None
+    _check(lib().pigo_blur_faces(desc, n, fptr, face_cap, cptr, C.byref(params), flags, sptr))
 
 
 class DeviceFrames:

@@ -35,7 +35,7 @@ struct TimingSlot {
 static TimingSlot g_tslot[T_NSLOTS];
 static std::mutex g_tmu;
 static const char* kSlotNames[T_NSLOTS] = {"tiled", "gather", "deep", "finalize", "cluster", "puploc", "gray", "seeds", "rottab", "ycbcr", "gray_images", "merge", "region",
-                                             "puploc_warp"};
+                                             "puploc_warp", "blur"};
 
 void timing_reset() {
   std::lock_guard<std::mutex> g(g_tmu);
@@ -2487,6 +2487,261 @@ int pigo_shard_plan(const pigo_image* images, int nimages, const double* angles,
   const std::vector<int> cut = plan_shards(ip.wins, angles, nshards);
   *n_used = (int)cut.size() - 1;
   if (first) std::copy(cut.begin(), cut.end(), first);
+  return PIGO_OK;
+}
+
+}  // extern "C"
+
+// ---- face blur of decoded images (pigo_blur_faces, pigo_blur_decoded) ----------------------------------------------------------
+// The formats the blur writes: one byte per channel.
+static bool blur_format(int format) {
+  return format == PIGO_DECODED_YCBCR || format == PIGO_DECODED_NRGBA || format == PIGO_DECODED_RGBA || format == PIGO_DECODED_GRAY ||
+         format == PIGO_DECODED_CMYK;
+}
+
+// What both blur calls check before any device work: the sources as pigo_gray_images checks them, their formats, no repeated
+// descriptor (a plane is blurred once per call), the parameters and face_cap.
+static int check_blur_args(const pigo_decoded* src, int n, int face_cap, const pigo_blur_params* bp) {
+  int rc = check_decoded_args(src, n);
+  if (rc) return rc;
+  for (int i = 0; i < n; ++i)
+    if (!blur_format(src[i].format))
+      return set_err(PIGO_E_INVALID, "source %d: format %d cannot be blurred (YCbCr, NRGBA, RGBA, Gray and CMYK can)", i, src[i].format);
+  std::vector<size_t> off;
+  std::vector<char> first;
+  arena_layout(src, n, off, first);
+  for (int i = 0; i < n; ++i)
+    if (!first[i]) return set_err(PIGO_E_INVALID, "source %d repeats an earlier descriptor", i);
+  if (!bp) return set_err(PIGO_E_INVALID, "null blur params");
+  if (bp->radius < 0 || bp->radius > 1023) return set_err(PIGO_E_INVALID, "radius %d outside 0..1023", bp->radius);
+  for (double r : {bp->disc_ratio, bp->radius_ratio})
+    if (!(r >= 0.0 && r <= 16.0)) return set_err(PIGO_E_INVALID, "disc_ratio and radius_ratio must be in 0..16");
+  if (std::isnan(bp->min_q)) return set_err(PIGO_E_INVALID, "NaN min_q");
+  if (face_cap < 0) return set_err(PIGO_E_INVALID, "negative face_cap");
+  return PIGO_OK;
+}
+
+// Samples per row (in bytes) and rows of plane k of a blur source; 0 rows: the format has no plane k.
+struct PlaneRows {
+  size_t row_bytes;
+  int rows;
+};
+static PlaneRows blur_plane_rows(const pigo_decoded& d, int k) {
+  if (d.format == PIGO_DECODED_YCBCR && k > 0) {
+    const int ys = chroma_yshift(d.subsample);
+    const YCbCrExtent e = ycbcr_extent(d.subsample, d.min_x, d.min_y, d.width, d.height, d.stride[0], d.stride[1]);
+    return PlaneRows{(size_t)e.c_cols, ((d.min_y + d.height - 1) >> ys) - (d.min_y >> ys) + 1};
+  }
+  if (k > 0) return PlaneRows{0, 0};
+  return PlaneRows{(size_t)d.width * (d.format == PIGO_DECODED_YCBCR ? 1 : decoded_bpp(d.format)), d.height};
+}
+
+// Host planes of blur sources into w->frames (each 256-byte aligned, the bytes from the rectangle's origin to its last
+// sample); dev[i] = src[i] with those device copies as its planes.
+static int stage_blur_planes(Workspace* w, const pigo_decoded* src, int n, cudaStream_t st, std::vector<pigo_decoded>& dev) {
+  std::vector<size_t> at((size_t)n * 3);
+  size_t total = 0;
+  for (int i = 0; i < n; ++i)
+    for (int k = 0; k < 3; ++k) {
+      at[(size_t)i * 3 + k] = total;
+      total += (decoded_plane_bytes(src[i], k) + 255) & ~(size_t)255;
+    }
+  const int rc = w->frames.reserve(total + 256);
+  if (rc) return rc;
+  for (int i = 0; i < n; ++i)
+    for (int k = 0; k < 3; ++k) {
+      const size_t b = decoded_plane_bytes(src[i], k);
+      if (!b) continue;
+      uint8_t* d = (uint8_t*)w->frames.p + at[(size_t)i * 3 + k];
+      CUDA_TRY(cudaMemcpyAsync(d, src[i].plane[k], b, cudaMemcpyHostToDevice, st));
+      dev[i].plane[k] = d;
+    }
+  return PIGO_OK;
+}
+
+// The device copies back into the host planes: each row's samples only, never the bytes past a row's end.
+static int unstage_blur_planes(const std::vector<pigo_decoded>& dev, const pigo_decoded* src, int n, cudaStream_t st) {
+  for (int i = 0; i < n; ++i)
+    for (int k = 0; k < 3; ++k) {
+      const PlaneRows pr = blur_plane_rows(src[i], k);
+      if (pr.rows == 0) continue;
+      const size_t pitch = (size_t)src[i].stride[k == 0 ? 0 : 1];
+      CUDA_TRY(cudaMemcpy2DAsync((void*)src[i].plane[k], pitch, dev[i].plane[k], pitch, pr.row_bytes, pr.rows, cudaMemcpyDeviceToHost, st));
+    }
+  return PIGO_OK;
+}
+
+// The blur of the device planes of dsrc[0..n) around faces [n][cap] / n_faces [n] (device pointers) on st, with w's scratch:
+// the planes' summed-area tables (scratch_a), the entries' luma maps (scratch_b), the face records and entry firsts
+// (scratch_c), and the plane / entry tables made here (img_tab).
+static int blur_on(int dev, Workspace* w, cudaStream_t st, const pigo_decoded* dsrc, int n, const pigo_det* d_faces, int cap,
+                   const int32_t* d_nfaces, const pigo_blur_params& bp) {
+  auto round256 = [](size_t b) { return (b + 255) & ~(size_t)255; };
+  std::vector<BlurUnit> units;
+  std::vector<BlurEntry> entries(n);
+  std::vector<uint64_t> rf(1, 0), sf(1, 0), pf(1, 0);
+  std::vector<size_t> sat_at, map_at(n);
+  size_t sat_bytes = 0, map_bytes = 0;
+  for (int i = 0; i < n; ++i) {
+    const pigo_decoded& d = dsrc[i];
+    map_at[i] = map_bytes;
+    map_bytes += round256((size_t)d.width * d.height * 4);
+    entries[i].width = d.width;
+    entries[i].height = d.height;
+    for (int k = 0; k < 3; ++k) {
+      const PlaneRows pr = blur_plane_rows(d, k);
+      if (pr.rows == 0) continue;
+      BlurUnit u{};
+      u.plane = (uint8_t*)d.plane[k];
+      u.entry = i;
+      u.chans = d.format == PIGO_DECODED_YCBCR || d.format == PIGO_DECODED_GRAY ? 1 : 4;
+      u.w = (int)(pr.row_bytes / u.chans);
+      u.h = pr.rows;
+      u.stride = d.stride[k == 0 ? 0 : 1];
+      if (k > 0) {
+        u.xs = chroma_xshift(d.subsample); u.ys = chroma_yshift(d.subsample);
+        u.min_x = d.min_x; u.min_y = d.min_y;
+      }
+      sat_at.push_back(sat_bytes);
+      sat_bytes += round256((size_t)u.w * u.h * u.chans * 4);
+      rf.push_back(rf.back() + (uint64_t)u.h);
+      sf.push_back(sf.back() + ((uint64_t)u.w * u.chans + 31) / 32);
+      pf.push_back(pf.back() + (uint64_t)u.w * u.h);
+      units.push_back(u);
+    }
+  }
+  const int nunits = (int)units.size();
+  const size_t rec_bytes = round256((size_t)n * cap * sizeof(BlurFace));
+  int rc = PIGO_OK;
+  if ((rc = w->scratch_a.reserve(sat_bytes + 256)) || (rc = w->scratch_b.reserve(map_bytes + 256)) ||
+      (rc = w->scratch_c.reserve(rec_bytes + ((size_t)n + 1) * 8)))
+    return rc;
+  for (int u = 0; u < nunits; ++u) units[u].sat = (uint32_t*)((uint8_t*)w->scratch_a.p + sat_at[u]);
+  for (int i = 0; i < n; ++i) entries[i].map = (uint32_t*)((uint8_t*)w->scratch_b.p + map_at[i]);
+  // one upload: units, entries, then the three per-plane work tables
+  const size_t o_ent = round256((size_t)nunits * sizeof(BlurUnit)), o_rf = o_ent + round256((size_t)n * sizeof(BlurEntry));
+  const size_t tab = ((size_t)nunits + 1) * sizeof(uint64_t), o_sf = o_rf + round256(tab), o_pf = o_sf + round256(tab);
+  std::vector<uint8_t> blob(o_pf + tab);
+  memcpy(blob.data(), units.data(), (size_t)nunits * sizeof(BlurUnit));
+  memcpy(blob.data() + o_ent, entries.data(), (size_t)n * sizeof(BlurEntry));
+  memcpy(blob.data() + o_rf, rf.data(), tab);
+  memcpy(blob.data() + o_sf, sf.data(), tab);
+  memcpy(blob.data() + o_pf, pf.data(), tab);
+  if ((rc = w->img_tab.reserve(blob.size()))) return rc;
+  uint8_t* t = (uint8_t*)w->img_tab.p;
+  CUDA_TRY(cudaMemcpyAsync(t, blob.data(), blob.size(), cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaMemsetAsync(w->scratch_b.p, 0, map_bytes, st));
+  BlurArgs A{};
+  A.units = (const BlurUnit*)t; A.entries = (const BlurEntry*)(t + o_ent);
+  A.row_first = (const uint64_t*)(t + o_rf); A.strip_first = (const uint64_t*)(t + o_sf); A.px_first = (const uint64_t*)(t + o_pf);
+  A.faces = d_faces; A.n_faces = d_nfaces;
+  A.recs = (BlurFace*)w->scratch_c.p; A.entry_first = (uint64_t*)((uint8_t*)w->scratch_c.p + rec_bytes);
+  A.nunits = nunits; A.n = n; A.cap = cap; A.radius = bp.radius;
+  A.min_q = bp.min_q; A.disc_ratio = bp.disc_ratio; A.radius_ratio = bp.radius_ratio;
+  launch_blur(A, rf.back(), sf.back(), pf.back(), device_sms(dev), st);
+  CUDA_TRY(cudaGetLastError());
+  return PIGO_OK;
+}
+
+extern "C" {
+
+int pigo_blur_faces(const pigo_decoded* src, int n, const pigo_det* faces, int face_cap, const int* n_faces, const pigo_blur_params* bp,
+                    unsigned flags, void* stream_) {
+  int rc = check_blur_args(src, n, face_cap, bp);
+  if (rc) return rc;
+  if (n > 0 && !n_faces) return set_err(PIGO_E_INVALID, "null n_faces");
+  if (n > 0 && face_cap > 0 && !faces) return set_err(PIGO_E_INVALID, "null faces");
+  if ((rc = ensure_device())) return rc;
+  if ((rc = refuse_capture("pigo_blur_faces", stream_))) return rc;
+  if (n == 0) return PIGO_OK;
+  const int dev = default_device();
+  Borrow w(g_misc_pool[dev], stream_);
+  if (w.rc) return w.rc;
+  cudaStream_t st = w.st;
+  const bool planes_dev = flags & PIGO_FRAMES_DEVICE, faces_dev = flags & PIGO_FACES_DEVICE;
+  std::vector<pigo_decoded> dsrc(src, src + n);
+  if (!planes_dev && (rc = stage_blur_planes(w, src, n, st, dsrc))) return rc;
+  const pigo_det* d_faces = faces;
+  const int32_t* d_nfaces = n_faces;
+  if (!faces_dev) {
+    const size_t fb = (size_t)n * face_cap * sizeof(pigo_det);
+    if ((rc = w->raw.reserve(fb + 256)) || (rc = w->nout.reserve((size_t)n * 4))) return rc;
+    if (fb) CUDA_TRY(cudaMemcpyAsync(w->raw.p, faces, fb, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(w->nout.p, n_faces, (size_t)n * 4, cudaMemcpyHostToDevice, st));
+    d_faces = (const pigo_det*)w->raw.p;
+    d_nfaces = (const int32_t*)w->nout.p;
+  }
+  cudaEvent_t copied = nullptr;
+  if (planes_dev && stream_ && !faces_dev) {   // host faces are the caller's again once copied; the blur may still run
+    if (!(copied = w->copy_event(0))) return set_err(PIGO_E_CUDA, "event creation failed");
+    CUDA_TRY(cudaEventRecord(copied, st));
+  }
+  if ((rc = blur_on(dev, w, st, dsrc.data(), n, d_faces, face_cap, d_nfaces, *bp))) return rc;
+  if (!planes_dev && (rc = unstage_blur_planes(dsrc, src, n, st))) return rc;
+  if (!planes_dev || !stream_) CUDA_TRY(cudaStreamSynchronize(st));
+  else if (copied) CUDA_TRY(cudaEventSynchronize(copied));
+  return PIGO_OK;
+}
+
+int pigo_blur_decoded(const pigo_cascade* face, const pigo_decoded* src, int n, const pigo_cascade_params* cparams, const double* angles,
+                      double iou_threshold, int det_cap, const pigo_blur_params* bp, pigo_det* faces, int face_cap, int* n_faces,
+                      unsigned flags, void* stream_) {
+  int rc = check_blur_args(src, n, face_cap, bp);
+  if (rc) return rc;
+  if (n > 0 && !cparams) return set_err(PIGO_E_INVALID, "null cparams");
+  if (det_cap < 0) return set_err(PIGO_E_INVALID, "negative det_cap");
+  const std::vector<pigo_image> geo = decoded_geometry(src, n);
+  if ((rc = check_images_args(face, geo.data(), n, faces, face_cap, n_faces))) return rc;
+  ImagePlans ip;
+  if ((rc = images_prologue("pigo_blur_decoded", geo.data(), n, cparams, stream_, ip)) || n == 0) return rc;
+  const int dev = default_device();
+  pigo_cascade* c = const_cast<pigo_cascade*>(face);
+  Borrow w(g_misc_pool[dev], stream_);
+  if (w.rc) return w.rc;
+  cudaStream_t st = w.st;
+  const bool planes_dev = flags & PIGO_FRAMES_DEVICE;
+  const int dcap = det_cap > 0 ? det_cap : 2048;
+  // 1. the planes on the device (host planes cross PCIe here, once), converted to the detector's gray images
+  std::vector<pigo_decoded> dsrc(src, src + n);
+  if (!planes_dev && (rc = stage_blur_planes(w, src, n, st, dsrc))) return rc;
+  std::vector<size_t> off;
+  std::vector<char> first;
+  const size_t gray_bytes = arena_layout(dsrc.data(), n, off, first);
+  if ((rc = w->gray_arena.reserve(gray_bytes + 256))) return rc;
+  uint8_t* gray = (uint8_t*)w->gray_arena.p;
+  if ((rc = gray_images_on(dev, dsrc.data(), n, off, first, gray, PIGO_FRAMES_DEVICE, st))) return rc;
+  std::vector<pigo_image> images(n);
+  for (int i = 0; i < n; ++i) images[i] = pigo_image{gray + off[i], src[i].height, src[i].width, src[i].width};
+  // 2. the scan and 3. the clusters, every cluster kept (at most det_cap per entry)
+  const size_t nd = (size_t)n * dcap;
+  if ((rc = w->raw.reserve(nd * sizeof(pigo_det))) || (rc = w->out.reserve(nd * sizeof(pigo_det))) || (rc = w->nout.reserve((size_t)n * 8)))
+    return rc;
+  pigo_det *d_raw = (pigo_det*)w->raw.p, *d_cl = (pigo_det*)w->out.p;
+  int32_t *d_cnt = (int32_t*)w->nout.p, *d_ncl = d_cnt + n;
+  std::vector<double> uniform;
+  if ((rc = scan_images_on(c, dev, images.data(), n, ip, angles_or(angles, 0.0, n, uniform), d_raw, dcap, d_cnt, PIGO_FRAMES_DEVICE | PIGO_OUT_DEVICE,
+                           st)))
+    return rc;
+  CUDA_TRY(cudaMemsetAsync(d_cl, 0, nd * sizeof(pigo_det), st));
+  if ((rc = cluster_batch_on(dev, d_raw, d_cnt, n, dcap, iou_threshold, d_cl, dcap, d_ncl, PIGO_OUT_DEVICE, st))) return rc;
+  // the counts and the faces that fit to the host: an entry past det_cap must fail before any plane is written
+  std::vector<int32_t> cnt(2 * (size_t)n);
+  CUDA_TRY(cudaMemcpyAsync(cnt.data(), d_cnt, cnt.size() * 4, cudaMemcpyDeviceToHost, st));
+  if (face_cap > 0) {
+    memset(faces, 0, (size_t)n * face_cap * sizeof(pigo_det));
+    CUDA_TRY(cudaMemcpy2DAsync(faces, (size_t)face_cap * sizeof(pigo_det), d_cl, (size_t)dcap * sizeof(pigo_det),
+                               (size_t)std::min(face_cap, dcap) * sizeof(pigo_det), n, cudaMemcpyDeviceToHost, st));
+  }
+  CUDA_TRY(cudaStreamSynchronize(st));
+  for (int i = 0; i < n; ++i)
+    if (cnt[i] > dcap) return set_err(PIGO_E_CAP, "entry %d has %d raw detections, det_cap is %d", i, cnt[i], dcap);
+  std::copy(cnt.begin() + n, cnt.end(), n_faces);
+  // 4. the blur around every cluster, and the host planes back (once)
+  if ((rc = blur_on(dev, w, st, dsrc.data(), n, d_cl, dcap, d_ncl, *bp))) return rc;
+  if (!planes_dev && (rc = unstage_blur_planes(dsrc, src, n, st))) return rc;
+  if (!planes_dev || !stream_) CUDA_TRY(cudaStreamSynchronize(st));
+  for (int i = 0; i < n; ++i)
+    if (n_faces[i] > face_cap) return set_err(PIGO_E_CAP, "entry %d has %d faces, face_cap is %d", i, n_faces[i], face_cap);
   return PIGO_OK;
 }
 

@@ -23,7 +23,7 @@ void raise_dyn_smem(const void* fn, int bytes);
 // brackets, inside T_TILED, only the fused launches that run the region role (after their tensor maps were encoded);
 // T_PUPLOC_WARP brackets, inside T_PUPLOC, only the launches of the 64-bit warp-per-perturbation kernel (puploc_kernel).
 enum TimeSlot { T_TILED = 0, T_GATHER, T_DEEP, T_FINALIZE, T_CLUSTER, T_PUPLOC, T_GRAY, T_SEEDS, T_ROTTAB, T_YCBCR, T_GRAY_IMAGES, T_MERGE, T_REGION,
-                T_PUPLOC_WARP, T_NSLOTS };
+                T_PUPLOC_WARP, T_BLUR, T_NSLOTS };
 void timing_reset();
 void walk_stats_reset();
 long long walk_stats_query(int which);
@@ -184,6 +184,40 @@ struct GraySrc {
   uint8_t* dst;              // the source's slot in the arena: height rows of width bytes
   int32_t format, sub, min_x, min_y, width, height, stride0, stride1;
 };
+
+// ---- face blur (blur.cu) ---------------------------------------------------------------------------------
+// One plane of a blur call, pointers on the device: h rows of w samples of `chans` bytes (1, or 4 for NRGBA, RGBA and CMYK).
+// A chroma plane of a YCbCr entry has its subsampling shifts xs, ys and the rectangle origin (min_x, min_y), which place each
+// sample's anchor luma pixel; every other plane has all four 0.
+struct BlurUnit {
+  uint8_t* plane;
+  uint32_t* sat;    // the plane's summed-area table, [h][w][chans] uint32 (mod 2^32)
+  int32_t entry, stride, w, h, chans, xs, ys, min_x, min_y;
+};
+// One entry of a blur call: its luma size and map, [height][width] uint32 = 0 (not covered) or Rmax + 1.
+struct BlurEntry {
+  uint32_t* map;
+  int32_t width, height;
+};
+// Face k of an entry as blur_plan_kernel leaves it: centre, d^2, first disc row inside the image, R, and its first work item
+// (one item per disc row inside the image) counted from the entry's first.
+struct BlurFace {
+  long long row, col, d2;
+  uint64_t first;
+  int32_t r0, R;
+};
+struct BlurArgs {
+  const BlurUnit* units;
+  const BlurEntry* entries;
+  const uint64_t *row_first, *strip_first, *px_first;   // per plane: first row / 32-column strip / sample of the call (host-made)
+  const pigo_det* faces;                                // [n][cap]
+  const int32_t* n_faces;                               // [n], clamped to 0..cap
+  BlurFace* recs;                                       // [n][cap]
+  uint64_t* entry_first;                                // [n + 1]: first disc-row work item of each entry
+  int32_t nunits, n, cap, radius;
+  double min_q, disc_ratio, radius_ratio;
+};
+void launch_blur(const BlurArgs& A, uint64_t rows, uint64_t strips, uint64_t samples, int num_sms, cudaStream_t st);
 
 // The formats gray_images_kernel<true> converts: Gray16, RGBA64, NRGBA64, CMYK and Paletted.
 __host__ __device__ __forceinline__ bool decoded_wide(int format) { return format >= PIGO_DECODED_GRAY16; }
